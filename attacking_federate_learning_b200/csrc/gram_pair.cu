@@ -13,15 +13,21 @@
 //                    error of d2 = s_ii + s_jj - 2 s_ij then scales with the distances to an honest client -
 //                    main.py:28 makes ids >= f honest - instead of with ||g||^2).  Per 16 columns:
 //                        S += b1_I b1_J^T,  S += b1_I b2_J^T,  S += b2_I b1_J^T      (dropped: b2 b2^T, ~2^-17)
+//                    With one tile (N <= 128) every pair is on the diagonal tile, so the converters write 2 b2 (exact)
+//                    and two products suffice: M += b1 b1^T + b1 (2 b2)^T, and S = (M + M^T) / 2, formed in float64
+//                    from the split sums (pair_reduce_kernel keeps both triangles, pair_to_sqdist_kernel adds them).
+//                    Its boxes have N rounded up to 8 rows; rows past them stay zero from the kernel's start.
 //       kModeTf32x2  fp32 clients, 32-column k-blocks delivered by TMA already swizzled (SWIZZLE_128B).  The
 //                    converter truncates the box in place to hi = the top 10 mantissa bits and writes lo = g - hi
 //                    at the same offsets 16 KB further; per 8 columns S += hi hi^T + hi lo^T + lo hi^T (dropped:
 //                    lo lo^T, <= 2^-20 relative).  No centring.
 //       kModeBf16In  bf16 clients: TMA delivers ready-made SWIZZLE_128B operand tiles, S += g_I g_J^T exactly
 //                    (only the fp32 accumulation rounds), no converter pass.
-//     EVERY pair - diagonal ones too - issues the same sequence on the same K partition, so two clients with
-//     identical rows get bit-identical s_ii, s_jj and s_ij wherever their tiles are, and their distance is exactly 0
-//     (ALIE makes rows 0..f-1 one array; Krum's [1, 0, 2, ...] tie-break depends on it).
+//     With more than one tile EVERY pair - diagonal ones too - issues the same sequence on the same K partition, so two
+//     clients with identical rows get bit-identical s_ii, s_jj and s_ij wherever their tiles are, and their distance is
+//     exactly 0 (ALIE makes rows 0..f-1 one array; Krum's [1, 0, 2, ...] tie-break depends on it).  The one-tile
+//     symmetric form keeps this: identical rows i, k give M_ik = M_ki = M_ii = M_kk bit for bit, and M_ij + M_ji =
+//     M_kj + M_jk.  (Across tiles an off-diagonal pair would need all three products to match the diagonal ones.)
 //   * Two consumer warpgroups own rows 0..63 and 64..127 of the I tile and issue wgmma.m64n128 with both operands
 //     read from shared memory.  The tensor core truncates while it accumulates, so its chains stay short: the
 //     register accumulator restarts every `flush` k-blocks and is added (round to nearest) to a running fp32 sum.
@@ -44,6 +50,7 @@ constexpr int kPPartElems = 128 * 128;       // S per (pair, split)
 
 struct PairParams {
   int n, tiles, pairs, splits;
+  int box_rows;         // rows per TMA box: 128, or with one bf16x2 tile N rounded up to 8
   int kblocks;          // ceil(d / columns per k-block)
   int flush;            // k-blocks per tensor-core accumulation chain
   int center;           // kModeBf16x2: 0 no centring, 1 subtract cvec, 2 (N <= 128) subtract the mean of box rows crow0..
@@ -63,9 +70,12 @@ __device__ __forceinline__ void sts64_p(uint32_t addr, uint32_t a, uint32_t b) {
 }
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
-template <int kMode>
+// kSym: kModeBf16x2 with one tile, the symmetric two-product form on boxes of p.box_rows <= 128 rows (a template
+// parameter: a runtime branch between the two MMA sequences makes ptxas fence every k-block's wgmma issue)
+template <int kMode, bool kSym>
 __global__ void __launch_bounds__(kPThreads, 1)
 gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
+  static_assert(!kSym || kMode == kModeBf16x2, "the symmetric form is a bf16x2 form");
   constexpr uint32_t kBoxBytes = kMode == kModeBf16x2 ? kPSlotBytes : kPSlotBytes / 2;
   constexpr int kCols = kMode == kModeTf32x2 ? 32 : kPCols;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -85,7 +95,23 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
   const uint32_t ring = smem_u32(smem);
   // box b of this CTA (b = k-block * nbx + which tile) lives in ring slot b % kPSlots
   auto phase_of = [](int b) -> uint32_t { return static_cast<uint32_t>(b / kPSlots) & 1u; };
+  // Converter wait for box b.  The slot's previous box b - kPSlots belongs to another converter warp, and TMA loads do
+  // not complete in issue order: while that box is still in flight raw_full is one phase behind, and a parity wait for
+  // box b would pass at once.  So first wait until the previous box has been converted (hence has landed).  Parity
+  // waits only tell adjacent phases apart; both are valid here: conv_done is at the previous box's phase or one past
+  // it (box b, which only this warp converts, has not been), and then raw_full is at box b's phase or one past it.
+  auto wait_raw = [&](int b) {
+    if (b >= kPSlots) mbar_wait_fast(&conv_done[b % kPSlots], phase_of(b - kPSlots));
+    mbar_wait_fast(&raw_full[b % kPSlots], phase_of(b));
+  };
+  const uint32_t box_bytes = kSym ? static_cast<uint32_t>(p.box_rows) * 256u : kBoxBytes;
 
+  if (kSym) {
+    // rows box_rows..127 of every slot: zero bf16 atoms, written once here and never again by TMA or the converters
+    for (uint32_t o = box_bytes + threadIdx.x * 16u; o < kPSlotBytes; o += kPThreads * 16u)
+      for (int s = 0; s < kPSlots; ++s) sts128(ring + static_cast<uint32_t>(s) * kPSlotBytes + o, make_float4(0.f, 0.f, 0.f, 0.f));
+    fence_proxy_async_smem();                               // the wgmma reads them through the async proxy
+  }
   if (threadIdx.x == 0) {
     for (int s = 0; s < kPSlots; ++s) {
       mbar_init(&raw_full[s], 1);
@@ -105,7 +131,7 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
         for (int b = 0; b < nboxes; ++b) {
           const int s = b % kPSlots;
           mbar_wait(&slot_free[s], phase_of(b) ^ 1u);
-          mbar_arrive_expect_tx(&raw_full[s], kBoxBytes);
+          mbar_arrive_expect_tx(&raw_full[s], box_bytes);
           tma_load_2d(smem + static_cast<size_t>(s) * kPSlotBytes, &tmap, &raw_full[s],
                       (split + (b / nbx) * p.splits) * kCols, ((b % nbx) == 0 ? ti : tj) * 128, pol);
         }
@@ -129,11 +155,13 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
         const int64_t col = static_cast<int64_t>(split + (box / nbx) * p.splits) * kPCols + c16 * 4;
         return __ldg(reinterpret_cast<const float4*>(p.cvec + col));
       };
+      const int units = box_bytes / 2048u;
+      constexpr float two = kSym ? 2.f : 1.f;               // kSym: the second atom is 2 b2 (exact, a power of 2)
       float4 cen = load_center(w);
       for (int box = w; box < nboxes; box += kConverters) {
         const int s = box % kPSlots;
         const float4 cnext = load_center(box + kConverters);   // in flight while this box is converted
-        mbar_wait_fast(&raw_full[s], phase_of(box));
+        wait_raw(box);
         const uint32_t base = ring + static_cast<uint32_t>(s) * kPSlotBytes;
         if (p.center == 2) {
           // one tile: the centre rows are part of this box, so the centre costs no extra HBM traffic; same summation
@@ -152,18 +180,18 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
 #pragma unroll
         for (int u = 0; u < 4; ++u) v[u] = lds128(base + src_lane + static_cast<uint32_t>(u) * 512u);
 #pragma unroll 1
-        for (int unit = 0; unit < 16; ++unit) {
+        for (int unit = 0; unit < units; ++unit) {
           uint32_t h[4][2], l[4][2];
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             const float x0 = v[u].x - cen.x, x1 = v[u].y - cen.y, x2 = v[u].z - cen.z, x3 = v[u].w - cen.w;
             h[u][0] = pack_bf16x2_rn_p(x0, x1);
             h[u][1] = pack_bf16x2_rn_p(x2, x3);
-            l[u][0] = pack_bf16x2_rn_p(x0 - __uint_as_float(h[u][0] << 16), x1 - __uint_as_float(h[u][0] & 0xFFFF0000u));
-            l[u][1] = pack_bf16x2_rn_p(x2 - __uint_as_float(h[u][1] << 16), x3 - __uint_as_float(h[u][1] & 0xFFFF0000u));
+            l[u][0] = pack_bf16x2_rn_p(two * (x0 - __uint_as_float(h[u][0] << 16)), two * (x1 - __uint_as_float(h[u][0] & 0xFFFF0000u)));
+            l[u][1] = pack_bf16x2_rn_p(two * (x2 - __uint_as_float(h[u][1] << 16)), two * (x3 - __uint_as_float(h[u][1] & 0xFFFF0000u)));
           }
           const uint32_t ub = base + static_cast<uint32_t>(unit) * 2048u;
-          if (unit + 1 < 16) {                              // next unit's loads before this unit's stores
+          if (unit + 1 < units) {                           // next unit's loads before this unit's stores
 #pragma unroll
             for (int u = 0; u < 4; ++u) v[u] = lds128(ub + 2048u + src_lane + static_cast<uint32_t>(u) * 512u);
           }
@@ -183,7 +211,7 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
       const int w = warp - 1;
       for (int box = w; box < nboxes; box += kConverters) {
         const int s = box % kPSlots;
-        mbar_wait_fast(&raw_full[s], phase_of(box));
+        wait_raw(box);
         const uint32_t base = ring + static_cast<uint32_t>(s) * kPSlotBytes + static_cast<uint32_t>(lane) * 16u;
 #pragma unroll 1
         for (int c0 = 0; c0 < 1024; c0 += 8 * 32) {         // 1024 16-byte chunks per 16 KB box
@@ -245,6 +273,12 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
             wgmma_m64n128k8_tf32(acc, d_1i + 2 * ks, d_2j + 2 * ks, 1u);           // hi_I lo_J^T
             wgmma_m64n128k8_tf32(acc, d_2i + 2 * ks, d_1j + 2 * ks, 1u);           // lo_I hi_J^T
           }
+        } else if (kSym) {
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            wgmma_m64n128k16_bf16(acc, d_1i + 2 * ks, d_1j + 2 * ks, first | ks);  // b1 b1^T
+            wgmma_m64n128k16_bf16(acc, d_1i + 2 * ks, d_2j + 2 * ks, 1u);          // b1 (2 b2)^T
+          }
         } else {
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {
@@ -278,10 +312,11 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
 }
 
 // Split reduction of the lower-triangular tile pairs: S[i][j] (i >= j, float64) = sum over splits, in a fixed order
-// (threadIdx.y owns a contiguous range, the kPSy partial sums are added in order).
+// (threadIdx.y owns a contiguous range, the kPSy partial sums are added in order).  sym (one bf16x2 tile, whose
+// partials hold M, not S): every j, so that S[i][j] + S[j][i] = 2 S_ij for pair_to_sqdist_kernel.
 constexpr int kPSy = 8;
 __global__ void __launch_bounds__(128 * kPSy)
-pair_reduce_kernel(const float* __restrict__ parts, int n, int splits, double* __restrict__ S) {
+pair_reduce_kernel(const float* __restrict__ parts, int n, int splits, int sym, double* __restrict__ S) {
   __shared__ double sh[kPSy][128];
   const int i = blockIdx.x, tj = blockIdx.y;
   const int ti = i >> 7, ii = i & 127;
@@ -291,12 +326,13 @@ pair_reduce_kernel(const float* __restrict__ parts, int n, int splits, double* _
   const int pair = ti * (ti + 1) / 2 + tj;
   const float* base = parts + static_cast<size_t>(pair) * splits * kPPartElems + ii * 128 + jj;
   const int s0 = splits * sy / kPSy, s1 = splits * (sy + 1) / kPSy;
+  const bool want = (sym || j <= i) && j < n;
   double acc = 0.0;
-  if (j <= i && j < n)
+  if (want)
     for (int s = s0; s < s1; ++s) acc += static_cast<double>(base[static_cast<size_t>(s) * kPPartElems]);
   sh[sy][jj] = acc;
   __syncthreads();
-  if (sy == 0 && j <= i && j < n) {
+  if (sy == 0 && want) {
     double t = sh[0][jj];
 #pragma unroll
     for (int y = 1; y < kPSy; ++y) t += sh[y][jj];
@@ -305,15 +341,18 @@ pair_reduce_kernel(const float* __restrict__ parts, int n, int splits, double* _
 }
 
 // d2_ij = (S_hh + S_ll) - 2 S_hl with h = max(i, j), l = min(i, j): exactly symmetric, zero diagonal, and exactly
-// zero between clients whose rows are identical.
-__global__ void pair_to_sqdist_kernel(const double* __restrict__ S, int n, double* __restrict__ d2) {
+// zero between clients whose rows are identical.  sym: 2 S_hl = S[h][l] + S[l][h], the split sums of M_hl and M_lh
+// (a floating-point addition is commutative, so identical rows still give bit-identical table rows).
+__global__ void pair_to_sqdist_kernel(const double* __restrict__ S, int n, int sym, double* __restrict__ d2) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = blockIdx.y;
   if (j >= n) return;
   double v = 0.0;
   if (i != j) {
     const int lo = min(i, j), hi = max(i, j);
-    v = (S[static_cast<size_t>(hi) * n + hi] + S[static_cast<size_t>(lo) * n + lo]) - 2.0 * S[static_cast<size_t>(hi) * n + lo];
+    const double s_hl = S[static_cast<size_t>(hi) * n + lo];
+    v = (S[static_cast<size_t>(hi) * n + hi] + S[static_cast<size_t>(lo) * n + lo]) -
+        (sym ? s_hl + S[static_cast<size_t>(lo) * n + hi] : 2.0 * s_hl);
   }
   d2[static_cast<size_t>(i) * n + j] = v;
 }
@@ -358,14 +397,14 @@ size_t pair_parts_bytes(int n, int64_t d) {
   return static_cast<size_t>(pairs) * pair_splits(n, d) * kPPartElems * sizeof(float);
 }
 
-template <int kMode>
+template <int kMode, bool kSym>
 static int launch_mode(const CUtensorMap& tmap, const PairParams& p, cudaStream_t stream) {
   const size_t smem = static_cast<size_t>(kPSlots) * kPSlotBytes + 1024;
   static int smem_attr_done[kMaxDevices] = {0};
-  AFL_CUDA(ensure_dyn_smem(gram_pair_kernel<kMode>, static_cast<int>(smem), smem_attr_done));
+  AFL_CUDA(ensure_dyn_smem(gram_pair_kernel<kMode, kSym>, static_cast<int>(smem), smem_attr_done));
   {
     ProfScope ps("gram_pair", stream);
-    gram_pair_kernel<kMode><<<p.pairs * p.splits, kPThreads, smem, stream>>>(tmap, p);
+    gram_pair_kernel<kMode, kSym><<<p.pairs * p.splits, kPThreads, smem, stream>>>(tmap, p);
   }
   AFL_LAUNCH_CHECK("gram_pair_kernel");
   return AFL_OK;
@@ -388,6 +427,8 @@ int launch_pair(const void* Gv, int mode, int n, int64_t d, int64_t ld, float* p
   const int cols = mode == kModeTf32x2 ? 32 : kPCols;
   PairParams p{};
   p.n = n; p.tiles = (n + 127) / 128; p.pairs = p.tiles * (p.tiles + 1) / 2;
+  const int sym = mode == kModeBf16x2 && p.tiles == 1;     // the kernel's kSym
+  p.box_rows = sym ? (n + 7) / 8 * 8 : 128;
   p.splits = pair_splits(n, d);
   p.kblocks = static_cast<int>((d + cols - 1) / cols);
   // `flush` counts 64-column k-blocks of 12 chained bf16 MMAs.  A split-TF32 k-block already chains 12 MMAs over 32 columns,
@@ -409,20 +450,21 @@ int launch_pair(const void* Gv, int mode, int n, int64_t d, int64_t ld, float* p
   CUtensorMap tmap;
   const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(d), static_cast<cuuint64_t>(n)};
   const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ld) * (bf16 ? 2 : 4)};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(cols), 128};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(cols), static_cast<cuuint32_t>(p.box_rows)};
   const cuuint32_t estride[2] = {1, 1};
   CUresult r = enc(&tmap, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(Gv), gdim,
                    gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    mode == kModeBf16x2 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed: %d", static_cast<int>(r)); return AFL_ERR_CUDA; }
-  int rc = mode == kModeBf16x2 ? launch_mode<kModeBf16x2>(tmap, p, stream)
-         : mode == kModeTf32x2 ? launch_mode<kModeTf32x2>(tmap, p, stream)
-                               : launch_mode<kModeBf16In>(tmap, p, stream);
+  int rc = sym                   ? launch_mode<kModeBf16x2, true>(tmap, p, stream)
+         : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, false>(tmap, p, stream)
+         : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, false>(tmap, p, stream)
+                               : launch_mode<kModeBf16In, false>(tmap, p, stream);
   if (rc) return rc;
-  pair_reduce_kernel<<<dim3(n, p.tiles), dim3(128, kPSy), 0, stream>>>(parts, n, p.splits, S);
+  pair_reduce_kernel<<<dim3(n, p.tiles), dim3(128, kPSy), 0, stream>>>(parts, n, p.splits, sym, S);
   AFL_LAUNCH_CHECK("pair_reduce_kernel");
-  pair_to_sqdist_kernel<<<dim3((n + 127) / 128, n), 128, 0, stream>>>(S, n, d2_out);
+  pair_to_sqdist_kernel<<<dim3((n + 127) / 128, n), 128, 0, stream>>>(S, n, sym, d2_out);
   AFL_LAUNCH_CHECK("pair_to_sqdist_kernel");
   return AFL_OK;
 }

@@ -81,11 +81,10 @@ def krum_from_sqdist(d2: torch.Tensor, users_count: int, corrupted_count: int, i
     L = nat.lib()
     with torch.cuda.device(d2.device):
         ws = Workspace.get(d2.device, "select", L.afl_select_workspace_bytes(n))
-        scratch = Workspace.get(d2.device, "dist", n * n * 4)
         if idx is None:
             idx = torch.empty(1, dtype=torch.int32, device=d2.device)
-        nat.check(L.afl_krum_from_sqdist(d2.data_ptr(), n, users_count, corrupted_count, scratch.data_ptr(),
-                                         idx.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(d2)))
+        nat.check(L.afl_krum_from_sqdist(d2.data_ptr(), n, users_count, corrupted_count, idx.data_ptr(),
+                                         ws.data_ptr(), ws.numel(), _stream_ptr(d2)))
     return idx
 
 

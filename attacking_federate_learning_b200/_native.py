@@ -33,7 +33,7 @@ SIGNATURES = {
     "afl_sqdist_to_dist": (_i, [_vp, _i, _vp, _vp]),
     "afl_select_workspace_bytes": (_sz, [_i]),
     "afl_krum_select": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
-    "afl_krum_from_sqdist": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "afl_krum_from_sqdist": (_i, [_vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "afl_bulyan_select": (_i, [_vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "afl_trimmed_mean": (_i, [_vp, _i, _i64, _i64, _i, _vp, _i, _i, _vp, _vp]),
     "afl_gather_row": (_i, [_vp, _i, _i64, _i64, _i, _vp, _vp, _vp]),

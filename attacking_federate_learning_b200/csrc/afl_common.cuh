@@ -52,6 +52,22 @@ static inline cudaError_t ensure_dyn_smem(K kernel, int bytes, int (&done)[kMaxD
 
 constexpr int kMaxWorld = 16;            // ranks of one peer-exchange context (csrc/xgpu.cu)
 
+// Arguments of the Krum kernel (csrc/select.cu).  The row of distances comes from `dist` (a caller's fp32 table) when
+// it is set, otherwise from the float64 d2 tables tab[0..world), summed in rank order; with world > 1 the kernel first
+// waits until `flags` reach `epoch` and reads the peers' tables through their mappings.
+struct KrumParams {
+  const double* tab[kMaxWorld];
+  const unsigned long long* flags;
+  unsigned long long epoch;
+  int world;
+  const float* dist;
+  int n, take;
+  float* score;                           // [n]
+  unsigned int* done;                     // last-CTA counter: zero at launch, reset by the kernel
+  int* idx_dev;
+  int* idx_host; int* status_host;        // mapped host words of the peer path, or NULL
+};
+
 // Optional CUDA-event bracket around a kernel launch (active only after afl_profile_enable(1)).
 struct ProfScope {
   ProfScope(const char* name, cudaStream_t stream);
@@ -95,6 +111,35 @@ __device__ __forceinline__ uint4 ldg_stream_u4(const uint4* p) {
   return r;
 }
 __device__ __forceinline__ float bf16_bits_to_f32(uint32_t b16) { return __uint_as_float(b16 << 16); }
+
+// ------------------------------------------------------------------------------------------------
+// peer-memory exchange (csrc/xgpu.cu): epoch flags and the peers' tables
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ double ld_peer_f64(const double* p) {       // never served from a stale L1 line
+  double v;
+  asm volatile("ld.volatile.global.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// Wait (bounded) until every rank has published `epoch`.  Returns false on timeout.
+__device__ __forceinline__ bool wait_flags(const unsigned long long* flags, int world, unsigned long long epoch) {
+  __shared__ int s_ok;
+  if (threadIdx.x == 0) s_ok = 1;
+  __syncthreads();
+  if (static_cast<int>(threadIdx.x) < world) {
+    const long long t0 = clock64();
+    while (ld_acquire_sys(flags + threadIdx.x) < epoch) {
+      if (clock64() - t0 > (1ll << 33)) { s_ok = 0; break; }           // ~4 s: a peer died or never launched
+    }
+  }
+  __syncthreads();
+  return s_ok != 0;
+}
 
 // ------------------------------------------------------------------------------------------------
 // mbarrier

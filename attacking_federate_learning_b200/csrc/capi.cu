@@ -100,6 +100,8 @@ namespace select {
 size_t workspace_bytes(int n);
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
                 void* ws, size_t ws_bytes, cudaStream_t stream);
+int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
+                     size_t ws_bytes, cudaStream_t stream);
 int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out, void* ws, size_t ws_bytes,
                   cudaStream_t stream);
 }
@@ -229,8 +231,7 @@ static int defend_host(const char* rule, const float* G, int n, int64_t d, int64
   }
   int host_idx = -1;
   if (r == R_KRUM) {
-    rc = gram::sqdist_to_dist(d2_acc, n, dist, c.comp); if (rc) return rc;
-    rc = select::krum_select(dist, n, users_count, f, sel, nullptr, sel_ws, c.ws_bytes - gram_ws_bytes, c.comp); if (rc) return rc;
+    rc = select::krum_from_sqdist(d2_acc, n, users_count, f, sel, sel_ws, c.ws_bytes - gram_ws_bytes, c.comp); if (rc) return rc;
     AFL_CUDA(cudaMemcpyAsync(&host_idx, sel, sizeof(int), cudaMemcpyDeviceToHost, c.comp));
     AFL_CUDA(cudaStreamSynchronize(c.comp));
     if (idx_out) *idx_out = host_idx;
@@ -313,12 +314,10 @@ int afl_krum_select(const float* dist, int n, int users_count, int corrupted_cou
   return select::krum_select(dist, n, users_count, corrupted_count, idx_out, scores_out, workspace, workspace_bytes,
                              static_cast<cudaStream_t>(stream));
 }
-int afl_krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, float* dist_scratch,
-                         int* idx_out, void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = gram::sqdist_to_dist(d2, n, dist_scratch, static_cast<cudaStream_t>(stream));
-  if (rc) return rc;
-  return select::krum_select(dist_scratch, n, users_count, corrupted_count, idx_out, nullptr, workspace,
-                             workspace_bytes, static_cast<cudaStream_t>(stream));
+int afl_krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  return select::krum_from_sqdist(d2, n, users_count, corrupted_count, idx_out, workspace, workspace_bytes,
+                                  static_cast<cudaStream_t>(stream));
 }
 int afl_bulyan_select(const float* dist, int n, int users_count, int corrupted_count, int* sel_out, void* workspace,
                       size_t workspace_bytes, void* stream) {

@@ -1,18 +1,22 @@
-// Krum scoring / argmin (defences.py:23-42) and Bulyan's selection loop (defences.py:57-68) on a
-// dense n x n fp32 distance table that is small enough (<= 64 MB at n = 4096) to live in L2.
+// Krum (defences.py:23-42) and Bulyan's selection loop (defences.py:57-68) on an n x n distance table that is small
+// enough (<= 64 MB of fp32 at n = 4096) to live in L2.
 //
-//   row_sort_kernel      one CTA per user: bitonic-sort the user's n-1 distances (value, index) in shared
-//                        memory; emit the sorted values, the sorted neighbour indices, the inverse
-//                        permutation (rank of every neighbour) and the reference's Krum score
-//                        (sequential ascending fp32 sum of the first `take` values — Python's
-//                        sum(sorted(...)[:m])).
-//   krum_argmin_kernel   strict-< argmin from (1e20, -1) in the reference's visit order [1,0,2,...].
+//   krum_tail_kernel     one CTA per user u: u's n-1 distances -> bitonic sort in shared memory -> ascending sequential
+//                        fp32 sum of the `take` smallest (defences.py:33-34) -> score[u]; the last CTA to finish does the
+//                        strict-< argmin from (1e20, -1) in the dict order [1, 0, 2, ...] (defences.py:35-37).  The row
+//                        is Sqdist (float64 d2 tables summed in rank order -> (float)sqrt(max(s, 0)), 32-bit keys) or Dist
+//                        (a caller's fp32 table: 64-bit (|value|, neighbour) keys, the table's own values summed in that
+//                        order, so a user-supplied table keeps the sign and NaN of its entries).
+//   row_sort_kernel      Bulyan: one CTA per user sorts the user's n-1 distances (value, index) and emits the sorted
+//                        values, the sorted neighbour indices and the inverse permutation (rank of every neighbour).
 //   bulyan_rounds_kernel one persistent CTA runs all theta rounds.  Removal of the selected user is an
 //                        O(1) update per remaining user: its kept set (the m_r smallest alive distances)
 //                        loses either the removed neighbour or its current largest kept element, tracked
 //                        by a boundary pointer that only ever moves left over the pre-sorted row.  Scores
 //                        are kept in float64, so every round's score is the exact sum of the fp32
 //                        distances (the reference's fp32 sequential sum differs by rounding noise only).
+#include <type_traits>
+
 #include "afl_common.cuh"
 
 namespace afl {
@@ -20,11 +24,11 @@ namespace select {
 
 constexpr int kMaxN = 4096;
 
+// Workspace: Bulyan's sorted rows, or Krum's [last-CTA counter | 256 B][score: n floats].
 struct SortWs {
   float* sval;      // [n][n]   sorted distances of row u (first n-1 entries valid)
   uint16_t* sidx;   // [n][n]   neighbour index at each sorted position
   uint16_t* rank;   // [n][n]   rank[u][v] = sorted position of neighbour v in row u
-  float* score;     // [n]      Krum score (fp32, reference arithmetic)
 };
 
 static size_t ws_bytes_for(int n) {
@@ -38,42 +42,163 @@ static SortWs carve(void* ws, int n) {
   SortWs w;
   w.sval = reinterpret_cast<float*>(p); p += align_up(nn * 4, 256);
   w.sidx = reinterpret_cast<uint16_t*>(p); p += align_up(nn * 2, 256);
-  w.rank = reinterpret_cast<uint16_t*>(p); p += align_up(nn * 2, 256);
-  w.score = reinterpret_cast<float*>(p);
+  w.rank = reinterpret_cast<uint16_t*>(p);
   return w;
 }
 
+// The reference's visit order [1, 0, 2, 3, ...]: position of user u, and (the map is its own inverse) user at position u.
 __device__ __forceinline__ int visit_pos(int u) { return u == 1 ? 0 : (u == 0 ? 1 : u); }
 
-// take: number of smallest distances summed (already resolved from Python slice semantics).
-__global__ void __launch_bounds__(256)
-row_sort_kernel(const float* __restrict__ dist, int n, int take, SortWs w) {
-  extern __shared__ unsigned long long keys[];
-  const int u = blockIdx.x;
-  int P = 1;
-  while (P < n) P <<= 1;
-  for (int v = threadIdx.x; v < P; v += blockDim.x) {
-    unsigned long long k = ~0ull;
-    if (v < n && v != u) {
-      // distances are >= 0 (or NaN): the IEEE bit pattern orders like the value; NaN sorts last.
-      const uint32_t bits = __float_as_uint(dist[static_cast<size_t>(u) * n + v]) & 0x7FFFFFFFu;
-      k = (static_cast<unsigned long long>(bits) << 32) | static_cast<unsigned>(v);
-    }
-    keys[v] = k;
-  }
-  __syncthreads();
+// Ascending bitonic sort of keys[0, P), P a power of two, by the whole block.  The keys must be visible to the block.
+template <typename Key>
+__device__ __forceinline__ void block_bitonic_sort(Key* keys, int P) {
   for (int size = 2; size <= P; size <<= 1) {
     for (int stride = size >> 1; stride > 0; stride >>= 1) {
       for (int t = threadIdx.x; t < (P >> 1); t += blockDim.x) {
         const int lo = ((t / stride) * (stride << 1)) + (t % stride);
         const int hi = lo + stride;
         const bool up = ((lo & size) == 0);
-        const unsigned long long a = keys[lo], b = keys[hi];
+        const Key a = keys[lo], b = keys[hi];
         if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
       }
       __syncthreads();
     }
   }
+}
+
+// (score, visit position) order: strict < on the score, ties to the earlier-visited user.  Start from
+// (+inf, 0x7fffffff) and feed only eligible scores (< 1e20, never NaN), so the minimum does not depend on the order.
+template <typename T>
+__device__ __forceinline__ void argmin_combine(T& best, int& best_pos, T v, int pos) {
+  if (v < best || (v == best && pos < best_pos)) { best = v; best_pos = pos; }
+}
+
+// Block-wide argmin of every thread's (best, best_pos); kWarps = blockDim.x / 32.  Returns, in thread 0, the winning
+// user or -1 when no thread saw an eligible score.
+template <int kWarps, typename T>
+__device__ __forceinline__ int block_argmin_user(T best, int best_pos) {
+  __shared__ T s_val[kWarps];
+  __shared__ int s_pos[kWarps];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+    argmin_combine(best, best_pos, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, best_pos, o));
+  if ((threadIdx.x & 31) == 0) { s_val[threadIdx.x >> 5] = best; s_pos[threadIdx.x >> 5] = best_pos; }
+  __syncthreads();
+  if (threadIdx.x >= 32) return -1;
+  const bool have = threadIdx.x < kWarps;
+  best = have ? s_val[threadIdx.x] : static_cast<T>(__int_as_float(0x7f800000));
+  best_pos = have ? s_pos[threadIdx.x] : 0x7fffffff;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+    argmin_combine(best, best_pos, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, best_pos, o));
+  return best_pos == 0x7fffffff ? -1 : visit_pos(best_pos);
+}
+
+// Sort key of an fp32 distance: distances are >= 0 (or NaN), so the IEEE bit pattern orders like the value (NaN last);
+// the neighbour in the low word keeps the sort stable.
+__device__ __forceinline__ unsigned long long dist_key(float d, int v) {
+  return (static_cast<unsigned long long>(__float_as_uint(d) & 0x7FFFFFFFu) << 32) | static_cast<unsigned>(v);
+}
+
+static int python_slice_take(int m, int len) {   // len(errors[:m])
+  if (m >= 0) return m < len ? m : len;
+  const int t = len + m;
+  return t > 0 ? t : 0;
+}
+
+enum KrumSource { kSqdist, kDist };
+template <KrumSource kSrc>
+using KrumKey = typename std::conditional<kSrc == kSqdist, uint32_t, unsigned long long>::type;
+
+template <KrumSource kSrc>
+__device__ __forceinline__ KrumKey<kSrc> krum_key(const KrumParams& p, int u, int v) {
+  const size_t e = static_cast<size_t>(u) * p.n + v;
+  if constexpr (kSrc == kSqdist) {
+    double s = 0.0;
+    for (int r = 0; r < p.world; ++r)                                    // fixed rank order: identical sum on every rank
+      s += p.world > 1 ? ld_peer_f64(p.tab[r] + e) : p.tab[0][e];
+    const float dist = static_cast<float>(sqrt(s > 0.0 ? s : 0.0));     // defences.py:20 (np.float32 norm)
+    return __float_as_uint(dist) & 0x7FFFFFFFu;                          // >= 0: the bit pattern orders like the value
+  } else {
+    return dist_key(p.dist[e], v);
+  }
+}
+
+// The distance a sorted key stands for: the key itself, or the table's original bits (keeps a NaN a NaN).
+template <KrumSource kSrc>
+__device__ __forceinline__ float krum_value(const KrumParams& p, int u, KrumKey<kSrc> k) {
+  if constexpr (kSrc == kSqdist) return __uint_as_float(k);
+  else return p.dist[static_cast<size_t>(u) * p.n + static_cast<int>(k & 0xFFFFFFFFu)];
+}
+
+template <KrumSource kSrc>
+__global__ void __launch_bounds__(256)
+krum_tail_kernel(const KrumParams p) {
+  using Key = KrumKey<kSrc>;
+  extern __shared__ __align__(8) unsigned char smem[];
+  Key* keys = reinterpret_cast<Key*>(smem);                              // P row keys
+  __shared__ int s_last;
+  const int u = blockIdx.x, n = p.n;
+  if constexpr (kSrc == kSqdist) {
+    if (p.world > 1 && !wait_flags(p.flags, p.world, p.epoch)) {
+      if (threadIdx.x == 0 && u == 0) { *p.status_host = 1; *p.idx_host = -1; *p.idx_dev = -1; }
+      return;
+    }
+  }
+  int P = 1;
+  while (P < n) P <<= 1;
+  for (int v = threadIdx.x; v < P; v += blockDim.x) keys[v] = (v < n && v != u) ? krum_key<kSrc>(p, u, v) : ~Key(0);
+  __syncthreads();
+  block_bitonic_sort(keys, P);
+  if (threadIdx.x == 0) {
+    float s = 0.f;                                                       // Python: sum() starts at int 0; ascending fp32 adds
+    for (int pos = 0; pos < p.take; ++pos) s = s + krum_value<kSrc>(p, u, keys[pos]);
+    p.score[u] = s;
+    __threadfence();
+    s_last = (atomicAdd(p.done, 1u) == static_cast<unsigned>(n - 1)) ? 1 : 0;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  // ---- the last CTA: strict-< argmin from (1e20, -1) in the reference's visit order
+  __threadfence();
+  float best = __int_as_float(0x7f800000);
+  int best_pos = 0x7fffffff;
+  for (int v = threadIdx.x; v < n; v += blockDim.x) {
+    const float s = __ldcg(p.score + v);
+    if (n >= 2 && static_cast<double>(s) < 1e20) argmin_combine(best, best_pos, s, visit_pos(v));   // vs the Python float 1e20
+  }
+  const int idx = block_argmin_user<256 / 32>(best, best_pos);
+  if (threadIdx.x == 0) {
+    *p.idx_dev = idx;
+    if (p.idx_host) { *p.idx_host = idx; *p.status_host = 0; }
+    *p.done = 0u;                                                        // ready for the next step
+    __threadfence_system();
+  }
+}
+
+// Fills p.take and launches the kernel for the row source p selects.  p.done must be zero.
+int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream) {
+  p.take = python_slice_take(users_count - corrupted_count, p.n - 1);
+  int P = 1; while (P < p.n) P <<= 1;
+  {
+    ProfScope ps("krum_tail", stream);
+    if (p.dist) krum_tail_kernel<kDist><<<p.n, 256, static_cast<size_t>(P) * sizeof(KrumKey<kDist>), stream>>>(p);
+    else krum_tail_kernel<kSqdist><<<p.n, 256, static_cast<size_t>(P) * sizeof(KrumKey<kSqdist>), stream>>>(p);
+  }
+  AFL_LAUNCH_CHECK("krum_tail_kernel");
+  return AFL_OK;
+}
+
+__global__ void __launch_bounds__(256)
+row_sort_kernel(const float* __restrict__ dist, int n, SortWs w) {
+  extern __shared__ unsigned long long keys[];
+  const int u = blockIdx.x;
+  int P = 1;
+  while (P < n) P <<= 1;
+  for (int v = threadIdx.x; v < P; v += blockDim.x)
+    keys[v] = (v < n && v != u) ? dist_key(dist[static_cast<size_t>(u) * n + v], v) : ~0ull;
+  __syncthreads();
+  block_bitonic_sort(keys, P);
   const size_t base = static_cast<size_t>(u) * n;
   for (int pos = threadIdx.x; pos < n; pos += blockDim.x) {
     const unsigned long long k = keys[pos];
@@ -88,50 +213,6 @@ row_sort_kernel(const float* __restrict__ dist, int n, int take, SortWs w) {
       w.rank[base + u] = static_cast<uint16_t>(pos);
     }
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float s = 0.f;                                        // Python: sum() starts at int 0
-    for (int pos = 0; pos < take; ++pos) s = s + w.sval[base + pos];
-    w.score[u] = s;
-  }
-}
-
-__global__ void __launch_bounds__(1024)
-krum_argmin_kernel(const float* __restrict__ score, int n, int* __restrict__ idx_out, float* __restrict__ scores_out) {
-  __shared__ float s_val[32];
-  __shared__ int s_pos[32];
-  float best = __int_as_float(0x7f800000);   // +inf
-  int best_pos = 0x7fffffff;
-  for (int u = threadIdx.x; u < n; u += blockDim.x) {
-    const float s = score[u];
-    if (scores_out) scores_out[u] = s;
-    if (n >= 2 && static_cast<double>(s) < 1e20) {       // first comparison is against the Python float 1e20
-      const int pos = visit_pos(u);
-      if (s < best || (s == best && pos < best_pos)) { best = s; best_pos = pos; }
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int op = __shfl_xor_sync(0xffffffffu, best_pos, o);
-    if (ov < best || (ov == best && op < best_pos)) { best = ov; best_pos = op; }
-  }
-  if ((threadIdx.x & 31) == 0) { s_val[threadIdx.x >> 5] = best; s_pos[threadIdx.x >> 5] = best_pos; }
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    best = s_val[threadIdx.x]; best_pos = s_pos[threadIdx.x];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-      const int op = __shfl_xor_sync(0xffffffffu, best_pos, o);
-      if (ov < best || (ov == best && op < best_pos)) { best = ov; best_pos = op; }
-    }
-    if (threadIdx.x == 0) {
-      int idx = -1;
-      if (best_pos != 0x7fffffff) idx = best_pos == 0 ? 1 : (best_pos == 1 ? 0 : best_pos);
-      *idx_out = idx;
-    }
-  }
 }
 
 constexpr int kRowsPerThread = kMaxN / 1024;
@@ -139,8 +220,6 @@ constexpr int kRowsPerThread = kMaxN / 1024;
 __global__ void __launch_bounds__(1024, 1)
 bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, SortWs w, int* __restrict__ sel_out) {
   __shared__ uint8_t alive[kMaxN];
-  __shared__ double r_val[32];
-  __shared__ int r_pos[32];
   __shared__ int s_winner;
 
   const int tid = threadIdx.x;
@@ -170,34 +249,13 @@ bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, So
 #pragma unroll
     for (int r = 0; r < kRowsPerThread; ++r) {
       const int u = tid + r * 1024;
-      if (u < n && alive[u] && score[r] < 1e20) {
-        const int pos = visit_pos(u);
-        if (score[r] < best || (score[r] == best && pos < best_pos)) { best = score[r]; best_pos = pos; }
-      }
+      if (u < n && alive[u] && score[r] < 1e20) argmin_combine(best, best_pos, score[r], visit_pos(u));
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double ov = __shfl_xor_sync(0xffffffffu, best, o);
-      const int op = __shfl_xor_sync(0xffffffffu, best_pos, o);
-      if (ov < best || (ov == best && op < best_pos)) { best = ov; best_pos = op; }
-    }
-    if ((tid & 31) == 0) { r_val[tid >> 5] = best; r_pos[tid >> 5] = best_pos; }
-    __syncthreads();
-    if (tid < 32) {
-      best = r_val[tid]; best_pos = r_pos[tid];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const double ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int op = __shfl_xor_sync(0xffffffffu, best_pos, o);
-        if (ov < best || (ov == best && op < best_pos)) { best = ov; best_pos = op; }
-      }
-      if (tid == 0) {
-        int idx = -1;
-        if (best_pos != 0x7fffffff) idx = best_pos == 0 ? 1 : (best_pos == 1 ? 0 : best_pos);
-        s_winner = idx;
-        sel_out[round] = idx;
-        if (idx >= 0) alive[idx] = 0;
-      }
+    const int idx = block_argmin_user<1024 / 32>(best, best_pos);
+    if (tid == 0) {
+      s_winner = idx;
+      sel_out[round] = idx;
+      if (idx >= 0) alive[idx] = 0;
     }
     __syncthreads();
     const int s = s_winner;
@@ -231,37 +289,41 @@ bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, So
 
 size_t workspace_bytes(int n) { return ws_bytes_for(n < 1 ? 1 : n); }
 
-static int python_slice_take(int m, int len) {   // len(errors[:m])
-  if (m >= 0) return m < len ? m : len;
-  const int t = len + m;
-  return t > 0 ? t : 0;
-}
-
-static int run_sort(const float* dist, int n, int take, void* ws, size_t ws_bytes, cudaStream_t stream, SortWs* out) {
+static int check_ws(int n, void* ws, size_t ws_bytes) {
   if (n > kMaxN) { set_error("selection kernels support n <= %d clients (got %d)", kMaxN, n); return AFL_ERR_UNSUPPORTED; }
   if (!ws || ws_bytes < ws_bytes_for(n) || (reinterpret_cast<uintptr_t>(ws) % 256) != 0) {
     set_error("selection workspace too small or misaligned (%zu < %zu)", ws_bytes, ws_bytes_for(n));
     return AFL_ERR_WORKSPACE;
   }
-  SortWs w = carve(ws, n);
-  int P = 1; while (P < n) P <<= 1;
-  ProfScope ps("row_sort", stream);
-  row_sort_kernel<<<n, 256, static_cast<size_t>(P) * sizeof(unsigned long long), stream>>>(dist, n, take, w);
-  AFL_LAUNCH_CHECK("row_sort_kernel");
-  *out = w;
   return AFL_OK;
+}
+
+// Krum on a workspace: the counter lives in its first 4 bytes (cleared here: workspaces are not initialised), the
+// scores behind it unless the caller wants them.
+static int krum_on_workspace(KrumParams p, int users_count, int corrupted_count, float* scores_out, void* ws,
+                             size_t ws_bytes, cudaStream_t stream) {
+  int rc = check_ws(p.n, ws, ws_bytes);
+  if (rc) return rc;
+  p.done = static_cast<unsigned int*>(ws);
+  p.score = scores_out ? scores_out : reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
+  AFL_CUDA(cudaMemsetAsync(p.done, 0, sizeof(unsigned int), stream));
+  return krum_tail(p, users_count, corrupted_count, stream);
 }
 
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
                 void* ws, size_t ws_bytes, cudaStream_t stream) {
   if (!dist || !idx_out || n < 1) { set_error("afl_krum_select: bad argument"); return AFL_ERR_BAD_ARG; }
-  const int take = python_slice_take(users_count - corrupted_count, n - 1);
-  SortWs w;
-  int rc = run_sort(dist, n, take, ws, ws_bytes, stream, &w);
-  if (rc) return rc;
-  krum_argmin_kernel<<<1, 1024, 0, stream>>>(w.score, n, idx_out, scores_out);
-  AFL_LAUNCH_CHECK("krum_argmin_kernel");
-  return AFL_OK;
+  KrumParams p{};
+  p.dist = dist; p.n = n; p.idx_dev = idx_out;
+  return krum_on_workspace(p, users_count, corrupted_count, scores_out, ws, ws_bytes, stream);
+}
+
+int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
+                     size_t ws_bytes, cudaStream_t stream) {
+  if (!d2 || !idx_out || n < 1) { set_error("afl_krum_from_sqdist: bad argument"); return AFL_ERR_BAD_ARG; }
+  KrumParams p{};
+  p.tab[0] = d2; p.world = 1; p.n = n; p.idx_dev = idx_out;
+  return krum_on_workspace(p, users_count, corrupted_count, nullptr, ws, ws_bytes, stream);
 }
 
 int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out, void* ws, size_t ws_bytes,
@@ -276,9 +338,15 @@ int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out
     return AFL_ERR_UNSUPPORTED;
   }
   const int theta = users_count - 2 * f;
-  SortWs w;
-  int rc = run_sort(dist, n, python_slice_take(users_count - f, n - 1), ws, ws_bytes, stream, &w);
+  int rc = check_ws(n, ws, ws_bytes);
   if (rc) return rc;
+  const SortWs w = carve(ws, n);
+  int P = 1; while (P < n) P <<= 1;
+  {
+    ProfScope ps("row_sort", stream);
+    row_sort_kernel<<<n, 256, static_cast<size_t>(P) * sizeof(unsigned long long), stream>>>(dist, n, w);
+  }
+  AFL_LAUNCH_CHECK("row_sort_kernel");
   ProfScope ps("bulyan_rounds", stream);
   bulyan_rounds_kernel<<<1, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out);
   AFL_LAUNCH_CHECK("bulyan_rounds_kernel");

@@ -1,4 +1,4 @@
-// The one exchange step of the D-sharded path (SURVEY 8e) over NVLink peer memory, and the fused Krum tail.
+// The one exchange step of the D-sharded path (SURVEY 8e) over NVLink peer memory.
 //
 // Every rank owns ONE cudaMalloc'ed block, exported with cudaIpcGetMemHandle and mapped by its peers:
 //     [table 0: n_max^2 float64][table 1][flags: world x u64][done counter]
@@ -10,11 +10,10 @@
 // tree on the latency path of an 80 KB (N = 100) .. 8 MB (N = 1000) table.  Two tables alternate by epoch: a rank can
 // run at most one step ahead of the slowest peer (its consumer kernel waits for everybody's publish of that epoch).
 //
-//   krum_tail_kernel   one CTA per client u: [wait] -> sum of the ranks' d2 rows -> sqrt -> bitonic sort of the row ->
-//                      ascending sequential fp32 sum of the `take` smallest (defences.py:33-34) -> score[u]; the last
-//                      CTA to finish does the strict-< argmin in the dict order [1, 0, 2, ...] (defences.py:35-37) and
-//                      writes the index to the device AND to mapped pinned host memory, so a Krum step ends with one
-//                      stream synchronisation instead of a blocking 4-byte memcpy.
+// Consumers:
+//   Krum               the Krum kernel (csrc/select.cu) reads the ranks' tables itself and writes the index to the device
+//                      AND to mapped pinned host memory, so a Krum step ends with one stream synchronisation instead of
+//                      a blocking 4-byte memcpy.
 //   xgpu_sum_kernel    [wait] -> elementwise sum of the ranks' tables into a local table (Bulyan keeps its own selection
 //                      kernels).
 #include <string.h>
@@ -25,6 +24,9 @@ namespace afl {
 namespace gram {
 int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, double* d2_out, void* ws, size_t ws_bytes,
                    int flags, cudaStream_t stream);
+}
+namespace select {
+int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream);
 }
 namespace xgpu {
 
@@ -43,130 +45,14 @@ struct Ctx {
   int* status_host_devptr;
 };
 
-struct TailParams {
-  const double* tab[kMaxWorld];         // the ranks' partial tables of this epoch (tab[0] only when world == 1)
-  const unsigned long long* flags;      // own flags
-  unsigned long long epoch;
-  int world, n, take;
-  float* score;
-  unsigned int* done;
-  int* idx_dev; int* idx_host; int* status_host;
-};
-
-__device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
   asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-__device__ __forceinline__ double ld_peer_f64(const double* p) {       // never served from a stale L1 line
-  double v;
-  asm volatile("ld.volatile.global.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory");
-  return v;
-}
-
-// Wait (bounded) until every rank has published `epoch`.  Returns false on timeout.
-__device__ __forceinline__ bool wait_flags(const unsigned long long* flags, int world, unsigned long long epoch) {
-  __shared__ int s_ok;
-  if (threadIdx.x == 0) s_ok = 1;
-  __syncthreads();
-  if (static_cast<int>(threadIdx.x) < world) {
-    const long long t0 = clock64();
-    while (ld_acquire_sys(flags + threadIdx.x) < epoch) {
-      if (clock64() - t0 > (1ll << 33)) { s_ok = 0; break; }           // ~4 s: a peer died or never launched
-    }
-  }
-  __syncthreads();
-  return s_ok != 0;
-}
-
 struct PublishParams { unsigned long long* flag[kMaxWorld]; int world, rank; unsigned long long epoch; };
 __global__ void publish_kernel(const PublishParams p) {
   if (threadIdx.x < p.world) {
     __threadfence_system();                                              // the table written by earlier kernels of this stream
     st_release_sys(p.flag[threadIdx.x] + p.rank, p.epoch);
-  }
-}
-
-__device__ __forceinline__ int visit_pos(int u) { return u == 1 ? 0 : (u == 0 ? 1 : u); }
-
-__global__ void __launch_bounds__(256)
-krum_tail_kernel(const TailParams p) {
-  extern __shared__ uint32_t keys[];                                     // P2 distance bit patterns
-  __shared__ float s_val[8];
-  __shared__ int s_pos[8];
-  __shared__ int s_last;
-  const int u = blockIdx.x, n = p.n;
-  if (p.world > 1 && !wait_flags(p.flags, p.world, p.epoch)) {
-    if (threadIdx.x == 0 && u == 0) { *p.status_host = 1; *p.idx_host = -1; *p.idx_dev = -1; }
-    return;
-  }
-  int P2 = 1;
-  while (P2 < n) P2 <<= 1;
-  for (int v = threadIdx.x; v < P2; v += blockDim.x) {
-    uint32_t k = 0xFFFFFFFFu;
-    if (v < n && v != u) {
-      double s = 0.0;
-      for (int r = 0; r < p.world; ++r)                                  // fixed rank order: identical sum on every rank
-        s += p.world > 1 ? ld_peer_f64(p.tab[r] + static_cast<size_t>(u) * n + v) : p.tab[0][static_cast<size_t>(u) * n + v];
-      const float dist = static_cast<float>(sqrt(s > 0.0 ? s : 0.0));   // defences.py:20 (np.float32 norm)
-      k = __float_as_uint(dist) & 0x7FFFFFFFu;                           // >= 0 or NaN: bit pattern orders like the value
-    }
-    keys[v] = k;
-  }
-  __syncthreads();
-  for (int size = 2; size <= P2; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int t = threadIdx.x; t < (P2 >> 1); t += blockDim.x) {
-        const int lo = ((t / stride) * (stride << 1)) + (t % stride);
-        const int hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const uint32_t a = keys[lo], b = keys[hi];
-        if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-      }
-      __syncthreads();
-    }
-  }
-  if (threadIdx.x == 0) {
-    float s = 0.f;                                                       // Python: sum() starts at int 0; ascending fp32 adds
-    for (int pos = 0; pos < p.take; ++pos) s = s + __uint_as_float(keys[pos]);
-    p.score[u] = s;
-    __threadfence();
-    s_last = (atomicAdd(p.done, 1u) == static_cast<unsigned>(n - 1)) ? 1 : 0;
-  }
-  __syncthreads();
-  if (!s_last) return;
-  // ---- the last CTA: strict-< argmin from (1e20, -1) in the reference's visit order
-  __threadfence();
-  float best = __int_as_float(0x7f800000);
-  int best_pos = 0x7fffffff;
-  for (int v = threadIdx.x; v < n; v += blockDim.x) {
-    const float s = __ldcg(p.score + v);
-    if (n >= 2 && static_cast<double>(s) < 1e20) {
-      const int pos = visit_pos(v);
-      if (s < best || (s == best && pos < best_pos)) { best = s; best_pos = pos; }
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int op = __shfl_xor_sync(0xffffffffu, best_pos, o);
-    if (ov < best || (ov == best && op < best_pos)) { best = ov; best_pos = op; }
-  }
-  if ((threadIdx.x & 31) == 0) { s_val[threadIdx.x >> 5] = best; s_pos[threadIdx.x >> 5] = best_pos; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < static_cast<int>(blockDim.x >> 5); ++w)
-      if (s_val[w] < best || (s_val[w] == best && s_pos[w] < best_pos)) { best = s_val[w]; best_pos = s_pos[w]; }
-    int idx = -1;
-    if (best_pos != 0x7fffffff) idx = best_pos == 0 ? 1 : (best_pos == 1 ? 0 : best_pos);
-    *p.idx_dev = idx;
-    *p.idx_host = idx;
-    *p.status_host = 0;
-    *p.done = 0u;                                                        // ready for the next step
-    __threadfence_system();
   }
 }
 
@@ -259,14 +145,9 @@ static int publish(Ctx* c, cudaStream_t stream) {
   return AFL_OK;
 }
 
-static int python_slice_take(int m, int len) {   // len(errors[:m])
-  if (m >= 0) return m < len ? m : len;
-  const int t = len + m;
-  return t > 0 ? t : 0;
-}
-
-// Whole sharded Krum step on this rank's [n, d_local] shard: partial table -> publish -> fused tail.  Enqueues only;
-// *idx_host_out points to mapped pinned memory holding the index once `stream` has been synchronised.
+// Whole sharded Krum step on this rank's [n, d_local] shard: partial table -> publish -> Krum kernel on the ranks'
+// tables.  Enqueues only; *idx_host_out points to mapped pinned memory holding the index once `stream` has been
+// synchronised.
 int krum_step(void* ctx, const void* G, int n, int64_t d, int64_t ld, int dtype, int users_count, int corrupted_count,
               void* ws, size_t ws_bytes, int flags, cudaStream_t stream, int** idx_host_out, int** status_host_out,
               int** idx_dev_out) {
@@ -279,20 +160,15 @@ int krum_step(void* ctx, const void* G, int n, int64_t d, int64_t ld, int dtype,
   if (rc) return rc;
   rc = publish(c, stream);
   if (rc) return rc;
-  TailParams tp{};
-  for (int r = 0; r < c->world; ++r) tp.tab[r] = table_of(c, r, c->epoch);
-  tp.flags = reinterpret_cast<const unsigned long long*>(c->block + flags_offset(c));
-  tp.epoch = c->epoch; tp.world = c->world; tp.n = n;
-  tp.take = python_slice_take(users_count - corrupted_count, n - 1);
-  tp.score = c->score;
-  tp.done = reinterpret_cast<unsigned int*>(c->block + flags_offset(c) + sizeof(unsigned long long) * kMaxWorld);
-  tp.idx_dev = c->idx_dev; tp.idx_host = c->idx_host_devptr; tp.status_host = c->status_host_devptr;
-  int P2 = 1; while (P2 < n) P2 <<= 1;
-  {
-    ProfScope ps("krum_tail", stream);
-    krum_tail_kernel<<<n, 256, static_cast<size_t>(P2) * sizeof(uint32_t), stream>>>(tp);
-  }
-  AFL_LAUNCH_CHECK("krum_tail_kernel");
+  KrumParams kp{};
+  for (int r = 0; r < c->world; ++r) kp.tab[r] = table_of(c, r, c->epoch);
+  kp.flags = reinterpret_cast<const unsigned long long*>(c->block + flags_offset(c));
+  kp.epoch = c->epoch; kp.world = c->world; kp.n = n;
+  kp.score = c->score;
+  kp.done = reinterpret_cast<unsigned int*>(c->block + flags_offset(c) + sizeof(unsigned long long) * kMaxWorld);
+  kp.idx_dev = c->idx_dev; kp.idx_host = c->idx_host_devptr; kp.status_host = c->status_host_devptr;
+  rc = select::krum_tail(kp, users_count, corrupted_count, stream);
+  if (rc) return rc;
   if (idx_host_out) *idx_host_out = c->idx_host;
   if (status_host_out) *status_host_out = c->status_host;
   if (idx_dev_out) *idx_dev_out = c->idx_dev;

@@ -96,16 +96,18 @@ class ShardedAggregator:
             assert users_count >= 2 * corrupted_count + 1, ('users_count>=2*corrupted_count + 3', users_count, corrupted_count)
         peer = self._peer_context(G_shard.shape[0], G_shard.device) if G_shard.is_cuda else None
         if peer is not None:
-            # hot path: ONE FFI crossing: Gram -> publish -> fused tail (peer-memory sum, sqrt, sort, score, argmin),
-            # index through mapped pinned memory, one stream synchronisation
+            # hot path (any world size, including 1): ONE FFI crossing: Gram -> publish -> Krum kernel on the ranks'
+            # tables (peer-memory sum, sqrt, sort, score, argmin), index through mapped pinned memory, one stream
+            # synchronisation
             idx = peer.krum(G_shard, users_count, corrupted_count)
         elif hasattr(self.k, "krum_from_sqdist"):
-            # two FFI crossings + the NCCL all-reduce, persistent buffers, one 4-byte D2H sync
+            # peer path off: two FFI crossings + the NCCL all-reduce, then the same Krum kernel on the summed d2 table;
+            # persistent buffers, one 4-byte D2H sync
             d2, idx_dev = self._buffers(G_shard.shape[0], G_shard.device)
             self.k.sqdist_partial(G_shard, 0, d2)
             self._allreduce_table(d2)
             idx = int(self.k.krum_from_sqdist(d2, users_count, corrupted_count, idx_dev).item())
-        else:
+        else:                                            # kernels without krum_from_sqdist (the NumPy stand-in)
             idx = int(self.k.krum_select(self.distances(G_shard), users_count, corrupted_count).reshape(-1)[0].item())
         return idx if return_index else G_shard[idx]
 
@@ -142,7 +144,7 @@ class ShardedAggregator:
         if self.world == 1:
             return "none"
         if self._peer is not None:
-            return "NVLink peer-memory sum inside the fused tail kernel (csrc/xgpu.cu)"
+            return "NVLink peer-memory sum inside the Krum kernel (csrc/xgpu.cu, csrc/select.cu)"
         return "NCCL all-reduce" + (f" (peer path off: {self._peer_error})" if self._peer_error else "")
 
     def defend(self, name, G_shard, users_count, corrupted_count):

@@ -76,7 +76,7 @@ uint64_t afl_launch_count(void);
 /* ---- in-library kernel timing (measurement aid for bench.py) -----------------------------------
  * While enabled, the dominant kernel of every entry point is bracketed by CUDA events on the stream it
  * is launched on.  afl_profile_read(name, ...) waits for the recorded events of kernel `name`
- * ("gram_pair", "sqdist_simt", "trimmed_mean", "alie", "mean", "row_sort", "bulyan_rounds"),
+ * ("gram_pair", "sqdist_simt", "trimmed_mean", "alie", "mean", "krum_tail", "row_sort", "bulyan_rounds"),
  * returns their summed duration and launch count, and forgets them.  on = 1: every bracketed kernel; on = 2: only the
  * dominant kernel of a rule (gram_pair, sqdist_simt, trimmed_mean, mean, alie) - one pair of events per step. */
 int afl_profile_enable(int on);
@@ -108,10 +108,11 @@ size_t afl_select_workspace_bytes(int n);
 int afl_krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out,
                     float* scores_out, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Convenience: afl_sqdist_to_dist + afl_krum_select in one call (one FFI crossing per aggregation after
- * the all-reduce).  dist_scratch: device float[n*n]. */
-int afl_krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, float* dist_scratch,
-                         int* idx_out, void* workspace, size_t workspace_bytes, void* stream);
+/* The same selection straight from an (all-reduced) squared-distance table d2 (device float64[n*n]): the
+ * distances are (float)sqrt(max(d2, 0)) as in afl_sqdist_to_dist, computed inside the Krum kernel, so the
+ * index equals afl_krum_select(afl_sqdist_to_dist(d2)).  One call per aggregation after the all-reduce. */
+int afl_krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out,
+                         void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- Bulyan selection:  defences.py:57-68 ------------------------------------------------------
  * theta = users_count - 2f rounds of Krum-with-removal on one distance table; sel_out (device

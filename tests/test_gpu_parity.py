@@ -199,7 +199,7 @@ def test_krum_matches_oracle(api, n, d, f, seed):
     row = D.krum(Gd, n, f)
     assert row.data_ptr() == Gd[want].data_ptr()                              # a view, like the reference
     from attacking_federate_learning_b200.sharded import ShardedAggregator
-    assert ShardedAggregator().krum(Gd, n, f, return_index=True) == want      # fused afl_krum_from_sqdist path
+    assert ShardedAggregator().krum(Gd, n, f, return_index=True) == want      # peer context, world 1 (afl_krum_sharded)
     # Tensor-core tables vs the float64 arbiter.  Both tensor kernels carry a small UNIFORM scale bias
     # (tensor-core accumulation truncates; the bf16x2 kernel also drops the b2*b2 term) which cannot
     # change any ranking; what must be tiny is the pair-to-pair SPREAD of the relative error.
@@ -235,6 +235,41 @@ def test_identical_rows_tie_goes_to_user_1(api):
         assert all(torch.equal(dist[0, f:], dist[i, f:]) for i in range(1, f))
         assert int(dev.krum_select(dist, n, f).item()) == 1
     assert orc.krum(G, n, f, return_index=True) == 1
+
+
+@pytest.mark.parametrize("n,d,f,seed", [(100, 40960, 24, 11), (300, 8192, 70, 12)])
+def test_krum_routes_agree(api, n, d, f, seed):
+    """Every Krum entry point runs the same kernel on the same d2 table: same index, and scores that are the
+    reference's sequential fp32 sum over the sorted fp32 row."""
+    D, _, dev, _ = api
+    from attacking_federate_learning_b200.sharded import ShardedAggregator
+    rng = np.random.default_rng(seed)
+    G = hetero(rng, n, d)
+    G[:f] = orc.alie_attack([G[i].copy() for i in range(f)], 1.5)[0]          # identical rows: exact score ties
+    Gd = torch.from_numpy(G).cuda()
+    d2 = dev.sqdist_partial(Gd)
+    dist = dev.sqdist_to_dist(d2)
+    idx, scores = dev.krum_select(dist, n, f, want_scores=True)
+    want = int(idx.item())
+    row = D.krum(G, n, f)                                                     # host-buffer C entry point
+    assert np.shares_memory(row, G) and (row.ctypes.data - G.ctypes.data) == want * G.strides[0]
+    assert D.krum(Gd, n, f, return_index=True) == want
+    assert ShardedAggregator().krum(Gd, n, f, return_index=True) == want
+    assert int(dev.krum_from_sqdist(d2, n, f).item()) == want
+    table = dist.cpu().numpy()
+    take = n - f
+    ref = np.empty(n, np.float32)
+    for u in range(n):
+        s = np.float32(0)
+        for v in np.sort(np.delete(table[u], u))[:take]:
+            s = np.float32(s + v)
+        ref[u] = s
+    assert np.array_equal(scores.cpu().numpy().view(np.uint32), ref.view(np.uint32))
+    best, best_u = 1e20, -1                                                   # defences.py:35-37 on these scores
+    for u in orc.visit_order(n):
+        if ref[u] < best:
+            best, best_u = ref[u], u
+    assert want == best_u
 
 
 @pytest.mark.parametrize("n,f,seed", [(31, 7, 0), (100, 24, 1), (203, 50, 2), (500, 100, 3)])

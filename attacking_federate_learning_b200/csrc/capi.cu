@@ -1,5 +1,6 @@
 // extern "C" surface declared in include/afl_b200.h, error plumbing, and the one-call host-buffer API.
 #include <stdarg.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include <atomic>
@@ -125,15 +126,36 @@ __global__ void add_f64_kernel(double* __restrict__ acc, const double* __restric
 }
 
 // ------------------------------------------------------------------------------------------------
-// Host-buffer path: cached device staging + a copy stream that runs ahead of the compute stream.
+// Host-buffer path: the matrix stays in host memory and is streamed through a bounded device staging area.
+//
+//   * Column slabs of `slab_cols` columns go through a ring of kRingSlots device slots: the copy stream fills
+//     slot s % slots while the compute stream runs the kernels of the slab before it.  `freed[slot]` is
+//     recorded on the compute stream after the last kernel that reads the slot, and the copy stream waits on
+//     it before overwriting the slot.
+//   * Krum sums one d2 table per slab (sqdist_partial + add_f64_kernel, in slab order); TrimmedMean and
+//     NoDefense finish each slab's columns as soon as its kernel has run.
+//   * Bulyan keeps slabs 0 .. R-1 resident (as many as the budget holds) and streams the rest.  After
+//     selection, stage 2 runs once over the resident columns with row_index = sel; for the other columns it
+//     re-streams only the theta selected rows, packed in selection order, and runs the same trimmed mean with
+//     row_index = NULL.  When the whole matrix fits, R covers every slab and nothing is streamed twice.
+//   * Budget: free device memory plus what this context already holds, minus 1 GiB, capped by the
+//     environment variable AFL_HOST_DEVICE_BYTES (read on every call).
+//
+// Results depend only on the input, n, d, ld and slab_cols: every kernel is column-wise or sums per-slab
+// tables in slab order, so neither the budget, the ring depth nor the resident prefix changes a bit.  For the
+// same reason the slab width is never narrowed to fit a small budget: the call fails instead.
 // ------------------------------------------------------------------------------------------------
+constexpr int kRingSlots = 3;
+constexpr size_t kHeadroom = size_t(1) << 30;
+
 struct HostCtx {
   std::mutex mu;
-  void* mat = nullptr; size_t mat_bytes = 0;       // resident [n, ld_dev] fp32 matrix
+  void* stage = nullptr; size_t stage_bytes = 0;   // Bulyan's resident prefix, then the ring slots
   void* ws = nullptr; size_t ws_bytes = 0;          // kernel workspace
   void* small = nullptr; size_t small_bytes = 0;    // d2 tables, dist, indices, output vector
   cudaStream_t copy = nullptr, comp = nullptr;
-  cudaEvent_t ev[64];
+  cudaEvent_t ready = nullptr;                      // slab landed (recorded on copy, waited on at once by comp)
+  cudaEvent_t freed[kRingSlots];                    // compute stream is done reading the slot
   bool init = false;
 };
 static HostCtx g_ctx[kMaxDevices];
@@ -144,6 +166,18 @@ static int ensure(void** p, size_t* have, size_t want) {
   AFL_CUDA(cudaMalloc(p, want));
   *have = want;
   return AFL_OK;
+}
+
+// Device bytes the host path may hold on this call.
+static size_t host_budget(size_t free_b, size_t held) {
+  size_t b = free_b + held > kHeadroom ? free_b + held - kHeadroom : 0;
+  if (const char* e = getenv("AFL_HOST_DEVICE_BYTES")) {
+    if (*e) {
+      const unsigned long long cap = strtoull(e, nullptr, 10);
+      if (cap < b) b = static_cast<size_t>(cap);
+    }
+  }
+  return b;
 }
 
 static int defend_host(const char* rule, const float* G, int n, int64_t d, int64_t ld, int users_count, int f,
@@ -170,68 +204,133 @@ static int defend_host(const char* rule, const float* G, int n, int64_t d, int64
   if (!c.init) {
     AFL_CUDA(cudaStreamCreateWithFlags(&c.copy, cudaStreamNonBlocking));
     AFL_CUDA(cudaStreamCreateWithFlags(&c.comp, cudaStreamNonBlocking));
-    for (auto& e : c.ev) AFL_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    AFL_CUDA(cudaEventCreateWithFlags(&c.ready, cudaEventDisableTiming));
+    for (auto& e : c.freed) AFL_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     c.init = true;
   }
+  struct Drain {                                  // every return leaves both streams idle: no copy still reads G
+    HostCtx& c;
+    ~Drain() { cudaStreamSynchronize(c.copy); cudaStreamSynchronize(c.comp); }
+  } drain{c};
+  const bool table = r == R_KRUM || r == R_BULYAN;
+  const int theta = r == R_BULYAN ? users_count - 2 * f : 0;
   const int64_t ld_dev = (d + 31) / 32 * 32;          // padded pitch: TMA + 16-byte loads always apply
-  const size_t mat_bytes = static_cast<size_t>(n) * ld_dev * sizeof(float);
-  size_t free_b = 0, total_b = 0;
-  AFL_CUDA(cudaMemGetInfo(&free_b, &total_b));
-  if (mat_bytes > c.mat_bytes && mat_bytes + (size_t(1) << 30) > free_b + c.mat_bytes) {   // keep 1 GiB of headroom
-    set_error("afl_defend_host: %zu-byte matrix does not fit on this GPU; shard the parameter dimension", mat_bytes);
-    return AFL_ERR_UNSUPPORTED;
-  }
-  int rc = ensure(&c.mat, &c.mat_bytes, mat_bytes);
-  if (rc) return rc;
   if (slab_cols <= 0) slab_cols = (int64_t(96) << 20) / (static_cast<int64_t>(n) * 4);   // ~96 MB per slab
   slab_cols = (slab_cols + 31) / 32 * 32;
   if (slab_cols < 32) slab_cols = 32;
+  if (slab_cols > ld_dev) slab_cols = ld_dev;         // one slab either way; keeps the slots no wider than the matrix
   const int nslab = static_cast<int>((d + slab_cols - 1) / slab_cols);
   const size_t nn = static_cast<size_t>(n) * n;
-  const size_t ws_need = (r == R_KRUM || r == R_BULYAN)
-                             ? align_up(gram::workspace_bytes(n, slab_cols, AFL_F32, 0), 256) + select::workspace_bytes(n)
-                             : 256;
-  rc = ensure(&c.ws, &c.ws_bytes, ws_need);
-  if (rc) return rc;
-  const size_t small_need = align_up(nn * 8, 256) * 2 + align_up(nn * 4, 256) + align_up(static_cast<size_t>(n) * 4, 256) +
-                            align_up(static_cast<size_t>(d) * 4, 256) + 1024;
-  rc = ensure(&c.small, &c.small_bytes, small_need);
-  if (rc) return rc;
-  uint8_t* sp = static_cast<uint8_t*>(c.small);
-  double* d2_acc = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
-  double* d2_part = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
-  float* dist = reinterpret_cast<float*>(sp); sp += align_up(nn * 4, 256);
-  int* sel = reinterpret_cast<int*>(sp); sp += align_up(static_cast<size_t>(n) * 4, 256);
-  float* out_dev = reinterpret_cast<float*>(sp);
-  float* mat = static_cast<float*>(c.mat);
-  void* gram_ws = c.ws;
-  const size_t gram_ws_bytes = (r == R_KRUM || r == R_BULYAN) ? align_up(gram::workspace_bytes(n, slab_cols, AFL_F32, 0), 256) : 0;
-  void* sel_ws = static_cast<uint8_t*>(c.ws) + gram_ws_bytes;
+  const int sel_len = n > theta ? n : theta;         // also the rows of a slot: Bulyan's second pass packs theta rows
 
+  // ---- device footprint: workspaces and tables (fixed), then the resident prefix and the ring
+  const size_t gram_ws_bytes = table ? align_up(gram::workspace_bytes(n, slab_cols, AFL_F32, 0), 256) : 0;
+  const size_t ws_need = table ? gram_ws_bytes + select::workspace_bytes(n) : 256;
+  const size_t small_need = (table ? align_up(nn * 8, 256) * 2 + align_up(nn * 4, 256) : 0) +
+                            align_up(static_cast<size_t>(sel_len) * 4, 256) +
+                            (r != R_KRUM ? align_up(static_cast<size_t>(d) * 4, 256) : 0) + 1024;
+  const size_t slab_bytes = static_cast<size_t>(n) * slab_cols * sizeof(float);
+  const size_t slot_bytes = align_up(static_cast<size_t>(sel_len) * slab_cols * sizeof(float), 256);
+  size_t free_b = 0, total_b = 0;
+  AFL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const size_t budget = host_budget(free_b, c.stage_bytes + c.ws_bytes + c.small_bytes);
+  const size_t fixed = ws_need + small_need;
+  const size_t full_res = align_up(static_cast<size_t>(n) * ld_dev * sizeof(float), 256);
+  int R = 0, slots = 0;                               // resident slabs, ring slots
+  if (r == R_BULYAN && fixed + full_res <= budget) {
+    R = nslab;
+  } else {
+    const int min_slots = nslab < 2 ? nslab : 2;
+    if (fixed + min_slots * slot_bytes > budget) {
+      set_error("afl_defend_host: needs %zu bytes of device memory (%d staging slots of %zu bytes for %lld-column slabs, "
+                "plus %zu bytes of tables and workspaces) but may use %zu (free memory less 1 GiB, capped by "
+                "AFL_HOST_DEVICE_BYTES); use narrower slabs or a larger budget",
+                fixed + min_slots * slot_bytes, min_slots, slot_bytes, static_cast<long long>(slab_cols), fixed, budget);
+      return AFL_ERR_UNSUPPORTED;
+    }
+    slots = min_slots;
+    if (r == R_BULYAN) {                              // spend the rest on resident slabs: they are not re-streamed
+      const size_t spare = budget - fixed - slots * slot_bytes;
+      const size_t fit = spare > 256 ? (spare - 256) / slab_bytes : 0;
+      R = static_cast<int>(fit < static_cast<size_t>(nslab - 1) ? fit : static_cast<size_t>(nslab - 1));
+    } else {
+      const int most = nslab < kRingSlots ? nslab : kRingSlots;
+      while (slots < most && fixed + (slots + 1) * slot_bytes <= budget) ++slots;
+    }
+  }
+  const int64_t ld_res = R == nslab ? ld_dev : R * slab_cols;   // resident pitch
+  const int64_t d_res = R == nslab ? d : R * slab_cols;        // resident columns
+  const size_t res_bytes = align_up(static_cast<size_t>(n) * ld_res * sizeof(float), 256);
+  const size_t stage_need = res_bytes + slots * slot_bytes;
+
+  // release cached buffers that are larger than this call needs when keeping them would exceed the budget
+  void** bufs[3] = {&c.stage, &c.ws, &c.small};
+  size_t* have[3] = {&c.stage_bytes, &c.ws_bytes, &c.small_bytes};
+  const size_t want[3] = {stage_need, ws_need, small_need};
+  size_t keep = 0;
+  for (int i = 0; i < 3; ++i) keep += *have[i] > want[i] ? *have[i] : want[i];
+  if (keep > budget)
+    for (int i = 0; i < 3; ++i)
+      if (*have[i] > want[i]) { AFL_CUDA(cudaFree(*bufs[i])); *bufs[i] = nullptr; *have[i] = 0; }
+  for (int i = 0; i < 3; ++i) {
+    const int rc = ensure(bufs[i], have[i], want[i]);
+    if (rc) return rc;
+  }
+
+  uint8_t* sp = static_cast<uint8_t*>(c.small);
+  double* d2_acc = nullptr; double* d2_part = nullptr; float* dist = nullptr;
+  if (table) {
+    d2_acc = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
+    d2_part = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
+    dist = reinterpret_cast<float*>(sp); sp += align_up(nn * 4, 256);
+  }
+  int* sel = reinterpret_cast<int*>(sp); sp += align_up(static_cast<size_t>(sel_len) * 4, 256);
+  float* out_dev = reinterpret_cast<float*>(sp);
+  float* res = static_cast<float*>(c.stage);
+  float* ring = reinterpret_cast<float*>(static_cast<uint8_t*>(c.stage) + res_bytes);
+  const int64_t slot_elems = static_cast<int64_t>(slot_bytes / sizeof(float));
+  void* gram_ws = c.ws;
+  void* sel_ws = static_cast<uint8_t*>(c.ws) + gram_ws_bytes;
+  const size_t sel_ws_bytes = c.ws_bytes - gram_ws_bytes;
+  int rc = AFL_OK;
+  int64_t ring_i = 0;                                 // ring slabs issued so far (pass 1 and pass 2)
+
+  // next ring slot: the copy stream waits until the compute stream has finished reading it
+  auto next_slot = [&](int* slot, float** m) -> cudaError_t {
+    *slot = static_cast<int>(ring_i % slots);
+    *m = ring + *slot * slot_elems;
+    return ring_i++ >= slots ? cudaStreamWaitEvent(c.copy, c.freed[*slot], 0) : cudaSuccess;
+  };
+
+  // ---- pass 1: every column once
   for (int s = 0; s < nslab; ++s) {
     const int64_t c0 = static_cast<int64_t>(s) * slab_cols;
     const int64_t w = (d - c0 < slab_cols) ? d - c0 : slab_cols;
-    if (s >= 64) AFL_CUDA(cudaEventSynchronize(c.ev[s % 64]));     // event slot reuse
-    AFL_CUDA(cudaMemcpy2DAsync(mat + c0, ld_dev * sizeof(float), G + c0, ld * sizeof(float), w * sizeof(float), n,
+    int slot = -1;
+    float* m = res + c0;
+    if (s >= R) AFL_CUDA(next_slot(&slot, &m));
+    const int64_t mld = s < R ? ld_res : slab_cols;
+    AFL_CUDA(cudaMemcpy2DAsync(m, mld * sizeof(float), G + c0, ld * sizeof(float), w * sizeof(float), n,
                                cudaMemcpyHostToDevice, c.copy));
-    AFL_CUDA(cudaEventRecord(c.ev[s % 64], c.copy));
-    AFL_CUDA(cudaStreamWaitEvent(c.comp, c.ev[s % 64], 0));
-    if (r == R_KRUM || r == R_BULYAN) {
-      rc = gram::sqdist_partial(mat + c0, n, w, ld_dev, AFL_F32, d2_part, gram_ws, gram_ws_bytes, 0, c.comp);
+    AFL_CUDA(cudaEventRecord(c.ready, c.copy));
+    AFL_CUDA(cudaStreamWaitEvent(c.comp, c.ready, 0));
+    if (table) {
+      rc = gram::sqdist_partial(m, n, w, mld, AFL_F32, d2_part, gram_ws, gram_ws_bytes, 0, c.comp);
       if (rc) return rc;
       add_f64_kernel<<<static_cast<unsigned>((nn + 255) / 256), 256, 0, c.comp>>>(d2_acc, d2_part, nn, s == 0);
       AFL_LAUNCH_CHECK("add_f64_kernel");
     } else if (r == R_TM) {
-      rc = tmean::trimmed_mean(mat + c0, n, w, ld_dev, AFL_F32, nullptr, n, f, out_dev + c0, c.comp);
+      rc = tmean::trimmed_mean(m, n, w, mld, AFL_F32, nullptr, n, f, out_dev + c0, c.comp);
       if (rc) return rc;
     } else {
-      rc = colstats::mean(mat + c0, n, w, ld_dev, AFL_F32, out_dev + c0, c.comp);
+      rc = colstats::mean(m, n, w, mld, AFL_F32, out_dev + c0, c.comp);
       if (rc) return rc;
     }
+    if (slot >= 0) AFL_CUDA(cudaEventRecord(c.freed[slot], c.comp));
   }
-  int host_idx = -1;
   if (r == R_KRUM) {
-    rc = select::krum_from_sqdist(d2_acc, n, users_count, f, sel, sel_ws, c.ws_bytes - gram_ws_bytes, c.comp); if (rc) return rc;
+    int host_idx = -1;
+    rc = select::krum_from_sqdist(d2_acc, n, users_count, f, sel, sel_ws, sel_ws_bytes, c.comp); if (rc) return rc;
     AFL_CUDA(cudaMemcpyAsync(&host_idx, sel, sizeof(int), cudaMemcpyDeviceToHost, c.comp));
     AFL_CUDA(cudaStreamSynchronize(c.comp));
     if (idx_out) *idx_out = host_idx;
@@ -243,15 +342,34 @@ static int defend_host(const char* rule, const float* G, int n, int64_t d, int64
   }
   if (r == R_BULYAN) {
     rc = gram::sqdist_to_dist(d2_acc, n, dist, c.comp); if (rc) return rc;
-    rc = select::bulyan_select(dist, n, users_count, f, sel, sel_ws, c.ws_bytes - gram_ws_bytes, c.comp); if (rc) return rc;
-    const int theta = users_count - 2 * f;
-    rc = tmean::trimmed_mean(mat, n, d, ld_dev, AFL_F32, sel, theta, 2 * f, out_dev, c.comp); if (rc) return rc;
-    int last_sel = 0;                                  // a failed round marks itself and every later round with -1
-    AFL_CUDA(cudaMemcpyAsync(&last_sel, sel + (theta - 1), sizeof(int), cudaMemcpyDeviceToHost, c.comp));
+    rc = select::bulyan_select(dist, n, users_count, f, sel, sel_ws, sel_ws_bytes, c.comp); if (rc) return rc;
+    if (R > 0) {                                      // stage 2 over the resident columns
+      rc = tmean::trimmed_mean(res, n, d_res, ld_res, AFL_F32, sel, theta, 2 * f, out_dev, c.comp); if (rc) return rc;
+    }
+    std::vector<int> hsel(static_cast<size_t>(theta));
+    AFL_CUDA(cudaMemcpyAsync(hsel.data(), sel, static_cast<size_t>(theta) * sizeof(int), cudaMemcpyDeviceToHost, c.comp));
     AFL_CUDA(cudaStreamSynchronize(c.comp));
-    if (last_sel < 0) {
+    if (hsel[theta - 1] < 0) {                        // a failed round marks itself and every later round with -1
       set_error("bulyan: a selection round found no eligible user (NaN or >= 1e20 scores); the reference raises KeyError(-1)");
       return AFL_ERR_NO_WINNER;
+    }
+    // ---- pass 2: the theta selected rows of the streamed columns, packed in selection order.  The kernel is
+    // column-wise, so the slab may be as wide as a slot holds.
+    const int64_t w2 = slot_elems / theta / 32 * 32;
+    for (int64_t c0 = d_res; c0 < d; c0 += w2) {
+      const int64_t w = (d - c0 < w2) ? d - c0 : w2;
+      int slot = -1;
+      float* m = nullptr;
+      AFL_CUDA(next_slot(&slot, &m));
+      for (int i = 0; i < theta; ++i) {
+        const int row = hsel[i] < 0 ? hsel[i] + n : hsel[i];
+        AFL_CUDA(cudaMemcpyAsync(m + static_cast<int64_t>(i) * w2, G + static_cast<int64_t>(row) * ld + c0,
+                                 w * sizeof(float), cudaMemcpyHostToDevice, c.copy));
+      }
+      AFL_CUDA(cudaEventRecord(c.ready, c.copy));
+      AFL_CUDA(cudaStreamWaitEvent(c.comp, c.ready, 0));
+      rc = tmean::trimmed_mean(m, theta, w, w2, AFL_F32, nullptr, theta, 2 * f, out_dev + c0, c.comp); if (rc) return rc;
+      AFL_CUDA(cudaEventRecord(c.freed[slot], c.comp));
     }
   }
   AFL_CUDA(cudaMemcpyAsync(out_host, out_dev, static_cast<size_t>(d) * sizeof(float), cudaMemcpyDeviceToHost, c.comp));

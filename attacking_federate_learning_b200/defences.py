@@ -13,7 +13,11 @@ Reference surface mirrored (file:line in /root/reference):
 `users_grads` may be
   * a NumPy float32 [N, D] array (what server.py:35 holds): the call goes through the host-buffer
     C entry point `afl_defend_host` (H2D staging overlapped with the kernels) and returns NumPy —
-    `krum` returns a *view* of the winning row exactly like the reference;
+    `krum` returns a *view* of the winning row exactly like the reference.  The matrix may be larger
+    than the GPU: column slabs are streamed through a bounded device budget (free memory less 1 GiB,
+    capped by the environment variable AFL_HOST_DEVICE_BYTES); a budget too small for two slabs and
+    the N x N tables raises NotImplementedError stating the bytes needed.  `krum(..., return_index=True)`
+    and `_krum_create_distances` still upload the whole matrix;
   * a torch.cuda float32 / bfloat16 [N, D] tensor: device-resident path, returns torch tensors
     (fp32), `krum` again returns a view `users_grads[idx]`.
 There is no CPU implementation in this package.

@@ -179,10 +179,16 @@ int afl_sqdist_allreduce(void* ctx, const void* G, int n, int64_t d, int64_t ld,
 
 /* ---- one-call host-buffer API (what a cgo/ctypes binding of server.py:87 would call) ----------
  * rule: "NoDefense" | "Krum" | "TrimmedMean" | "Bulyan" (defences.py:4-8).  G_host: n x d fp32 in
- * host memory, pitch ld.  The call stages column slabs through device memory (H2D copies overlap the
- * kernels), runs the rule, and writes the aggregated gradient to out_host[d] (fp32) and, for Krum,
- * the winning index to *idx_out (may be NULL).  Blocking.  Reference assert failures map to
- * AFL_ERR_PRECONDITION.  `slab_cols` = columns per staging slab (0 = default). */
+ * host memory, pitch ld.  The call streams column slabs through a bounded device staging area (H2D
+ * copies overlap the kernels), runs the rule, and writes the aggregated gradient to out_host[d] (fp32)
+ * and, for Krum, the winning index to *idx_out (may be NULL).  Blocking.  Reference assert failures
+ * map to AFL_ERR_PRECONDITION.  `slab_cols` = columns per staging slab (0 = default, about 96 MB).
+ * The matrix does not have to fit the GPU: Krum, TrimmedMean and NoDefense stream every slab through a
+ * ring of slots; Bulyan keeps as many leading slabs resident as the budget allows and re-streams only its
+ * selected rows for the other columns.  Budget: free device memory plus what the call already holds,
+ * minus 1 GiB, capped by the environment variable AFL_HOST_DEVICE_BYTES (bytes, read on every call).
+ * If two slots and the n x n tables do not fit, AFL_ERR_UNSUPPORTED (the message states the bytes needed).
+ * Results depend only on the input, n, d, ld and slab_cols, never on the budget or the free memory. */
 int afl_defend_host(const char* rule, const float* G_host, int n, int64_t d, int64_t ld,
                     int users_count, int corrupted_count, float* out_host, int* idx_out,
                     int64_t slab_cols);

@@ -294,6 +294,12 @@ __device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t a_
 // correct; a centre close to the clients' common component keeps ||g - c||^2 (which the dropped-term and
 // accumulation biases scale with) of the order of the distances themselves.  Ids >= f are honest (main.py:28).
 constexpr int kGramCenterRows = 8;
+// A centre row with an inf in a column would turn every client's g - c there into inf or NaN: that column is not
+// centred (c = 0), so only the rows that hold the inf get non-finite operands.
+__device__ __forceinline__ float gram_center_finite(float c) { return isfinite(c) ? c : 0.f; }
+__device__ __forceinline__ float4 gram_center_finite(float4 c) {
+  return make_float4(gram_center_finite(c.x), gram_center_finite(c.y), gram_center_finite(c.z), gram_center_finite(c.w));
+}
 __device__ __forceinline__ float4 gram_center(const float* cref, int rows, int64_t ld, int64_t col, int64_t d) {
   // always kGramCenterRows loads, all issued before the first add (a runtime trip count would serialise 8 dependent
   // L2 round trips per k-block); with fewer clients the last row is simply counted more than once - any centre is valid
@@ -313,7 +319,7 @@ __device__ __forceinline__ float4 gram_center(const float* cref, int rows, int64
 #pragma unroll
   for (int r = 0; r < kGramCenterRows; ++r) { cx += t[r].x; cy += t[r].y; cz += t[r].z; cw += t[r].w; }
   const float inv = 1.0f / static_cast<float>(kGramCenterRows);
-  return make_float4(cx * inv, cy * inv, cz * inv, cw * inv);
+  return gram_center_finite(make_float4(cx * inv, cy * inv, cz * inv, cw * inv));
 }
 
 

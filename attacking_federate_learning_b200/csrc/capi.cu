@@ -98,6 +98,7 @@ int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, doubl
 int sqdist_to_dist(const double* d2, int n, float* dist, cudaStream_t stream);
 }
 namespace select {
+int max_clients();
 size_t workspace_bytes(int n);
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
                 void* ws, size_t ws_bytes, cudaStream_t stream);
@@ -198,6 +199,10 @@ static int defend_host(const char* rule, const float* G, int n, int64_t d, int64
   if (r == R_BULYAN && users_count < 4 * f + 3) {
     set_error("bulyan: users_count >= 4*corrupted_count + 3 violated (%d, %d)", users_count, f);
     return AFL_ERR_PRECONDITION;
+  }
+  if ((r == R_KRUM || r == R_BULYAN) && n > select::max_clients()) {   // before any copy or launch
+    set_error("afl_defend_host: %s supports n <= %d clients (got %d)", rule, select::max_clients(), n);
+    return AFL_ERR_UNSUPPORTED;
   }
   HostCtx& c = g_ctx[current_device()];          // streams, events and buffers belong to the current device
   std::lock_guard<std::mutex> lock(c.mu);

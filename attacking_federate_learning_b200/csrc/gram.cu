@@ -88,7 +88,8 @@ __global__ void sqdist_to_dist_kernel(const double* __restrict__ d2, int n, floa
   if (e >= static_cast<size_t>(n) * n) return;
   const int i = static_cast<int>(e / n), j = static_cast<int>(e % n);
   const double v = d2[e];
-  dist[e] = (i == j) ? 0.f : static_cast<float>(sqrt(v > 0.0 ? v : 0.0));
+  // a negative cancellation residue is 0; NaN (two SIMT rows with the same infinity in one column) stays NaN
+  dist[e] = (i == j) ? 0.f : static_cast<float>(sqrt(v > 0.0 ? v : (v == v ? 0.0 : v)));
 }
 
 // tensor-core tile-pair kernel (gram_pair.cu)

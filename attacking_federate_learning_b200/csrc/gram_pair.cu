@@ -174,7 +174,7 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
 #pragma unroll
           for (int r = 0; r < kGramCenterRows; ++r) { cen.x += t[r].x; cen.y += t[r].y; cen.z += t[r].z; cen.w += t[r].w; }
           const float inv = 1.0f / static_cast<float>(kGramCenterRows);
-          cen = make_float4(cen.x * inv, cen.y * inv, cen.z * inv, cen.w * inv);
+          cen = gram_center_finite(make_float4(cen.x * inv, cen.y * inv, cen.z * inv, cen.w * inv));
         }
         float4 v[4];
 #pragma unroll
@@ -343,6 +343,8 @@ pair_reduce_kernel(const float* __restrict__ parts, int n, int splits, int sym, 
 // d2_ij = (S_hh + S_ll) - 2 S_hl with h = max(i, j), l = min(i, j): exactly symmetric, zero diagonal, and exactly
 // zero between clients whose rows are identical.  sym: 2 S_hl = S[h][l] + S[l][h], the split sums of M_hl and M_lh
 // (a floating-point addition is commutative, so identical rows still give bit-identical table rows).
+// A row with an inf (its split operands hold inf - inf = NaN) or whose squared norm overflows has a non-finite S_hh:
+// its distance to every other client is +inf, as the reference's fp32 norm of a difference that contains an inf.
 __global__ void pair_to_sqdist_kernel(const double* __restrict__ S, int n, int sym, double* __restrict__ d2) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = blockIdx.y;
@@ -350,9 +352,10 @@ __global__ void pair_to_sqdist_kernel(const double* __restrict__ S, int n, int s
   double v = 0.0;
   if (i != j) {
     const int lo = min(i, j), hi = max(i, j);
+    const double s_hh = S[static_cast<size_t>(hi) * n + hi], s_ll = S[static_cast<size_t>(lo) * n + lo];
     const double s_hl = S[static_cast<size_t>(hi) * n + lo];
-    v = (S[static_cast<size_t>(hi) * n + hi] + S[static_cast<size_t>(lo) * n + lo]) -
-        (sym ? s_hl + S[static_cast<size_t>(lo) * n + hi] : 2.0 * s_hl);
+    v = (isfinite(s_hh) && isfinite(s_ll)) ? (s_hh + s_ll) - (sym ? s_hl + S[static_cast<size_t>(lo) * n + hi] : 2.0 * s_hl)
+                                           : __longlong_as_double(0x7ff0000000000000ll);
   }
   d2[static_cast<size_t>(i) * n + j] = v;
 }

@@ -117,8 +117,9 @@ __device__ __forceinline__ KrumKey<kSrc> krum_key(const KrumParams& p, int u, in
     double s = 0.0;
     for (int r = 0; r < p.world; ++r)                                    // fixed rank order: identical sum on every rank
       s += p.world > 1 ? ld_peer_f64(p.tab[r] + e) : p.tab[0][e];
-    const float dist = static_cast<float>(sqrt(s > 0.0 ? s : 0.0));     // defences.py:20 (np.float32 norm)
-    return __float_as_uint(dist) & 0x7FFFFFFFu;                          // >= 0: the bit pattern orders like the value
+    // defences.py:20 (np.float32 norm); a negative cancellation residue is 0, a NaN stays NaN (sorts last, never eligible)
+    const float dist = static_cast<float>(sqrt(s > 0.0 ? s : (s == s ? 0.0 : s)));
+    return __float_as_uint(dist) & 0x7FFFFFFFu;                          // >= 0 or NaN: the bit pattern orders like the value
   } else {
     return dist_key(p.dist[e], v);
   }
@@ -287,6 +288,7 @@ bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, So
   }
 }
 
+int max_clients() { return kMaxN; }
 size_t workspace_bytes(int n) { return ws_bytes_for(n < 1 ? 1 : n); }
 
 static int check_ws(int n, void* ws, size_t ws_bytes) {

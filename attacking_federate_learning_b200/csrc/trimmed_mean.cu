@@ -164,6 +164,7 @@ __device__ __forceinline__ void warp_select(const float (&v)[S], int n, int r1, 
         return;
       }
       p = 0.5f * vmin + 0.5f * vmax;
+      if (vmin == -kInf) p = -__FLT_MAX__;          // a -inf group: the midpoint would be -inf, split the group off
       if (!(p > vmin)) p = vmax;
       model = false;
     }
@@ -542,9 +543,22 @@ __device__ __forceinline__ float general_column_impl(const Params& P, const uint
     int c_lo = 0, c_hi = n;
     col.med = med;
     if (!select_fast<S, true, BF16>(x, col, n, P.keep - 1, P.keep - 1, P.key_q * sd, P.key_density * inv_sd, lane, jx, scratch, lo, hi,
-                              c_lo, c_hi, sl, total, unused))
-      warp_select<S, true>(x, n, P.keep - 1, P.keep - 1, P.key_q * sd, P.key_density * inv_sd, lane, jx, scratch, lo, hi,
-                           c_lo, c_hi, sl, total, unused);
+                              c_lo, c_hi, sl, total, unused)) {
+      // General path.  Infinite deviations (an inf in the column, or fl32(x - med) overflowing) share the key +inf with
+      // the padded rows, so the bracket's upper count is the number of finite keys, not n.  When the keep boundary is
+      // at or past it, the threshold is +inf: every finite deviation is kept, and the infinite ones in row order
+      // (padded rows come after every real row, so tie_sum never reaches them).
+      int c_fin;
+      float s_fin = 0.f;
+      count_pass<S, true>(x, kInf, c_fin, s_fin);
+      if (P.keep > c_fin) {
+        total = warp_sum(s_fin + tie_sum<S>(x, kInf, P.keep - c_fin, jx, lane));
+      } else {
+        if (hi == kInf) c_hi = c_fin;
+        warp_select<S, true>(x, n, P.keep - 1, P.keep - 1, P.key_q * sd, P.key_density * inv_sd, lane, jx, scratch, lo, hi,
+                             c_lo, c_hi, sl, total, unused);
+      }
+    }
     res = __fadd_rn(__fdiv_rn(total, static_cast<float>(P.keep)), med);
   }
   return res;

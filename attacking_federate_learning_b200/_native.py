@@ -48,6 +48,9 @@ SIGNATURES = {
                               C.POINTER(C.POINTER(_i)), C.POINTER(C.POINTER(_i))]),
     "afl_sqdist_allreduce": (_i, [_vp, _vp, _i, _i64, _i64, _i, _vp, _vp, _sz, _i, _vp, C.POINTER(C.POINTER(_i))]),
     "afl_defend_host": (_i, [C.c_char_p, _vp, _i, _i64, _i64, _i, _i, _vp, C.POINTER(_i), _i64]),
+    "afl_sqdist_host": (_i, [_vp, _i, _i64, _i64, _vp, _i64]),
+    "afl_bulyan_host": (_i, [_vp, _i, _i64, _i64, _i, _i, _vp, _vp, _i64]),
+    "afl_alie_host": (_i, [_vp, _i, _i64, _d, _vp, _vp, _vp, _i64]),
 }
 
 _lib = None

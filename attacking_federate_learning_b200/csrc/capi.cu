@@ -128,17 +128,21 @@ __global__ void add_f64_kernel(double* __restrict__ acc, const double* __restric
 
 // ------------------------------------------------------------------------------------------------
 // Host-buffer path: the matrix stays in host memory and is streamed through a bounded device staging area.
+// Every host entry point (afl_defend_host, afl_sqdist_host, afl_bulyan_host, afl_alie_host) runs on the
+// helpers below: one HostCall per call, one stage() for the budget and buffers, one slot ring.
 //
 //   * Column slabs of `slab_cols` columns go through a ring of kRingSlots device slots: the copy stream fills
 //     slot s % slots while the compute stream runs the kernels of the slab before it.  `freed[slot]` is
 //     recorded on the compute stream after the last kernel that reads the slot, and the copy stream waits on
 //     it before overwriting the slot.
-//   * Krum sums one d2 table per slab (sqdist_partial + add_f64_kernel, in slab order); TrimmedMean and
-//     NoDefense finish each slab's columns as soon as its kernel has run.
+//   * Krum, Bulyan and afl_sqdist_host sum one d2 table per slab (sum_sqdist: sqdist_partial + add_f64_kernel,
+//     in slab order); TrimmedMean and NoDefense finish each slab's columns as soon as its kernel has run.
 //   * Bulyan keeps slabs 0 .. R-1 resident (as many as the budget holds) and streams the rest.  After
 //     selection, stage 2 runs once over the resident columns with row_index = sel; for the other columns it
 //     re-streams only the theta selected rows, packed in selection order, and runs the same trimmed mean with
 //     row_index = NULL.  When the whole matrix fits, R covers every slab and nothing is streamed twice.
+//   * ALIE packs the f separate user vectors of each slab into a slot (one copy per row) and runs the
+//     column-wise alie kernel on it.
 //   * Budget: free device memory plus what this context already holds, minus 1 GiB, capped by the
 //     environment variable AFL_HOST_DEVICE_BYTES (read on every call).
 //
@@ -153,7 +157,7 @@ struct HostCtx {
   std::mutex mu;
   void* stage = nullptr; size_t stage_bytes = 0;   // Bulyan's resident prefix, then the ring slots
   void* ws = nullptr; size_t ws_bytes = 0;          // kernel workspace
-  void* small = nullptr; size_t small_bytes = 0;    // d2 tables, dist, indices, output vector
+  void* small = nullptr; size_t small_bytes = 0;    // d2 tables, dist, indices, output vectors
   cudaStream_t copy = nullptr, comp = nullptr;
   cudaEvent_t ready = nullptr;                      // slab landed (recorded on copy, waited on at once by comp)
   cudaEvent_t freed[kRingSlots];                    // compute stream is done reading the slot
@@ -181,80 +185,92 @@ static size_t host_budget(size_t free_b, size_t held) {
   return b;
 }
 
-static int defend_host(const char* rule, const float* G, int n, int64_t d, int64_t ld, int users_count, int f,
-                       float* out_host, int* idx_out, int64_t slab_cols) {
-  enum { R_MEAN, R_KRUM, R_TM, R_BULYAN } r;
-  if (!strcmp(rule, "NoDefense")) r = R_MEAN;
-  else if (!strcmp(rule, "Krum")) r = R_KRUM;
-  else if (!strcmp(rule, "TrimmedMean")) r = R_TM;
-  else if (!strcmp(rule, "Bulyan")) r = R_BULYAN;
-  else { set_error("afl_defend_host: unknown rule '%s'", rule); return AFL_ERR_BAD_ARG; }
-  if (!G || n < 1 || d < 1 || ld < d) { set_error("afl_defend_host: bad argument"); return AFL_ERR_BAD_ARG; }
-  if (r != R_KRUM && !out_host) { set_error("afl_defend_host: out_host is required for %s", rule); return AFL_ERR_BAD_ARG; }
-  // the reference's asserts (defences.py:24-25, :56)
-  if (r == R_KRUM && users_count < 2 * f + 1) {
-    set_error("krum: users_count >= 2*corrupted_count + 1 violated (%d, %d)", users_count, f);
-    return AFL_ERR_PRECONDITION;
-  }
-  if (r == R_BULYAN && users_count < 4 * f + 3) {
-    set_error("bulyan: users_count >= 4*corrupted_count + 3 violated (%d, %d)", users_count, f);
-    return AFL_ERR_PRECONDITION;
-  }
-  if ((r == R_KRUM || r == R_BULYAN) && n > select::max_clients()) {   // before any copy or launch
-    set_error("afl_defend_host: %s supports n <= %d clients (got %d)", rule, select::max_clients(), n);
-    return AFL_ERR_UNSUPPORTED;
-  }
-  HostCtx& c = g_ctx[current_device()];          // streams, events and buffers belong to the current device
-  std::lock_guard<std::mutex> lock(c.mu);
-  if (!c.init) {
-    AFL_CUDA(cudaStreamCreateWithFlags(&c.copy, cudaStreamNonBlocking));
-    AFL_CUDA(cudaStreamCreateWithFlags(&c.comp, cudaStreamNonBlocking));
-    AFL_CUDA(cudaEventCreateWithFlags(&c.ready, cudaEventDisableTiming));
-    for (auto& e : c.freed) AFL_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    c.init = true;
-  }
-  struct Drain {                                  // every return leaves both streams idle: no copy still reads G
-    HostCtx& c;
-    ~Drain() { cudaStreamSynchronize(c.copy); cudaStreamSynchronize(c.comp); }
-  } drain{c};
-  const bool table = r == R_KRUM || r == R_BULYAN;
-  const int theta = r == R_BULYAN ? users_count - 2 * f : 0;
-  const int64_t ld_dev = (d + 31) / 32 * 32;          // padded pitch: TMA + 16-byte loads always apply
-  if (slab_cols <= 0) slab_cols = (int64_t(96) << 20) / (static_cast<int64_t>(n) * 4);   // ~96 MB per slab
+// Columns per slab: slab_cols rounded up to a multiple of 32 (0 = about 96 MB of `rows` rows), never wider than
+// the padded matrix.
+static int64_t slab_width(int64_t slab_cols, int rows, int64_t d) {
+  const int64_t ld_dev = (d + 31) / 32 * 32;
+  if (slab_cols <= 0) slab_cols = (int64_t(96) << 20) / (static_cast<int64_t>(rows) * 4);
   slab_cols = (slab_cols + 31) / 32 * 32;
   if (slab_cols < 32) slab_cols = 32;
-  if (slab_cols > ld_dev) slab_cols = ld_dev;         // one slab either way; keeps the slots no wider than the matrix
-  const int nslab = static_cast<int>((d + slab_cols - 1) / slab_cols);
-  const size_t nn = static_cast<size_t>(n) * n;
-  const int sel_len = n > theta ? n : theta;         // also the rows of a slot: Bulyan's second pass packs theta rows
+  return slab_cols > ld_dev ? ld_dev : slab_cols;
+}
 
-  // ---- device footprint: workspaces and tables (fixed), then the resident prefix and the ring
-  const size_t gram_ws_bytes = table ? align_up(gram::workspace_bytes(n, slab_cols, AFL_F32, 0), 256) : 0;
-  const size_t ws_need = table ? gram_ws_bytes + select::workspace_bytes(n) : 256;
-  const size_t small_need = (table ? align_up(nn * 8, 256) * 2 + align_up(nn * 4, 256) : 0) +
-                            align_up(static_cast<size_t>(sel_len) * 4, 256) +
-                            (r != R_KRUM ? align_up(static_cast<size_t>(d) * 4, 256) : 0) + 1024;
+// One call's hold on the current device's context: the lock, the streams and events (created once), and on
+// every return both streams drained, so that no copy still reads the caller's host buffers.
+struct HostCall {
+  HostCtx& c;
+  std::lock_guard<std::mutex> lock;
+  bool open = false;
+  HostCall() : c(g_ctx[current_device()]), lock(c.mu) {}
+  ~HostCall() {
+    if (open) { cudaStreamSynchronize(c.copy); cudaStreamSynchronize(c.comp); }
+  }
+  int begin() {
+    if (!c.init) {
+      AFL_CUDA(cudaStreamCreateWithFlags(&c.copy, cudaStreamNonBlocking));
+      AFL_CUDA(cudaStreamCreateWithFlags(&c.comp, cudaStreamNonBlocking));
+      AFL_CUDA(cudaEventCreateWithFlags(&c.ready, cudaEventDisableTiming));
+      for (auto& e : c.freed) AFL_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      c.init = true;
+    }
+    open = true;
+    return AFL_OK;
+  }
+  // the copy stream has issued a slab: the compute stream waits for it before the slab's kernels
+  cudaError_t landed() {
+    cudaError_t e = cudaEventRecord(c.ready, c.copy);
+    return e != cudaSuccess ? e : cudaStreamWaitEvent(c.comp, c.ready, 0);
+  }
+};
+
+// The staging area of one call, carved out of HostCtx::stage: slabs 0 .. R-1 resident at pitch ld_res, then
+// `slots` ring slots of slot_elems floats.
+struct Staging {
+  int nslab = 0, R = 0, slots = 0;
+  int64_t ld_res = 0, d_res = 0;                     // resident pitch and columns
+  float* res = nullptr;
+  float* ring = nullptr;
+  int64_t slot_elems = 0;
+  int64_t issued = 0;                                // ring slabs issued so far
+
+  // next ring slot: the copy stream waits until the compute stream has finished reading it
+  cudaError_t next_slot(HostCtx& c, int* slot, float** m) {
+    *slot = static_cast<int>(issued % slots);
+    *m = ring + *slot * slot_elems;
+    return issued++ >= slots ? cudaStreamWaitEvent(c.copy, c.freed[*slot], 0) : cudaSuccess;
+  }
+};
+
+// Fits a call into the budget and sizes the cached buffers: ws_need + small_need bytes are always held, plus
+// two or three ring slots of slot_rows x slab_cols floats.  With `resident` (Bulyan) the rest of the budget goes
+// to leading slabs of the n-row matrix that stay on the device (all of them when the matrix fits); otherwise the
+// ring gets a third slot when it fits.  `who` names the entry point in the error.
+static int stage(const char* who, HostCtx& c, int n, int64_t d, int64_t slab_cols, int slot_rows, size_t ws_need,
+                 size_t small_need, bool resident, Staging* st) {
+  const int64_t ld_dev = (d + 31) / 32 * 32;          // padded pitch: TMA + 16-byte loads always apply
+  const int nslab = static_cast<int>((d + slab_cols - 1) / slab_cols);
   const size_t slab_bytes = static_cast<size_t>(n) * slab_cols * sizeof(float);
-  const size_t slot_bytes = align_up(static_cast<size_t>(sel_len) * slab_cols * sizeof(float), 256);
+  const size_t slot_bytes = align_up(static_cast<size_t>(slot_rows) * slab_cols * sizeof(float), 256);
   size_t free_b = 0, total_b = 0;
   AFL_CUDA(cudaMemGetInfo(&free_b, &total_b));
   const size_t budget = host_budget(free_b, c.stage_bytes + c.ws_bytes + c.small_bytes);
   const size_t fixed = ws_need + small_need;
   const size_t full_res = align_up(static_cast<size_t>(n) * ld_dev * sizeof(float), 256);
   int R = 0, slots = 0;                               // resident slabs, ring slots
-  if (r == R_BULYAN && fixed + full_res <= budget) {
+  if (resident && fixed + full_res <= budget) {
     R = nslab;
   } else {
     const int min_slots = nslab < 2 ? nslab : 2;
     if (fixed + min_slots * slot_bytes > budget) {
-      set_error("afl_defend_host: needs %zu bytes of device memory (%d staging slots of %zu bytes for %lld-column slabs, "
+      set_error("%s: needs %zu bytes of device memory (%d staging slots of %zu bytes for %lld-column slabs, "
                 "plus %zu bytes of tables and workspaces) but may use %zu (free memory less 1 GiB, capped by "
                 "AFL_HOST_DEVICE_BYTES); use narrower slabs or a larger budget",
-                fixed + min_slots * slot_bytes, min_slots, slot_bytes, static_cast<long long>(slab_cols), fixed, budget);
+                who, fixed + min_slots * slot_bytes, min_slots, slot_bytes, static_cast<long long>(slab_cols), fixed,
+                budget);
       return AFL_ERR_UNSUPPORTED;
     }
     slots = min_slots;
-    if (r == R_BULYAN) {                              // spend the rest on resident slabs: they are not re-streamed
+    if (resident) {                                   // spend the rest on resident slabs: they are not re-streamed
       const size_t spare = budget - fixed - slots * slot_bytes;
       const size_t fit = spare > 256 ? (spare - 256) / slab_bytes : 0;
       R = static_cast<int>(fit < static_cast<size_t>(nslab - 1) ? fit : static_cast<size_t>(nslab - 1));
@@ -263,8 +279,7 @@ static int defend_host(const char* rule, const float* G, int n, int64_t d, int64
       while (slots < most && fixed + (slots + 1) * slot_bytes <= budget) ++slots;
     }
   }
-  const int64_t ld_res = R == nslab ? ld_dev : R * slab_cols;   // resident pitch
-  const int64_t d_res = R == nslab ? d : R * slab_cols;        // resident columns
+  const int64_t ld_res = R == nslab ? ld_dev : R * slab_cols;
   const size_t res_bytes = align_up(static_cast<size_t>(n) * ld_res * sizeof(float), 256);
   const size_t stage_need = res_bytes + slots * slot_bytes;
 
@@ -281,61 +296,191 @@ static int defend_host(const char* rule, const float* G, int n, int64_t d, int64
     const int rc = ensure(bufs[i], have[i], want[i]);
     if (rc) return rc;
   }
+  st->nslab = nslab; st->R = R; st->slots = slots;
+  st->ld_res = ld_res;
+  st->d_res = R == nslab ? d : R * slab_cols;
+  st->res = static_cast<float*>(c.stage);
+  st->ring = reinterpret_cast<float*>(static_cast<uint8_t*>(c.stage) + res_bytes);
+  st->slot_elems = static_cast<int64_t>(slot_bytes / sizeof(float));
+  st->issued = 0;
+  return AFL_OK;
+}
 
-  uint8_t* sp = static_cast<uint8_t*>(c.small);
-  double* d2_acc = nullptr; double* d2_part = nullptr; float* dist = nullptr;
-  if (table) {
-    d2_acc = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
-    d2_part = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
-    dist = reinterpret_cast<float*>(sp); sp += align_up(nn * 4, 256);
-  }
-  int* sel = reinterpret_cast<int*>(sp); sp += align_up(static_cast<size_t>(sel_len) * 4, 256);
-  float* out_dev = reinterpret_cast<float*>(sp);
-  float* res = static_cast<float*>(c.stage);
-  float* ring = reinterpret_cast<float*>(static_cast<uint8_t*>(c.stage) + res_bytes);
-  const int64_t slot_elems = static_cast<int64_t>(slot_bytes / sizeof(float));
-  void* gram_ws = c.ws;
-  void* sel_ws = static_cast<uint8_t*>(c.ws) + gram_ws_bytes;
-  const size_t sel_ws_bytes = c.ws_bytes - gram_ws_bytes;
-  int rc = AFL_OK;
-  int64_t ring_i = 0;                                 // ring slabs issued so far (pass 1 and pass 2)
-
-  // next ring slot: the copy stream waits until the compute stream has finished reading it
-  auto next_slot = [&](int* slot, float** m) -> cudaError_t {
-    *slot = static_cast<int>(ring_i % slots);
-    *m = ring + *slot * slot_elems;
-    return ring_i++ >= slots ? cudaStreamWaitEvent(c.copy, c.freed[*slot], 0) : cudaSuccess;
-  };
-
-  // ---- pass 1: every column once
-  for (int s = 0; s < nslab; ++s) {
+// Pass 1: every column of the n x d host matrix G (pitch ld) once, slab by slab into the resident prefix or the
+// ring.  kernel(m, mld, c0, w, s) enqueues slab s (columns c0 .. c0+w-1 at m, pitch mld) on the compute stream.
+template <typename Kernel>
+static int pass1(HostCall& call, Staging& st, const float* G, int n, int64_t d, int64_t ld, int64_t slab_cols,
+                 Kernel kernel) {
+  HostCtx& c = call.c;
+  for (int s = 0; s < st.nslab; ++s) {
     const int64_t c0 = static_cast<int64_t>(s) * slab_cols;
     const int64_t w = (d - c0 < slab_cols) ? d - c0 : slab_cols;
     int slot = -1;
-    float* m = res + c0;
-    if (s >= R) AFL_CUDA(next_slot(&slot, &m));
-    const int64_t mld = s < R ? ld_res : slab_cols;
+    float* m = st.res + c0;
+    if (s >= st.R) AFL_CUDA(st.next_slot(c, &slot, &m));
+    const int64_t mld = s < st.R ? st.ld_res : slab_cols;
     AFL_CUDA(cudaMemcpy2DAsync(m, mld * sizeof(float), G + c0, ld * sizeof(float), w * sizeof(float), n,
                                cudaMemcpyHostToDevice, c.copy));
-    AFL_CUDA(cudaEventRecord(c.ready, c.copy));
-    AFL_CUDA(cudaStreamWaitEvent(c.comp, c.ready, 0));
-    if (table) {
-      rc = gram::sqdist_partial(m, n, w, mld, AFL_F32, d2_part, gram_ws, gram_ws_bytes, 0, c.comp);
-      if (rc) return rc;
-      add_f64_kernel<<<static_cast<unsigned>((nn + 255) / 256), 256, 0, c.comp>>>(d2_acc, d2_part, nn, s == 0);
-      AFL_LAUNCH_CHECK("add_f64_kernel");
-    } else if (r == R_TM) {
-      rc = tmean::trimmed_mean(m, n, w, mld, AFL_F32, nullptr, n, f, out_dev + c0, c.comp);
-      if (rc) return rc;
-    } else {
-      rc = colstats::mean(m, n, w, mld, AFL_F32, out_dev + c0, c.comp);
-      if (rc) return rc;
-    }
+    AFL_CUDA(call.landed());
+    const int rc = kernel(m, mld, c0, w, s);
+    if (rc) return rc;
     if (slot >= 0) AFL_CUDA(cudaEventRecord(c.freed[slot], c.comp));
   }
+  return AFL_OK;
+}
+
+// Pass 1 into the summed n x n float64 d2 table: sqdist_partial per slab into d2_part, added into d2_acc in slab
+// order.  Krum, Bulyan and afl_sqdist_host all build their table here.
+static int sum_sqdist(HostCall& call, Staging& st, const float* G, int n, int64_t d, int64_t ld, int64_t slab_cols,
+                      double* d2_acc, double* d2_part, void* gram_ws, size_t gram_ws_bytes) {
+  const size_t nn = static_cast<size_t>(n) * n;
+  cudaStream_t comp = call.c.comp;
+  return pass1(call, st, G, n, d, ld, slab_cols, [&](const float* m, int64_t mld, int64_t, int64_t w, int s) -> int {
+    const int rc = gram::sqdist_partial(m, n, w, mld, AFL_F32, d2_part, gram_ws, gram_ws_bytes, 0, comp);
+    if (rc) return rc;
+    add_f64_kernel<<<static_cast<unsigned>((nn + 255) / 256), 256, 0, comp>>>(d2_acc, d2_part, nn, s == 0);
+    AFL_LAUNCH_CHECK("add_f64_kernel");
+    return AFL_OK;
+  });
+}
+
+static int sqdist_host(const float* G, int n, int64_t d, int64_t ld, double* d2_out, int64_t slab_cols) {
+  if (!G || !d2_out || n < 1 || d < 1 || ld < d) { set_error("afl_sqdist_host: bad argument"); return AFL_ERR_BAD_ARG; }
+  HostCall call;
+  int rc = call.begin(); if (rc) return rc;
+  slab_cols = slab_width(slab_cols, n, d);
+  const size_t nn = static_cast<size_t>(n) * n;
+  const size_t gram_ws_bytes = align_up(gram::workspace_bytes(n, slab_cols, AFL_F32, 0), 256);
+  Staging st;
+  rc = stage("afl_sqdist_host", call.c, n, d, slab_cols, n, gram_ws_bytes, align_up(nn * 8, 256), false, &st);
+  if (rc) return rc;
+  rc = sum_sqdist(call, st, G, n, d, ld, slab_cols, d2_out, static_cast<double*>(call.c.small), call.c.ws, gram_ws_bytes);
+  if (rc) return rc;
+  AFL_CUDA(cudaStreamSynchronize(call.c.comp));
+  return AFL_OK;
+}
+
+static int bulyan_host(const char* who, const float* G, int n, int64_t d, int64_t ld, int users_count, int f,
+                       float* out_host, int* sel_host, int64_t slab_cols) {
+  if (!G || n < 1 || d < 1 || ld < d) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
+  if (!out_host) { set_error("%s: out_host is required for Bulyan", who); return AFL_ERR_BAD_ARG; }
+  if (users_count < 4 * f + 3) {                      // the reference's assert (defences.py:56)
+    set_error("bulyan: users_count >= 4*corrupted_count + 3 violated (%d, %d)", users_count, f);
+    return AFL_ERR_PRECONDITION;
+  }
+  if (n > select::max_clients()) {                    // before any copy or launch
+    set_error("%s: Bulyan supports n <= %d clients (got %d)", who, select::max_clients(), n);
+    return AFL_ERR_UNSUPPORTED;
+  }
+  HostCall call;
+  int rc = call.begin(); if (rc) return rc;
+  HostCtx& c = call.c;
+  const int theta = users_count - 2 * f;
+  slab_cols = slab_width(slab_cols, n, d);
+  const size_t nn = static_cast<size_t>(n) * n;
+  const int sel_len = n > theta ? n : theta;         // also the rows of a slot: the second pass packs theta rows
+  const size_t gram_ws_bytes = align_up(gram::workspace_bytes(n, slab_cols, AFL_F32, 0), 256);
+  const size_t small_need = align_up(nn * 8, 256) * 2 + align_up(nn * 4, 256) +
+                            align_up(static_cast<size_t>(sel_len) * 4, 256) + align_up(static_cast<size_t>(d) * 4, 256) + 1024;
+  Staging st;
+  rc = stage(who, c, n, d, slab_cols, sel_len, gram_ws_bytes + select::workspace_bytes(n), small_need, true, &st);
+  if (rc) return rc;
+  uint8_t* sp = static_cast<uint8_t*>(c.small);
+  double* d2_acc = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
+  double* d2_part = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
+  float* dist = reinterpret_cast<float*>(sp); sp += align_up(nn * 4, 256);
+  int* sel = reinterpret_cast<int*>(sp); sp += align_up(static_cast<size_t>(sel_len) * 4, 256);
+  float* out_dev = reinterpret_cast<float*>(sp);
+  void* sel_ws = static_cast<uint8_t*>(c.ws) + gram_ws_bytes;
+  const size_t sel_ws_bytes = c.ws_bytes - gram_ws_bytes;
+
+  rc = sum_sqdist(call, st, G, n, d, ld, slab_cols, d2_acc, d2_part, c.ws, gram_ws_bytes); if (rc) return rc;
+  rc = gram::sqdist_to_dist(d2_acc, n, dist, c.comp); if (rc) return rc;
+  rc = select::bulyan_select(dist, n, users_count, f, sel, sel_ws, sel_ws_bytes, c.comp); if (rc) return rc;
+  if (st.R > 0) {                                     // stage 2 over the resident columns
+    rc = tmean::trimmed_mean(st.res, n, st.d_res, st.ld_res, AFL_F32, sel, theta, 2 * f, out_dev, c.comp);
+    if (rc) return rc;
+  }
+  std::vector<int> hsel(static_cast<size_t>(theta));
+  AFL_CUDA(cudaMemcpyAsync(hsel.data(), sel, static_cast<size_t>(theta) * sizeof(int), cudaMemcpyDeviceToHost, c.comp));
+  AFL_CUDA(cudaStreamSynchronize(c.comp));
+  if (sel_host) memcpy(sel_host, hsel.data(), static_cast<size_t>(theta) * sizeof(int));
+  if (hsel[theta - 1] < 0) {                          // a failed round marks itself and every later round with -1
+    set_error("bulyan: a selection round found no eligible user (NaN or >= 1e20 scores); the reference raises KeyError(-1)");
+    return AFL_ERR_NO_WINNER;
+  }
+  // ---- pass 2: the theta selected rows of the streamed columns, packed in selection order.  The kernel is
+  // column-wise, so the slab may be as wide as a slot holds.
+  const int64_t w2 = st.slot_elems / theta / 32 * 32;
+  for (int64_t c0 = st.d_res; c0 < d; c0 += w2) {
+    const int64_t w = (d - c0 < w2) ? d - c0 : w2;
+    int slot = -1;
+    float* m = nullptr;
+    AFL_CUDA(st.next_slot(c, &slot, &m));
+    for (int i = 0; i < theta; ++i) {
+      const int row = hsel[i] < 0 ? hsel[i] + n : hsel[i];
+      AFL_CUDA(cudaMemcpyAsync(m + static_cast<int64_t>(i) * w2, G + static_cast<int64_t>(row) * ld + c0,
+                               w * sizeof(float), cudaMemcpyHostToDevice, c.copy));
+    }
+    AFL_CUDA(call.landed());
+    rc = tmean::trimmed_mean(m, theta, w, w2, AFL_F32, nullptr, theta, 2 * f, out_dev + c0, c.comp); if (rc) return rc;
+    AFL_CUDA(cudaEventRecord(c.freed[slot], c.comp));
+  }
+  AFL_CUDA(cudaMemcpyAsync(out_host, out_dev, static_cast<size_t>(d) * sizeof(float), cudaMemcpyDeviceToHost, c.comp));
+  AFL_CUDA(cudaStreamSynchronize(c.comp));
+  return AFL_OK;
+}
+
+static int defend_host(const char* rule, const float* G, int n, int64_t d, int64_t ld, int users_count, int f,
+                       float* out_host, int* idx_out, int64_t slab_cols) {
+  enum { R_MEAN, R_KRUM, R_TM } r;
+  if (!strcmp(rule, "NoDefense")) r = R_MEAN;
+  else if (!strcmp(rule, "Krum")) r = R_KRUM;
+  else if (!strcmp(rule, "TrimmedMean")) r = R_TM;
+  else if (!strcmp(rule, "Bulyan")) {
+    const int rc = bulyan_host("afl_defend_host", G, n, d, ld, users_count, f, out_host, nullptr, slab_cols);
+    if (rc == AFL_OK && idx_out) *idx_out = -1;
+    return rc;
+  }
+  else { set_error("afl_defend_host: unknown rule '%s'", rule); return AFL_ERR_BAD_ARG; }
+  if (!G || n < 1 || d < 1 || ld < d) { set_error("afl_defend_host: bad argument"); return AFL_ERR_BAD_ARG; }
+  if (r != R_KRUM && !out_host) { set_error("afl_defend_host: out_host is required for %s", rule); return AFL_ERR_BAD_ARG; }
+  // the reference's assert (defences.py:24-25)
+  if (r == R_KRUM && users_count < 2 * f + 1) {
+    set_error("krum: users_count >= 2*corrupted_count + 1 violated (%d, %d)", users_count, f);
+    return AFL_ERR_PRECONDITION;
+  }
+  if (r == R_KRUM && n > select::max_clients()) {   // before any copy or launch
+    set_error("afl_defend_host: %s supports n <= %d clients (got %d)", rule, select::max_clients(), n);
+    return AFL_ERR_UNSUPPORTED;
+  }
+  HostCall call;
+  int rc = call.begin(); if (rc) return rc;
+  HostCtx& c = call.c;
+  const bool table = r == R_KRUM;
+  slab_cols = slab_width(slab_cols, n, d);
+  const size_t nn = static_cast<size_t>(n) * n;
+
+  // ---- device footprint: workspaces and tables (fixed), then the ring
+  const size_t gram_ws_bytes = table ? align_up(gram::workspace_bytes(n, slab_cols, AFL_F32, 0), 256) : 0;
+  const size_t ws_need = table ? gram_ws_bytes + select::workspace_bytes(n) : 256;
+  const size_t small_need = (table ? align_up(nn * 8, 256) * 2 + align_up(nn * 4, 256) : 0) +
+                            align_up(static_cast<size_t>(n) * 4, 256) +
+                            (r != R_KRUM ? align_up(static_cast<size_t>(d) * 4, 256) : 0) + 1024;
+  Staging st;
+  rc = stage("afl_defend_host", c, n, d, slab_cols, n, ws_need, small_need, false, &st);
+  if (rc) return rc;
+
+  uint8_t* sp = static_cast<uint8_t*>(c.small);
   if (r == R_KRUM) {
+    double* d2_acc = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256);
+    double* d2_part = reinterpret_cast<double*>(sp); sp += align_up(nn * 8, 256) + align_up(nn * 4, 256);
+    int* sel = reinterpret_cast<int*>(sp);
+    rc = sum_sqdist(call, st, G, n, d, ld, slab_cols, d2_acc, d2_part, c.ws, gram_ws_bytes); if (rc) return rc;
     int host_idx = -1;
-    rc = select::krum_from_sqdist(d2_acc, n, users_count, f, sel, sel_ws, sel_ws_bytes, c.comp); if (rc) return rc;
+    rc = select::krum_from_sqdist(d2_acc, n, users_count, f, sel, static_cast<uint8_t*>(c.ws) + gram_ws_bytes,
+                                  c.ws_bytes - gram_ws_bytes, c.comp);
+    if (rc) return rc;
     AFL_CUDA(cudaMemcpyAsync(&host_idx, sel, sizeof(int), cudaMemcpyDeviceToHost, c.comp));
     AFL_CUDA(cudaStreamSynchronize(c.comp));
     if (idx_out) *idx_out = host_idx;
@@ -345,41 +490,60 @@ static int defend_host(const char* rule, const float* G, int n, int64_t d, int64
     }
     return AFL_OK;
   }
-  if (r == R_BULYAN) {
-    rc = gram::sqdist_to_dist(d2_acc, n, dist, c.comp); if (rc) return rc;
-    rc = select::bulyan_select(dist, n, users_count, f, sel, sel_ws, sel_ws_bytes, c.comp); if (rc) return rc;
-    if (R > 0) {                                      // stage 2 over the resident columns
-      rc = tmean::trimmed_mean(res, n, d_res, ld_res, AFL_F32, sel, theta, 2 * f, out_dev, c.comp); if (rc) return rc;
-    }
-    std::vector<int> hsel(static_cast<size_t>(theta));
-    AFL_CUDA(cudaMemcpyAsync(hsel.data(), sel, static_cast<size_t>(theta) * sizeof(int), cudaMemcpyDeviceToHost, c.comp));
-    AFL_CUDA(cudaStreamSynchronize(c.comp));
-    if (hsel[theta - 1] < 0) {                        // a failed round marks itself and every later round with -1
-      set_error("bulyan: a selection round found no eligible user (NaN or >= 1e20 scores); the reference raises KeyError(-1)");
-      return AFL_ERR_NO_WINNER;
-    }
-    // ---- pass 2: the theta selected rows of the streamed columns, packed in selection order.  The kernel is
-    // column-wise, so the slab may be as wide as a slot holds.
-    const int64_t w2 = slot_elems / theta / 32 * 32;
-    for (int64_t c0 = d_res; c0 < d; c0 += w2) {
-      const int64_t w = (d - c0 < w2) ? d - c0 : w2;
-      int slot = -1;
-      float* m = nullptr;
-      AFL_CUDA(next_slot(&slot, &m));
-      for (int i = 0; i < theta; ++i) {
-        const int row = hsel[i] < 0 ? hsel[i] + n : hsel[i];
-        AFL_CUDA(cudaMemcpyAsync(m + static_cast<int64_t>(i) * w2, G + static_cast<int64_t>(row) * ld + c0,
-                                 w * sizeof(float), cudaMemcpyHostToDevice, c.copy));
-      }
-      AFL_CUDA(cudaEventRecord(c.ready, c.copy));
-      AFL_CUDA(cudaStreamWaitEvent(c.comp, c.ready, 0));
-      rc = tmean::trimmed_mean(m, theta, w, w2, AFL_F32, nullptr, theta, 2 * f, out_dev + c0, c.comp); if (rc) return rc;
-      AFL_CUDA(cudaEventRecord(c.freed[slot], c.comp));
-    }
-  }
+  float* out_dev = reinterpret_cast<float*>(sp + align_up(static_cast<size_t>(n) * 4, 256));
+  rc = pass1(call, st, G, n, d, ld, slab_cols, [&](const float* m, int64_t mld, int64_t c0, int64_t w, int) -> int {
+    if (r == R_TM) return tmean::trimmed_mean(m, n, w, mld, AFL_F32, nullptr, n, f, out_dev + c0, c.comp);
+    return colstats::mean(m, n, w, mld, AFL_F32, out_dev + c0, c.comp);
+  });
+  if (rc) return rc;
   AFL_CUDA(cudaMemcpyAsync(out_host, out_dev, static_cast<size_t>(d) * sizeof(float), cudaMemcpyDeviceToHost, c.comp));
   AFL_CUDA(cudaStreamSynchronize(c.comp));
   if (idx_out) *idx_out = -1;
+  return AFL_OK;
+}
+
+static int alie_host(const float* const* rows, int f, int64_t d, double z, float* mu_out, float* sigma_out,
+                     float* crafted_out, int64_t slab_cols) {
+  if (!rows || f < 1 || d < 1) { set_error("afl_alie_host: bad argument"); return AFL_ERR_BAD_ARG; }
+  for (int i = 0; i < f; ++i)
+    if (!rows[i]) { set_error("afl_alie_host: rows[%d] is NULL", i); return AFL_ERR_BAD_ARG; }
+  HostCall call;
+  int rc = call.begin(); if (rc) return rc;
+  HostCtx& c = call.c;
+  slab_cols = slab_width(slab_cols, f, d);
+  // device copies of the outputs; crafted_out == mu_out shares one, the in-place aliasing afl_alie reproduces
+  float* outs[3] = {mu_out, sigma_out, crafted_out != mu_out ? crafted_out : nullptr};
+  const size_t vec_bytes = align_up(static_cast<size_t>(d) * 4, 256);
+  size_t small_need = 1024;
+  for (float* o : outs) small_need += o ? vec_bytes : 0;
+  Staging st;
+  rc = stage("afl_alie_host", c, f, d, slab_cols, f, 256, small_need, false, &st);
+  if (rc) return rc;
+  float* dev[3] = {nullptr, nullptr, nullptr};
+  uint8_t* sp = static_cast<uint8_t*>(c.small);
+  for (int k = 0; k < 3; ++k)
+    if (outs[k]) { dev[k] = reinterpret_cast<float*>(sp); sp += vec_bytes; }
+  float* crafted_dev = crafted_out == mu_out ? dev[0] : dev[2];
+
+  // each slab: the f row segments packed into one slot at pitch slab_cols, then the column-wise alie kernel
+  for (int64_t c0 = 0; c0 < d; c0 += slab_cols) {
+    const int64_t w = (d - c0 < slab_cols) ? d - c0 : slab_cols;
+    int slot = -1;
+    float* m = nullptr;
+    AFL_CUDA(st.next_slot(c, &slot, &m));
+    for (int i = 0; i < f; ++i)
+      AFL_CUDA(cudaMemcpyAsync(m + static_cast<int64_t>(i) * slab_cols, rows[i] + c0, w * sizeof(float),
+                               cudaMemcpyHostToDevice, c.copy));
+    AFL_CUDA(call.landed());
+    rc = colstats::alie(m, f, w, slab_cols, AFL_F32, z, dev[0] ? dev[0] + c0 : nullptr, dev[1] ? dev[1] + c0 : nullptr,
+                        crafted_dev ? crafted_dev + c0 : nullptr, nullptr, 0, c.comp);
+    if (rc) return rc;
+    AFL_CUDA(cudaEventRecord(c.freed[slot], c.comp));
+  }
+  for (int k = 0; k < 3; ++k)
+    if (outs[k])
+      AFL_CUDA(cudaMemcpyAsync(outs[k], dev[k], static_cast<size_t>(d) * sizeof(float), cudaMemcpyDeviceToHost, c.comp));
+  AFL_CUDA(cudaStreamSynchronize(c.comp));
   return AFL_OK;
 }
 
@@ -480,6 +644,20 @@ int afl_defend_host(const char* rule, const float* G_host, int n, int64_t d, int
                     int corrupted_count, float* out_host, int* idx_out, int64_t slab_cols) {
   if (!rule) { set_error("afl_defend_host: rule is NULL"); return AFL_ERR_BAD_ARG; }
   return defend_host(rule, G_host, n, d, ld, users_count, corrupted_count, out_host, idx_out, slab_cols);
+}
+
+int afl_sqdist_host(const float* G_host, int n, int64_t d, int64_t ld, double* d2_out, int64_t slab_cols) {
+  return sqdist_host(G_host, n, d, ld, d2_out, slab_cols);
+}
+
+int afl_bulyan_host(const float* G_host, int n, int64_t d, int64_t ld, int users_count, int corrupted_count,
+                    float* out_host, int* sel_host, int64_t slab_cols) {
+  return bulyan_host("afl_bulyan_host", G_host, n, d, ld, users_count, corrupted_count, out_host, sel_host, slab_cols);
+}
+
+int afl_alie_host(const float* const* rows, int f, int64_t d, double z, float* mu_out, float* sigma_out,
+                  float* crafted_out, int64_t slab_cols) {
+  return alie_host(rows, f, d, z, mu_out, sigma_out, crafted_out, slab_cols);
 }
 
 }  // extern "C"

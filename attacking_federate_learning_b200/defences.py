@@ -16,8 +16,10 @@ Reference surface mirrored (file:line in /root/reference):
     `krum` returns a *view* of the winning row exactly like the reference.  The matrix may be larger
     than the GPU: column slabs are streamed through a bounded device budget (free memory less 1 GiB,
     capped by the environment variable AFL_HOST_DEVICE_BYTES); a budget too small for two slabs and
-    the N x N tables raises NotImplementedError stating the bytes needed.  `krum(..., return_index=True)`
-    and `_krum_create_distances` still upload the whole matrix;
+    the N x N tables raises NotImplementedError stating the bytes needed.  `_krum_create_distances` and
+    `krum(..., return_index=True)` stream the matrix into the same slab-summed distance table
+    (`afl_sqdist_host`), so `krum(G, n, f)` is `G[krum(G, n, f, return_index=True)]`;
+    `bulyan(..., return_selection=True)` also returns the selection (`afl_bulyan_host`);
   * a torch.cuda float32 / bfloat16 [N, D] tensor: device-resident path, returns torch tensors
     (fp32), `krum` again returns a view `users_grads[idx]`.
 There is no CPU implementation in this package.
@@ -123,15 +125,25 @@ def no_defense(users_grads, users_count, corrupted_count):
     return out
 
 
+def _host_sqdist(G: np.ndarray):
+    """Squared-distance table (float64 [n, n] torch.cuda) of a host matrix, streamed in slabs (afl_sqdist_host):
+    the table the host Krum call selects on."""
+    import torch
+    n, d = G.shape
+    d2 = torch.empty((n, n), dtype=torch.float64, device="cuda")
+    torch.cuda.current_stream().synchronize()        # the call writes d2 from its own stream
+    nat.check(nat.lib().afl_sqdist_host(G.ctypes.data, n, d, G.strides[0] // 4, d2.data_ptr(), 0))
+    return d2
+
+
 def _krum_create_distances(users_grads):
     """Pairwise L2 distances of all clients as a DistanceTable (dense [n, n] fp32 on the GPU)."""
-    import torch
     from . import _device as dev
     if _is_torch_cuda(users_grads):
-        G = users_grads
+        d2 = dev.sqdist_partial(users_grads)
     else:
-        G = torch.from_numpy(_as_host_matrix(users_grads)).cuda()
-    return DistanceTable(dev.sqdist_to_dist(dev.sqdist_partial(G)))
+        d2 = _host_sqdist(_as_host_matrix(users_grads))
+    return DistanceTable(dev.sqdist_to_dist(d2))
 
 
 def _table_from_mapping(distances):
@@ -159,12 +171,10 @@ def krum(users_grads, users_count, corrupted_count, distances=None, return_index
         assert users_count >= 2 * corrupted_count + 1, ('users_count>=2*corrupted_count + 3', users_count, corrupted_count)
     if distances is None and not _is_torch_cuda(users_grads):
         G = _as_host_matrix(users_grads)
-        if not return_index:
-            _, idx = _host_call(DefenseTypes.Krum, G, users_count, corrupted_count, want_out=False)
-        else:
-            # return_index=True skips the reference's assert; the host entry point enforces it, so use
-            # the device path for the (rare) unchecked call
-            return krum(_to_cuda(G), users_count, corrupted_count, None, True, debug)
+        if return_index:                                 # no assert, as in the reference: select on the same table
+            from . import _device as dev
+            return int(dev.krum_from_sqdist(_host_sqdist(G), users_count, corrupted_count).item())
+        _, idx = _host_call(DefenseTypes.Krum, G, users_count, corrupted_count, want_out=False)
         return G[idx]
     from . import _device as dev
     users = None
@@ -185,11 +195,6 @@ def krum(users_grads, users_count, corrupted_count, distances=None, return_index
     return users_grads[idx]
 
 
-def _to_cuda(G: np.ndarray):
-    import torch
-    return torch.from_numpy(G).cuda()
-
-
 def trimmed_mean(users_grads, users_count, corrupted_count):
     if _is_torch_cuda(users_grads):
         from . import _device as dev
@@ -208,8 +213,13 @@ def bulyan(users_grads, users_count, corrupted_count, return_selection=False):
         if sel.numel() and int(sel[-1].item()) < 0:      # a failed round marks itself and all later rounds with -1
             raise KeyError(-1)                           # defences.py:66 `distances.pop(-1)`
         return (out, sel) if return_selection else out
-    out, _ = _host_call(DefenseTypes.Bulyan, _as_host_matrix(users_grads), users_count, corrupted_count)
-    return out
+    G = _as_host_matrix(users_grads)
+    n, d = G.shape
+    out = np.empty((d,), np.float32)
+    sel = np.empty((users_count - 2 * corrupted_count,), np.int32)
+    nat.check(nat.lib().afl_bulyan_host(G.ctypes.data, n, d, G.strides[0] // 4, int(users_count), int(corrupted_count),
+                                        out.ctypes.data, sel.ctypes.data, 0))
+    return (out, sel) if return_selection else out
 
 
 defend = {DefenseTypes.Krum: krum,

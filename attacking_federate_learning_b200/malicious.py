@@ -8,17 +8,50 @@ backdoor.py:108-, is model code and out of scope: the caller passes it in).  `us
 objects with `.grads`, `.original_params`, `.learning_rate` exactly as the reference expects; `.grads`
 may be NumPy float32 vectors or torch.cuda vectors.  As in the reference, after `attack()` every
 malicious user holds THE SAME array object; for DriftAttack that object is also `self.grads_mean`
-(mutated in place); `self.grads_stdev` keeps sigma.  All arithmetic runs on the GPU: NumPy inputs are
-copied to the device and the results copied back.
+(mutated in place); `self.grads_stdev` keeps sigma.  All arithmetic runs on the GPU.  With NumPy
+gradients `attack()` streams column slabs of the users' own arrays to the device (`afl_alie_host`, within
+the host-buffer budget of `defences.py`), so no stacked f x D copy exists on the host or the device; the
+statistics come back as NumPy vectors.
 """
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
+
+from . import _native as nat
 
 
 def _is_cuda(x):
     import torch
     return isinstance(x, torch.Tensor) and x.is_cuda
+
+
+def _host_rows(users):
+    """The users' gradients as C-contiguous 1-D float32 arrays; only arrays that are not already so are converted."""
+    rows = []
+    for u in users:
+        g = u.grads
+        if not (isinstance(g, np.ndarray) and g.dtype == np.float32 and g.ndim == 1 and g.flags.c_contiguous):
+            g = np.ascontiguousarray(np.asarray(g, np.float32))
+        if g.ndim != 1:
+            raise ValueError("users' grads must be 1-D vectors")
+        if rows and g.shape != rows[0].shape:
+            raise ValueError("all input arrays must have the same shape")       # what np.stack raises
+        rows.append(g)
+    return rows
+
+
+def _host_alie(users, z, crafted: bool):
+    """(mu, sigma) of the users' NumPy gradients, one afl_alie_host call.  crafted=True: mu is overwritten in place
+    by mu - z*sigma (the reference's aliasing); otherwise z is unused."""
+    rows = _host_rows(users)
+    f, d = len(rows), rows[0].size
+    mu, sigma = np.empty(d, np.float32), np.empty(d, np.float32)
+    ptrs = (C.c_void_p * f)(*[r.ctypes.data for r in rows])
+    nat.check(nat.lib().afl_alie_host(ptrs, f, d, float(z), mu.ctypes.data, sigma.ctypes.data,
+                                      mu.ctypes.data if crafted else None, 0))
+    return mu, sigma
 
 
 def _to_dev(x):
@@ -37,22 +70,15 @@ class Attack(object):
     def attack(self, users):
         if len(users) == 0:
             return
-        import torch
-        from . import _device as dev
-
-        first = users[0].grads
-        on_gpu = _is_cuda(first)
-        if on_gpu:
-            rows = torch.stack([u.grads for u in users])
-        else:
-            rows = torch.from_numpy(np.ascontiguousarray(np.stack([np.asarray(u.grads, np.float32) for u in users]))).cuda()
         fused = self.num_std != 0 and self._fused_drift()
         # malicious.py:17-18 (mu, sigma); with the fused DriftAttack also malicious.py:35 in the same pass
-        crafted, mu, sigma = dev.alie(rows, self.num_std if fused else 0.0, None, alias_mean=fused)
-        if on_gpu:
-            self.grads_mean, self.grads_stdev = mu, sigma
+        if _is_cuda(users[0].grads):
+            import torch
+            from . import _device as dev
+            rows = torch.stack([u.grads for u in users])
+            _, self.grads_mean, self.grads_stdev = dev.alie(rows, self.num_std if fused else 0.0, None, alias_mean=fused)
         else:
-            self.grads_mean, self.grads_stdev = mu.cpu().numpy(), sigma.cpu().numpy()
+            self.grads_mean, self.grads_stdev = _host_alie(users, self.num_std if fused else 0.0, fused)
         if self.num_std == 0:                               # malicious.py:20-21: statistics only
             return
         if fused:

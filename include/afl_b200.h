@@ -193,6 +193,32 @@ int afl_defend_host(const char* rule, const float* G_host, int n, int64_t d, int
                     int users_count, int corrupted_count, float* out_host, int* idx_out,
                     int64_t slab_cols);
 
+/* The rest of the host-buffer surface.  Each call is blocking, runs on the current device, streams
+ * column slabs within afl_defend_host's budget (same AFL_ERR_UNSUPPORTED "needs N bytes" error) and
+ * rounds `slab_cols` the same way; results depend only on the input and slab_cols.
+ *
+ * afl_sqdist_host — defences.py:16-21  _krum_create_distances.  Writes the n x n float64 squared-
+ * distance table of the host matrix into d2_out (device float64[n*n], caller-owned), summed slab by
+ * slab in slab order: the table afl_defend_host("Krum", ...) builds from the same arguments, bit for
+ * bit.  No client limit: past 4096 clients every slab runs the SIMT kernel (afl_sqdist_partial). */
+int afl_sqdist_host(const float* G_host, int n, int64_t d, int64_t ld, double* d2_out, int64_t slab_cols);
+
+/* afl_bulyan_host — defences.py:55-70  bulyan.  afl_defend_host("Bulyan", ...) is this call with
+ * sel_host = NULL.  sel_host (host int[users_count - 2*corrupted_count], may be NULL) receives the
+ * selection in selection order, also on AFL_ERR_NO_WINNER, where the failed rounds hold -1.
+ * AFL_ERR_PRECONDITION unless users_count >= 4f+3; n <= 4096 clients. */
+int afl_bulyan_host(const float* G_host, int n, int64_t d, int64_t ld, int users_count, int corrupted_count,
+                    float* out_host, int* sel_host, int64_t slab_cols);
+
+/* afl_alie_host — malicious.py:14-19,35  Attack.attack + DriftAttack._attack_grads on host gradients.
+ * rows: f separate host vectors of d fp32 (the users' own arrays; no stacked matrix is needed).  Each
+ * slab packs the f row segments into a device slot and runs afl_alie on it.  mu_out, sigma_out,
+ * crafted_out: host fp32[d], each may be NULL, with afl_alie's contract (bcast_rows = NULL):
+ * crafted_out == mu_out reproduces the reference's in-place aliasing.  The column sums run down the
+ * rows in float64, so the outputs equal one afl_alie over the stacked matrix, bit for bit. */
+int afl_alie_host(const float* const* rows, int f, int64_t d, double z, float* mu_out, float* sigma_out,
+                  float* crafted_out, int64_t slab_cols);
+
 #ifdef __cplusplus
 }
 #endif

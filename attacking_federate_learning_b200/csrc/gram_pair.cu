@@ -16,7 +16,8 @@
 //                    With one tile (N <= 128) every pair is on the diagonal tile, so the converters write 2 b2 (exact)
 //                    and two products suffice: M += b1 b1^T + b1 (2 b2)^T, and S = (M + M^T) / 2, formed in float64
 //                    from the split sums (pair_reduce_kernel keeps both triangles, pair_to_sqdist_kernel adds them).
-//                    Its boxes have N rounded up to 8 rows; rows past them stay zero from the kernel's start.
+//                    Its boxes have N rounded up to 8 rows (kSymN); rows past them stay zero from the kernel's start,
+//                    and its MMAs are m64nNk16 with N = kSymN, so no tensor work is spent on columns past the box.
 //       kModeTf32x2  fp32 clients, 32-column k-blocks delivered by TMA already swizzled (SWIZZLE_128B).  The
 //                    converter truncates the box in place to hi = the top 10 mantissa bits and writes lo = g - hi
 //                    at the same offsets 16 KB further; per 8 columns S += hi hi^T + hi lo^T + lo hi^T (dropped:
@@ -70,12 +71,62 @@ __device__ __forceinline__ void sts64_p(uint32_t addr, uint32_t a, uint32_t b) {
 }
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
-// kSym: kModeBf16x2 with one tile, the symmetric two-product form on boxes of p.box_rows <= 128 rows (a template
-// parameter: a runtime branch between the two MMA sequences makes ptxas fence every k-block's wgmma issue)
-template <int kMode, bool kSym>
+// wgmma.m64nNk16 (bf16 operands from shared memory, fp32 accumulate) for N = 56, 64, ..., 112: thread t of the
+// warpgroup holds N / 2 accumulators.  The asm operand lists are built by macros; IA, IB, IK are the operand numbers
+// of the two descriptors and `keep`, which follow the N / 2 accumulators.
+#define AFL_R28 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, " \
+                "%22, %23, %24, %25, %26, %27"
+#define AFL_R32 AFL_R28 ", %28, %29, %30, %31"
+#define AFL_R36 AFL_R32 ", %32, %33, %34, %35"
+#define AFL_R40 AFL_R36 ", %36, %37, %38, %39"
+#define AFL_R44 AFL_R40 ", %40, %41, %42, %43"
+#define AFL_R48 AFL_R44 ", %44, %45, %46, %47"
+#define AFL_R52 AFL_R48 ", %48, %49, %50, %51"
+#define AFL_R56 AFL_R52 ", %52, %53, %54, %55"
+#define AFL_F4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define AFL_C28 AFL_F4(0), AFL_F4(4), AFL_F4(8), AFL_F4(12), AFL_F4(16), AFL_F4(20), AFL_F4(24)
+#define AFL_C32 AFL_C28, AFL_F4(28)
+#define AFL_C36 AFL_C32, AFL_F4(32)
+#define AFL_C40 AFL_C36, AFL_F4(36)
+#define AFL_C44 AFL_C40, AFL_F4(40)
+#define AFL_C48 AFL_C44, AFL_F4(44)
+#define AFL_C52 AFL_C48, AFL_F4(48)
+#define AFL_C56 AFL_C52, AFL_F4(52)
+#define AFL_WGMMA_BF16_N(N, K, IA, IB, IK)                                                                          \
+  __device__ __forceinline__ void wgmma_m64nNk16_bf16(float (&d)[K], uint64_t a_desc, uint64_t b_desc, uint32_t keep) { \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #IK ", 0;\n\t"                                               \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 {" AFL_R##K "}, %" #IA ", %" #IB             \
+                 ", p, 1, 1, 0, 0;\n\t}\n"                                                                            \
+                 : AFL_C##K : "l"(a_desc), "l"(b_desc), "r"(keep));                                                   \
+  }
+AFL_WGMMA_BF16_N(56, 28, 28, 29, 30)
+AFL_WGMMA_BF16_N(64, 32, 32, 33, 34)
+AFL_WGMMA_BF16_N(72, 36, 36, 37, 38)
+AFL_WGMMA_BF16_N(80, 40, 40, 41, 42)
+AFL_WGMMA_BF16_N(88, 44, 44, 45, 46)
+AFL_WGMMA_BF16_N(96, 48, 48, 49, 50)
+AFL_WGMMA_BF16_N(104, 52, 52, 53, 54)
+AFL_WGMMA_BF16_N(112, 56, 56, 57, 58)
+#undef AFL_WGMMA_BF16_N
+#undef AFL_F4
+
+// keeps the compiler from touching accumulator registers across a wgmma_wait
+template <int K>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[K]) {
+#pragma unroll
+  for (int i = 0; i < K; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// kSymN > 0: kModeBf16x2 with one tile, the symmetric two-product form on boxes of kSymN = p.box_rows rows (N rounded
+// up to 8, 56..112), with wgmma.m64nNk16 for N = kSymN: no tensor work on columns past the box.  (A template
+// parameter: a runtime branch between the two MMA sequences makes ptxas fence every k-block's wgmma issue.)
+template <int kMode, int kSymN>
 __global__ void __launch_bounds__(kPThreads, 1)
 gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
-  static_assert(!kSym || kMode == kModeBf16x2, "the symmetric form is a bf16x2 form");
+  constexpr bool kSym = kSymN != 0;
+  static_assert(!kSym || (kMode == kModeBf16x2 && kSymN % 8 == 0 && kSymN >= 56 && kSymN <= 112),
+                "the symmetric form is a bf16x2 form on 8-row units, and warpgroup 2's rows 64.. must exist");
+  constexpr int kAcc = kSym ? kSymN / 2 : 64;               // accumulators per thread (m64nN: N / 2)
   constexpr uint32_t kBoxBytes = kMode == kModeBf16x2 ? kPSlotBytes : kPSlotBytes / 2;
   constexpr int kCols = kMode == kModeTf32x2 ? 32 : kPCols;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -233,9 +284,9 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
     // ===================== MMA: warpgroup c owns rows 64c .. 64c+63 of the I tile =====================
     const int c = wg - 1;
     const int wq = warp & 3;
-    float acc[64], run[64];
+    float acc[kAcc], run[kAcc];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) { acc[i] = 0.f; run[i] = 0.f; }
+    for (int i = 0; i < kAcc; ++i) { acc[i] = 0.f; run[i] = 0.f; }
     // operand layout: kModeBf16x2 alternates 1 KB b1 / b2 atoms (8-row groups 2 KB apart); the other two modes are
     // plain SWIZZLE_128B tiles (8-row groups 1 KB apart), kModeTf32x2 with lo one box further
     constexpr uint32_t kSbo = kMode == kModeBf16x2 ? 2048u : 1024u;
@@ -262,7 +313,13 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
         const uint64_t d_1j = wgmma_desc_sw128(s_j, kSbo), d_2j = wgmma_desc_sw128(s_j + kSecond, kSbo);
         wgmma_fence();
         const uint32_t first = it != it_begin;            // 0: this chain's first MMA overwrites the accumulator
-        if (kMode == kModeTf32x2 && p.single_pass) {
+        if constexpr (kSym) {
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            wgmma_m64nNk16_bf16(acc, d_1i + 2 * ks, d_1j + 2 * ks, first | ks);    // b1 b1^T
+            wgmma_m64nNk16_bf16(acc, d_1i + 2 * ks, d_2j + 2 * ks, 1u);            // b1 (2 b2)^T
+          }
+        } else if (kMode == kModeTf32x2 && p.single_pass) {
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks)                    // 4 x 32 bytes = one 128-byte swizzle row of K
             wgmma_m64n128k8_tf32(acc, d_1i + 2 * ks, d_1j + 2 * ks, first | ks);   // hi_I hi_J^T
@@ -272,12 +329,6 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
             wgmma_m64n128k8_tf32(acc, d_1i + 2 * ks, d_1j + 2 * ks, first | ks);   // hi_I hi_J^T
             wgmma_m64n128k8_tf32(acc, d_1i + 2 * ks, d_2j + 2 * ks, 1u);           // hi_I lo_J^T
             wgmma_m64n128k8_tf32(acc, d_2i + 2 * ks, d_1j + 2 * ks, 1u);           // lo_I hi_J^T
-          }
-        } else if (kSym) {
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            wgmma_m64n128k16_bf16(acc, d_1i + 2 * ks, d_1j + 2 * ks, first | ks);  // b1 b1^T
-            wgmma_m64n128k16_bf16(acc, d_1i + 2 * ks, d_2j + 2 * ks, 1u);          // b1 (2 b2)^T
           }
         } else {
 #pragma unroll
@@ -297,16 +348,16 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
       }
       wgmma_wait<0>();
       release(it_end - 1);
-      wgmma_fence_operands(acc);
+      wgmma_fence_acc(acc);
 #pragma unroll
-      for (int i = 0; i < 64; ++i) run[i] += acc[i];
+      for (int i = 0; i < kAcc; ++i) run[i] += acc[i];
     }
     // accumulator fragment of m64nN: element i of thread (warp wq, lane) is row 16 wq + lane/4 + 8 ((i/2) % 2),
-    // column 8 (i/4) + 2 (lane % 4) + i % 2
+    // column 8 (i/4) + 2 (lane % 4) + i % 2; kSym writes columns 0..kSymN-1 only
     float* out = p.parts + (static_cast<size_t>(pair) * p.splits + split) * kPPartElems +
                  static_cast<size_t>(64 * c + 16 * wq + (lane >> 2)) * 128 + 2 * (lane & 3);
 #pragma unroll
-    for (int i = 0; i < 64; i += 2)
+    for (int i = 0; i < kAcc; i += 2)
       *reinterpret_cast<float2*>(out + ((i >> 1) & 1) * 8 * 128 + (i >> 2) * 8) = make_float2(run[i], run[i + 1]);
   }
 }
@@ -400,17 +451,33 @@ size_t pair_parts_bytes(int n, int64_t d) {
   return static_cast<size_t>(pairs) * pair_splits(n, d) * kPPartElems * sizeof(float);
 }
 
-template <int kMode, bool kSym>
+template <int kMode, int kSymN>
 static int launch_mode(const CUtensorMap& tmap, const PairParams& p, cudaStream_t stream) {
   const size_t smem = static_cast<size_t>(kPSlots) * kPSlotBytes + 1024;
   static int smem_attr_done[kMaxDevices] = {0};
-  AFL_CUDA(ensure_dyn_smem(gram_pair_kernel<kMode, kSym>, static_cast<int>(smem), smem_attr_done));
+  AFL_CUDA(ensure_dyn_smem(gram_pair_kernel<kMode, kSymN>, static_cast<int>(smem), smem_attr_done));
   {
     ProfScope ps("gram_pair", stream);
-    gram_pair_kernel<kMode, kSym><<<p.pairs * p.splits, kPThreads, smem, stream>>>(tmap, p);
+    gram_pair_kernel<kMode, kSymN><<<p.pairs * p.splits, kPThreads, smem, stream>>>(tmap, p);
   }
   AFL_LAUNCH_CHECK("gram_pair_kernel");
   return AFL_OK;
+}
+
+// the one-tile symmetric form: one instance per box height (gram.cu:make_plan runs it for 49 <= N <= 112)
+static int launch_sym(const CUtensorMap& tmap, const PairParams& p, cudaStream_t stream) {
+  switch (p.box_rows) {
+    case 56: return launch_mode<kModeBf16x2, 56>(tmap, p, stream);
+    case 64: return launch_mode<kModeBf16x2, 64>(tmap, p, stream);
+    case 72: return launch_mode<kModeBf16x2, 72>(tmap, p, stream);
+    case 80: return launch_mode<kModeBf16x2, 80>(tmap, p, stream);
+    case 88: return launch_mode<kModeBf16x2, 88>(tmap, p, stream);
+    case 96: return launch_mode<kModeBf16x2, 96>(tmap, p, stream);
+    case 104: return launch_mode<kModeBf16x2, 104>(tmap, p, stream);
+    case 112: return launch_mode<kModeBf16x2, 112>(tmap, p, stream);
+  }
+  set_error("gram_pair_kernel: no one-tile bf16x2 instance for %d clients (49..112)", p.n);
+  return AFL_ERR_UNSUPPORTED;
 }
 
 // G: fp32 [n, d] (pitch multiple of 4 elements) or bf16 (kModeBf16In, pitch multiple of 8), 16-byte aligned.
@@ -430,7 +497,7 @@ int launch_pair(const void* Gv, int mode, int n, int64_t d, int64_t ld, float* p
   const int cols = mode == kModeTf32x2 ? 32 : kPCols;
   PairParams p{};
   p.n = n; p.tiles = (n + 127) / 128; p.pairs = p.tiles * (p.tiles + 1) / 2;
-  const int sym = mode == kModeBf16x2 && p.tiles == 1;     // the kernel's kSym
+  const int sym = mode == kModeBf16x2 && p.tiles == 1;     // the kernel's kSymN > 0
   p.box_rows = sym ? (n + 7) / 8 * 8 : 128;
   p.splits = pair_splits(n, d);
   p.kblocks = static_cast<int>((d + cols - 1) / cols);
@@ -460,10 +527,10 @@ int launch_pair(const void* Gv, int mode, int n, int64_t d, int64_t ld, float* p
                    mode == kModeBf16x2 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed: %d", static_cast<int>(r)); return AFL_ERR_CUDA; }
-  int rc = sym                   ? launch_mode<kModeBf16x2, true>(tmap, p, stream)
-         : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, false>(tmap, p, stream)
-         : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, false>(tmap, p, stream)
-                               : launch_mode<kModeBf16In, false>(tmap, p, stream);
+  int rc = sym                   ? launch_sym(tmap, p, stream)
+         : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, 0>(tmap, p, stream)
+         : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, 0>(tmap, p, stream)
+                               : launch_mode<kModeBf16In, 0>(tmap, p, stream);
   if (rc) return rc;
   pair_reduce_kernel<<<dim3(n, p.tiles), dim3(128, kPSy), 0, stream>>>(parts, n, p.splits, sym, S);
   AFL_LAUNCH_CHECK("pair_reduce_kernel");

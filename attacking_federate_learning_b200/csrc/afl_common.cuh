@@ -212,14 +212,14 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
-// 2-D tiled load, completes `bytes` on the mbarrier.  c0 = innermost (column) coord, c1 = row coord.
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0,
-                                            int c1, uint64_t cache_policy) {
+// 3-D tiled load, completes `bytes` on the mbarrier.  c0 = innermost (column) coord, c1 = row coord, c2 = problem.
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0,
+                                            int c1, int c2, uint64_t cache_policy) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
+      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "l"(cache_policy)
+        "r"(c2), "l"(cache_policy)
       : "memory");
 }
 __device__ __forceinline__ uint64_t policy_evict_normal() {

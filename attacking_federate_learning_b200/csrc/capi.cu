@@ -93,28 +93,40 @@ int sm_count() {
 
 namespace gram {
 size_t workspace_bytes(int n, int64_t d, int dtype, int flags);
+size_t workspace_bytes(int n, int64_t d, int dtype, int flags, int batch);
 int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, double* d2_out, void* ws, size_t ws_bytes,
                    int flags, cudaStream_t stream);
-int sqdist_to_dist(const double* d2, int n, float* dist, cudaStream_t stream);
+int sqdist_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, double* d2_out,
+                   void* ws, size_t ws_bytes, int flags, cudaStream_t stream);
+int sqdist_to_dist(const double* d2, int n, float* dist, cudaStream_t stream, int batch = 1);
 }
 namespace select {
 int max_clients();
 size_t workspace_bytes(int n);
+size_t workspace_bytes(int n, int batch);
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
                 void* ws, size_t ws_bytes, cudaStream_t stream);
 int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
-                     size_t ws_bytes, cudaStream_t stream);
+                     size_t ws_bytes, cudaStream_t stream, int batch = 1);
 int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out, void* ws, size_t ws_bytes,
-                  cudaStream_t stream);
+                  cudaStream_t stream, int batch = 1);
 }
 namespace tmean {
 int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
                  int corrupted_count, float* out, cudaStream_t stream);
+int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
+                         int corrupted_count, float* out, int batch, int64_t g_batch, int ri_batch, int64_t out_batch,
+                         cudaStream_t stream);
 }
 namespace colstats {
 int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream);
+int mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, int batch, int64_t g_batch,
+                 int64_t out_batch, cudaStream_t stream);
 int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
          float* crafted_out, float* bcast, int64_t bcast_ld, cudaStream_t stream);
+int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
+                 float* crafted_out, float* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
+                 int64_t bcast_batch, cudaStream_t stream);
 int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* idx_dev, float* out,
                cudaStream_t stream);
 int momentum_step(float* w, float* v, const float* g, int64_t d, float momentum, float lr, cudaStream_t stream);
@@ -547,6 +559,99 @@ static int alie_host(const float* const* rows, int f, int64_t d, double z, float
   return AFL_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Batched device calls: `batch` same-shape problems of n <= 128 clients, problem b at G + b * batch_stride, each
+// computed by the same kernels as one problem (the batch is a grid dimension), so every problem's result is the
+// single call's.  Scratch per rule (the tables first, so that a caller can read them after the call):
+//   Krum   [d2: batch x n x n float64][gram workspace][selection workspace]
+//   Bulyan [d2: batch x n x n float64][dist: batch x n x n fp32][gram workspace][selection workspace]
+// ------------------------------------------------------------------------------------------------
+constexpr int kBatchMaxClients = 128;            // one Gram tile
+constexpr int kBatchMax = 65535;                 // grid y / z limit
+
+enum BatchedRule { B_BAD, B_MEAN, B_KRUM, B_TM, B_BULYAN };
+static BatchedRule batched_rule(const char* rule) {
+  if (!rule) return B_BAD;
+  if (!strcmp(rule, "NoDefense")) return B_MEAN;
+  if (!strcmp(rule, "Krum")) return B_KRUM;
+  if (!strcmp(rule, "TrimmedMean")) return B_TM;
+  if (!strcmp(rule, "Bulyan")) return B_BULYAN;
+  return B_BAD;
+}
+
+// Shape checks shared by afl_defend_batched and afl_alie_batched, before any CUDA call.
+static int check_batch(const char* who, const void* G, int batch, int64_t batch_stride, int rows, int64_t d, int64_t ld,
+                       int dtype) {
+  if (!G || rows < 1 || d < 1 || ld < d) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
+  if (batch < 1) { set_error("%s: batch must be >= 1 (got %d)", who, batch); return AFL_ERR_BAD_ARG; }
+  if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
+  if (rows > kBatchMaxClients) {
+    set_error("%s: batched problems support n <= %d clients (got %d)", who, kBatchMaxClients, rows);
+    return AFL_ERR_UNSUPPORTED;
+  }
+  if (batch > 1 && batch_stride < static_cast<int64_t>(rows - 1) * ld + d) {
+    set_error("%s: batch_stride %lld is negative or makes problems overlap (a problem spans %lld elements)", who,
+              static_cast<long long>(batch_stride), static_cast<long long>(static_cast<int64_t>(rows - 1) * ld + d));
+    return AFL_ERR_BAD_ARG;
+  }
+  if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("%s: dtype", who); return AFL_ERR_UNSUPPORTED; }
+  return AFL_OK;
+}
+
+static size_t batched_ws_parts(BatchedRule r, int batch, int n, int64_t d, int dtype, size_t* gram_ws, size_t* tabs) {
+  const size_t nn = static_cast<size_t>(batch) * n * n;
+  *gram_ws = align_up(gram::workspace_bytes(n, d, dtype, 0, batch), 256);
+  *tabs = align_up(nn * 8, 256) + (r == B_BULYAN ? align_up(nn * 4, 256) : 0);
+  return *gram_ws + *tabs + select::workspace_bytes(n, batch);
+}
+
+static int defend_batched(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                          int dtype, int users_count, int f, float* out, int* idx_out, int* sel_out, void* ws,
+                          size_t ws_bytes, cudaStream_t stream) {
+  const BatchedRule r = batched_rule(rule);
+  if (r == B_BAD) { set_error("afl_defend_batched: unknown rule '%s'", rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
+  int rc = check_batch("afl_defend_batched", G, batch, batch_stride, n, d, ld, dtype);
+  if (rc) return rc;
+  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out) || f < 0) {
+    set_error("afl_defend_batched: %s needs %s", rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
+    return AFL_ERR_BAD_ARG;
+  }
+  if (r == B_KRUM && users_count < 2 * f + 1) {         // the reference's assert (defences.py:24-25)
+    set_error("krum: users_count >= 2*corrupted_count + 1 violated (%d, %d)", users_count, f);
+    return AFL_ERR_PRECONDITION;
+  }
+  if (r == B_BULYAN && users_count < 4 * f + 3) {       // the reference's assert (defences.py:56)
+    set_error("bulyan: users_count >= 4*corrupted_count + 3 violated (%d, %d)", users_count, f);
+    return AFL_ERR_PRECONDITION;
+  }
+  if (r == B_BULYAN && users_count != n) {
+    set_error("afl_defend_batched: Bulyan's users_count (%d) must equal the number of rows (%d)", users_count, n);
+    return AFL_ERR_UNSUPPORTED;
+  }
+  if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream);
+  if (r == B_TM)
+    return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, f, out, batch, batch_stride, 0, d, stream);
+  size_t gram_ws = 0, tabs = 0;
+  const size_t need = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
+    set_error("afl_defend_batched: workspace too small or misaligned (%zu < %zu)", ws_bytes, need);
+    return AFL_ERR_WORKSPACE;
+  }
+  uint8_t* p = static_cast<uint8_t*>(ws);
+  const size_t nn = static_cast<size_t>(batch) * n * n;
+  double* d2 = reinterpret_cast<double*>(p);
+  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
+  void* sel_ws = p + tabs + gram_ws;
+  const size_t sel_ws_bytes = ws_bytes - tabs - gram_ws;
+  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream);
+  if (rc) return rc;
+  if (r == B_KRUM) return select::krum_from_sqdist(d2, n, users_count, f, idx_out, sel_ws, sel_ws_bytes, stream, batch);
+  const int theta = users_count - 2 * f;
+  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
+  rc = select::bulyan_select(dist, n, users_count, f, sel_out, sel_ws, sel_ws_bytes, stream, batch); if (rc) return rc;
+  return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, theta, 2 * f, out, batch, batch_stride, theta, d, stream);
+}
+
 }  // namespace afl
 
 using namespace afl;
@@ -658,6 +763,34 @@ int afl_bulyan_host(const float* G_host, int n, int64_t d, int64_t ld, int users
 int afl_alie_host(const float* const* rows, int f, int64_t d, double z, float* mu_out, float* sigma_out,
                   float* crafted_out, int64_t slab_cols) {
   return alie_host(rows, f, d, z, mu_out, sigma_out, crafted_out, slab_cols);
+}
+
+size_t afl_batched_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
+  const BatchedRule r = batched_rule(rule);
+  if (r == B_BAD || batch < 1 || batch > kBatchMax || n < 1 || n > kBatchMaxClients || d < 1) return 0;
+  if (r == B_MEAN || r == B_TM) return 256;
+  size_t gram_ws = 0, tabs = 0;
+  return batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+}
+
+int afl_defend_batched(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                       int dtype, int users_count, int corrupted_count, float* out, int* idx_out, int* sel_out,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+  return defend_batched(rule, G, batch, batch_stride, n, d, ld, dtype, users_count, corrupted_count, out, idx_out, sel_out,
+                        workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int afl_alie_batched(const void* G_mal, int batch, int64_t batch_stride, int f, int64_t d, int64_t ld, int dtype, double z,
+                     float* mu_out, float* sigma_out, float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride,
+                     int64_t bcast_ld, void* stream) {
+  int rc = check_batch("afl_alie_batched", G_mal, batch, batch_stride, f, d, ld, dtype);
+  if (rc) return rc;
+  if (bcast_rows && (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(f - 1) * bcast_ld + d))) {
+    set_error("afl_alie_batched: bcast_ld / bcast_batch_stride make the written rows overlap");
+    return AFL_ERR_BAD_ARG;
+  }
+  return colstats::alie_batched(G_mal, f, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast_rows, bcast_ld, batch,
+                                batch_stride, d, bcast_batch_stride, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
 // HBM-bound column kernels: plain mean (defences.py:13-14), the ALIE mu/sigma/perturb reduction
 // (malicious.py:18-19,35), Krum's row gather, and the server momentum step (server.py:89-90).
 // All of them stream the row-major [n, d] matrix once with 16-byte loads; a thread owns VEC adjacent
-// columns and walks down the rows, so every warp-level load is one contiguous segment of a row.
+// columns and walks down the rows, so every warp-level load is one contiguous segment of a row.  mean and
+// alie take a batch of same-shape problems in grid y (input at b * g_batch, outputs at b * out_batch).
 #include "afl_common.cuh"
 
 namespace afl {
@@ -74,9 +75,12 @@ __device__ __forceinline__ Pack<VEC> load_rows(const T* p) {
 // np.mean(axis=0) on a C-contiguous array, so fp32 results are bit-identical to the reference.
 template <typename T, int VEC>
 __global__ void __launch_bounds__(kBlock)
-mean_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, float* __restrict__ out) {
+mean_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, float* __restrict__ out, int64_t g_batch,
+            int64_t out_batch) {
   const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * VEC;
   if (c0 >= d) return;
+  G += blockIdx.y * g_batch;
+  out += blockIdx.y * out_batch;
   float acc[VEC];
 #pragma unroll
   for (int k = 0; k < VEC; ++k) acc[k] = 0.f;
@@ -110,9 +114,11 @@ mean_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, float* __rest
 template <typename T, int VEC, bool COHERENT>
 __global__ void __launch_bounds__(kBlock)
 alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict__ mu_out,
-            float* __restrict__ sigma_out, float* __restrict__ crafted_out, float* bcast, int64_t bcast_ld) {
+            float* __restrict__ sigma_out, float* __restrict__ crafted_out, float* bcast, int64_t bcast_ld,
+            int64_t g_batch, int64_t out_batch, int64_t bcast_batch) {
   const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * VEC;
   if (c0 >= d) return;
+  G += blockIdx.y * g_batch;
   const T* p = G + c0;
   double s1[VEC], s2[VEC];
 #pragma unroll
@@ -141,6 +147,7 @@ alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict
     }
   }
   const double inv = 1.0 / static_cast<double>(f);
+  const int64_t o = blockIdx.y * out_batch + c0;         // this thread's first output element
   float crafted[VEC];
 #pragma unroll
   for (int k = 0; k < VEC; ++k) {
@@ -151,12 +158,13 @@ alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict
     const float sigma = static_cast<float>(sqrt(var));
     crafted[k] = __fsub_rn(mu, __fmul_rn(z, sigma));
     if (c0 + k < d) {
-      if (sigma_out) sigma_out[c0 + k] = sigma;
-      if (mu_out && mu_out != crafted_out) mu_out[c0 + k] = mu;
-      if (crafted_out) crafted_out[c0 + k] = crafted[k];
+      if (sigma_out) sigma_out[o + k] = sigma;
+      if (mu_out && mu_out != crafted_out) mu_out[o + k] = mu;
+      if (crafted_out) crafted_out[o + k] = crafted[k];
     }
   }
   if (bcast) {
+    bcast += blockIdx.y * bcast_batch;
     // server.py:82-83 copies the one aliased array into every malicious row: f row segments of VEC floats,
     // written as 16-byte stores when the destination allows it (all of this thread's reads are done)
     const bool v16 = (VEC % 4 == 0) && (c0 + VEC <= d) && (bcast_ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(bcast) & 15) == 0);
@@ -218,44 +226,55 @@ band_kernel(const float* mu, const float* sigma, float z, const float* x, float*
   }
 }
 
-static bool vec_ok(const void* G, int64_t ld, int dtype) {
+// 16-byte loads need an aligned base, pitch and (batch > 1) batch pitch
+static bool vec_ok(const void* G, int64_t ld, int dtype, int batch, int64_t g_batch) {
   const int64_t es = dtype == AFL_F32 ? 4 : 2;
-  return (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0);
+  return (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0) && (batch == 1 || (g_batch * es) % 16 == 0);
 }
 
-int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream) {
+int mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, int batch, int64_t g_batch,
+                 int64_t out_batch, cudaStream_t stream) {
   if (!G || !out || n < 1 || d < 1 || ld < d) { set_error("afl_mean: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
-  const bool v = vec_ok(G, ld, dtype);
+  const bool v = vec_ok(G, ld, dtype, batch, g_batch);
   const int vec = v ? (dtype == AFL_F32 ? 4 : 8) : 1;
-  const unsigned grid = static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock));
+  const dim3 grid(static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock)), batch);
   ProfScope ps("mean", stream);
+#define AFL_MEAN_LAUNCH(T, V) mean_kernel<T, V><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, out, g_batch, out_batch)
   if (dtype == AFL_F32) {
-    if (v) mean_kernel<float, 4><<<grid, kBlock, 0, stream>>>(static_cast<const float*>(G), n, d, ld, out);
-    else mean_kernel<float, 1><<<grid, kBlock, 0, stream>>>(static_cast<const float*>(G), n, d, ld, out);
+    if (v) AFL_MEAN_LAUNCH(float, 4);
+    else AFL_MEAN_LAUNCH(float, 1);
   } else {
-    if (v) mean_kernel<__nv_bfloat16, 8><<<grid, kBlock, 0, stream>>>(static_cast<const __nv_bfloat16*>(G), n, d, ld, out);
-    else mean_kernel<__nv_bfloat16, 1><<<grid, kBlock, 0, stream>>>(static_cast<const __nv_bfloat16*>(G), n, d, ld, out);
+    if (v) AFL_MEAN_LAUNCH(__nv_bfloat16, 8);
+    else AFL_MEAN_LAUNCH(__nv_bfloat16, 1);
   }
+#undef AFL_MEAN_LAUNCH
   AFL_LAUNCH_CHECK("mean_kernel");
   return AFL_OK;
 }
 
-int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
-         float* crafted_out, float* bcast, int64_t bcast_ld, cudaStream_t stream) {
+int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream) {
+  return mean_batched(G, n, d, ld, dtype, out, 1, 0, 0, stream);
+}
+
+// `batch` problems: G + b * g_batch; mu/sigma/crafted + b * out_batch; bcast + b * bcast_batch
+int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
+                 float* crafted_out, float* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
+                 int64_t bcast_batch, cudaStream_t stream) {
   if (!G || f < 1 || d < 1 || ld < d || (bcast && bcast_ld < d)) { set_error("afl_alie: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_alie: dtype"); return AFL_ERR_UNSUPPORTED; }
-  const bool v = vec_ok(G, ld, dtype);
+  const bool v = vec_ok(G, ld, dtype, batch, g_batch);
   const int vec = v ? (dtype == AFL_F32 ? 4 : 8) : 1;
-  const unsigned grid = static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock));
+  const dim3 grid(static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock)), batch);
   const float zf = static_cast<float>(z);
   ProfScope ps("alie", stream);
   // the reference writes the crafted vector back over the malicious rows (main.py:68 -> server.py:82-83): when the
-  // broadcast target overlaps the input, read it coherently (no ld.global.nc on memory this launch writes)
-  const uintptr_t g0 = reinterpret_cast<uintptr_t>(G), g1 = g0 + static_cast<uintptr_t>((static_cast<int64_t>(f - 1) * ld + d) * (dtype == AFL_F32 ? 4 : 2));
-  const uintptr_t b0 = reinterpret_cast<uintptr_t>(bcast), b1 = b0 + static_cast<uintptr_t>((static_cast<int64_t>(f - 1) * bcast_ld + d) * 4);
+  // broadcast target overlaps the input (any problem's), read it coherently (no ld.global.nc on memory this launch writes)
+  const int64_t last = static_cast<int64_t>(batch - 1);
+  const uintptr_t g0 = reinterpret_cast<uintptr_t>(G), g1 = g0 + static_cast<uintptr_t>((last * g_batch + static_cast<int64_t>(f - 1) * ld + d) * (dtype == AFL_F32 ? 4 : 2));
+  const uintptr_t b0 = reinterpret_cast<uintptr_t>(bcast), b1 = b0 + static_cast<uintptr_t>((last * bcast_batch + static_cast<int64_t>(f - 1) * bcast_ld + d) * 4);
   const bool coh = bcast && b0 < g1 && g0 < b1;
-#define AFL_ALIE_LAUNCH(T, V, C) alie_kernel<T, V, C><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), f, d, ld, zf, mu_out, sigma_out, crafted_out, bcast, bcast_ld)
+#define AFL_ALIE_LAUNCH(T, V, C) alie_kernel<T, V, C><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), f, d, ld, zf, mu_out, sigma_out, crafted_out, bcast, bcast_ld, g_batch, out_batch, bcast_batch)
   if (dtype == AFL_F32) {
     if (v) { if (coh) AFL_ALIE_LAUNCH(float, 4, true); else AFL_ALIE_LAUNCH(float, 4, false); }
     else { if (coh) AFL_ALIE_LAUNCH(float, 1, true); else AFL_ALIE_LAUNCH(float, 1, false); }
@@ -266,6 +285,11 @@ int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float
 #undef AFL_ALIE_LAUNCH
   AFL_LAUNCH_CHECK("alie_kernel");
   return AFL_OK;
+}
+
+int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
+         float* crafted_out, float* bcast, int64_t bcast_ld, cudaStream_t stream) {
+  return alie_batched(G, f, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast, bcast_ld, 1, 0, 0, 0, stream);
 }
 
 int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* idx_dev, float* out,

@@ -22,14 +22,18 @@ template <> __device__ __forceinline__ float load_elem<__nv_bfloat16>(const __nv
   return __bfloat162float(*p);
 }
 
+// blockIdx.z = problem of a batch (matrix at G + z * batch_stride, partials at part + z * splits * n * n).
 template <typename T>
 __global__ void __launch_bounds__(256)
-sqdist_simt_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, int splits, double* __restrict__ part) {
+sqdist_simt_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, int64_t batch_stride, int splits,
+                   double* __restrict__ part) {
   __shared__ float As[32][33], Bs[32][33];
   const int tiles = (n + 31) / 32;
   const int ti = blockIdx.x / tiles, tj = blockIdx.x % tiles;
   if (tj > ti) return;                                  // lower triangle (incl. diagonal tiles)
   const int split = blockIdx.y;
+  G += blockIdx.z * batch_stride;
+  part += static_cast<size_t>(blockIdx.z) * splits * n * n;
   const int64_t chunks = (d + 31) / 32;
   const int64_t c0 = chunks * split / splits, c1 = chunks * (split + 1) / splits;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -75,6 +79,8 @@ __global__ void sqdist_simt_reduce_kernel(const double* __restrict__ part, int n
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = blockIdx.y;
   if (j >= n) return;
+  part += static_cast<size_t>(blockIdx.z) * splits * n * n;   // problem blockIdx.z
+  d2 += static_cast<size_t>(blockIdx.z) * n * n;
   double v = 0.0;
   if (i != j) {
     const int hi = max(i, j), lo = min(i, j);
@@ -83,21 +89,22 @@ __global__ void sqdist_simt_reduce_kernel(const double* __restrict__ part, int n
   d2[static_cast<size_t>(i) * n + j] = v;
 }
 
-__global__ void sqdist_to_dist_kernel(const double* __restrict__ d2, int n, float* __restrict__ dist) {
+// `total` = batch * n * n: the tables of a batch are consecutive
+__global__ void sqdist_to_dist_kernel(const double* __restrict__ d2, int n, size_t total, float* __restrict__ dist) {
   const size_t e = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (e >= static_cast<size_t>(n) * n) return;
-  const int i = static_cast<int>(e / n), j = static_cast<int>(e % n);
+  if (e >= total) return;
+  const size_t r = e % (static_cast<size_t>(n) * n);
+  const int i = static_cast<int>(r / n), j = static_cast<int>(r % n);
   const double v = d2[e];
   // a negative cancellation residue is 0; NaN (two SIMT rows with the same infinity in one column) stays NaN
   dist[e] = (i == j) ? 0.f : static_cast<float>(sqrt(v > 0.0 ? v : (v == v ? 0.0 : v)));
 }
 
 // tensor-core tile-pair kernel (gram_pair.cu)
-int pair_splits(int n, int64_t d);
-size_t pair_parts_bytes(int n, int64_t d);
+size_t pair_parts_bytes(int n, int64_t d, int batch);
 size_t pair_center_bytes(int64_t d);
-int launch_pair(const void* G, int mode, int n, int64_t d, int64_t ld, float* parts, double* S, float* cvec, double* d2_out,
-                int flush, int center, int single_pass, cudaStream_t stream);
+int launch_pair(const void* G, int mode, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, float* parts,
+                double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -114,18 +121,21 @@ static int env_int(const char* name, int dflt) {
   return (v && *v) ? atoi(v) : dflt;
 }
 
-static bool tensor_eligible(const void* G, int n, int64_t d, int64_t ld, int dtype) {
+// batch > 1 adds the batch pitch to the alignment TMA needs, and a pitch that keeps the problems apart (the 3-D tensor map)
+static bool tensor_eligible(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype) {
   const int64_t per16 = dtype == AFL_F32 ? 4 : 8;           // elements per 16 bytes: TMA needs 16-byte aligned rows
   return (dtype == AFL_F32 || dtype == AFL_BF16) && (ld % per16 == 0) && (reinterpret_cast<uintptr_t>(G) % 16 == 0) && n >= 1 &&
-         d >= 1 && n <= 4096 && d < (int64_t(1) << 31) - 64;
+         d >= 1 && n <= 4096 && d < (int64_t(1) << 31) - 64 &&
+         (batch == 1 || (batch_stride % per16 == 0 && batch_stride >= static_cast<int64_t>(n) * ld));
 }
 
 // fp32 operands default to the centred bf16x2 split for N > 128 and for the streaming shapes (64 <= N_pad <= 112,
 // D >= 32768); elsewhere, and with AFL_GRAM_TF32X2 / AFL_GRAM_SINGLE_PASS, to the split-TF32 operands (smaller
-// uniform bias, no centring).
-static Plan make_plan(const void* G, int n, int64_t d, int64_t ld, int dtype, int flags) {
+// uniform bias, no centring).  A batch chooses like one problem of its shape; its split counts see batch times the
+// CTAs of one problem, and AFL_GRAM_SPLITS overrides both paths' split count.
+static Plan make_plan(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, int flags) {
   Plan pl{};
-  pl.tensor = !(flags & AFL_GRAM_FORCE_SIMT) && tensor_eligible(G, n, d, ld, dtype);
+  pl.tensor = !(flags & AFL_GRAM_FORCE_SIMT) && tensor_eligible(G, batch, batch_stride, n, d, ld, dtype);
   const int sms = sm_count();
   if (pl.tensor) {
     const int nb = (n + 15) & ~15;
@@ -133,34 +143,37 @@ static Plan make_plan(const void* G, int n, int64_t d, int64_t ld, int dtype, in
     if (dtype == AFL_BF16) pl.mode = kModeBf16In;
     else if ((flags & (AFL_GRAM_SINGLE_PASS | AFL_GRAM_TF32X2)) || !(n > 128 || streaming)) pl.mode = kModeTf32x2;
     else pl.mode = kModeBf16x2;
-    pl.parts_bytes = pair_parts_bytes(n, d);
-    pl.s_bytes = align_up(static_cast<size_t>(n) * n * sizeof(double), 256);
+    pl.parts_bytes = pair_parts_bytes(n, d, batch);
+    pl.s_bytes = align_up(static_cast<size_t>(batch) * n * n * sizeof(double), 256);
     pl.total = pl.parts_bytes + pl.s_bytes + pair_center_bytes(d);
   } else {
     const int t32 = (n + 31) / 32;
     int64_t chunks = (d + 31) / 32;
-    int s = (sms * 8) / (t32 * (t32 + 1) / 2); if (s < 1) s = 1;
+    int s = (sms * 8) / (t32 * (t32 + 1) / 2 * batch); if (s < 1) s = 1;
+    if (env_int("AFL_GRAM_SPLITS", 0) > 0) s = env_int("AFL_GRAM_SPLITS", 0);
     if (s > chunks) s = static_cast<int>(chunks);
     if (s > 1024) s = 1024;
     pl.simt_splits = s;
-    pl.total = static_cast<size_t>(s) * n * n * sizeof(double);
+    pl.total = static_cast<size_t>(s) * batch * n * n * sizeof(double);
   }
   pl.total = align_up(pl.total, 256);
   return pl;
 }
 
-size_t workspace_bytes(int n, int64_t d, int dtype, int flags) {
+size_t workspace_bytes(int n, int64_t d, int dtype, int flags, int batch) {
   // Upper bound that holds for either path (the pointer alignment is unknown here).
-  Plan a = make_plan(reinterpret_cast<const void*>(16), n, d, 8, dtype, flags & ~AFL_GRAM_FORCE_SIMT);
-  Plan b = make_plan(reinterpret_cast<const void*>(16), n, d, 8, dtype, flags | AFL_GRAM_FORCE_SIMT);
+  Plan a = make_plan(reinterpret_cast<const void*>(16), batch, static_cast<int64_t>(n) * 8, n, d, 8, dtype, flags & ~AFL_GRAM_FORCE_SIMT);
+  Plan b = make_plan(reinterpret_cast<const void*>(16), batch, static_cast<int64_t>(n) * 8, n, d, 8, dtype, flags | AFL_GRAM_FORCE_SIMT);
   return (a.total > b.total ? a.total : b.total) + 256;
 }
 
-int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, double* d2_out, void* ws, size_t ws_bytes,
-                   int flags, cudaStream_t stream) {
+// `batch` problems of the same shape, problem b at G + b * batch_stride elements; d2_out: batch consecutive n x n tables.
+// One problem is batch = 1 (batch_stride unused).
+int sqdist_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, double* d2_out,
+                   void* ws, size_t ws_bytes, int flags, cudaStream_t stream) {
   if (!G || !d2_out || n < 1 || d < 1 || ld < d) { set_error("afl_sqdist_partial: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_sqdist_partial: dtype"); return AFL_ERR_UNSUPPORTED; }
-  Plan pl = make_plan(G, n, d, ld, dtype, flags);
+  Plan pl = make_plan(G, batch, batch_stride, n, d, ld, dtype, flags);
   if ((flags & AFL_GRAM_FORCE_TCGEN05) && !pl.tensor) {
     set_error("afl_sqdist_partial: tensor-core path needs a 16-byte aligned base, 16-byte aligned pitch, n <= 4096");
     return AFL_ERR_UNSUPPORTED;
@@ -169,26 +182,27 @@ int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, doubl
     set_error("afl_sqdist_partial: workspace too small or misaligned (%zu < %zu)", ws_bytes, pl.total);
     return AFL_ERR_WORKSPACE;
   }
-  const dim3 rblock(128), rgrid((n + 127) / 128, n);
+  const dim3 rblock(128), rgrid((n + 127) / 128, n, batch);
   if (pl.tensor) {
     // translation invariance: bf16x2 operands are converted as g - (mean of the last 8 clients) unless switched off
     const int center = !(flags & AFL_GRAM_NO_CENTER) && env_int("AFL_GRAM_CENTER", 1) != 0;
     float* parts = static_cast<float*>(ws);
     double* S = reinterpret_cast<double*>(static_cast<uint8_t*>(ws) + pl.parts_bytes);
     float* cvec = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + pl.parts_bytes + pl.s_bytes);
-    return launch_pair(G, pl.mode, n, d, ld, parts, S, cvec, d2_out, env_int("AFL_GRAM_FLUSH", 4), center,
-                       (flags & AFL_GRAM_SINGLE_PASS) ? 1 : 0, stream);
+    return launch_pair(G, pl.mode, batch, batch_stride, n, d, ld, parts, S, cvec, d2_out, env_int("AFL_GRAM_FLUSH", 4),
+                       center, (flags & AFL_GRAM_SINGLE_PASS) ? 1 : 0, stream);
   } else {
     const int t32 = (n + 31) / 32;
     double* part = static_cast<double*>(ws);
-    const dim3 grid(t32 * t32, pl.simt_splits);
+    const dim3 grid(t32 * t32, pl.simt_splits, batch);
     {
       ProfScope ps("sqdist_simt", stream);
       if (dtype == AFL_F32)
-        sqdist_simt_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const float*>(G), n, d, ld, pl.simt_splits, part);
+        sqdist_simt_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const float*>(G), n, d, ld, batch_stride,
+                                                            pl.simt_splits, part);
       else
         sqdist_simt_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(G), n, d, ld,
-                                                                     pl.simt_splits, part);
+                                                                     batch_stride, pl.simt_splits, part);
     }
     AFL_LAUNCH_CHECK("sqdist_simt_kernel");
     sqdist_simt_reduce_kernel<<<rgrid, rblock, 0, stream>>>(part, n, pl.simt_splits, d2_out);
@@ -197,10 +211,18 @@ int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, doubl
   return AFL_OK;
 }
 
-int sqdist_to_dist(const double* d2, int n, float* dist, cudaStream_t stream) {
+size_t workspace_bytes(int n, int64_t d, int dtype, int flags) { return workspace_bytes(n, d, dtype, flags, 1); }
+
+int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, double* d2_out, void* ws, size_t ws_bytes,
+                   int flags, cudaStream_t stream) {
+  return sqdist_batched(G, 1, 0, n, d, ld, dtype, d2_out, ws, ws_bytes, flags, stream);
+}
+
+// batch consecutive n x n tables
+int sqdist_to_dist(const double* d2, int n, float* dist, cudaStream_t stream, int batch) {
   if (!d2 || !dist || n < 1) { set_error("afl_sqdist_to_dist: bad argument"); return AFL_ERR_BAD_ARG; }
-  const size_t total = static_cast<size_t>(n) * n;
-  sqdist_to_dist_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(d2, n, dist);
+  const size_t total = static_cast<size_t>(batch) * n * n;
+  sqdist_to_dist_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(d2, n, total, dist);
   AFL_LAUNCH_CHECK("sqdist_to_dist_kernel");
   return AFL_OK;
 }

@@ -3,7 +3,8 @@
 //
 //   * The N x N table is cut into T = ceil(N/128) row tiles; only the T(T+1)/2 pairs (I >= J) are computed.
 //     CTA = (pair, K split); split s owns the k-blocks s, s+S, s+2S, ... and writes its partial S tile to a private
-//     slot, which pair_reduce_kernel sums in a fixed order in float64 (bit-reproducible).
+//     slot, which pair_reduce_kernel sums in a fixed order in float64 (bit-reproducible).  A batch of same-shape one-tile
+//     problems adds grid dimension y = problem (a 3-D tensor map {d, n, batch}), with one private slot per (problem, split).
 //   * One TMA box {k-block columns x 128 rows} per tile and k-block lands in a 7-slot ring of 32 KB slots (rows past
 //     N and columns past D are zero-filled).  Three operand formats (`kMode`):
 //       kModeBf16x2  fp32 clients, 64-column k-blocks.  A converter warp rewrites the slot IN PLACE: every 8-row
@@ -183,8 +184,8 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
           const int s = b % kPSlots;
           mbar_wait(&slot_free[s], phase_of(b) ^ 1u);
           mbar_arrive_expect_tx(&raw_full[s], box_bytes);
-          tma_load_2d(smem + static_cast<size_t>(s) * kPSlotBytes, &tmap, &raw_full[s],
-                      (split + (b / nbx) * p.splits) * kCols, ((b % nbx) == 0 ? ti : tj) * 128, pol);
+          tma_load_3d(smem + static_cast<size_t>(s) * kPSlotBytes, &tmap, &raw_full[s],
+                      (split + (b / nbx) * p.splits) * kCols, ((b % nbx) == 0 ? ti : tj) * 128, blockIdx.y, pol);
         }
       }
     } else if (kMode == kModeBf16x2) {
@@ -354,7 +355,7 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
     }
     // accumulator fragment of m64nN: element i of thread (warp wq, lane) is row 16 wq + lane/4 + 8 ((i/2) % 2),
     // column 8 (i/4) + 2 (lane % 4) + i % 2; kSym writes columns 0..kSymN-1 only
-    float* out = p.parts + (static_cast<size_t>(pair) * p.splits + split) * kPPartElems +
+    float* out = p.parts + ((static_cast<size_t>(blockIdx.y) * p.pairs + pair) * p.splits + split) * kPPartElems +
                  static_cast<size_t>(64 * c + 16 * wq + (lane >> 2)) * 128 + 2 * (lane & 3);
 #pragma unroll
     for (int i = 0; i < kAcc; i += 2)
@@ -364,7 +365,7 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
 
 // Split reduction of the lower-triangular tile pairs: S[i][j] (i >= j, float64) = sum over splits, in a fixed order
 // (threadIdx.y owns a contiguous range, the kPSy partial sums are added in order).  sym (one bf16x2 tile, whose
-// partials hold M, not S): every j, so that S[i][j] + S[j][i] = 2 S_ij for pair_to_sqdist_kernel.
+// partials hold M, not S): every j, so that S[i][j] + S[j][i] = 2 S_ij for pair_to_sqdist_kernel.  blockIdx.z = problem.
 constexpr int kPSy = 8;
 __global__ void __launch_bounds__(128 * kPSy)
 pair_reduce_kernel(const float* __restrict__ parts, int n, int splits, int sym, double* __restrict__ S) {
@@ -374,7 +375,8 @@ pair_reduce_kernel(const float* __restrict__ parts, int n, int splits, int sym, 
   if (tj > ti) return;
   const int jj = threadIdx.x, sy = threadIdx.y;
   const int j = tj * 128 + jj;
-  const int pair = ti * (ti + 1) / 2 + tj;
+  const int pair = (blockIdx.z * gridDim.y * (gridDim.y + 1)) / 2 + ti * (ti + 1) / 2 + tj;
+  S += static_cast<size_t>(blockIdx.z) * n * n;
   const float* base = parts + static_cast<size_t>(pair) * splits * kPPartElems + ii * 128 + jj;
   const int s0 = splits * sy / kPSy, s1 = splits * (sy + 1) / kPSy;
   const bool want = (sym || j <= i) && j < n;
@@ -400,6 +402,8 @@ __global__ void pair_to_sqdist_kernel(const double* __restrict__ S, int n, int s
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = blockIdx.y;
   if (j >= n) return;
+  S += static_cast<size_t>(blockIdx.z) * n * n;                 // problem blockIdx.z
+  d2 += static_cast<size_t>(blockIdx.z) * n * n;
   double v = 0.0;
   if (i != j) {
     const int lo = min(i, j), hi = max(i, j);
@@ -425,9 +429,10 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 // K splits per tile pair: the kernel runs one CTA per SM, so choose the split count whose pairs * splits CTAs fill
-// whole waves of SMs best (up to 4 waves; e.g. N = 1000 on 132 SMs: 36 pairs x 11 = 3 full waves instead of 108 CTAs)
-int pair_splits(int n, int64_t d) {
-  const int tiles = (n + 127) / 128, pairs = tiles * (tiles + 1) / 2;
+// whole waves of SMs best (up to 4 waves; e.g. N = 1000 on 132 SMs: 36 pairs x 11 = 3 full waves instead of 108 CTAs).
+// A batch counts pairs x batch CTAs per split, so its partials stay near 4 waves of tiles instead of growing with it.
+int pair_splits(int n, int64_t d, int batch) {
+  const int tiles = (n + 127) / 128, pairs = tiles * (tiles + 1) / 2 * batch;
   const int64_t kblocks = (d + kPCols - 1) / kPCols;
   const int sms = sm_count();
   int s = 1;
@@ -446,46 +451,48 @@ int pair_splits(int n, int64_t d) {
   return s < 1 ? 1 : s;
 }
 size_t pair_center_bytes(int64_t d) { return align_up(static_cast<size_t>((d + kPCols - 1) / kPCols * kPCols) * sizeof(float), 256); }
-size_t pair_parts_bytes(int n, int64_t d) {
+size_t pair_parts_bytes(int n, int64_t d, int batch) {
   const int tiles = (n + 127) / 128, pairs = tiles * (tiles + 1) / 2;
-  return static_cast<size_t>(pairs) * pair_splits(n, d) * kPPartElems * sizeof(float);
+  return static_cast<size_t>(pairs) * batch * pair_splits(n, d, batch) * kPPartElems * sizeof(float);
 }
 
 template <int kMode, int kSymN>
-static int launch_mode(const CUtensorMap& tmap, const PairParams& p, cudaStream_t stream) {
+static int launch_mode(const CUtensorMap& tmap, const PairParams& p, int batch, cudaStream_t stream) {
   const size_t smem = static_cast<size_t>(kPSlots) * kPSlotBytes + 1024;
   static int smem_attr_done[kMaxDevices] = {0};
   AFL_CUDA(ensure_dyn_smem(gram_pair_kernel<kMode, kSymN>, static_cast<int>(smem), smem_attr_done));
   {
     ProfScope ps("gram_pair", stream);
-    gram_pair_kernel<kMode, kSymN><<<p.pairs * p.splits, kPThreads, smem, stream>>>(tmap, p);
+    gram_pair_kernel<kMode, kSymN><<<dim3(p.pairs * p.splits, batch), kPThreads, smem, stream>>>(tmap, p);
   }
   AFL_LAUNCH_CHECK("gram_pair_kernel");
   return AFL_OK;
 }
 
 // the one-tile symmetric form: one instance per box height (gram.cu:make_plan runs it for 49 <= N <= 112)
-static int launch_sym(const CUtensorMap& tmap, const PairParams& p, cudaStream_t stream) {
+static int launch_sym(const CUtensorMap& tmap, const PairParams& p, int batch, cudaStream_t stream) {
   switch (p.box_rows) {
-    case 56: return launch_mode<kModeBf16x2, 56>(tmap, p, stream);
-    case 64: return launch_mode<kModeBf16x2, 64>(tmap, p, stream);
-    case 72: return launch_mode<kModeBf16x2, 72>(tmap, p, stream);
-    case 80: return launch_mode<kModeBf16x2, 80>(tmap, p, stream);
-    case 88: return launch_mode<kModeBf16x2, 88>(tmap, p, stream);
-    case 96: return launch_mode<kModeBf16x2, 96>(tmap, p, stream);
-    case 104: return launch_mode<kModeBf16x2, 104>(tmap, p, stream);
-    case 112: return launch_mode<kModeBf16x2, 112>(tmap, p, stream);
+    case 56: return launch_mode<kModeBf16x2, 56>(tmap, p, batch, stream);
+    case 64: return launch_mode<kModeBf16x2, 64>(tmap, p, batch, stream);
+    case 72: return launch_mode<kModeBf16x2, 72>(tmap, p, batch, stream);
+    case 80: return launch_mode<kModeBf16x2, 80>(tmap, p, batch, stream);
+    case 88: return launch_mode<kModeBf16x2, 88>(tmap, p, batch, stream);
+    case 96: return launch_mode<kModeBf16x2, 96>(tmap, p, batch, stream);
+    case 104: return launch_mode<kModeBf16x2, 104>(tmap, p, batch, stream);
+    case 112: return launch_mode<kModeBf16x2, 112>(tmap, p, batch, stream);
   }
   set_error("gram_pair_kernel: no one-tile bf16x2 instance for %d clients (49..112)", p.n);
   return AFL_ERR_UNSUPPORTED;
 }
 
-// G: fp32 [n, d] (pitch multiple of 4 elements) or bf16 (kModeBf16In, pitch multiple of 8), 16-byte aligned.
-// parts: pair_parts_bytes(); S: n*n doubles; cvec: pair_center_bytes().
-int launch_pair(const void* Gv, int mode, int n, int64_t d, int64_t ld, float* parts, double* S, float* cvec, double* d2_out,
-                int flush, int center, int single_pass, cudaStream_t stream) {
+// G: `batch` problems of fp32 [n, d] (pitch multiple of 4 elements) or bf16 (kModeBf16In, pitch multiple of 8), 16-byte
+// aligned, problem b at G + b * batch_stride elements (batch > 1: one tile, a 16-byte multiple >= n * ld).
+// parts: pair_parts_bytes(); S and d2_out: batch * n * n doubles; cvec: pair_center_bytes().
+int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, float* parts,
+                double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream) {
   const float* G = static_cast<const float*>(Gv);
   const bool bf16 = mode == kModeBf16In;
+  if (batch > 1 && n > 128) { set_error("gram_pair_kernel: batched problems are one tile (n <= 128, got %d)", n); return AFL_ERR_UNSUPPORTED; }
   static EncodeTiledFn enc = nullptr;
   if (!enc) {
     void* fp = nullptr;
@@ -499,7 +506,7 @@ int launch_pair(const void* Gv, int mode, int n, int64_t d, int64_t ld, float* p
   p.n = n; p.tiles = (n + 127) / 128; p.pairs = p.tiles * (p.tiles + 1) / 2;
   const int sym = mode == kModeBf16x2 && p.tiles == 1;     // the kernel's kSymN > 0
   p.box_rows = sym ? (n + 7) / 8 * 8 : 128;
-  p.splits = pair_splits(n, d);
+  p.splits = pair_splits(n, d, batch);
   p.kblocks = static_cast<int>((d + cols - 1) / cols);
   // `flush` counts 64-column k-blocks of 12 chained bf16 MMAs.  A split-TF32 k-block already chains 12 MMAs over 32 columns,
   // and its truncation bias grows with the chain: one k-block per chain keeps it within that format's 2e-6 budget.
@@ -518,23 +525,25 @@ int launch_pair(const void* Gv, int mode, int n, int64_t d, int64_t ld, float* p
     AFL_LAUNCH_CHECK("pair_center_kernel");
   }
   CUtensorMap tmap;
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(d), static_cast<cuuint64_t>(n)};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ld) * (bf16 ? 2 : 4)};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(cols), static_cast<cuuint32_t>(p.box_rows)};
-  const cuuint32_t estride[2] = {1, 1};
-  CUresult r = enc(&tmap, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(Gv), gdim,
+  const cuuint64_t es = bf16 ? 2 : 4;
+  const cuuint64_t gdim[3] = {static_cast<cuuint64_t>(d), static_cast<cuuint64_t>(n), static_cast<cuuint64_t>(batch)};
+  const cuuint64_t gstride[2] = {static_cast<cuuint64_t>(ld) * es,
+                                 static_cast<cuuint64_t>(batch > 1 ? batch_stride : n * ld) * es};
+  const cuuint32_t box[3] = {static_cast<cuuint32_t>(cols), static_cast<cuuint32_t>(p.box_rows), 1};
+  const cuuint32_t estride[3] = {1, 1, 1};
+  CUresult r = enc(&tmap, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(Gv), gdim,
                    gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    mode == kModeBf16x2 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed: %d", static_cast<int>(r)); return AFL_ERR_CUDA; }
-  int rc = sym                   ? launch_sym(tmap, p, stream)
-         : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, 0>(tmap, p, stream)
-         : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, 0>(tmap, p, stream)
-                               : launch_mode<kModeBf16In, 0>(tmap, p, stream);
+  int rc = sym                   ? launch_sym(tmap, p, batch, stream)
+         : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, 0>(tmap, p, batch, stream)
+         : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, 0>(tmap, p, batch, stream)
+                               : launch_mode<kModeBf16In, 0>(tmap, p, batch, stream);
   if (rc) return rc;
-  pair_reduce_kernel<<<dim3(n, p.tiles), dim3(128, kPSy), 0, stream>>>(parts, n, p.splits, sym, S);
+  pair_reduce_kernel<<<dim3(n, p.tiles, batch), dim3(128, kPSy), 0, stream>>>(parts, n, p.splits, sym, S);
   AFL_LAUNCH_CHECK("pair_reduce_kernel");
-  pair_to_sqdist_kernel<<<dim3((n + 127) / 128, n), 128, 0, stream>>>(S, n, sym, d2_out);
+  pair_to_sqdist_kernel<<<dim3((n + 127) / 128, n, batch), 128, 0, stream>>>(S, n, sym, d2_out);
   AFL_LAUNCH_CHECK("pair_to_sqdist_kernel");
   return AFL_OK;
 }

@@ -1,5 +1,6 @@
 // Krum (defences.py:23-42) and Bulyan's selection loop (defences.py:57-68) on an n x n distance table that is small
-// enough (<= 64 MB of fp32 at n = 4096) to live in L2.
+// enough (<= 64 MB of fp32 at n = 4096) to live in L2.  A batch of same-shape problems (consecutive tables) adds the
+// problem to the grid: y for krum_tail_kernel and row_sort_kernel, x for bulyan_rounds_kernel.
 //
 //   krum_tail_kernel     one CTA per user u: u's n-1 distances -> bitonic sort in shared memory -> ascending sequential
 //                        fp32 sum of the `take` smallest (defences.py:33-34) -> score[u]; the last CTA to finish does the
@@ -9,7 +10,7 @@
 //                        order, so a user-supplied table keeps the sign and NaN of its entries).
 //   row_sort_kernel      Bulyan: one CTA per user sorts the user's n-1 distances (value, index) and emits the sorted
 //                        values, the sorted neighbour indices and the inverse permutation (rank of every neighbour).
-//   bulyan_rounds_kernel one persistent CTA runs all theta rounds.  Removal of the selected user is an
+//   bulyan_rounds_kernel one persistent CTA per problem runs all theta rounds.  Removal of the selected user is an
 //                        O(1) update per remaining user: its kept set (the m_r smallest alive distances)
 //                        loses either the removed neighbour or its current largest kept element, tracked
 //                        by a boundary pointer that only ever moves left over the pre-sorted row.  Scores
@@ -24,20 +25,21 @@ namespace select {
 
 constexpr int kMaxN = 4096;
 
-// Workspace: Bulyan's sorted rows, or Krum's [last-CTA counter | 256 B][score: n floats].
+// Workspace of `batch` problems: Bulyan's sorted rows, or Krum's [last-CTA counters: batch, padded to 256 B][scores:
+// batch x n floats].  Problem b's rows are at b * n * n in each array.
 struct SortWs {
-  float* sval;      // [n][n]   sorted distances of row u (first n-1 entries valid)
-  uint16_t* sidx;   // [n][n]   neighbour index at each sorted position
-  uint16_t* rank;   // [n][n]   rank[u][v] = sorted position of neighbour v in row u
+  float* sval;      // [batch][n][n]   sorted distances of row u (first n-1 entries valid)
+  uint16_t* sidx;   // [batch][n][n]   neighbour index at each sorted position
+  uint16_t* rank;   // [batch][n][n]   rank[u][v] = sorted position of neighbour v in row u
 };
 
-static size_t ws_bytes_for(int n) {
-  const size_t nn = static_cast<size_t>(n) * n;
-  return align_up(nn * 4, 256) + 2 * align_up(nn * 2, 256) + align_up(static_cast<size_t>(n) * 4, 256) + 256;
+static size_t ws_bytes_for(int n, int batch) {
+  const size_t nn = static_cast<size_t>(n) * n * batch;
+  return align_up(nn * 4, 256) + 2 * align_up(nn * 2, 256) + align_up(static_cast<size_t>(n) * batch * 4, 256) + 256;
 }
 
-static SortWs carve(void* ws, int n) {
-  const size_t nn = static_cast<size_t>(n) * n;
+static SortWs carve(void* ws, int n, int batch) {
+  const size_t nn = static_cast<size_t>(n) * n * batch;
   uint8_t* p = static_cast<uint8_t*>(ws);
   SortWs w;
   w.sval = reinterpret_cast<float*>(p); p += align_up(nn * 4, 256);
@@ -111,8 +113,8 @@ template <KrumSource kSrc>
 using KrumKey = typename std::conditional<kSrc == kSqdist, uint32_t, unsigned long long>::type;
 
 template <KrumSource kSrc>
-__device__ __forceinline__ KrumKey<kSrc> krum_key(const KrumParams& p, int u, int v) {
-  const size_t e = static_cast<size_t>(u) * p.n + v;
+__device__ __forceinline__ KrumKey<kSrc> krum_key(const KrumParams& p, size_t off, int u, int v) {
+  const size_t e = off + static_cast<size_t>(u) * p.n + v;
   if constexpr (kSrc == kSqdist) {
     double s = 0.0;
     for (int r = 0; r < p.world; ++r)                                    // fixed rank order: identical sum on every rank
@@ -127,9 +129,9 @@ __device__ __forceinline__ KrumKey<kSrc> krum_key(const KrumParams& p, int u, in
 
 // The distance a sorted key stands for: the key itself, or the table's original bits (keeps a NaN a NaN).
 template <KrumSource kSrc>
-__device__ __forceinline__ float krum_value(const KrumParams& p, int u, KrumKey<kSrc> k) {
+__device__ __forceinline__ float krum_value(const KrumParams& p, size_t off, int u, KrumKey<kSrc> k) {
   if constexpr (kSrc == kSqdist) return __uint_as_float(k);
-  else return p.dist[static_cast<size_t>(u) * p.n + static_cast<int>(k & 0xFFFFFFFFu)];
+  else return p.dist[off + static_cast<size_t>(u) * p.n + static_cast<int>(k & 0xFFFFFFFFu)];
 }
 
 template <KrumSource kSrc>
@@ -139,7 +141,9 @@ krum_tail_kernel(const KrumParams p) {
   extern __shared__ __align__(8) unsigned char smem[];
   Key* keys = reinterpret_cast<Key*>(smem);                              // P row keys
   __shared__ int s_last;
-  const int u = blockIdx.x, n = p.n;
+  const int u = blockIdx.x, n = p.n, b = blockIdx.y;                     // user u of problem b
+  const size_t off = static_cast<size_t>(b) * n * n;
+  float* score = p.score + static_cast<size_t>(b) * n;
   if constexpr (kSrc == kSqdist) {
     if (p.world > 1 && !wait_flags(p.flags, p.world, p.epoch)) {
       if (threadIdx.x == 0 && u == 0) { *p.status_host = 1; *p.idx_host = -1; *p.idx_dev = -1; }
@@ -148,15 +152,15 @@ krum_tail_kernel(const KrumParams p) {
   }
   int P = 1;
   while (P < n) P <<= 1;
-  for (int v = threadIdx.x; v < P; v += blockDim.x) keys[v] = (v < n && v != u) ? krum_key<kSrc>(p, u, v) : ~Key(0);
+  for (int v = threadIdx.x; v < P; v += blockDim.x) keys[v] = (v < n && v != u) ? krum_key<kSrc>(p, off, u, v) : ~Key(0);
   __syncthreads();
   block_bitonic_sort(keys, P);
   if (threadIdx.x == 0) {
     float s = 0.f;                                                       // Python: sum() starts at int 0; ascending fp32 adds
-    for (int pos = 0; pos < p.take; ++pos) s = s + krum_value<kSrc>(p, u, keys[pos]);
-    p.score[u] = s;
+    for (int pos = 0; pos < p.take; ++pos) s = s + krum_value<kSrc>(p, off, u, keys[pos]);
+    score[u] = s;
     __threadfence();
-    s_last = (atomicAdd(p.done, 1u) == static_cast<unsigned>(n - 1)) ? 1 : 0;
+    s_last = (atomicAdd(p.done + b, 1u) == static_cast<unsigned>(n - 1)) ? 1 : 0;
   }
   __syncthreads();
   if (!s_last) return;
@@ -165,26 +169,27 @@ krum_tail_kernel(const KrumParams p) {
   float best = __int_as_float(0x7f800000);
   int best_pos = 0x7fffffff;
   for (int v = threadIdx.x; v < n; v += blockDim.x) {
-    const float s = __ldcg(p.score + v);
+    const float s = __ldcg(score + v);
     if (n >= 2 && static_cast<double>(s) < 1e20) argmin_combine(best, best_pos, s, visit_pos(v));   // vs the Python float 1e20
   }
   const int idx = block_argmin_user<256 / 32>(best, best_pos);
   if (threadIdx.x == 0) {
-    *p.idx_dev = idx;
+    p.idx_dev[b] = idx;
     if (p.idx_host) { *p.idx_host = idx; *p.status_host = 0; }
-    *p.done = 0u;                                                        // ready for the next step
+    p.done[b] = 0u;                                                      // ready for the next step
     __threadfence_system();
   }
 }
 
-// Fills p.take and launches the kernel for the row source p selects.  p.done must be zero.
-int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream) {
+// Fills p.take and launches the kernel for the row source p selects, grid (n, batch).  p.done[0 .. batch) must be zero.
+int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream, int batch) {
   p.take = python_slice_take(users_count - corrupted_count, p.n - 1);
   int P = 1; while (P < p.n) P <<= 1;
   {
     ProfScope ps("krum_tail", stream);
-    if (p.dist) krum_tail_kernel<kDist><<<p.n, 256, static_cast<size_t>(P) * sizeof(KrumKey<kDist>), stream>>>(p);
-    else krum_tail_kernel<kSqdist><<<p.n, 256, static_cast<size_t>(P) * sizeof(KrumKey<kSqdist>), stream>>>(p);
+    const dim3 grid(p.n, batch);
+    if (p.dist) krum_tail_kernel<kDist><<<grid, 256, static_cast<size_t>(P) * sizeof(KrumKey<kDist>), stream>>>(p);
+    else krum_tail_kernel<kSqdist><<<grid, 256, static_cast<size_t>(P) * sizeof(KrumKey<kSqdist>), stream>>>(p);
   }
   AFL_LAUNCH_CHECK("krum_tail_kernel");
   return AFL_OK;
@@ -194,6 +199,8 @@ __global__ void __launch_bounds__(256)
 row_sort_kernel(const float* __restrict__ dist, int n, SortWs w) {
   extern __shared__ unsigned long long keys[];
   const int u = blockIdx.x;
+  const size_t off = static_cast<size_t>(blockIdx.y) * n * n;           // problem blockIdx.y
+  dist += off; w.sval += off; w.sidx += off; w.rank += off;
   int P = 1;
   while (P < n) P <<= 1;
   for (int v = threadIdx.x; v < P; v += blockDim.x)
@@ -222,6 +229,9 @@ __global__ void __launch_bounds__(1024, 1)
 bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, SortWs w, int* __restrict__ sel_out) {
   __shared__ uint8_t alive[kMaxN];
   __shared__ int s_winner;
+  const size_t off = static_cast<size_t>(blockIdx.x) * n * n;           // one CTA per problem
+  dist += off; w.sval += off; w.sidx += off; w.rank += off;
+  sel_out += static_cast<size_t>(blockIdx.x) * theta;
 
   const int tid = threadIdx.x;
   double score[kRowsPerThread];
@@ -289,27 +299,29 @@ bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, So
 }
 
 int max_clients() { return kMaxN; }
-size_t workspace_bytes(int n) { return ws_bytes_for(n < 1 ? 1 : n); }
+size_t workspace_bytes(int n, int batch) { return ws_bytes_for(n < 1 ? 1 : n, batch < 1 ? 1 : batch); }
+size_t workspace_bytes(int n) { return workspace_bytes(n, 1); }
 
-static int check_ws(int n, void* ws, size_t ws_bytes) {
+static int check_ws(int n, int batch, void* ws, size_t ws_bytes) {
   if (n > kMaxN) { set_error("selection kernels support n <= %d clients (got %d)", kMaxN, n); return AFL_ERR_UNSUPPORTED; }
-  if (!ws || ws_bytes < ws_bytes_for(n) || (reinterpret_cast<uintptr_t>(ws) % 256) != 0) {
-    set_error("selection workspace too small or misaligned (%zu < %zu)", ws_bytes, ws_bytes_for(n));
+  if (!ws || ws_bytes < ws_bytes_for(n, batch) || (reinterpret_cast<uintptr_t>(ws) % 256) != 0) {
+    set_error("selection workspace too small or misaligned (%zu < %zu)", ws_bytes, ws_bytes_for(n, batch));
     return AFL_ERR_WORKSPACE;
   }
   return AFL_OK;
 }
 
-// Krum on a workspace: the counter lives in its first 4 bytes (cleared here: workspaces are not initialised), the
-// scores behind it unless the caller wants them.
-static int krum_on_workspace(KrumParams p, int users_count, int corrupted_count, float* scores_out, void* ws,
+// Krum on a workspace: the batch counters live at its start (cleared here: workspaces are not initialised), the
+// scores behind them unless the caller wants them.
+static int krum_on_workspace(KrumParams p, int batch, int users_count, int corrupted_count, float* scores_out, void* ws,
                              size_t ws_bytes, cudaStream_t stream) {
-  int rc = check_ws(p.n, ws, ws_bytes);
+  int rc = check_ws(p.n, batch, ws, ws_bytes);
   if (rc) return rc;
   p.done = static_cast<unsigned int*>(ws);
-  p.score = scores_out ? scores_out : reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
-  AFL_CUDA(cudaMemsetAsync(p.done, 0, sizeof(unsigned int), stream));
-  return krum_tail(p, users_count, corrupted_count, stream);
+  p.score = scores_out ? scores_out
+                       : reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + align_up(static_cast<size_t>(batch) * 4, 256));
+  AFL_CUDA(cudaMemsetAsync(p.done, 0, static_cast<size_t>(batch) * sizeof(unsigned int), stream));
+  return krum_tail(p, users_count, corrupted_count, stream, batch);
 }
 
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
@@ -317,19 +329,21 @@ int krum_select(const float* dist, int n, int users_count, int corrupted_count, 
   if (!dist || !idx_out || n < 1) { set_error("afl_krum_select: bad argument"); return AFL_ERR_BAD_ARG; }
   KrumParams p{};
   p.dist = dist; p.n = n; p.idx_dev = idx_out;
-  return krum_on_workspace(p, users_count, corrupted_count, scores_out, ws, ws_bytes, stream);
+  return krum_on_workspace(p, 1, users_count, corrupted_count, scores_out, ws, ws_bytes, stream);
 }
 
+// d2: batch consecutive n x n tables; idx_out[batch]
 int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
-                     size_t ws_bytes, cudaStream_t stream) {
+                     size_t ws_bytes, cudaStream_t stream, int batch) {
   if (!d2 || !idx_out || n < 1) { set_error("afl_krum_from_sqdist: bad argument"); return AFL_ERR_BAD_ARG; }
   KrumParams p{};
   p.tab[0] = d2; p.world = 1; p.n = n; p.idx_dev = idx_out;
-  return krum_on_workspace(p, users_count, corrupted_count, nullptr, ws, ws_bytes, stream);
+  return krum_on_workspace(p, batch, users_count, corrupted_count, nullptr, ws, ws_bytes, stream);
 }
 
+// dist: batch consecutive n x n tables; sel_out[batch][theta]
 int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out, void* ws, size_t ws_bytes,
-                  cudaStream_t stream) {
+                  cudaStream_t stream, int batch) {
   if (!dist || !sel_out || n < 1 || f < 0) { set_error("afl_bulyan_select: bad argument"); return AFL_ERR_BAD_ARG; }
   if (users_count < 4 * f + 3) {
     set_error("bulyan: users_count >= 4*corrupted_count + 3 violated (%d, %d)", users_count, f);
@@ -340,17 +354,17 @@ int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out
     return AFL_ERR_UNSUPPORTED;
   }
   const int theta = users_count - 2 * f;
-  int rc = check_ws(n, ws, ws_bytes);
+  int rc = check_ws(n, batch, ws, ws_bytes);
   if (rc) return rc;
-  const SortWs w = carve(ws, n);
+  const SortWs w = carve(ws, n, batch);
   int P = 1; while (P < n) P <<= 1;
   {
     ProfScope ps("row_sort", stream);
-    row_sort_kernel<<<n, 256, static_cast<size_t>(P) * sizeof(unsigned long long), stream>>>(dist, n, w);
+    row_sort_kernel<<<dim3(n, batch), 256, static_cast<size_t>(P) * sizeof(unsigned long long), stream>>>(dist, n, w);
   }
   AFL_LAUNCH_CHECK("row_sort_kernel");
   ProfScope ps("bulyan_rounds", stream);
-  bulyan_rounds_kernel<<<1, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out);
+  bulyan_rounds_kernel<<<batch, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out);
   AFL_LAUNCH_CHECK("bulyan_rounds_kernel");
   return AFL_OK;
 }

@@ -43,6 +43,8 @@ struct Params {
   int n_rows;             // participating rows
   int n_total;            // rows of G (bounds for row_index)
   int keep;               // effective number of kept devs (python slice semantics applied), >= 0
+  int64_t g_batch, out_batch;   // problem blockIdx.y: G, out and row_index advance by these (elements)
+  int ri_batch;
   float med_density;      // 0.39894228 * n      (ranks per unit value at the centre of a unit Gaussian)
   float key_q;            // Gaussian guess of the |dev| threshold in sigmas
   float key_density;      // 2 * phi(key_q) * n  (ranks per unit |dev| at that threshold, unit sigma)
@@ -403,7 +405,8 @@ __device__ __forceinline__ void stage_tile(const Params& P, uint32_t* tile, int6
   const int es = BF16 ? 2 : 4;
   const int cols_per_tile = BF16 ? 32 : 16;
   const uint32_t sentinel = BF16 ? 0x7F807F80u : 0x7F800000u;
-  const uint8_t* base = static_cast<const uint8_t*>(P.G);
+  const uint8_t* base = static_cast<const uint8_t*>(P.G) + static_cast<int64_t>(blockIdx.y) * P.g_batch * es;
+  const int* row_index = P.row_index ? P.row_index + static_cast<int64_t>(blockIdx.y) * P.ri_batch : nullptr;
   constexpr int kIters = (32 * S * 4) / kThreads;      // S/2
   const bool full_tile = P.vec_ok && (col0 + cols_per_tile <= P.d);
   const int rowq = tid >> 2, j = tid & 3, l = rowq & 31, hi2 = tid >> 7;
@@ -417,9 +420,9 @@ __device__ __forceinline__ void stage_tile(const Params& P, uint32_t* tile, int6
     // (branch-free: rows past n_rows re-read the last row and are replaced by the sentinel at the store)
     int gr[kIters];
     const int last = P.n_rows - 1;
-    if (P.row_index) {
+    if (row_index) {
 #pragma unroll
-      for (int it = 0; it < kIters; ++it) gr[it] = P.row_index[min(it * 64 + rowq, last)];
+      for (int it = 0; it < kIters; ++it) gr[it] = row_index[min(it * 64 + rowq, last)];
 #pragma unroll
       for (int it = 0; it < kIters; ++it) gr[it] = gr[it] < 0 ? gr[it] + P.n_total : gr[it];
     } else {
@@ -450,7 +453,7 @@ __device__ __forceinline__ void stage_tile(const Params& P, uint32_t* tile, int6
     const int r = it * 64 + rowq;
     uint32_t w[4] = {sentinel, sentinel, sentinel, sentinel};
     if (r < P.n_rows) {
-      int gr = P.row_index ? P.row_index[r] : r;
+      int gr = row_index ? row_index[r] : r;
       gr = gr < 0 ? gr + P.n_total : gr;
       const uint8_t* src = base + (static_cast<int64_t>(gr) * P.ld + c) * es;
       w[0] = w[1] = w[2] = w[3] = 0u;
@@ -593,7 +596,7 @@ trimmed_mean_kernel(const Params P) {
       const int64_t col = col0 + (BF16 ? 2 * cw + half : cw);
       if (col >= P.d) break;                         // warp-uniform
       const float res = general_column_impl<S, BF16>(P, tile, cw, half, scratch, lane);
-      if (lane == 0) P.out[col] = res;
+      if (lane == 0) P.out[static_cast<int64_t>(blockIdx.y) * P.out_batch + col] = res;
     }
   }
 }
@@ -641,9 +644,10 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
   const int es = bf16 ? 2 : 4;
   const int cols = bf16 ? 8 : 4;
   const int64_t col0 = static_cast<int64_t>(blockIdx.x) * cols;
-  const uint8_t* base = static_cast<const uint8_t*>(P.G);
+  const uint8_t* base = static_cast<const uint8_t*>(P.G) + static_cast<int64_t>(blockIdx.y) * P.g_batch * es;
+  const int* row_index = P.row_index ? P.row_index + static_cast<int64_t>(blockIdx.y) * P.ri_batch : nullptr;
   for (int r = tid; r < n; r += blockDim.x) {
-    int gr = P.row_index ? P.row_index[r] : r;
+    int gr = row_index ? row_index[r] : r;
     gr = gr < 0 ? gr + P.n_total : gr;
     const uint8_t* src = base + (static_cast<int64_t>(gr) * P.ld + col0) * es;
     uint32_t w[4] = {0u, 0u, 0u, 0u};
@@ -696,7 +700,7 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
       const float total = warp_sum(part);
       res = __fadd_rn(__fdiv_rn(total, static_cast<float>(P.keep)), med);
     }
-    if (lane == 0) P.out[col] = res;
+    if (lane == 0) P.out[static_cast<int64_t>(blockIdx.y) * P.out_batch + col] = res;
   }
 }
 
@@ -727,10 +731,10 @@ static double norm_ppf(double pr) {   // Acklam's rational approximation, |error
 }
 
 template <int S>
-static int launch(const Params& P, int dtype, cudaStream_t stream) {
+static int launch(const Params& P, int dtype, int batch, cudaStream_t stream) {
   const size_t smem = static_cast<size_t>(S) * 2048 + kWarps * kScratchWords * 4;
   const int cols = dtype == AFL_BF16 ? 32 : 16;
-  const unsigned grid = static_cast<unsigned>(ceil_div64(P.d, cols));
+  const dim3 grid(static_cast<unsigned>(ceil_div64(P.d, cols)), batch);
   ProfScope ps("trimmed_mean", stream);
   if (dtype == AFL_BF16) {
     AFL_CUDA(cudaFuncSetAttribute(trimmed_mean_kernel<S, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -743,8 +747,10 @@ static int launch(const Params& P, int dtype, cudaStream_t stream) {
   return AFL_OK;
 }
 
-int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
-                 int corrupted_count, float* out, cudaStream_t stream) {
+// `batch` problems (grid y): problem b reads G + b * g_batch and row_index + b * ri_batch, and writes out + b * out_batch.
+int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
+                         int corrupted_count, float* out, int batch, int64_t g_batch, int ri_batch, int64_t out_batch,
+                         cudaStream_t stream) {
   if (!G || !out || n < 1 || d < 1 || ld < d || n_rows < 1) { set_error("afl_trimmed_mean: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_trimmed_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
   if (n_rows > kLargeMaxRows) {
@@ -756,33 +762,39 @@ int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const i
   const int keep = k >= 0 ? (k < n_rows ? k : n_rows) : (n_rows + k > 0 ? n_rows + k : 0);
   Params P{};
   P.G = G; P.row_index = row_index; P.out = out; P.d = d; P.ld = ld; P.n_rows = n_rows; P.n_total = n; P.keep = keep;
+  P.g_batch = g_batch; P.out_batch = out_batch; P.ri_batch = ri_batch;
   P.med_density = 0.3989422804f * static_cast<float>(n_rows);
   const double frac = keep > 0 ? (static_cast<double>(keep) - 0.5) / n_rows : 0.5;
   const double q = norm_ppf(0.5 * (1.0 + (frac < 0.999999 ? frac : 0.999999)));
   P.key_q = static_cast<float>(q);
   P.key_density = static_cast<float>(2.0 * 0.3989422804014327 * exp(-0.5 * q * q) * n_rows);
   const int64_t es = dtype == AFL_F32 ? 4 : 2;
-  P.vec_ok = (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0);
+  P.vec_ok = (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0) && (batch == 1 || (g_batch * es) % 16 == 0);
   if (n_rows > 1024) {
     const size_t smem = static_cast<size_t>(n_rows) * 16;
     const int cols = dtype == AFL_BF16 ? 8 : 4;
     static int smem_attr_done[kMaxDevices] = {0};
     AFL_CUDA(ensure_dyn_smem(trimmed_mean_large_kernel, static_cast<int>(kLargeMaxRows) * 16, smem_attr_done));
     ProfScope ps("trimmed_mean", stream);
-    trimmed_mean_large_kernel<<<static_cast<unsigned>(ceil_div64(d, cols)), 256, smem, stream>>>(P, dtype == AFL_BF16 ? 1 : 0);
+    trimmed_mean_large_kernel<<<dim3(static_cast<unsigned>(ceil_div64(d, cols)), batch), 256, smem, stream>>>(P, dtype == AFL_BF16 ? 1 : 0);
     AFL_LAUNCH_CHECK("trimmed_mean_large_kernel");
     return AFL_OK;
   }
   // S = slots per lane, a multiple of 4 with 32 * S >= n_rows: the work per column is proportional to S, not to n_rows
   // (Bulyan's second stage at N = 1000, f = 240 selects 520 rows: S = 20 instead of 32)
-  if (n_rows <= 128) return launch<4>(P, dtype, stream);
-  if (n_rows <= 256) return launch<8>(P, dtype, stream);
-  if (n_rows <= 384) return launch<12>(P, dtype, stream);
-  if (n_rows <= 512) return launch<16>(P, dtype, stream);
-  if (n_rows <= 640) return launch<20>(P, dtype, stream);
-  if (n_rows <= 768) return launch<24>(P, dtype, stream);
-  if (n_rows <= 896) return launch<28>(P, dtype, stream);
-  return launch<32>(P, dtype, stream);
+  if (n_rows <= 128) return launch<4>(P, dtype, batch, stream);
+  if (n_rows <= 256) return launch<8>(P, dtype, batch, stream);
+  if (n_rows <= 384) return launch<12>(P, dtype, batch, stream);
+  if (n_rows <= 512) return launch<16>(P, dtype, batch, stream);
+  if (n_rows <= 640) return launch<20>(P, dtype, batch, stream);
+  if (n_rows <= 768) return launch<24>(P, dtype, batch, stream);
+  if (n_rows <= 896) return launch<28>(P, dtype, batch, stream);
+  return launch<32>(P, dtype, batch, stream);
+}
+
+int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
+                 int corrupted_count, float* out, cudaStream_t stream) {
+  return trimmed_mean_batched(G, n, d, ld, dtype, row_index, n_rows, corrupted_count, out, 1, 0, 0, 0, stream);
 }
 
 }  // namespace tmean

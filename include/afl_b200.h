@@ -219,6 +219,43 @@ int afl_bulyan_host(const float* G_host, int n, int64_t d, int64_t ld, int users
 int afl_alie_host(const float* const* rows, int f, int64_t d, double z, float* mu_out, float* sigma_out,
                   float* crafted_out, int64_t slab_cols);
 
+/* ---- batched device calls: many same-shape problems, one launch per stage --------------------------
+ * `batch` independent problems of n <= 128 clients (one Gram tile), problem b at G + b * batch_stride
+ * ELEMENTS, each with the same n, d, ld, users_count and corrupted_count.  The batch is a grid dimension
+ * of the same kernels the single calls run, so every problem's result is the single device call's on
+ * that problem (bit for bit: distance table, Krum index, Bulyan selection and output, trimmed mean,
+ * mean, ALIE statistics; the Gram kernels' split count is chosen for the whole batch, so pin it with the
+ * environment variable AFL_GRAM_SPLITS when comparing distance tables).  Device pointers; the calls only
+ * enqueue work.  The tensor-core Gram path needs a 16-byte aligned base, ld and batch_stride with
+ * batch_stride >= n * ld; anything else runs the SIMT Gram kernel.  Limits, checked before any CUDA call:
+ * n > 128 or batch > 65535 -> AFL_ERR_UNSUPPORTED; batch < 1, a NULL pointer, or (batch > 1) a
+ * batch_stride smaller than one problem's span ((n - 1) * ld + d) -> AFL_ERR_BAD_ARG.
+ *
+ * afl_defend_batched — defences.py:73-75 defend[rule] per problem.  rule as afl_defend_host.
+ *   "Krum"        defences.py:23-42:  idx_out (device int[batch]) receives each problem's index (or -1);
+ *                 users_count >= 2f+1 else AFL_ERR_PRECONDITION.
+ *   "Bulyan"      defences.py:55-70:  out (device fp32[batch][d]) and sel_out (device int[batch][theta],
+ *                 theta = users_count - 2f, selection order; a round with no eligible user writes -1 from
+ *                 that round on in that problem's row, the other problems are unaffected); users_count
+ *                 >= 4f+3 else AFL_ERR_PRECONDITION, and users_count == n.
+ *   "TrimmedMean" defences.py:44-52 and "NoDefense" defences.py:13-14:  out (device fp32[batch][d]).
+ * workspace: afl_batched_workspace_bytes(rule, batch, n, d, dtype) bytes, 256-byte aligned (0 on bad
+ * arguments); TrimmedMean and NoDefense use none.  For Krum and Bulyan it begins with the batch's
+ * squared-distance tables (float64[batch][n][n], afl_sqdist_partial's table of each problem), which the
+ * caller may read once the call's work has run. */
+size_t afl_batched_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype);
+int afl_defend_batched(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                       int64_t ld, int dtype, int users_count, int corrupted_count, float* out, int* idx_out,
+                       int* sel_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* afl_alie_batched — malicious.py:10-27,34-36 per problem: afl_alie on rows 0..f-1 of every problem.
+ * mu_out, sigma_out, crafted_out: device fp32[batch][d] (each may be NULL; crafted_out == mu_out
+ * reproduces the reference's aliasing).  bcast_rows (may be NULL): the crafted vector of problem b is
+ * written into rows 0..f-1 of bcast_rows + b * bcast_batch_stride (pitch bcast_ld), server.py:82-83. */
+int afl_alie_batched(const void* G_mal, int batch, int64_t batch_stride, int f, int64_t d, int64_t ld,
+                     int dtype, double z, float* mu_out, float* sigma_out, float* crafted_out,
+                     float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -54,6 +54,11 @@ SIGNATURES = {
     "afl_batched_workspace_bytes": (_sz, [C.c_char_p, _i, _i, _i64, _i]),
     "afl_defend_batched": (_i, [C.c_char_p, _vp, _i, _i64, _i, _i64, _i64, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "afl_alie_batched": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _d, _vp, _vp, _vp, _vp, _i64, _i64, _vp]),
+    "afl_batched_each_workspace_bytes": (_sz, [C.c_char_p, _i, _i, _i64, _i]),
+    "afl_defend_batched_each": (_i, [C.c_char_p, _vp, _i, _i64, _i, _i64, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz,
+                                     _vp]),
+    "afl_alie_batched_each": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp,
+                                   _sz, _vp]),
 }
 
 _lib = None

@@ -7,14 +7,18 @@ Every problem keeps the reference's semantics exactly: problem b's result is wha
 `G[b]`, bit for bit (C ABI `afl_defend_batched` / `afl_alie_batched`).
 
 Inputs are torch.cuda float32 / bfloat16 tensors `[B, N, D]` with `stride(2) == 1` and N <= 128 clients (one
-Gram tile); every problem shares N, D, `users_count` and `corrupted_count`.  Nothing here synchronises the
-host except `bulyan`, which checks for a failed selection round as `defences.bulyan` does.
+Gram tile); every problem shares N, D and `users_count`.  `corrupted_count` (and `alie_rows`' `num_std`) is
+either one number for every problem or a host sequence of B values (list, tuple, NumPy array, CPU tensor), one
+per problem (C ABI `afl_defend_batched_each` / `afl_alie_batched_each`), so that a grid over the malicious
+share and z runs as one batch.  Nothing here synchronises the host except `bulyan`, which checks for a failed
+selection round as `defences.bulyan` does.
 
 The server's momentum step needs no batched form: `_device.momentum_step` on contiguous `[B, D]` weights,
 velocity and gradients is already the batched step (server.py:89-90 is element-wise).
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 from . import _native as nat
@@ -33,10 +37,39 @@ def _check(G: torch.Tensor):
     return B, N, D, ld, G.stride(0)
 
 
-def _defend(rule: str, G: torch.Tensor, users_count: int, corrupted_count: int, out=None, idx=None, sel=None):
+def _per_problem(x, B: int, name: str, dtype):
+    """None when x is one number for every problem, else its B per-problem values as a contiguous host array."""
+    if isinstance(x, torch.Tensor):
+        if x.dim() == 0:
+            return None
+        if x.is_cuda:
+            raise TypeError(f"{name}: per-problem values must be on the host (reading a CUDA tensor would synchronise)")
+        x = x.numpy()
+    if np.ndim(x) == 0:
+        return None
+    a = np.asarray(x)
+    if dtype == np.int32 and a.size and not np.issubdtype(a.dtype, np.integer):
+        raise TypeError(f"{name}: per-problem counts must be integers (got {a.dtype})")
+    if a.ndim != 1 or a.shape[0] != B:
+        raise ValueError(f"{name}: expected one value per problem ({B}), got shape {a.shape}")
+    return np.ascontiguousarray(a, dtype=dtype)
+
+
+def _defend(rule: str, G: torch.Tensor, users_count: int, corrupted_count, out=None, idx=None, sel=None):
     B, N, D, ld, bs = _check(G)
     L = nat.lib()
+    fs = _per_problem(corrupted_count, B, "corrupted_count", np.int32)
     with torch.cuda.device(G.device):
+        if fs is not None:
+            nbytes = L.afl_batched_each_workspace_bytes(rule.encode(), B, N, D, dtype_code(G))
+            ws = Workspace.get(G.device, "batched", nbytes)
+            nat.check(L.afl_defend_batched_each(rule.encode(), G.data_ptr(), B, bs, N, D, ld, dtype_code(G),
+                                                int(users_count), fs.ctypes.data,
+                                                None if out is None else out.data_ptr(),
+                                                None if idx is None else idx.data_ptr(),
+                                                None if sel is None else sel.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                _stream_ptr(G)))
+            return
         nbytes = L.afl_batched_workspace_bytes(rule.encode(), B, N, D, dtype_code(G))
         ws = Workspace.get(G.device, "batched", nbytes) if nbytes else None
         nat.check(L.afl_defend_batched(rule.encode(), G.data_ptr(), B, bs, N, D, ld, dtype_code(G), int(users_count),
@@ -47,8 +80,9 @@ def _defend(rule: str, G: torch.Tensor, users_count: int, corrupted_count: int, 
 
 
 def krum(users_grads, users_count, corrupted_count, return_index=False):
-    """Per problem defences.krum: the winning rows `G[arange(B), idx]` ([B, D], input dtype), or with
-    return_index the device int32 [B] indices (-1 where no user is eligible).  No host synchronisation."""
+    """Per problem defences.krum (corrupted_count: one int or B of them): the winning rows `G[arange(B), idx]`
+    ([B, D], input dtype), or with return_index the device int32 [B] indices (-1 where no user is eligible).
+    No host synchronisation."""
     B = users_grads.shape[0]
     idx = torch.empty(B, dtype=torch.int32, device=users_grads.device)
     _defend(DefenseTypes.Krum, users_grads, users_count, corrupted_count, idx=idx)
@@ -75,15 +109,24 @@ def no_defense(users_grads, users_count, corrupted_count):
 
 def bulyan(users_grads, users_count, corrupted_count, return_selection=False):
     """Per problem defences.bulyan: fp32 [B, D] and, with return_selection, the int32 [B, theta] selections.
-    Raises KeyError(-1) when any problem's last selection is -1 (a round found no eligible user), as
-    `defences.bulyan` does for one problem."""
-    assert users_count >= 4 * corrupted_count + 3
+    With one corrupted_count per problem the selections are [B, theta_max], theta_max = users_count - 2 min(f):
+    problem b's theta_b = users_count - 2 f_b rounds, then -2 ("no such round").  Raises KeyError(-1) when any
+    problem's last round is -1 (a round found no eligible user), as `defences.bulyan` does for one problem."""
     B, _, D = users_grads.shape
-    theta = users_count - 2 * corrupted_count
+    fs = _per_problem(corrupted_count, B, "corrupted_count", np.int32)
+    if fs is None:
+        assert users_count >= 4 * corrupted_count + 3
+        theta = users_count - 2 * corrupted_count
+    else:                                                # each problem's assert is checked by the call
+        theta = max(users_count - 2 * int(fs.min()), 1) if B else 1
     out = torch.empty((B, D), dtype=torch.float32, device=users_grads.device)
     sel = torch.empty((B, theta), dtype=torch.int32, device=users_grads.device)
-    _defend(DefenseTypes.Bulyan, users_grads, users_count, corrupted_count, out=out, sel=sel)
-    if bool((sel[:, -1] < 0).any()):                     # defences.py:66 `distances.pop(-1)`
+    _defend(DefenseTypes.Bulyan, users_grads, users_count, corrupted_count if fs is None else fs, out=out, sel=sel)
+    if fs is None:
+        last = sel[:, -1]
+    else:
+        last = sel.cpu()[torch.arange(B), torch.from_numpy(users_count - 2 * fs.astype(np.int64) - 1)]
+    if bool((last < 0).any()):                           # defences.py:66 `distances.pop(-1)`
         raise KeyError(-1)
     return (out, sel) if return_selection else out
 
@@ -97,7 +140,16 @@ def alie_rows(users_grads, corrupted_count, num_std):
     """Per problem malicious.Attack.attack_rows (DriftAttack): the malicious users are rows 0..f-1 of every
     problem.  Returns (crafted, mu, sigma), each fp32 [B, D] (mu is the unperturbed mean), and writes crafted
     = mu - num_std * sigma into those rows in place (fp32 directly; bf16 through a cast, as attack_rows does).
-    With num_std == 0 the rows are left alone, as attack_rows does.  None when corrupted_count <= 0."""
+    With num_std == 0 the rows are left alone, as attack_rows does.  None when corrupted_count <= 0.
+
+    corrupted_count and num_std may each be one number or B of them (host sequences).  Per problem, f_b <= N;
+    f_b = 0 leaves the problem's rows alone and its crafted, mu and sigma are NaN; z_b = 0 computes the
+    statistics (crafted = mu) and leaves the rows alone."""
+    B = users_grads.shape[0]
+    fs = _per_problem(corrupted_count, B, "corrupted_count", np.int32)
+    zs = _per_problem(num_std, B, "num_std", np.float64)
+    if fs is not None or zs is not None:
+        return _alie_rows_each(users_grads, corrupted_count if fs is None else fs, num_std if zs is None else zs)
     f = int(corrupted_count)
     if f <= 0:
         return None
@@ -113,4 +165,27 @@ def alie_rows(users_grads, corrupted_count, num_std):
                                              _stream_ptr(users_grads)))
     if write and bcast is None:
         users_grads[:, :f] = crafted[:, None, :].to(users_grads.dtype)
+    return crafted, mu, sigma
+
+
+def _alie_rows_each(users_grads, fs, zs):
+    B, N, D, ld, bs = _check(users_grads)
+    fs = np.ascontiguousarray(np.broadcast_to(np.asarray(fs, np.int32), (B,)))
+    zs = np.ascontiguousarray(np.broadcast_to(np.asarray(zs, np.float64), (B,)))
+    dev = users_grads.device
+    mu, sigma, crafted = (torch.empty((B, D), dtype=torch.float32, device=dev) for _ in range(3))
+    write = (fs > 0) & (zs != 0)
+    bcast = users_grads if write.any() and users_grads.dtype == torch.float32 else None
+    L = nat.lib()
+    with torch.cuda.device(dev):
+        nbytes = L.afl_batched_each_workspace_bytes(b"ALIE", B, N, D, dtype_code(users_grads))
+        ws = Workspace.get(dev, "batched_alie", nbytes)
+        nat.check(L.afl_alie_batched_each(users_grads.data_ptr(), B, bs, N, D, ld, dtype_code(users_grads),
+                                          fs.ctypes.data, zs.ctypes.data, mu.data_ptr(), sigma.data_ptr(),
+                                          crafted.data_ptr(), None if bcast is None else bcast.data_ptr(), bs, ld,
+                                          ws.data_ptr(), ws.numel(), _stream_ptr(users_grads)))
+    if write.any() and bcast is None:                    # bf16: rows r < f_b of the problems that write, via a cast
+        b_idx, r_idx = np.nonzero(write[:, None] & (np.arange(N)[None, :] < fs[:, None]))
+        b_idx, r_idx = (torch.from_numpy(x).pin_memory().to(dev, non_blocking=True) for x in (b_idx, r_idx))
+        users_grads[b_idx, r_idx] = crafted[b_idx].to(users_grads.dtype)
     return crafted, mu, sigma

@@ -52,6 +52,27 @@ static inline cudaError_t ensure_dyn_smem(K kernel, int bytes, int (&done)[kMaxD
 
 constexpr int kMaxWorld = 16;            // ranks of one peer-exchange context (csrc/xgpu.cu)
 
+// Trimmed-mean constants (csrc/trimmed_mean.cu, tmean::shape) of `n_rows` participating rows and a corrupted count.
+struct TmShape {
+  int n_rows;             // participating rows
+  int keep;               // effective number of kept devs (python slice semantics applied), >= 0
+  float med_density;      // 0.39894228 * n_rows (ranks per unit value at the centre of a unit Gaussian)
+  float key_q;            // Gaussian guess of the |dev| threshold in sigmas
+  float key_density;      // 2 * phi(key_q) * n_rows (ranks per unit |dev| at that threshold, unit sigma)
+};
+
+// One problem of a per-problem batched call (afl_defend_batched_each, afl_alie_batched_each): the values the single
+// call derives on the host from that problem's corrupted_count and z.  The table of `batch` rows sits at the start of
+// the caller's workspace; the kernels read row blockIdx.y (Bulyan's rounds: blockIdx.x) when handed a table.
+struct ProblemParams {
+  int f;                  // corrupted_count: Bulyan's first-round keep, ALIE's rows
+  int take;               // Krum: len(sorted(...)[:users_count - f])
+  int theta;              // Bulyan: users_count - 2f rounds
+  int write;              // ALIE: crafted is written over rows 0..f-1 (f > 0 and z != 0)
+  float z;                // ALIE: (float)z
+  TmShape tm;             // TrimmedMean: n rows and f; Bulyan's second stage: theta rows and 2f
+};
+
 // Arguments of the Krum kernel (csrc/select.cu).  The row of distances comes from `dist` (a caller's fp32 table) when
 // it is set, otherwise from the float64 d2 tables tab[0..world), summed in rank order; with world > 1 the kernel first
 // waits until `flags` reach `epoch` and reads the peers' tables through their mappings.
@@ -62,6 +83,7 @@ struct KrumParams {
   int world;
   const float* dist;
   int n, take;
+  const ProblemParams* each;              // per-problem take, or NULL: `take` for every problem
   float* score;                           // [n]
   unsigned int* done;                     // last-CTA counter: zero at launch, reset by the kernel
   int* idx_dev;

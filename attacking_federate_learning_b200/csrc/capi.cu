@@ -107,16 +107,18 @@ size_t workspace_bytes(int n, int batch);
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
                 void* ws, size_t ws_bytes, cudaStream_t stream);
 int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
-                     size_t ws_bytes, cudaStream_t stream, int batch = 1);
+                     size_t ws_bytes, cudaStream_t stream, int batch = 1, const ProblemParams* each = nullptr);
 int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out, void* ws, size_t ws_bytes,
-                  cudaStream_t stream, int batch = 1);
+                  cudaStream_t stream, int batch = 1, const ProblemParams* each = nullptr);
+int krum_take(int n, int users_count, int corrupted_count);
 }
 namespace tmean {
 int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
                  int corrupted_count, float* out, cudaStream_t stream);
 int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
                          int corrupted_count, float* out, int batch, int64_t g_batch, int ri_batch, int64_t out_batch,
-                         cudaStream_t stream);
+                         cudaStream_t stream, const ProblemParams* each = nullptr);
+TmShape shape(int n_rows, int corrupted_count);
 }
 namespace colstats {
 int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream);
@@ -126,7 +128,7 @@ int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float
          float* crafted_out, float* bcast, int64_t bcast_ld, cudaStream_t stream);
 int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
                  float* crafted_out, float* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
-                 int64_t bcast_batch, cudaStream_t stream);
+                 int64_t bcast_batch, cudaStream_t stream, const ProblemParams* each = nullptr);
 int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* idx_dev, float* out,
                cudaStream_t stream);
 int momentum_step(float* w, float* v, const float* g, int64_t d, float momentum, float lr, cudaStream_t stream);
@@ -565,6 +567,10 @@ static int alie_host(const float* const* rows, int f, int64_t d, double z, float
 // single call's.  Scratch per rule (the tables first, so that a caller can read them after the call):
 //   Krum   [d2: batch x n x n float64][gram workspace][selection workspace]
 //   Bulyan [d2: batch x n x n float64][dist: batch x n x n fp32][gram workspace][selection workspace]
+// The per-problem calls (*_each) take corrupted_count (and ALIE's z) per problem.  Their host arrays become one
+// ProblemParams row per problem, built here with the single call's own host code (krum_take, tmean::shape) and copied
+// to the start of the workspace; the scalar call's layout follows it.  The scalar calls pass no table and run as they
+// always have.
 // ------------------------------------------------------------------------------------------------
 constexpr int kBatchMaxClients = 128;            // one Gram tile
 constexpr int kBatchMax = 65535;                 // grid y / z limit
@@ -579,7 +585,7 @@ static BatchedRule batched_rule(const char* rule) {
   return B_BAD;
 }
 
-// Shape checks shared by afl_defend_batched and afl_alie_batched, before any CUDA call.
+// Shape checks shared by the batched calls, before any CUDA call.
 static int check_batch(const char* who, const void* G, int batch, int64_t batch_stride, int rows, int64_t d, int64_t ld,
                        int dtype) {
   if (!G || rows < 1 || d < 1 || ld < d) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
@@ -598,46 +604,101 @@ static int check_batch(const char* who, const void* G, int batch, int64_t batch_
   return AFL_OK;
 }
 
+// Per-problem counts: non-NULL, each in [0, f_cap]; their range in *fmin, *fmax.
+static int check_counts(const char* who, const int* fs, int batch, int f_cap, int* fmin, int* fmax) {
+  if (!fs) { set_error("%s: the per-problem corrupted counts are NULL", who); return AFL_ERR_BAD_ARG; }
+  *fmin = fs[0]; *fmax = fs[0];
+  for (int b = 0; b < batch; ++b) {
+    if (fs[b] < 0 || fs[b] > f_cap) {
+      set_error("%s: corrupted count %d of problem %d is outside [0, %d]", who, fs[b], b, f_cap);
+      return AFL_ERR_BAD_ARG;
+    }
+    *fmin = fs[b] < *fmin ? fs[b] : *fmin;
+    *fmax = fs[b] > *fmax ? fs[b] : *fmax;
+  }
+  return AFL_OK;
+}
+
+static size_t table_bytes(int batch) { return align_up(static_cast<size_t>(batch) * sizeof(ProblemParams), 256); }
+
+// The rule's scratch after the table (0: the rule needs none).
 static size_t batched_ws_parts(BatchedRule r, int batch, int n, int64_t d, int dtype, size_t* gram_ws, size_t* tabs) {
+  *gram_ws = 0; *tabs = 0;
+  if (r != B_KRUM && r != B_BULYAN) return 0;
   const size_t nn = static_cast<size_t>(batch) * n * n;
   *gram_ws = align_up(gram::workspace_bytes(n, d, dtype, 0, batch), 256);
   *tabs = align_up(nn * 8, 256) + (r == B_BULYAN ? align_up(nn * 4, 256) : 0);
   return *gram_ws + *tabs + select::workspace_bytes(n, batch);
 }
 
+// Workspace check, then the table built by `row(b, ProblemParams&)` copied to the workspace start (pageable source:
+// the copy has taken the values when cudaMemcpyAsync returns).  Returns the device table in *table.
+template <typename Row>
+static int upload_table(const char* who, int batch, void* ws, size_t ws_bytes, size_t need, cudaStream_t stream,
+                        Row row, const ProblemParams** table) {
+  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
+    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
+    return AFL_ERR_WORKSPACE;
+  }
+  std::vector<ProblemParams> host(static_cast<size_t>(batch));
+  for (int b = 0; b < batch; ++b) row(b, host[b]);
+  AFL_CUDA(cudaMemcpyAsync(ws, host.data(), host.size() * sizeof(ProblemParams), cudaMemcpyHostToDevice, stream));
+  *table = static_cast<const ProblemParams*>(ws);
+  return AFL_OK;
+}
+
+// fs == NULL: every problem has corrupted_count f (afl_defend_batched).  Otherwise problem b has fs[b]
+// (afl_defend_batched_each): f is unused, the preconditions hold per problem, and the workspace starts with the table.
 static int defend_batched(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
-                          int dtype, int users_count, int f, float* out, int* idx_out, int* sel_out, void* ws,
-                          size_t ws_bytes, cudaStream_t stream) {
+                          int dtype, int users_count, int f, const int* fs, float* out, int* idx_out, int* sel_out,
+                          void* ws, size_t ws_bytes, cudaStream_t stream) {
+  const char* who = fs ? "afl_defend_batched_each" : "afl_defend_batched";
   const BatchedRule r = batched_rule(rule);
-  if (r == B_BAD) { set_error("afl_defend_batched: unknown rule '%s'", rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
-  int rc = check_batch("afl_defend_batched", G, batch, batch_stride, n, d, ld, dtype);
+  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
   if (rc) return rc;
-  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out) || f < 0) {
-    set_error("afl_defend_batched: %s needs %s", rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
+  int fmin = f, fmax = f;
+  if (fs && (rc = check_counts(who, fs, batch, INT32_MAX / 4, &fmin, &fmax))) return rc;
+  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out) || fmin < 0) {
+    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
     return AFL_ERR_BAD_ARG;
   }
-  if (r == B_KRUM && users_count < 2 * f + 1) {         // the reference's assert (defences.py:24-25)
-    set_error("krum: users_count >= 2*corrupted_count + 1 violated (%d, %d)", users_count, f);
-    return AFL_ERR_PRECONDITION;
-  }
-  if (r == B_BULYAN && users_count < 4 * f + 3) {       // the reference's assert (defences.py:56)
-    set_error("bulyan: users_count >= 4*corrupted_count + 3 violated (%d, %d)", users_count, f);
+  // the reference's asserts (defences.py:24-25, 56), per problem
+  const int need_f = r == B_KRUM ? 2 * fmax + 1 : r == B_BULYAN ? 4 * fmax + 3 : 0;
+  if (users_count < need_f) {
+    const char* what = r == B_KRUM ? "krum: users_count >= 2*corrupted_count + 1" : "bulyan: users_count >= 4*corrupted_count + 3";
+    int b = 0;
+    while (fs && fs[b] != fmax) ++b;
+    if (fs) set_error("%s violated (%d, %d) in problem %d", what, users_count, fmax, b);
+    else set_error("%s violated (%d, %d)", what, users_count, f);
     return AFL_ERR_PRECONDITION;
   }
   if (r == B_BULYAN && users_count != n) {
-    set_error("afl_defend_batched: Bulyan's users_count (%d) must equal the number of rows (%d)", users_count, n);
+    set_error("%s: Bulyan's users_count (%d) must equal the number of rows (%d)", who, users_count, n);
     return AFL_ERR_UNSUPPORTED;
+  }
+  size_t gram_ws = 0, tabs = 0;
+  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  const ProblemParams* each = nullptr;
+  uint8_t* p = static_cast<uint8_t*>(ws);
+  if (fs && r != B_MEAN) {                              // NoDefense ignores f, as the reference does
+    rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch) + rule_ws, stream, [&](int b, ProblemParams& q) {
+      q.f = fs[b];
+      q.take = select::krum_take(n, users_count, fs[b]);
+      q.theta = users_count - 2 * fs[b];
+      q.tm = r == B_BULYAN ? tmean::shape(q.theta, 2 * fs[b]) : tmean::shape(n, fs[b]);
+    }, &each);
+    if (rc) return rc;
+    p += table_bytes(batch);
+    ws_bytes -= table_bytes(batch);
   }
   if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream);
   if (r == B_TM)
-    return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, f, out, batch, batch_stride, 0, d, stream);
-  size_t gram_ws = 0, tabs = 0;
-  const size_t need = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
-  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
-    set_error("afl_defend_batched: workspace too small or misaligned (%zu < %zu)", ws_bytes, need);
+    return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, fmin, out, batch, batch_stride, 0, d, stream, each);
+  if (ws_bytes < rule_ws || !p || reinterpret_cast<uintptr_t>(p) % 256 != 0) {
+    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, rule_ws);
     return AFL_ERR_WORKSPACE;
   }
-  uint8_t* p = static_cast<uint8_t*>(ws);
   const size_t nn = static_cast<size_t>(batch) * n * n;
   double* d2 = reinterpret_cast<double*>(p);
   float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
@@ -645,11 +706,45 @@ static int defend_batched(const char* rule, const void* G, int batch, int64_t ba
   const size_t sel_ws_bytes = ws_bytes - tabs - gram_ws;
   rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream);
   if (rc) return rc;
-  if (r == B_KRUM) return select::krum_from_sqdist(d2, n, users_count, f, idx_out, sel_ws, sel_ws_bytes, stream, batch);
-  const int theta = users_count - 2 * f;
+  if (r == B_KRUM)
+    return select::krum_from_sqdist(d2, n, users_count, fmin, idx_out, sel_ws, sel_ws_bytes, stream, batch, each);
+  const int theta = users_count - 2 * fmin;             // the row length of sel_out
   rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
-  rc = select::bulyan_select(dist, n, users_count, f, sel_out, sel_ws, sel_ws_bytes, stream, batch); if (rc) return rc;
-  return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, theta, 2 * f, out, batch, batch_stride, theta, d, stream);
+  rc = select::bulyan_select(dist, n, users_count, fmin, sel_out, sel_ws, sel_ws_bytes, stream, batch, each);
+  if (rc) return rc;
+  return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, theta, 2 * fmin, out, batch, batch_stride, theta, d,
+                                     stream, each);
+}
+
+// fs == NULL: rows 0..f-1 and z in every problem of f-row problems (afl_alie_batched).  Otherwise problem b has n rows of
+// which fs[b] are malicious, and its own z (afl_alie_batched_each); the workspace holds the table.
+static int alie_batched(const char* who, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                        int dtype, int f, double z, const int* fs, const double* zs, float* mu_out, float* sigma_out,
+                        float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* ws,
+                        size_t ws_bytes, cudaStream_t stream) {
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
+  if (rc) return rc;
+  int fmin = f, fmax = f;
+  if (fs) {
+    if (!zs) { set_error("%s: the per-problem attack strengths are NULL", who); return AFL_ERR_BAD_ARG; }
+    if ((rc = check_counts(who, fs, batch, n, &fmin, &fmax))) return rc;
+  }
+  if (bcast_rows && fmax > 0 &&
+      (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(fmax - 1) * bcast_ld + d))) {
+    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  const ProblemParams* each = nullptr;
+  if (fs) {
+    rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch), stream, [&](int b, ProblemParams& q) {
+      q.f = fs[b];
+      q.z = static_cast<float>(zs[b]);
+      q.write = fs[b] > 0 && zs[b] != 0.0;             // malicious.py:20-21: z == 0 computes the statistics only
+    }, &each);
+    if (rc) return rc;
+  }
+  return colstats::alie_batched(G, fmax, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast_rows, bcast_ld, batch,
+                                batch_stride, d, bcast_batch_stride, stream, each);
 }
 
 }  // namespace afl
@@ -773,24 +868,48 @@ size_t afl_batched_workspace_bytes(const char* rule, int batch, int n, int64_t d
   return batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
 }
 
+size_t afl_batched_each_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
+  const bool alie = rule && !strcmp(rule, "ALIE");
+  const BatchedRule r = batched_rule(rule);
+  if ((r == B_BAD && !alie) || batch < 1 || batch > kBatchMax || n < 1 || n > kBatchMaxClients || d < 1) return 0;
+  size_t gram_ws = 0, tabs = 0;
+  return table_bytes(batch) + batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+}
+
 int afl_defend_batched(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
                        int dtype, int users_count, int corrupted_count, float* out, int* idx_out, int* sel_out,
                        void* workspace, size_t workspace_bytes, void* stream) {
-  return defend_batched(rule, G, batch, batch_stride, n, d, ld, dtype, users_count, corrupted_count, out, idx_out, sel_out,
-                        workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  return defend_batched(rule, G, batch, batch_stride, n, d, ld, dtype, users_count, corrupted_count, nullptr, out, idx_out,
+                        sel_out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int afl_defend_batched_each(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                            int64_t ld, int dtype, int users_count, const int* corrupted_counts, float* out, int* idx_out,
+                            int* sel_out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!corrupted_counts) {
+    set_error("afl_defend_batched_each: the per-problem corrupted counts are NULL");
+    return AFL_ERR_BAD_ARG;
+  }
+  return defend_batched(rule, G, batch, batch_stride, n, d, ld, dtype, users_count, 0, corrupted_counts, out, idx_out,
+                        sel_out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 int afl_alie_batched(const void* G_mal, int batch, int64_t batch_stride, int f, int64_t d, int64_t ld, int dtype, double z,
                      float* mu_out, float* sigma_out, float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride,
                      int64_t bcast_ld, void* stream) {
-  int rc = check_batch("afl_alie_batched", G_mal, batch, batch_stride, f, d, ld, dtype);
-  if (rc) return rc;
-  if (bcast_rows && (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(f - 1) * bcast_ld + d))) {
-    set_error("afl_alie_batched: bcast_ld / bcast_batch_stride make the written rows overlap");
-    return AFL_ERR_BAD_ARG;
-  }
-  return colstats::alie_batched(G_mal, f, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast_rows, bcast_ld, batch,
-                                batch_stride, d, bcast_batch_stride, static_cast<cudaStream_t>(stream));
+  return alie_batched("afl_alie_batched", G_mal, batch, batch_stride, f, d, ld, dtype, f, z, nullptr, nullptr, mu_out,
+                      sigma_out, crafted_out, bcast_rows, bcast_batch_stride, bcast_ld, nullptr, 0,
+                      static_cast<cudaStream_t>(stream));
+}
+
+int afl_alie_batched_each(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                          const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
+                          float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  if (!f) { set_error("afl_alie_batched_each: the per-problem corrupted counts are NULL"); return AFL_ERR_BAD_ARG; }
+  return alie_batched("afl_alie_batched_each", G, batch, batch_stride, n, d, ld, dtype, 0, 0.0, f, z, mu_out, sigma_out,
+                      crafted_out, bcast_rows, bcast_batch_stride, bcast_ld, workspace, workspace_bytes,
+                      static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -111,13 +111,20 @@ mean_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, float* __rest
 // E[x^2] - E[x]^2 is accurate even when one client is orders of magnitude larger than the column's sigma (the
 // round-1 version shifted by the first row in fp32 and lost ~1e-5 relative there).  sigma = sqrt(population
 // variance); crafted = mu - z*sigma with the same two fp32 roundings as `grads_mean[:] -= num_std * grads_stdev[:]`.
+// With a table (each != NULL) problem b uses its own f, z and write flag; f = 0 reads and writes no row and gives NaN
+// statistics (the reference returns before computing any, malicious.py:11-12).
 template <typename T, int VEC, bool COHERENT>
 __global__ void __launch_bounds__(kBlock)
 alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict__ mu_out,
             float* __restrict__ sigma_out, float* __restrict__ crafted_out, float* bcast, int64_t bcast_ld,
-            int64_t g_batch, int64_t out_batch, int64_t bcast_batch) {
+            int64_t g_batch, int64_t out_batch, int64_t bcast_batch, const ProblemParams* __restrict__ each) {
   const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * VEC;
   if (c0 >= d) return;
+  if (each) {
+    const ProblemParams& q = each[blockIdx.y];
+    f = q.f; z = q.z;
+    if (!q.write) bcast = nullptr;
+  }
   G += blockIdx.y * g_batch;
   const T* p = G + c0;
   double s1[VEC], s2[VEC];
@@ -153,7 +160,7 @@ alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict
   for (int k = 0; k < VEC; ++k) {
     const double m = s1[k] * inv;
     double var = fma(-m, m, s2[k] * inv);
-    var = var > 0.0 ? var : 0.0;
+    var = var > 0.0 ? var : (f > 0 ? 0.0 : m);      // f = 0: m is NaN
     const float mu = static_cast<float>(m);
     const float sigma = static_cast<float>(sqrt(var));
     crafted[k] = __fsub_rn(mu, __fmul_rn(z, sigma));
@@ -257,11 +264,12 @@ int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cud
   return mean_batched(G, n, d, ld, dtype, out, 1, 0, 0, stream);
 }
 
-// `batch` problems: G + b * g_batch; mu/sigma/crafted + b * out_batch; bcast + b * bcast_batch
+// `batch` problems: G + b * g_batch; mu/sigma/crafted + b * out_batch; bcast + b * bcast_batch.  each (device, may be
+// NULL): per-problem f, z and write flag, f then being the largest problem's (0 allowed).
 int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
                  float* crafted_out, float* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
-                 int64_t bcast_batch, cudaStream_t stream) {
-  if (!G || f < 1 || d < 1 || ld < d || (bcast && bcast_ld < d)) { set_error("afl_alie: bad argument"); return AFL_ERR_BAD_ARG; }
+                 int64_t bcast_batch, cudaStream_t stream, const ProblemParams* each) {
+  if (!G || f < (each ? 0 : 1) || d < 1 || ld < d || (bcast && bcast_ld < d)) { set_error("afl_alie: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_alie: dtype"); return AFL_ERR_UNSUPPORTED; }
   const bool v = vec_ok(G, ld, dtype, batch, g_batch);
   const int vec = v ? (dtype == AFL_F32 ? 4 : 8) : 1;
@@ -273,8 +281,8 @@ int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double 
   const int64_t last = static_cast<int64_t>(batch - 1);
   const uintptr_t g0 = reinterpret_cast<uintptr_t>(G), g1 = g0 + static_cast<uintptr_t>((last * g_batch + static_cast<int64_t>(f - 1) * ld + d) * (dtype == AFL_F32 ? 4 : 2));
   const uintptr_t b0 = reinterpret_cast<uintptr_t>(bcast), b1 = b0 + static_cast<uintptr_t>((last * bcast_batch + static_cast<int64_t>(f - 1) * bcast_ld + d) * 4);
-  const bool coh = bcast && b0 < g1 && g0 < b1;
-#define AFL_ALIE_LAUNCH(T, V, C) alie_kernel<T, V, C><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), f, d, ld, zf, mu_out, sigma_out, crafted_out, bcast, bcast_ld, g_batch, out_batch, bcast_batch)
+  const bool coh = bcast && f > 0 && b0 < g1 && g0 < b1;
+#define AFL_ALIE_LAUNCH(T, V, C) alie_kernel<T, V, C><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), f, d, ld, zf, mu_out, sigma_out, crafted_out, bcast, bcast_ld, g_batch, out_batch, bcast_batch, each)
   if (dtype == AFL_F32) {
     if (v) { if (coh) AFL_ALIE_LAUNCH(float, 4, true); else AFL_ALIE_LAUNCH(float, 4, false); }
     else { if (coh) AFL_ALIE_LAUNCH(float, 1, true); else AFL_ALIE_LAUNCH(float, 1, false); }
@@ -289,7 +297,7 @@ int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double 
 
 int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
          float* crafted_out, float* bcast, int64_t bcast_ld, cudaStream_t stream) {
-  return alie_batched(G, f, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast, bcast_ld, 1, 0, 0, 0, stream);
+  return alie_batched(G, f, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast, bcast_ld, 1, 0, 0, 0, stream, nullptr);
 }
 
 int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* idx_dev, float* out,

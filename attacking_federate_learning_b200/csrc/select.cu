@@ -1,6 +1,8 @@
 // Krum (defences.py:23-42) and Bulyan's selection loop (defences.py:57-68) on an n x n distance table that is small
 // enough (<= 64 MB of fp32 at n = 4096) to live in L2.  A batch of same-shape problems (consecutive tables) adds the
-// problem to the grid: y for krum_tail_kernel and row_sort_kernel, x for bulyan_rounds_kernel.
+// problem to the grid: y for krum_tail_kernel and row_sort_kernel, x for bulyan_rounds_kernel.  A per-problem call
+// (afl_defend_batched_each) also hands krum_tail_kernel and bulyan_rounds_kernel its ProblemParams table: each problem
+// then reads its own take, or its own f and theta, instead of the scalar arguments.
 //
 //   krum_tail_kernel     one CTA per user u: u's n-1 distances -> bitonic sort in shared memory -> ascending sequential
 //                        fp32 sum of the `take` smallest (defences.py:33-34) -> score[u]; the last CTA to finish does the
@@ -157,7 +159,8 @@ krum_tail_kernel(const KrumParams p) {
   block_bitonic_sort(keys, P);
   if (threadIdx.x == 0) {
     float s = 0.f;                                                       // Python: sum() starts at int 0; ascending fp32 adds
-    for (int pos = 0; pos < p.take; ++pos) s = s + krum_value<kSrc>(p, off, u, keys[pos]);
+    const int take = p.each ? p.each[b].take : p.take;
+    for (int pos = 0; pos < take; ++pos) s = s + krum_value<kSrc>(p, off, u, keys[pos]);
     score[u] = s;
     __threadfence();
     s_last = (atomicAdd(p.done + b, 1u) == static_cast<unsigned>(n - 1)) ? 1 : 0;
@@ -181,9 +184,14 @@ krum_tail_kernel(const KrumParams p) {
   }
 }
 
+// Krum's score length for n clients: len(sorted(errors)[:users_count - corrupted_count]) over n - 1 distances.
+int krum_take(int n, int users_count, int corrupted_count) {
+  return python_slice_take(users_count - corrupted_count, n - 1);
+}
+
 // Fills p.take and launches the kernel for the row source p selects, grid (n, batch).  p.done[0 .. batch) must be zero.
 int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream, int batch) {
-  p.take = python_slice_take(users_count - corrupted_count, p.n - 1);
+  p.take = krum_take(p.n, users_count, corrupted_count);
   int P = 1; while (P < p.n) P <<= 1;
   {
     ProfScope ps("krum_tail", stream);
@@ -226,14 +234,20 @@ row_sort_kernel(const float* __restrict__ dist, int n, SortWs w) {
 constexpr int kRowsPerThread = kMaxN / 1024;
 
 __global__ void __launch_bounds__(1024, 1)
-bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, SortWs w, int* __restrict__ sel_out) {
+bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, SortWs w, int* __restrict__ sel_out,
+                     const ProblemParams* __restrict__ each) {
   __shared__ uint8_t alive[kMaxN];
   __shared__ int s_winner;
   const size_t off = static_cast<size_t>(blockIdx.x) * n * n;           // one CTA per problem
   dist += off; w.sval += off; w.sidx += off; w.rank += off;
-  sel_out += static_cast<size_t>(blockIdx.x) * theta;
+  sel_out += static_cast<size_t>(blockIdx.x) * theta;                    // with a table: theta = the longest problem's
 
   const int tid = threadIdx.x;
+  if (each) {                                                            // this problem's f and rounds; -2: no such round
+    const int theta_b = each[blockIdx.x].theta;
+    for (int r = theta_b + tid; r < theta; r += 1024) sel_out[r] = -2;
+    f = each[blockIdx.x].f; theta = theta_b;
+  }
   double score[kRowsPerThread];
   int bptr[kRowsPerThread];
 
@@ -332,18 +346,19 @@ int krum_select(const float* dist, int n, int users_count, int corrupted_count, 
   return krum_on_workspace(p, 1, users_count, corrupted_count, scores_out, ws, ws_bytes, stream);
 }
 
-// d2: batch consecutive n x n tables; idx_out[batch]
+// d2: batch consecutive n x n tables; idx_out[batch]; each (device, may be NULL): per-problem take
 int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
-                     size_t ws_bytes, cudaStream_t stream, int batch) {
+                     size_t ws_bytes, cudaStream_t stream, int batch, const ProblemParams* each) {
   if (!d2 || !idx_out || n < 1) { set_error("afl_krum_from_sqdist: bad argument"); return AFL_ERR_BAD_ARG; }
   KrumParams p{};
-  p.tab[0] = d2; p.world = 1; p.n = n; p.idx_dev = idx_out;
+  p.tab[0] = d2; p.world = 1; p.n = n; p.idx_dev = idx_out; p.each = each;
   return krum_on_workspace(p, batch, users_count, corrupted_count, nullptr, ws, ws_bytes, stream);
 }
 
-// dist: batch consecutive n x n tables; sel_out[batch][theta]
+// dist: batch consecutive n x n tables; sel_out[batch][theta], theta = users_count - 2f.  each (device, may be NULL):
+// per-problem f and theta; f is then the smallest problem's, so that every row of sel_out holds its problem's rounds.
 int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out, void* ws, size_t ws_bytes,
-                  cudaStream_t stream, int batch) {
+                  cudaStream_t stream, int batch, const ProblemParams* each) {
   if (!dist || !sel_out || n < 1 || f < 0) { set_error("afl_bulyan_select: bad argument"); return AFL_ERR_BAD_ARG; }
   if (users_count < 4 * f + 3) {
     set_error("bulyan: users_count >= 4*corrupted_count + 3 violated (%d, %d)", users_count, f);
@@ -364,7 +379,7 @@ int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out
   }
   AFL_LAUNCH_CHECK("row_sort_kernel");
   ProfScope ps("bulyan_rounds", stream);
-  bulyan_rounds_kernel<<<batch, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out);
+  bulyan_rounds_kernel<<<batch, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out, each);
   AFL_LAUNCH_CHECK("bulyan_rounds_kernel");
   return AFL_OK;
 }

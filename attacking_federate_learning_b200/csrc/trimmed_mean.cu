@@ -25,6 +25,9 @@
 //     the keep boundary cuts (ALIE's f identical rows, bf16 value collisions) is resolved in row order with ballots on
 //     the register-resident column (tie_sum).
 //   * More than 1024 rows: trimmed_mean_large_kernel (shared-memory strip, bisection on the integer image of the keys).
+//   * A batch (grid y) may carry a ProblemParams table: problem b then has its own participating rows, keep and pivot
+//     constants (tm).  Batches have n <= 128 rows, so only S = 4 has instances that read it (EACH); rows past a
+//     problem's n_rows are staged as +inf like the rows past n_rows of a single call.
 #include "afl_common.cuh"
 
 namespace afl {
@@ -40,14 +43,11 @@ struct Params {
   const int* row_index;   // may be null
   float* out;
   int64_t d, ld;
-  int n_rows;             // participating rows
   int n_total;            // rows of G (bounds for row_index)
-  int keep;               // effective number of kept devs (python slice semantics applied), >= 0
+  TmShape tm;             // participating rows, kept devs and the pivot model's constants
+  const ProblemParams* each;    // per-problem tm (trimmed_mean_kernel<4, *> only), or NULL: `tm` for every problem
   int64_t g_batch, out_batch;   // problem blockIdx.y: G, out and row_index advance by these (elements)
   int ri_batch;
-  float med_density;      // 0.39894228 * n      (ranks per unit value at the centre of a unit Gaussian)
-  float key_q;            // Gaussian guess of the |dev| threshold in sigmas
-  float key_density;      // 2 * phi(key_q) * n  (ranks per unit |dev| at that threshold, unit sigma)
   int vec_ok;
 };
 
@@ -399,7 +399,7 @@ __device__ __forceinline__ bool select_fast(const float (&v)[S], const ColRef& c
 // slot r>>5 of lane r&31; slot-group m = slot>>2 and the XOR-ed slot position are compile-time
 // functions of `it`, so every store below has an immediate offset from one of two per-thread bases.
 template <int S, bool BF16>
-__device__ __forceinline__ void stage_tile(const Params& P, uint32_t* tile, int64_t col0) {
+__device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, uint32_t* tile, int64_t col0) {
   constexpr int kGroups = S / 4;
   const int tid = threadIdx.x;
   const int es = BF16 ? 2 : 4;
@@ -419,7 +419,7 @@ __device__ __forceinline__ void stage_tile(const Params& P, uint32_t* tile, int6
     // instructions per load so that the whole path stays a few hundred bytes of code
     // (branch-free: rows past n_rows re-read the last row and are replaced by the sentinel at the store)
     int gr[kIters];
-    const int last = P.n_rows - 1;
+    const int last = sh.n_rows - 1;
     if (row_index) {
 #pragma unroll
       for (int it = 0; it < kIters; ++it) gr[it] = row_index[min(it * 64 + rowq, last)];
@@ -452,7 +452,7 @@ __device__ __forceinline__ void stage_tile(const Params& P, uint32_t* tile, int6
   for (int it = 0; it < kIters; ++it) {
     const int r = it * 64 + rowq;
     uint32_t w[4] = {sentinel, sentinel, sentinel, sentinel};
-    if (r < P.n_rows) {
+    if (r < sh.n_rows) {
       int gr = row_index ? row_index[r] : r;
       gr = gr < 0 ? gr + P.n_total : gr;
       const uint8_t* src = base + (static_cast<int64_t>(gr) * P.ld + c) * es;
@@ -480,7 +480,7 @@ __device__ __forceinline__ void stage_tile(const Params& P, uint32_t* tile, int6
 // ---------------- general per-column path (any data): one warp, one column ----------------
 // `half` selects the bf16 column inside the 32-bit word-column cw (ignored for fp32).
 template <int S, bool BF16>
-__device__ __forceinline__ float general_column_impl(const Params& P, const uint32_t* tile, int cw, int half,
+__device__ __forceinline__ float general_column_impl(const TmShape& P, const uint32_t* tile, int cw, int half,
                                                      uint32_t* scratch, int lane) {
   constexpr int kGroups = S / 4;
   const int n = P.n_rows;
@@ -570,8 +570,11 @@ __device__ __forceinline__ float general_column_impl(const Params& P, const uint
 constexpr int kScratchWords = 96;              // per warp: dense candidate list [32] (fast path) / (key,row) u64[32] + payload[32] (general path)
 
 // S <= 20 (up to 640 rows: Bulyan's second stage at N = 500 and N = 1000) leaves room for four CTAs per SM in shared memory; ask
-// the compiler for 64 registers there (resident warps are what hides the shuffle chains of the scans and sorts)
-template <int S, bool BF16>
+// the compiler for 64 registers there (resident warps are what hides the shuffle chains of the scans and sorts).
+// EACH: problem blockIdx.y's constants come from the per-problem table P.each (batches only, so S = 4).  A separate instance:
+// holding them in registers instead of reading the constant bank takes the fp32 kernel from 48 to 54 registers, which
+// would cost the single calls a fifth CTA per SM.
+template <int S, bool BF16, bool EACH>
 __global__ void __launch_bounds__(kThreads, (S <= 20 ? 4 : 3))      // (S = 24 fits 4 CTAs in shared memory too, but the fp32 instance spills at 64 registers)
 trimmed_mean_kernel(const Params P) {
   extern __shared__ __align__(1024) uint32_t tile[];     // [16 word-cols][S/4 groups][32 lanes][4 slots] + scratch
@@ -579,7 +582,9 @@ trimmed_mean_kernel(const Params P) {
   const int tid = threadIdx.x, warp = tid >> 5;
   const int cols_per_tile = BF16 ? 32 : 16;
   const int64_t col0 = static_cast<int64_t>(blockIdx.x) * cols_per_tile;
-  stage_tile<S, BF16>(P, tile, col0);
+  TmShape sh = P.tm;
+  if constexpr (EACH) sh = P.each[blockIdx.y].tm;
+  stage_tile<S, BF16>(P, sh, tile, col0);
   // read once, after staging: `volatile` keeps ptxas from re-reading the special register (S2R, ~50 cycles of
   // latency) in front of every scan and sort of the per-column code to save one register
   int lane = tid & 31, warp_o = warp;
@@ -595,7 +600,7 @@ trimmed_mean_kernel(const Params P) {
     for (int half = 0; half < (BF16 ? 2 : 1); ++half) {
       const int64_t col = col0 + (BF16 ? 2 * cw + half : cw);
       if (col >= P.d) break;                         // warp-uniform
-      const float res = general_column_impl<S, BF16>(P, tile, cw, half, scratch, lane);
+      const float res = general_column_impl<S, BF16>(sh, tile, cw, half, scratch, lane);
       if (lane == 0) P.out[static_cast<int64_t>(blockIdx.y) * P.out_batch + col] = res;
     }
   }
@@ -640,7 +645,7 @@ __global__ void __launch_bounds__(256, 1)
 trimmed_mean_large_kernel(const Params P, int bf16) {
   extern __shared__ __align__(16) uint32_t strip[];        // [n_rows][4 words]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = P.n_rows;
+  const int n = P.tm.n_rows;
   const int es = bf16 ? 2 : 4;
   const int cols = bf16 ? 8 : 4;
   const int64_t col0 = static_cast<int64_t>(blockIdx.x) * cols;
@@ -673,10 +678,10 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
     const float b = (n & 1) ? a : from_ord_bits(warp_kth_key<0>(strip, n, cis, bf16 != 0, 0.f, n >> 1, lane));
     const float med = (n & 1) ? a : __fdiv_rn(__fadd_rn(a, b), 2.0f);
     float res;
-    if (P.keep <= 0) {
+    if (P.tm.keep <= 0) {
       res = __int_as_float(0x7fc00000);
     } else {
-      const uint32_t To = warp_kth_key<1>(strip, n, cis, bf16 != 0, med, P.keep - 1, lane);   // threshold key (as ord bits)
+      const uint32_t To = warp_kth_key<1>(strip, n, cis, bf16 != 0, med, P.tm.keep - 1, lane);   // threshold key (as ord bits)
       // sum of the devs strictly below the threshold, then the first `need` of the tie group in row order
       float part = 0.f;
       int below = 0;
@@ -687,7 +692,7 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
         below += lt ? 1 : 0;
       }
       below = __reduce_add_sync(0xffffffffu, below);
-      int need = P.keep - below;
+      int need = P.tm.keep - below;
       for (int r0 = 0; r0 < n && need > 0; r0 += 32) {       // rows in order: r0 .. r0+31 <-> lanes 0..31
         const int r = r0 + lane;
         float dv = 0.f;
@@ -698,7 +703,7 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
         need -= __popc(m);
       }
       const float total = warp_sum(part);
-      res = __fadd_rn(__fdiv_rn(total, static_cast<float>(P.keep)), med);
+      res = __fadd_rn(__fdiv_rn(total, static_cast<float>(P.tm.keep)), med);
     }
     if (lane == 0) P.out[static_cast<int64_t>(blockIdx.y) * P.out_batch + col] = res;
   }
@@ -736,38 +741,48 @@ static int launch(const Params& P, int dtype, int batch, cudaStream_t stream) {
   const int cols = dtype == AFL_BF16 ? 32 : 16;
   const dim3 grid(static_cast<unsigned>(ceil_div64(P.d, cols)), batch);
   ProfScope ps("trimmed_mean", stream);
-  if (dtype == AFL_BF16) {
-    AFL_CUDA(cudaFuncSetAttribute(trimmed_mean_kernel<S, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    trimmed_mean_kernel<S, true><<<grid, kThreads, smem, stream>>>(P);
-  } else {
-    AFL_CUDA(cudaFuncSetAttribute(trimmed_mean_kernel<S, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    trimmed_mean_kernel<S, false><<<grid, kThreads, smem, stream>>>(P);
+  auto go = [&](auto kernel) -> int {
+    AFL_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    kernel<<<grid, kThreads, smem, stream>>>(P);
+    AFL_LAUNCH_CHECK("trimmed_mean_kernel");
+    return AFL_OK;
+  };
+  if constexpr (S == 4) {
+    if (P.each) return dtype == AFL_BF16 ? go(trimmed_mean_kernel<S, true, true>) : go(trimmed_mean_kernel<S, false, true>);
   }
-  AFL_LAUNCH_CHECK("trimmed_mean_kernel");
-  return AFL_OK;
+  return dtype == AFL_BF16 ? go(trimmed_mean_kernel<S, true, false>) : go(trimmed_mean_kernel<S, false, false>);
+}
+
+// The constants of n_rows participating rows and corrupted_count: number_to_consider = rows - f - 1 with Python slice
+// semantics for sorted(...)[:k] (defences.py:45,50), and the pivot model's Gaussian guesses.
+TmShape shape(int n_rows, int corrupted_count) {
+  TmShape t{};
+  const int k = n_rows - corrupted_count - 1;
+  t.n_rows = n_rows;
+  t.keep = k >= 0 ? (k < n_rows ? k : n_rows) : (n_rows + k > 0 ? n_rows + k : 0);
+  t.med_density = 0.3989422804f * static_cast<float>(n_rows);
+  const double frac = t.keep > 0 ? (static_cast<double>(t.keep) - 0.5) / n_rows : 0.5;
+  const double q = norm_ppf(0.5 * (1.0 + (frac < 0.999999 ? frac : 0.999999)));
+  t.key_q = static_cast<float>(q);
+  t.key_density = static_cast<float>(2.0 * 0.3989422804014327 * exp(-0.5 * q * q) * n_rows);
+  return t;
 }
 
 // `batch` problems (grid y): problem b reads G + b * g_batch and row_index + b * ri_batch, and writes out + b * out_batch.
+// each (device, may be NULL; n_rows <= 128): problem b's participating rows and constants are each[b].tm, at most n_rows.
 int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
                          int corrupted_count, float* out, int batch, int64_t g_batch, int ri_batch, int64_t out_batch,
-                         cudaStream_t stream) {
+                         cudaStream_t stream, const ProblemParams* each) {
   if (!G || !out || n < 1 || d < 1 || ld < d || n_rows < 1) { set_error("afl_trimmed_mean: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_trimmed_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
   if (n_rows > kLargeMaxRows) {
     set_error("afl_trimmed_mean: at most %d participating rows fit the shared-memory strip (got %d)", kLargeMaxRows, n_rows);
     return AFL_ERR_UNSUPPORTED;
   }
-  // number_to_consider = rows - f - 1, then Python slice semantics for sorted(...)[:k]   (defences.py:45,50)
-  const int k = n_rows - corrupted_count - 1;
-  const int keep = k >= 0 ? (k < n_rows ? k : n_rows) : (n_rows + k > 0 ? n_rows + k : 0);
+  if (each && n_rows > 128) { set_error("afl_trimmed_mean: a per-problem table needs n_rows <= 128"); return AFL_ERR_UNSUPPORTED; }
   Params P{};
-  P.G = G; P.row_index = row_index; P.out = out; P.d = d; P.ld = ld; P.n_rows = n_rows; P.n_total = n; P.keep = keep;
-  P.g_batch = g_batch; P.out_batch = out_batch; P.ri_batch = ri_batch;
-  P.med_density = 0.3989422804f * static_cast<float>(n_rows);
-  const double frac = keep > 0 ? (static_cast<double>(keep) - 0.5) / n_rows : 0.5;
-  const double q = norm_ppf(0.5 * (1.0 + (frac < 0.999999 ? frac : 0.999999)));
-  P.key_q = static_cast<float>(q);
-  P.key_density = static_cast<float>(2.0 * 0.3989422804014327 * exp(-0.5 * q * q) * n_rows);
+  P.G = G; P.row_index = row_index; P.out = out; P.d = d; P.ld = ld; P.n_total = n; P.tm = shape(n_rows, corrupted_count);
+  P.each = each; P.g_batch = g_batch; P.out_batch = out_batch; P.ri_batch = ri_batch;
   const int64_t es = dtype == AFL_F32 ? 4 : 2;
   P.vec_ok = (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0) && (batch == 1 || (g_batch * es) % 16 == 0);
   if (n_rows > 1024) {
@@ -794,7 +809,7 @@ int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype,
 
 int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
                  int corrupted_count, float* out, cudaStream_t stream) {
-  return trimmed_mean_batched(G, n, d, ld, dtype, row_index, n_rows, corrupted_count, out, 1, 0, 0, 0, stream);
+  return trimmed_mean_batched(G, n, d, ld, dtype, row_index, n_rows, corrupted_count, out, 1, 0, 0, 0, stream, nullptr);
 }
 
 }  // namespace tmean

@@ -256,6 +256,47 @@ int afl_alie_batched(const void* G_mal, int batch, int64_t batch_stride, int f, 
                      int dtype, double z, float* mu_out, float* sigma_out, float* crafted_out,
                      float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* stream);
 
+/* ---- per-problem batched calls: the same batches with corrupted_count (and ALIE's z) per problem ----------
+ * The reference's results come from grids over z (--num_std, main.py:109) and the malicious share (--mal-prop,
+ * main.py:106, f = int(mal_prop * N), main.py:21) as well as the seed.  These calls run such a grid as one batch:
+ * problem b's result is, bit for bit, the single device call's on G[b] with its own f_b (and z_b).  Every other
+ * argument, limit and stride rule is the scalar batched call's.  corrupted_counts / f / z are HOST arrays of `batch`
+ * values; the call validates them, builds one small table of per-problem kernel parameters (the values the single
+ * call derives: Krum's take, Bulyan's f and theta, the trimmed mean's kept count and pivot constants, ALIE's f, (float)z
+ * and whether it writes) and copies it to the start of the workspace with cudaMemcpyAsync on `stream`.  The arrays may
+ * be reused once the call returns.  Because that copy reads pageable memory, these calls cannot be captured into a
+ * CUDA graph.  Checked before any CUDA call: a NULL array or f_b < 0 (ALIE: also f_b > n) -> AFL_ERR_BAD_ARG; a
+ * workspace that is too small or not 256-byte aligned -> AFL_ERR_WORKSPACE; Krum's users_count >= 2f_b+1 and
+ * Bulyan's users_count >= 4f_b+3 for every b, else AFL_ERR_PRECONDITION naming the first failing problem.
+ *
+ * afl_batched_each_workspace_bytes(rule, ...) — rule as afl_defend_batched, or "ALIE"; 0 on bad arguments, otherwise
+ * at least afl_batched_workspace_bytes.  The parameter table comes first; for Krum and Bulyan the scalar call's layout
+ * follows it, so that the squared-distance tables start at byte T = afl_batched_each_workspace_bytes -
+ * afl_batched_workspace_bytes (the same tables the scalar call leaves at byte 0).
+ *
+ * afl_defend_batched_each — defences.py:73-75 defend[rule] per problem with f_b = corrupted_counts[b]:
+ *   "Krum"        defences.py:23-42, take_b = len(sorted(...)[:users_count - f_b]).
+ *   "TrimmedMean" defences.py:44-52, keep_b from n - f_b - 1 with Python slice semantics.
+ *   "NoDefense"   defences.py:13-14, f_b is ignored as in the reference (no table, no workspace).
+ *   "Bulyan"      defences.py:55-70, theta_b = users_count - 2f_b rounds, then the trimmed mean of those rows with
+ *                 2f_b.  sel_out is device int[batch][theta_max], theta_max = users_count - 2 * min_b f_b: problem b
+ *                 fills positions 0..theta_b-1 (-1 from a failed round on, as afl_defend_batched) and positions
+ *                 theta_b..theta_max-1 with -2 ("no such round"). */
+size_t afl_batched_each_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype);
+int afl_defend_batched_each(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                            int64_t ld, int dtype, int users_count, const int* corrupted_counts, float* out,
+                            int* idx_out, int* sel_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* afl_alie_batched_each — malicious.py:10-27,34-36 per problem (DriftAttack(z_b).attack_rows(G[b], f_b)): problems
+ * of n rows, of which rows 0..f_b-1 are malicious, f_b <= n.  Outputs and bcast_rows as afl_alie_batched.
+ * f_b = 0 reads and writes no row and that problem's mu, sigma and crafted are NaN (the reference returns before
+ * computing anything, malicious.py:11-12); z_b = 0 computes the statistics, crafted = mu - 0 * sigma, and writes no
+ * row (malicious.py:20-21). */
+int afl_alie_batched_each(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                          const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
+                          float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                          size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

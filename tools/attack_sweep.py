@@ -1,52 +1,52 @@
-"""ALIE z sweep (SURVEY 8d, Dist C): for every z the malicious rows 0..f-1 are replaced by mu - z*sigma on
-the device, then Krum and Bulyan run; reports attack success and checks the indices against the oracle on
-the same inputs (NumPy oracle up to n = 200, the plain-C float64 oracle beyond; Bulyan's sequence is required to
-match up to the first round whose top-1/top-2 margin is below 1e-5).
+"""ALIE z sweep (SURVEY 8d, Dist C) as one per-problem batch: problem i is the same client matrix attacked with z_i,
+so one batched.alie_rows call replaces rows 0..f-1 of every problem by mu - z_i*sigma, and one batched Krum and one
+batched Bulyan call aggregate them all.  Reports attack success per z and checks every problem's indices against the
+NumPy oracle on the same inputs (Bulyan's sequence is required to match up to the first round whose top-1/top-2 margin
+is below 1e-5).  The batched calls hold n <= 128 clients.
 usage: python tools/attack_sweep.py [n] [d] > attack_sweep.json"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
-from attacking_federate_learning_b200 import defences as D, malicious as M, metrics
-from oracle import ref_numpy as orc, c_oracle as co
+from attacking_federate_learning_b200 import batched as bt, metrics
+from oracle import ref_numpy as orc
 import time
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 100
 d = int(sys.argv[2]) if len(sys.argv) > 2 else 65536
+if n > 128:
+    sys.exit("attack_sweep.py runs the z sweep as one batch: n <= 128 clients")
 f = int(0.24 * n)
+zs = [0.25, 0.5, 1.0, 1.5, 2.0, 3.0]
 rng = np.random.default_rng(2026)
 base = (0.1 * rng.standard_normal(d) + rng.standard_normal((n, d)) * np.exp(0.25 * rng.standard_normal((n, 1)))).astype(np.float32)
+Gd = torch.from_numpy(base).cuda().expand(len(zs), n, d).contiguous()
+honest_mean = Gd[0, f:].mean(0)
+bt.alie_rows(Gd, f, zs)
+k = bt.krum(Gd, n, f, return_index=True).cpu().tolist()
+agg, sel = bt.bulyan(Gd, n, f, return_selection=True)
+torch.cuda.synchronize(); t0 = time.perf_counter()
+for _ in range(3):
+    bt.krum(Gd, n, f, return_index=True)
+torch.cuda.synchronize(); t_krum = (time.perf_counter() - t0) / 3
+t0 = time.perf_counter()
+for _ in range(3):
+    bt.bulyan(Gd, n, f)
+torch.cuda.synchronize(); t_bulyan = (time.perf_counter() - t0) / 3
 rows = []
-for z in (0.25, 0.5, 1.0, 1.5, 2.0, 3.0):
-    Gd = torch.from_numpy(base).cuda()
-    honest_mean = Gd[f:].mean(0)
-    M.DriftAttack(z).attack_rows(Gd, f)
-    G = Gd.cpu().numpy()
-    k = D.krum(Gd, n, f, return_index=True)
-    agg, sel = D.bulyan(Gd, n, f, return_selection=True)
-    torch.cuda.synchronize(); t0 = time.perf_counter()
-    for _ in range(3):
-        D.krum(Gd, n, f, return_index=True)
-    torch.cuda.synchronize(); t_krum = (time.perf_counter() - t0) / 3
-    t0 = time.perf_counter()
-    for _ in range(3):
-        D.bulyan(Gd, n, f)
-    torch.cuda.synchronize(); t_bulyan = (time.perf_counter() - t0) / 3
-    if n <= 200:
-        t64 = orc.pairwise_distances_f64(G)
-        k_ref, margin = orc.krum_select(t64, orc.visit_order(n), n, f, dtype=np.float64, with_margin=True)
-        sel_ref, margins = orc.bulyan_select(t64, n, f, dtype=np.float64, with_margins=True)
-    else:
-        t64 = np.sqrt(co.pairwise_sqdist(G))
-        k_ref, margin = co.krum_select(t64, n, f, with_margin=True)
-        sel_ref, margins = co.bulyan_select(t64, n, f, with_margins=True)
-    first_close = next((i for i, m in enumerate(margins) if 0.0 < m <= 1e-5), len(margins))
-    sel_l = sel.cpu().tolist()
-    rows.append({"z": z, "krum_index": int(k), "krum_matches_oracle": int(k) == int(k_ref), "krum_margin": float(margin),
-                 "krum_success": metrics.krum_attack_success(k, f),
-                 "krum_aggregations_per_s": 1.0 / t_krum, "bulyan_aggregations_per_s": 1.0 / t_bulyan,
+for i, z in enumerate(zs):
+    G = Gd[i].cpu().numpy()
+    t64 = orc.pairwise_distances_f64(G)
+    k_ref, margin = orc.krum_select(t64, orc.visit_order(n), n, f, dtype=np.float64, with_margin=True)
+    sel_ref, margins = orc.bulyan_select(t64, n, f, dtype=np.float64, with_margins=True)
+    first_close = next((j for j, m in enumerate(margins) if 0.0 < m <= 1e-5), len(margins))
+    sel_l = sel[i].cpu().tolist()
+    rows.append({"z": z, "krum_index": k[i], "krum_matches_oracle": k[i] == int(k_ref), "krum_margin": float(margin),
+                 "krum_success": metrics.krum_attack_success(k[i], f),
                  "bulyan_matches_oracle": sel_l[:first_close] == list(sel_ref)[:first_close],
                  "bulyan_rounds_required_exact": first_close, "bulyan_rounds": len(sel_l),
-                 "bulyan_malicious_fraction": metrics.bulyan_attack_success(sel.cpu().tolist(), f),
-                 "bulyan_rel_deviation": metrics.relative_deviation(agg, honest_mean),
-                 "krum_rel_deviation": metrics.relative_deviation(Gd[k], honest_mean)})
-print(json.dumps({"n": n, "d": d, "f": f, "sweep": rows}, indent=1))
+                 "bulyan_malicious_fraction": metrics.bulyan_attack_success(sel_l, f),
+                 "bulyan_rel_deviation": metrics.relative_deviation(agg[i], honest_mean),
+                 "krum_rel_deviation": metrics.relative_deviation(Gd[i, k[i]], honest_mean)})
+# one batched call aggregates every z: aggregations/s counts problems
+print(json.dumps({"n": n, "d": d, "f": f, "krum_aggregations_per_s": len(zs) / t_krum,
+                  "bulyan_aggregations_per_s": len(zs) / t_bulyan, "sweep": rows}, indent=1))

@@ -16,7 +16,9 @@ def dtype_code(t: torch.Tensor) -> int:
         return nat.AFL_F32
     if t.dtype == torch.bfloat16:
         return nat.AFL_BF16
-    raise NotImplementedError(f"users_grads dtype {t.dtype}: only float32 and bfloat16 are supported")
+    if t.dtype == torch.float16:
+        return nat.AFL_F16
+    raise NotImplementedError(f"users_grads dtype {t.dtype}: only float32, bfloat16 and float16 are supported")
 
 
 def check_matrix(G: torch.Tensor):

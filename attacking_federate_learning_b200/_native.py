@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libafl_b200.so")
 
 AFL_OK, AFL_ERR_BAD_ARG, AFL_ERR_PRECONDITION, AFL_ERR_CUDA, AFL_ERR_UNSUPPORTED, AFL_ERR_WORKSPACE, AFL_ERR_NO_WINNER = range(7)
-AFL_F32, AFL_BF16 = 0, 1
+AFL_F32, AFL_BF16, AFL_F16 = 0, 1, 2
 GRAM_AUTO, GRAM_FORCE_SIMT, GRAM_FORCE_TCGEN05, GRAM_SINGLE_PASS, GRAM_REWRITE_HI = 0, 1, 2, 4, 8
 GRAM_TF32X2 = 16
 GRAM_BF16X2 = 32

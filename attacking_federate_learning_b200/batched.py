@@ -6,7 +6,7 @@ Every problem keeps the reference's semantics exactly: problem b's result is wha
 (`defences.krum` / `bulyan` / `trimmed_mean` / `no_defense`, `malicious.Attack.attack_rows`) returns for
 `G[b]`, bit for bit (C ABI `afl_defend_batched` / `afl_alie_batched`).
 
-Inputs are torch.cuda float32 / bfloat16 tensors `[B, N, D]` with `stride(2) == 1` and N <= 128 clients (one
+Inputs are torch.cuda float32 / bfloat16 / float16 tensors `[B, N, D]` with `stride(2) == 1` and N <= 128 clients (one
 Gram tile); every problem shares N, D and `users_count`.  `corrupted_count` (and `alie_rows`' `num_std`) is
 either one number for every problem or a host sequence of B values (list, tuple, NumPy array, CPU tensor), one
 per problem (C ABI `afl_defend_batched_each` / `afl_alie_batched_each`), so that a grid over the malicious
@@ -139,7 +139,7 @@ defend = {DefenseTypes.Krum: krum,
 def alie_rows(users_grads, corrupted_count, num_std):
     """Per problem malicious.Attack.attack_rows (DriftAttack): the malicious users are rows 0..f-1 of every
     problem.  Returns (crafted, mu, sigma), each fp32 [B, D] (mu is the unperturbed mean), and writes crafted
-    = mu - num_std * sigma into those rows in place (fp32 directly; bf16 through a cast, as attack_rows does).
+    = mu - num_std * sigma into those rows in place (fp32 directly; bf16 and fp16 through a cast, as attack_rows does).
     With num_std == 0 the rows are left alone, as attack_rows does.  None when corrupted_count <= 0.
 
     corrupted_count and num_std may each be one number or B of them (host sequences).  Per problem, f_b <= N;
@@ -184,7 +184,7 @@ def _alie_rows_each(users_grads, fs, zs):
                                           fs.ctypes.data, zs.ctypes.data, mu.data_ptr(), sigma.data_ptr(),
                                           crafted.data_ptr(), None if bcast is None else bcast.data_ptr(), bs, ld,
                                           ws.data_ptr(), ws.numel(), _stream_ptr(users_grads)))
-    if write.any() and bcast is None:                    # bf16: rows r < f_b of the problems that write, via a cast
+    if write.any() and bcast is None:                    # bf16 / fp16: rows r < f_b of the problems that write, via a cast
         b_idx, r_idx = np.nonzero(write[:, None] & (np.arange(N)[None, :] < fs[:, None]))
         b_idx, r_idx = (torch.from_numpy(x).pin_memory().to(dev, non_blocking=True) for x in (b_idx, r_idx))
         users_grads[b_idx, r_idx] = crafted[b_idx].to(users_grads.dtype)

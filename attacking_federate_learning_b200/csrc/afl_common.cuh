@@ -5,6 +5,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -98,7 +99,7 @@ struct ProfScope {
 };
 
 // Operand formats of the tensor-core Gram kernel (csrc/gram_pair.cu)
-enum GramMode { kModeBf16x2 = 0, kModeTf32x2 = 1, kModeBf16In = 2 };
+enum GramMode { kModeBf16x2 = 0, kModeTf32x2 = 1, kModeBf16In = 2, kModeF16In = 3 };
 
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -133,6 +134,10 @@ __device__ __forceinline__ uint4 ldg_stream_u4(const uint4* p) {
   return r;
 }
 __device__ __forceinline__ float bf16_bits_to_f32(uint32_t b16) { return __uint_as_float(b16 << 16); }
+// fp16 in the low 16 bits -> fp32 (exact, subnormals and infinities included)
+__device__ __forceinline__ float f16_bits_to_f32(uint32_t b16) {
+  return __half2float(__ushort_as_half(static_cast<unsigned short>(b16)));
+}
 
 // ------------------------------------------------------------------------------------------------
 // peer-memory exchange (csrc/xgpu.cu): epoch flags and the peers' tables
@@ -276,23 +281,28 @@ __device__ __forceinline__ void wgmma_fence_operands(float (&d)[64]) {
   for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 // m64n128: thread t of the warpgroup holds 64 accumulators; keep == 0 overwrites D instead of accumulating.
-__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t keep) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1, 0, 0;\n\t}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-      "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-      "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-      "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-      "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-      "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-      "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-      "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a_desc), "l"(b_desc), "r"(keep));
-}
+// AB = the operand type of both 16-bit operands: bf16 or f16 (fp16 clients, kModeF16In).
+#define AFL_WGMMA_M64N128K16(NAME, AB)                                                                             \
+  __device__ __forceinline__ void NAME(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t keep) {       \
+    asm volatile(                                                                                                 \
+        "{\n\t.reg .pred p;\n\t"                                                                                  \
+        "setp.ne.b32 p, %66, 0;\n\t"                                                                              \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." AB "." AB " "                                              \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, " \
+        "%64, %65, p, 1, 1, 0, 0;\n\t}\n"                                                                         \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),         \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),     \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),   \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),   \
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),   \
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),   \
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),   \
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])    \
+        : "l"(a_desc), "l"(b_desc), "r"(keep));                                                                   \
+  }
+AFL_WGMMA_M64N128K16(wgmma_m64n128k16_bf16, "bf16")
+AFL_WGMMA_M64N128K16(wgmma_m64n128k16_f16, "f16")
+#undef AFL_WGMMA_M64N128K16
 __device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t keep) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"

@@ -600,7 +600,7 @@ static int check_batch(const char* who, const void* G, int batch, int64_t batch_
               static_cast<long long>(batch_stride), static_cast<long long>(static_cast<int64_t>(rows - 1) * ld + d));
     return AFL_ERR_BAD_ARG;
   }
-  if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("%s: dtype", who); return AFL_ERR_UNSUPPORTED; }
+  if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("%s: dtype", who); return AFL_ERR_UNSUPPORTED; }
   return AFL_OK;
 }
 

@@ -3,6 +3,8 @@
 // All of them stream the row-major [n, d] matrix once with 16-byte loads; a thread owns VEC adjacent
 // columns and walks down the rows, so every warp-level load is one contiguous segment of a row.  mean and
 // alie take a batch of same-shape problems in grid y (input at b * g_batch, outputs at b * out_batch).
+#include <type_traits>
+
 #include "afl_common.cuh"
 
 namespace afl {
@@ -13,7 +15,12 @@ constexpr int kUnroll = 8;
 
 template <int VEC> struct Pack { float v[VEC]; };
 
-// Load VEC consecutive columns of one row as fp32.  VEC = 4 (fp32, 16 B) or 8 (bf16, 16 B) or 1 (scalar).
+// One 16-bit element (low half of `b16`) of a bf16 or fp16 matrix as fp32 (exact).
+template <typename T> __device__ __forceinline__ float half_bits_to_f32(uint32_t b16);
+template <> __device__ __forceinline__ float half_bits_to_f32<__nv_bfloat16>(uint32_t b16) { return bf16_bits_to_f32(b16); }
+template <> __device__ __forceinline__ float half_bits_to_f32<__half>(uint32_t b16) { return f16_bits_to_f32(b16); }
+
+// Load VEC consecutive columns of one row as fp32.  VEC = 4 (fp32, 16 B) or 8 (bf16 / fp16, 16 B) or 1 (scalar).
 template <typename T, int VEC>
 __device__ __forceinline__ Pack<VEC> load_pack(const T* p);
 template <> __device__ __forceinline__ Pack<4> load_pack<float, 4>(const float* p) {
@@ -35,6 +42,18 @@ template <> __device__ __forceinline__ Pack<8> load_pack<__nv_bfloat16, 8>(const
 template <> __device__ __forceinline__ Pack<1> load_pack<__nv_bfloat16, 1>(const __nv_bfloat16* p) {
   return Pack<1>{{__bfloat162float(*p)}};
 }
+template <> __device__ __forceinline__ Pack<8> load_pack<__half, 8>(const __half* p) {
+  const uint4 t = ldg_stream_u4(reinterpret_cast<const uint4*>(p));
+  Pack<8> r;
+  const uint32_t w[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    r.v[2 * i] = f16_bits_to_f32(w[i] & 0xFFFFu);
+    r.v[2 * i + 1] = f16_bits_to_f32(w[i] >> 16);
+  }
+  return r;
+}
+template <> __device__ __forceinline__ Pack<1> load_pack<__half, 1>(const __half* p) { return Pack<1>{{__half2float(*p)}}; }
 
 // Coherent variants (no .nc, no L1 bypass hint): used when the kernel also WRITES the matrix it reads
 // (ALIE writing the crafted vector back into the malicious rows it just reduced).
@@ -56,11 +75,17 @@ __device__ __forceinline__ Pack<VEC> load_pack_coherent(const T* p) {
       uint32_t w[4];
       asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "l"(p) : "memory");
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { r.v[2 * i] = bf16_bits_to_f32(w[i] & 0xFFFFu); r.v[2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u); }
+      for (int i = 0; i < 4; ++i) {
+        if constexpr (std::is_same<T, __half>::value) {
+          r.v[2 * i] = f16_bits_to_f32(w[i] & 0xFFFFu); r.v[2 * i + 1] = f16_bits_to_f32(w[i] >> 16);
+        } else {
+          r.v[2 * i] = bf16_bits_to_f32(w[i] & 0xFFFFu); r.v[2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
+        }
+      }
     } else {
       uint16_t t;
       asm volatile("ld.global.u16 %0, [%1];" : "=h"(t) : "l"(p) : "memory");
-      r.v[0] = bf16_bits_to_f32(t);
+      r.v[0] = half_bits_to_f32<T>(t);
     }
   }
   return r;
@@ -242,7 +267,7 @@ static bool vec_ok(const void* G, int64_t ld, int dtype, int batch, int64_t g_ba
 int mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, int batch, int64_t g_batch,
                  int64_t out_batch, cudaStream_t stream) {
   if (!G || !out || n < 1 || d < 1 || ld < d) { set_error("afl_mean: bad argument"); return AFL_ERR_BAD_ARG; }
-  if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
+  if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
   const bool v = vec_ok(G, ld, dtype, batch, g_batch);
   const int vec = v ? (dtype == AFL_F32 ? 4 : 8) : 1;
   const dim3 grid(static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock)), batch);
@@ -251,9 +276,12 @@ int mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, float* 
   if (dtype == AFL_F32) {
     if (v) AFL_MEAN_LAUNCH(float, 4);
     else AFL_MEAN_LAUNCH(float, 1);
-  } else {
+  } else if (dtype == AFL_BF16) {
     if (v) AFL_MEAN_LAUNCH(__nv_bfloat16, 8);
     else AFL_MEAN_LAUNCH(__nv_bfloat16, 1);
+  } else {
+    if (v) AFL_MEAN_LAUNCH(__half, 8);
+    else AFL_MEAN_LAUNCH(__half, 1);
   }
 #undef AFL_MEAN_LAUNCH
   AFL_LAUNCH_CHECK("mean_kernel");
@@ -270,7 +298,7 @@ int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double 
                  float* crafted_out, float* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
                  int64_t bcast_batch, cudaStream_t stream, const ProblemParams* each) {
   if (!G || f < (each ? 0 : 1) || d < 1 || ld < d || (bcast && bcast_ld < d)) { set_error("afl_alie: bad argument"); return AFL_ERR_BAD_ARG; }
-  if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_alie: dtype"); return AFL_ERR_UNSUPPORTED; }
+  if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_alie: dtype"); return AFL_ERR_UNSUPPORTED; }
   const bool v = vec_ok(G, ld, dtype, batch, g_batch);
   const int vec = v ? (dtype == AFL_F32 ? 4 : 8) : 1;
   const dim3 grid(static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock)), batch);
@@ -286,9 +314,12 @@ int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double 
   if (dtype == AFL_F32) {
     if (v) { if (coh) AFL_ALIE_LAUNCH(float, 4, true); else AFL_ALIE_LAUNCH(float, 4, false); }
     else { if (coh) AFL_ALIE_LAUNCH(float, 1, true); else AFL_ALIE_LAUNCH(float, 1, false); }
-  } else {
+  } else if (dtype == AFL_BF16) {
     if (v) { if (coh) AFL_ALIE_LAUNCH(__nv_bfloat16, 8, true); else AFL_ALIE_LAUNCH(__nv_bfloat16, 8, false); }
     else { if (coh) AFL_ALIE_LAUNCH(__nv_bfloat16, 1, true); else AFL_ALIE_LAUNCH(__nv_bfloat16, 1, false); }
+  } else {
+    if (v) { if (coh) AFL_ALIE_LAUNCH(__half, 8, true); else AFL_ALIE_LAUNCH(__half, 8, false); }
+    else { if (coh) AFL_ALIE_LAUNCH(__half, 1, true); else AFL_ALIE_LAUNCH(__half, 1, false); }
   }
 #undef AFL_ALIE_LAUNCH
   AFL_LAUNCH_CHECK("alie_kernel");
@@ -309,6 +340,8 @@ int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int
     gather_row_kernel<float><<<static_cast<unsigned>(blocks), kBlock, 0, stream>>>(static_cast<const float*>(G), n, d, ld, idx_dev, out);
   else if (dtype == AFL_BF16)
     gather_row_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), kBlock, 0, stream>>>(static_cast<const __nv_bfloat16*>(G), n, d, ld, idx_dev, out);
+  else if (dtype == AFL_F16)
+    gather_row_kernel<__half><<<static_cast<unsigned>(blocks), kBlock, 0, stream>>>(static_cast<const __half*>(G), n, d, ld, idx_dev, out);
   else { set_error("afl_gather_row: dtype"); return AFL_ERR_UNSUPPORTED; }
   AFL_LAUNCH_CHECK("gather_row_kernel");
   return AFL_OK;

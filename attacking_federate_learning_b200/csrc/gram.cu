@@ -1,12 +1,12 @@
 // Pairwise squared distances of the N client rows (reference: defences.py:16-21
 // `_krum_create_distances`, the dominant cost of Krum and Bulyan).
 //
-// Tensor-core path (fp32 or bf16 input, 16-byte aligned rows): d2_ij = s_ii + s_jj - 2 s_ij with S = G G^T on the
-// Hopper warpgroup MMAs (csrc/gram_pair.cu), fp32 split into two bf16 or two TF32 terms, K split over CTAs and the
+// Tensor-core path (fp32, bf16 or fp16 input, 16-byte aligned rows): d2_ij = s_ii + s_jj - 2 s_ij with S = G G^T on the
+// Hopper warpgroup MMAs (csrc/gram_pair.cu), fp32 split into two bf16 or two TF32 terms, 16-bit clients as they are, K split over CTAs and the
 // partial tiles summed in a fixed order in float64 -> bit-reproducible, and identical rows give bit-identical
 // table rows (Krum's [1,0,2,...] tie-break relies on this).
 //
-// SIMT path (any pitch, fp32 or bf16): direct sum of squared fp32 differences, float64 accumulation.
+// SIMT path (any pitch, fp32, bf16 or fp16): direct sum of squared fp32 differences, float64 accumulation.
 // Used for misaligned pitches and as an independent check of the tensor path in the tests.
 #include "afl_common.cuh"
 
@@ -21,6 +21,7 @@ template <> __device__ __forceinline__ float load_elem<float>(const float* p) { 
 template <> __device__ __forceinline__ float load_elem<__nv_bfloat16>(const __nv_bfloat16* p) {
   return __bfloat162float(*p);
 }
+template <> __device__ __forceinline__ float load_elem<__half>(const __half* p) { return __half2float(*p); }
 
 // blockIdx.z = problem of a batch (matrix at G + z * batch_stride, partials at part + z * splits * n * n).
 template <typename T>
@@ -124,15 +125,16 @@ static int env_int(const char* name, int dflt) {
 // batch > 1 adds the batch pitch to the alignment TMA needs, and a pitch that keeps the problems apart (the 3-D tensor map)
 static bool tensor_eligible(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype) {
   const int64_t per16 = dtype == AFL_F32 ? 4 : 8;           // elements per 16 bytes: TMA needs 16-byte aligned rows
-  return (dtype == AFL_F32 || dtype == AFL_BF16) && (ld % per16 == 0) && (reinterpret_cast<uintptr_t>(G) % 16 == 0) && n >= 1 &&
+  return (dtype == AFL_F32 || dtype == AFL_BF16 || dtype == AFL_F16) && (ld % per16 == 0) && (reinterpret_cast<uintptr_t>(G) % 16 == 0) && n >= 1 &&
          d >= 1 && n <= 4096 && d < (int64_t(1) << 31) - 64 &&
          (batch == 1 || (batch_stride % per16 == 0 && batch_stride >= static_cast<int64_t>(n) * ld));
 }
 
 // fp32 operands default to the centred bf16x2 split for N > 128 and for the streaming shapes (64 <= N_pad <= 112,
 // D >= 32768); elsewhere, and with AFL_GRAM_TF32X2 / AFL_GRAM_SINGLE_PASS, to the split-TF32 operands (smaller
-// uniform bias, no centring).  A batch chooses like one problem of its shape; its split counts see batch times the
-// CTAs of one problem, and AFL_GRAM_SPLITS overrides both paths' split count.
+// uniform bias, no centring).  bf16 and fp16 clients are the operands themselves (kModeBf16In, kModeF16In); the fp32
+// operand flags do not apply to them.  A batch chooses like one problem of its shape; its split counts see batch times
+// the CTAs of one problem, and AFL_GRAM_SPLITS overrides both paths' split count.
 static Plan make_plan(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, int flags) {
   Plan pl{};
   pl.tensor = !(flags & AFL_GRAM_FORCE_SIMT) && tensor_eligible(G, batch, batch_stride, n, d, ld, dtype);
@@ -141,6 +143,7 @@ static Plan make_plan(const void* G, int batch, int64_t batch_stride, int n, int
     const int nb = (n + 15) & ~15;
     const bool streaming = nb >= 64 && nb <= 112 && d >= 32768;
     if (dtype == AFL_BF16) pl.mode = kModeBf16In;
+    else if (dtype == AFL_F16) pl.mode = kModeF16In;
     else if ((flags & (AFL_GRAM_SINGLE_PASS | AFL_GRAM_TF32X2)) || !(n > 128 || streaming)) pl.mode = kModeTf32x2;
     else pl.mode = kModeBf16x2;
     pl.parts_bytes = pair_parts_bytes(n, d, batch);
@@ -172,7 +175,7 @@ size_t workspace_bytes(int n, int64_t d, int dtype, int flags, int batch) {
 int sqdist_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, double* d2_out,
                    void* ws, size_t ws_bytes, int flags, cudaStream_t stream) {
   if (!G || !d2_out || n < 1 || d < 1 || ld < d) { set_error("afl_sqdist_partial: bad argument"); return AFL_ERR_BAD_ARG; }
-  if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_sqdist_partial: dtype"); return AFL_ERR_UNSUPPORTED; }
+  if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_sqdist_partial: dtype"); return AFL_ERR_UNSUPPORTED; }
   Plan pl = make_plan(G, batch, batch_stride, n, d, ld, dtype, flags);
   if ((flags & AFL_GRAM_FORCE_TCGEN05) && !pl.tensor) {
     set_error("afl_sqdist_partial: tensor-core path needs a 16-byte aligned base, 16-byte aligned pitch, n <= 4096");
@@ -200,9 +203,12 @@ int sqdist_batched(const void* G, int batch, int64_t batch_stride, int n, int64_
       if (dtype == AFL_F32)
         sqdist_simt_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const float*>(G), n, d, ld, batch_stride,
                                                             pl.simt_splits, part);
-      else
+      else if (dtype == AFL_BF16)
         sqdist_simt_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(G), n, d, ld,
                                                                      batch_stride, pl.simt_splits, part);
+      else
+        sqdist_simt_kernel<__half><<<grid, 256, 0, stream>>>(static_cast<const __half*>(G), n, d, ld, batch_stride,
+                                                              pl.simt_splits, part);
     }
     AFL_LAUNCH_CHECK("sqdist_simt_kernel");
     sqdist_simt_reduce_kernel<<<rgrid, rblock, 0, stream>>>(part, n, pl.simt_splits, d2_out);

@@ -25,6 +25,8 @@
 //                    lo lo^T, <= 2^-20 relative).  No centring.
 //       kModeBf16In  bf16 clients: TMA delivers ready-made SWIZZLE_128B operand tiles, S += g_I g_J^T exactly
 //                    (only the fp32 accumulation rounds), no converter pass.
+//       kModeF16In   fp16 clients: the same with FLOAT16 tiles and wgmma .f16 operands (an fp16 product is exact in
+//                    fp32 too).
 //     With more than one tile EVERY pair - diagonal ones too - issues the same sequence on the same K partition, so two
 //     clients with identical rows get bit-identical s_ii, s_jj and s_ij wherever their tiles are, and their distance is
 //     exactly 0 (ALIE makes rows 0..f-1 one array; Krum's [1, 0, 2, ...] tie-break depends on it).  The one-tile
@@ -294,8 +296,9 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
     constexpr uint32_t kSecond = kMode == kModeBf16x2 ? 1024u : kBoxBytes;
     const uint32_t a_off = static_cast<uint32_t>(c) * 8u * kSbo;
     const int ngroups = (nkb + p.flush - 1) / p.flush;
+    constexpr bool kDirect = kMode == kModeBf16In || kMode == kModeF16In;     // 16-bit clients: no converter pass
     auto wait_ready = [&](int b) {
-      mbar_wait_fast(kMode == kModeBf16In ? &raw_full[b % kPSlots] : &conv_done[b % kPSlots], phase_of(b));
+      mbar_wait_fast(kDirect ? &raw_full[b % kPSlots] : &conv_done[b % kPSlots], phase_of(b));
     };
     auto release = [&](int it) {
       if (lane == 0) {
@@ -331,6 +334,10 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
             wgmma_m64n128k8_tf32(acc, d_1i + 2 * ks, d_2j + 2 * ks, 1u);           // hi_I lo_J^T
             wgmma_m64n128k8_tf32(acc, d_2i + 2 * ks, d_1j + 2 * ks, 1u);           // lo_I hi_J^T
           }
+        } else if (kMode == kModeF16In) {
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks)
+            wgmma_m64n128k16_f16(acc, d_1i + 2 * ks, d_1j + 2 * ks, first | ks);     // g_I g_J^T
         } else {
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {
@@ -485,13 +492,13 @@ static int launch_sym(const CUtensorMap& tmap, const PairParams& p, int batch, c
   return AFL_ERR_UNSUPPORTED;
 }
 
-// G: `batch` problems of fp32 [n, d] (pitch multiple of 4 elements) or bf16 (kModeBf16In, pitch multiple of 8), 16-byte
-// aligned, problem b at G + b * batch_stride elements (batch > 1: one tile, a 16-byte multiple >= n * ld).
-// parts: pair_parts_bytes(); S and d2_out: batch * n * n doubles; cvec: pair_center_bytes().
+// G: `batch` problems of fp32 [n, d] (pitch multiple of 4 elements) or bf16 / fp16 (kModeBf16In / kModeF16In, pitch
+// multiple of 8), 16-byte aligned, problem b at G + b * batch_stride elements (batch > 1: one tile, a 16-byte multiple
+// >= n * ld).  parts: pair_parts_bytes(); S and d2_out: batch * n * n doubles; cvec: pair_center_bytes().
 int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, float* parts,
                 double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream) {
   const float* G = static_cast<const float*>(Gv);
-  const bool bf16 = mode == kModeBf16In;
+  const bool half16 = mode == kModeBf16In || mode == kModeF16In;    // 16-bit elements
   if (batch > 1 && n > 128) { set_error("gram_pair_kernel: batched problems are one tile (n <= 128, got %d)", n); return AFL_ERR_UNSUPPORTED; }
   static EncodeTiledFn enc = nullptr;
   if (!enc) {
@@ -525,13 +532,16 @@ int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n
     AFL_LAUNCH_CHECK("pair_center_kernel");
   }
   CUtensorMap tmap;
-  const cuuint64_t es = bf16 ? 2 : 4;
+  const cuuint64_t es = half16 ? 2 : 4;
+  const CUtensorMapDataType elem = mode == kModeBf16In ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                   : mode == kModeF16In ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                                        : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   const cuuint64_t gdim[3] = {static_cast<cuuint64_t>(d), static_cast<cuuint64_t>(n), static_cast<cuuint64_t>(batch)};
   const cuuint64_t gstride[2] = {static_cast<cuuint64_t>(ld) * es,
                                  static_cast<cuuint64_t>(batch > 1 ? batch_stride : n * ld) * es};
   const cuuint32_t box[3] = {static_cast<cuuint32_t>(cols), static_cast<cuuint32_t>(p.box_rows), 1};
   const cuuint32_t estride[3] = {1, 1, 1};
-  CUresult r = enc(&tmap, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(Gv), gdim,
+  CUresult r = enc(&tmap, elem, 3, const_cast<void*>(Gv), gdim,
                    gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    mode == kModeBf16x2 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -539,6 +549,7 @@ int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n
   int rc = sym                   ? launch_sym(tmap, p, batch, stream)
          : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, 0>(tmap, p, batch, stream)
          : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, 0>(tmap, p, batch, stream)
+         : mode == kModeF16In  ? launch_mode<kModeF16In, 0>(tmap, p, batch, stream)
                                : launch_mode<kModeBf16In, 0>(tmap, p, batch, stream);
   if (rc) return rc;
   pair_reduce_kernel<<<dim3(n, p.tiles, batch), dim3(128, kPSy), 0, stream>>>(parts, n, p.splits, sym, S);

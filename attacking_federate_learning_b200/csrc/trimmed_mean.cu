@@ -6,13 +6,16 @@
 //              out = fl32(fl32(sum(kept)/k) + med).
 //
 // Layout / mapping
-//   * A CTA owns a tile of 64 bytes per row (16 fp32 or 32 bf16 columns) x all rows.  Rows are read
+//   * A CTA owns a tile of 64 bytes per row (16 fp32 or 32 bf16 / fp16 columns) x all rows.  Rows are read
 //     with coalesced 16-byte loads (4 lanes per row segment) and scattered into shared memory in a
 //     [word-column][slot-group][lane] order with an XOR on the slot-in-group index, so that both the
 //     staging stores (STS.32) and the per-column reads (LDS.128) are bank-conflict free.
 //   * One warp then owns one word-column: lane l holds rows l, l+32, l+64, ... in registers
 //     (S slots per lane, S = 4, 8, 12, ..., 32: the smallest multiple of 4 with 32 S >= rows), so every pass over
 //     the column is pure register arithmetic plus one warp reduction.  Rows past N are staged as +inf.
+//   * Element formats (template parameter DT, an afl_dtype): fp32 occupies one word per column; bf16 and fp16 two
+//     columns per word, unpacked to fp32 (exactly) as the column is loaded into registers, so everything after the
+//     unpack is the fp32 arithmetic.
 //   * Selection, fast path (select_fast): ONE fused pass per order statistic with a bracket [a, b) aimed from the
 //     column's mean / sigma (median) or sigma and the normal quantile (|dev| threshold): it counts #{key < a}, sums
 //     the devs below a, and marks the in-bracket slots in a per-lane bit mask (4-5 instructions per value, in PTX).
@@ -254,17 +257,31 @@ __device__ __forceinline__ float warp_sort32(float v, int lane) {
   return KEYS ? __uint_as_float(__funnelshift_r(u, u, 1)) : v;
 }
 
+// One staged word as the fp32 value of the column that `sel` (unpack_sel) picks: fp32 as is; bf16 moved to the top
+// half by one PRMT; fp16 moved to the bottom half by one PRMT and converted.
+template <int DT>
+__device__ __forceinline__ float unpack_word(uint32_t w, uint32_t sel) {
+  if constexpr (DT == AFL_F32) return __uint_as_float(w);
+  else if constexpr (DT == AFL_BF16) return __uint_as_float(__byte_perm(w, 0u, sel));
+  else return f16_bits_to_f32(__byte_perm(w, 0u, sel));
+}
+template <int DT>
+__device__ __forceinline__ uint32_t unpack_sel(int half) {
+  if constexpr (DT == AFL_F16) return half ? 0x3232u : 0x1010u;
+  else return half ? 0x3244u : 0x1044u;
+}
+
 // Where a register-resident column lives in the shared-memory tile, so that a candidate can be re-read by a
 // run-time register index (a dynamic index into the register array itself would spill it to local memory).
 struct ColRef {
   const uint32_t* words;     // tile word of element 0 for this lane; element i is words[(i >> 2) * 128 + (i & 3)]
-  uint32_t unpack_sel;       // bf16: PRMT selector that moves the column's half of the word to the top (0x1044 / 0x3244)
+  uint32_t unpack_sel;       // 16-bit formats: PRMT selector of the column's half of the word (unpack_sel<DT>)
   float med;                 // KEYS: the median that was subtracted from the registers
 };
-template <bool BF16, bool KEYS>
+template <int DT, bool KEYS>
 __device__ __forceinline__ float col_fetch(const ColRef& c, int i) {
   const uint32_t w = c.words[(i >> 2) * 128 + (i & 3)];
-  const float x = BF16 ? __uint_as_float(__byte_perm(w, 0u, c.unpack_sel)) : __uint_as_float(w);
+  const float x = unpack_word<DT>(w, c.unpack_sel);
   return KEYS ? __fsub_rn(x, c.med) : x;
 }
 
@@ -300,7 +317,7 @@ __device__ __forceinline__ void fused_step(float v, float a, float b, uint32_t b
 // few candidates from the tile into a dense 32-entry list (exclusive prefix of the per-lane counts), and the
 // list is sorted with a 15-stage shuffle network.  Returns false (state updated: lo/c_lo/sum_lo or hi/c_hi
 // tightened where the pass proved a bound) when the general path has to take over.
-template <int S, bool KEYS, bool BF16>
+template <int S, bool KEYS, int DT>
 __device__ __forceinline__ bool select_fast(const float (&v)[S], const ColRef& col, int n, int r1, int r2, float p0,
                                             float density, int lane, int jx, uint32_t* scratch, float& lo, float& hi,
                                             int& c_lo, int& c_hi, float& sum_lo, float& out_a, float& out_b) {
@@ -336,7 +353,7 @@ __device__ __forceinline__ bool select_fast(const float (&v)[S], const ColRef& c
       }
       float* dense = reinterpret_cast<float*>(scratch);              // [32]
       int pos = incl - mine;
-      for (uint32_t m = inmask; m != 0u; m &= m - 1u) dense[pos++] = col_fetch<BF16, KEYS>(col, __ffs(m) - 1);
+      for (uint32_t m = inmask; m != 0u; m &= m - 1u) dense[pos++] = col_fetch<DT, KEYS>(col, __ffs(m) - 1);
       __syncwarp();
       const bool have = lane < cin;
       const float val = have ? dense[lane] : kInf;
@@ -398,13 +415,14 @@ __device__ __forceinline__ bool select_fast(const float (&v)[S], const ColRef& c
 // Thread t loads the 16-byte chunk j = t&3 of row (it*64 + t>>2) in iteration `it`.  Row r lives in
 // slot r>>5 of lane r&31; slot-group m = slot>>2 and the XOR-ed slot position are compile-time
 // functions of `it`, so every store below has an immediate offset from one of two per-thread bases.
-template <int S, bool BF16>
+template <int S, int DT>
 __device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, uint32_t* tile, int64_t col0) {
   constexpr int kGroups = S / 4;
+  constexpr bool W16 = DT != AFL_F32;                   // two 16-bit columns per word
   const int tid = threadIdx.x;
-  const int es = BF16 ? 2 : 4;
-  const int cols_per_tile = BF16 ? 32 : 16;
-  const uint32_t sentinel = BF16 ? 0x7F807F80u : 0x7F800000u;
+  const int es = W16 ? 2 : 4;
+  const int cols_per_tile = W16 ? 32 : 16;
+  const uint32_t sentinel = DT == AFL_F16 ? 0x7C007C00u : DT == AFL_BF16 ? 0x7F807F80u : 0x7F800000u;   // +inf
   const uint8_t* base = static_cast<const uint8_t*>(P.G) + static_cast<int64_t>(blockIdx.y) * P.g_batch * es;
   const int* row_index = P.row_index ? P.row_index + static_cast<int64_t>(blockIdx.y) * P.ri_batch : nullptr;
   constexpr int kIters = (32 * S * 4) / kThreads;      // S/2
@@ -457,7 +475,7 @@ __device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, u
       gr = gr < 0 ? gr + P.n_total : gr;
       const uint8_t* src = base + (static_cast<int64_t>(gr) * P.ld + c) * es;
       w[0] = w[1] = w[2] = w[3] = 0u;
-      if (BF16) {
+      if (W16) {
         const uint16_t* s16 = reinterpret_cast<const uint16_t*>(src);
 #pragma unroll
         for (int e = 0; e < 8; ++e)
@@ -478,8 +496,8 @@ __device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, u
 }
 
 // ---------------- general per-column path (any data): one warp, one column ----------------
-// `half` selects the bf16 column inside the 32-bit word-column cw (ignored for fp32).
-template <int S, bool BF16>
+// `half` selects the 16-bit column inside the 32-bit word-column cw (ignored for fp32).
+template <int S, int DT>
 __device__ __forceinline__ float general_column_impl(const TmShape& P, const uint32_t* tile, int cw, int half,
                                                      uint32_t* scratch, int lane) {
   constexpr int kGroups = S / 4;
@@ -487,17 +505,17 @@ __device__ __forceinline__ float general_column_impl(const TmShape& P, const uin
   const float fn = static_cast<float>(n);
   const int jx = (cw >> 2) & 3;
   const uint4* t4 = reinterpret_cast<const uint4*>(tile) + (cw * kGroups) * 32 + lane;
-  // bf16 -> fp32 is one PRMT with a run-time selector (`half` is a loop variable: a ?: costs two predicated instructions)
-  const uint32_t unpack_sel = half ? 0x3244u : 0x1044u;
-  ColRef col{reinterpret_cast<const uint32_t*>(t4), unpack_sel, 0.f};
+  // 16-bit -> fp32 is one PRMT with a run-time selector (`half` is a loop variable: a ?: costs two predicated
+  // instructions), plus the conversion for fp16
+  const uint32_t sel = unpack_sel<DT>(half);
+  ColRef col{reinterpret_cast<const uint32_t*>(t4), sel, 0.f};
   float x[S];
 #pragma unroll
   for (int m = 0; m < kGroups; ++m) {
     const uint4 t = t4[m * 32];
     const uint32_t w[4] = {t.x, t.y, t.z, t.w};
 #pragma unroll
-    for (int q = 0; q < 4; ++q)
-      x[4 * m + q] = BF16 ? __uint_as_float(__byte_perm(w[q], 0u, unpack_sel)) : __uint_as_float(w[q]);
+    for (int q = 0; q < 4; ++q) x[4 * m + q] = unpack_word<DT>(w[q], sel);
   }
 
   // mean / sigma of the column (pivot model only; never enters the result).  The kernel is instantiated with
@@ -528,7 +546,7 @@ __device__ __forceinline__ float general_column_impl(const TmShape& P, const uin
   {
     float lo = -kInf, hi = kInf, sl = 0.f;
     int c_lo = 0, c_hi = n;
-    if (!select_fast<S, false, BF16>(x, col, n, (n - 1) >> 1, n >> 1, mean, P.med_density * inv_sd, lane, jx, scratch, lo, hi, c_lo,
+    if (!select_fast<S, false, DT>(x, col, n, (n - 1) >> 1, n >> 1, mean, P.med_density * inv_sd, lane, jx, scratch, lo, hi, c_lo,
                                c_hi, sl, a, b))
       warp_select<S, false>(x, n, (n - 1) >> 1, n >> 1, mean, P.med_density * inv_sd, lane, jx, scratch, lo, hi, c_lo,
                             c_hi, 0.f, a, b);
@@ -545,7 +563,7 @@ __device__ __forceinline__ float general_column_impl(const TmShape& P, const uin
     float lo = -kInf, hi = kInf, sl = 0.f;
     int c_lo = 0, c_hi = n;
     col.med = med;
-    if (!select_fast<S, true, BF16>(x, col, n, P.keep - 1, P.keep - 1, P.key_q * sd, P.key_density * inv_sd, lane, jx, scratch, lo, hi,
+    if (!select_fast<S, true, DT>(x, col, n, P.keep - 1, P.keep - 1, P.key_q * sd, P.key_density * inv_sd, lane, jx, scratch, lo, hi,
                               c_lo, c_hi, sl, total, unused)) {
       // General path.  Infinite deviations (an inf in the column, or fl32(x - med) overflowing) share the key +inf with
       // the padded rows, so the bracket's upper count is the number of finite keys, not n.  When the keep boundary is
@@ -574,21 +592,22 @@ constexpr int kScratchWords = 96;              // per warp: dense candidate list
 // EACH: problem blockIdx.y's constants come from the per-problem table P.each (batches only, so S = 4).  A separate instance:
 // holding them in registers instead of reading the constant bank takes the fp32 kernel from 48 to 54 registers, which
 // would cost the single calls a fifth CTA per SM.
-template <int S, bool BF16, bool EACH>
+template <int S, int DT, bool EACH>
 __global__ void __launch_bounds__(kThreads, (S <= 20 ? 4 : 3))      // (S = 24 fits 4 CTAs in shared memory too, but the fp32 instance spills at 64 registers)
 trimmed_mean_kernel(const Params P) {
   extern __shared__ __align__(1024) uint32_t tile[];     // [16 word-cols][S/4 groups][32 lanes][4 slots] + scratch
   constexpr int kGroups = S / 4;
+  constexpr bool W16 = DT != AFL_F32;                    // bf16 / fp16: two columns per word-column
   const int tid = threadIdx.x, warp = tid >> 5;
-  const int cols_per_tile = BF16 ? 32 : 16;
+  const int cols_per_tile = W16 ? 32 : 16;
   const int64_t col0 = static_cast<int64_t>(blockIdx.x) * cols_per_tile;
   TmShape sh = P.tm;
   if constexpr (EACH) sh = P.each[blockIdx.y].tm;
-  stage_tile<S, BF16>(P, sh, tile, col0);
+  stage_tile<S, DT>(P, sh, tile, col0);
   // read once, after staging: `volatile` keeps ptxas from re-reading the special register (S2R, ~50 cycles of
   // latency) in front of every scan and sort of the per-column code to save one register
   int lane = tid & 31, warp_o = warp;
-  if (BF16 || S < 32) {       // (the fp32 S = 32 instance is at the 80-register limit: there it would only add spills)
+  if (W16 || S < 32) {        // (the fp32 S = 32 instance is at the 80-register limit: there it would only add spills)
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
     asm volatile("mov.u32 %0, %1;" : "=r"(warp_o) : "r"(warp));
   }
@@ -597,10 +616,10 @@ trimmed_mean_kernel(const Params P) {
 #pragma unroll 1
   for (int cw = warp_o; cw < kWordCols; cw += kWarps) {
 #pragma unroll 1
-    for (int half = 0; half < (BF16 ? 2 : 1); ++half) {
-      const int64_t col = col0 + (BF16 ? 2 * cw + half : cw);
+    for (int half = 0; half < (W16 ? 2 : 1); ++half) {
+      const int64_t col = col0 + (W16 ? 2 * cw + half : cw);
       if (col >= P.d) break;                         // warp-uniform
-      const float res = general_column_impl<S, BF16>(sh, tile, cw, half, scratch, lane);
+      const float res = general_column_impl<S, DT>(sh, tile, cw, half, scratch, lane);
       if (lane == 0) P.out[static_cast<int64_t>(blockIdx.y) * P.out_batch + col] = res;
     }
   }
@@ -614,21 +633,24 @@ trimmed_mean_kernel(const Params P) {
 // order with ballots.  Exact for any data; slow (a fallback: the reference has no client-count limit, defences.py:44-52).
 constexpr int kLargeMaxRows = 12288;          // 12288 rows x 16 B = 192 KB of shared memory
 
-__device__ __forceinline__ float strip_value(const uint32_t* strip, int row, int col_in_strip, bool bf16) {
-  if (!bf16) return __uint_as_float(strip[row * 4 + col_in_strip]);
+// w16: 16-bit elements, two per word (bf16, or fp16 when F16)
+template <bool F16>
+__device__ __forceinline__ float strip_value(const uint32_t* strip, int row, int col_in_strip, bool w16) {
+  if (!w16) return __uint_as_float(strip[row * 4 + col_in_strip]);
   const uint32_t w = strip[row * 4 + (col_in_strip >> 1)];
+  if (F16) return f16_bits_to_f32((col_in_strip & 1) ? (w >> 16) : w);
   return __uint_as_float((col_in_strip & 1) ? (w & 0xFFFF0000u) : (w << 16));
 }
 
 // k-th smallest (0-based) key among this warp's column, keys = ord_bits(f(value)); F = 0: value, F = 1: |fl32(value - med)|
-template <int F>
-__device__ __forceinline__ uint32_t warp_kth_key(const uint32_t* strip, int n, int cis, bool bf16, float med, int k, int lane) {
+template <int F, bool F16>
+__device__ __forceinline__ uint32_t warp_kth_key(const uint32_t* strip, int n, int cis, bool w16, float med, int k, int lane) {
   uint32_t lo = 0u, hi = 0xFFFFFFFFu;                      // invariant: count(key < lo) <= k < count(key <= hi)
   while (lo < hi) {
     const uint32_t mid = lo + ((hi - lo) >> 1);
     int c = 0;
     for (int r = lane; r < n; r += 32) {
-      float v = strip_value(strip, r, cis, bf16);
+      float v = strip_value<F16>(strip, r, cis, w16);
       if (F) v = fabsf(__fsub_rn(v, med));
       c += (ord_bits(v) <= mid) ? 1 : 0;
     }
@@ -641,6 +663,8 @@ __device__ __forceinline__ float from_ord_bits(uint32_t o) {
   return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
 }
 
+// bf16 != 0: 16-bit elements (bf16, or fp16 in the F16 instance)
+template <bool F16>
 __global__ void __launch_bounds__(256, 1)
 trimmed_mean_large_kernel(const Params P, int bf16) {
   extern __shared__ __align__(16) uint32_t strip[];        // [n_rows][4 words]
@@ -674,19 +698,19 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
   for (int cis = warp; cis < cols; cis += 8) {
     const int64_t col = col0 + cis;
     if (col >= P.d) break;
-    const float a = from_ord_bits(warp_kth_key<0>(strip, n, cis, bf16 != 0, 0.f, (n - 1) >> 1, lane));
-    const float b = (n & 1) ? a : from_ord_bits(warp_kth_key<0>(strip, n, cis, bf16 != 0, 0.f, n >> 1, lane));
+    const float a = from_ord_bits(warp_kth_key<0, F16>(strip, n, cis, bf16 != 0, 0.f, (n - 1) >> 1, lane));
+    const float b = (n & 1) ? a : from_ord_bits(warp_kth_key<0, F16>(strip, n, cis, bf16 != 0, 0.f, n >> 1, lane));
     const float med = (n & 1) ? a : __fdiv_rn(__fadd_rn(a, b), 2.0f);
     float res;
     if (P.tm.keep <= 0) {
       res = __int_as_float(0x7fc00000);
     } else {
-      const uint32_t To = warp_kth_key<1>(strip, n, cis, bf16 != 0, med, P.tm.keep - 1, lane);   // threshold key (as ord bits)
+      const uint32_t To = warp_kth_key<1, F16>(strip, n, cis, bf16 != 0, med, P.tm.keep - 1, lane);   // threshold key (as ord bits)
       // sum of the devs strictly below the threshold, then the first `need` of the tie group in row order
       float part = 0.f;
       int below = 0;
       for (int r = lane; r < n; r += 32) {
-        const float dv = __fsub_rn(strip_value(strip, r, cis, bf16 != 0), med);
+        const float dv = __fsub_rn(strip_value<F16>(strip, r, cis, bf16 != 0), med);
         const bool lt = ord_bits(fabsf(dv)) < To;
         part += lt ? dv : 0.f;
         below += lt ? 1 : 0;
@@ -697,7 +721,7 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
         const int r = r0 + lane;
         float dv = 0.f;
         bool tie = false;
-        if (r < n) { dv = __fsub_rn(strip_value(strip, r, cis, bf16 != 0), med); tie = ord_bits(fabsf(dv)) == To; }
+        if (r < n) { dv = __fsub_rn(strip_value<F16>(strip, r, cis, bf16 != 0), med); tie = ord_bits(fabsf(dv)) == To; }
         const unsigned m = __ballot_sync(0xffffffffu, tie);
         if (tie && __popc(m & ((1u << lane) - 1u)) < need) part += dv;
         need -= __popc(m);
@@ -738,7 +762,7 @@ static double norm_ppf(double pr) {   // Acklam's rational approximation, |error
 template <int S>
 static int launch(const Params& P, int dtype, int batch, cudaStream_t stream) {
   const size_t smem = static_cast<size_t>(S) * 2048 + kWarps * kScratchWords * 4;
-  const int cols = dtype == AFL_BF16 ? 32 : 16;
+  const int cols = dtype != AFL_F32 ? 32 : 16;
   const dim3 grid(static_cast<unsigned>(ceil_div64(P.d, cols)), batch);
   ProfScope ps("trimmed_mean", stream);
   auto go = [&](auto kernel) -> int {
@@ -748,9 +772,14 @@ static int launch(const Params& P, int dtype, int batch, cudaStream_t stream) {
     return AFL_OK;
   };
   if constexpr (S == 4) {
-    if (P.each) return dtype == AFL_BF16 ? go(trimmed_mean_kernel<S, true, true>) : go(trimmed_mean_kernel<S, false, true>);
+    if (P.each)
+      return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, true>)
+             : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, true>)
+                                : go(trimmed_mean_kernel<S, AFL_F32, true>);
   }
-  return dtype == AFL_BF16 ? go(trimmed_mean_kernel<S, true, false>) : go(trimmed_mean_kernel<S, false, false>);
+  return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, false>)
+         : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, false>)
+                            : go(trimmed_mean_kernel<S, AFL_F32, false>);
 }
 
 // The constants of n_rows participating rows and corrupted_count: number_to_consider = rows - f - 1 with Python slice
@@ -774,7 +803,7 @@ int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype,
                          int corrupted_count, float* out, int batch, int64_t g_batch, int ri_batch, int64_t out_batch,
                          cudaStream_t stream, const ProblemParams* each) {
   if (!G || !out || n < 1 || d < 1 || ld < d || n_rows < 1) { set_error("afl_trimmed_mean: bad argument"); return AFL_ERR_BAD_ARG; }
-  if (dtype != AFL_F32 && dtype != AFL_BF16) { set_error("afl_trimmed_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
+  if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_trimmed_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
   if (n_rows > kLargeMaxRows) {
     set_error("afl_trimmed_mean: at most %d participating rows fit the shared-memory strip (got %d)", kLargeMaxRows, n_rows);
     return AFL_ERR_UNSUPPORTED;
@@ -787,11 +816,17 @@ int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype,
   P.vec_ok = (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0) && (batch == 1 || (g_batch * es) % 16 == 0);
   if (n_rows > 1024) {
     const size_t smem = static_cast<size_t>(n_rows) * 16;
-    const int cols = dtype == AFL_BF16 ? 8 : 4;
-    static int smem_attr_done[kMaxDevices] = {0};
-    AFL_CUDA(ensure_dyn_smem(trimmed_mean_large_kernel, static_cast<int>(kLargeMaxRows) * 16, smem_attr_done));
+    const int cols = dtype != AFL_F32 ? 8 : 4;
+    const dim3 grid(static_cast<unsigned>(ceil_div64(d, cols)), batch);
+    static int smem_attr_done[kMaxDevices] = {0}, smem_attr_done_f16[kMaxDevices] = {0};
     ProfScope ps("trimmed_mean", stream);
-    trimmed_mean_large_kernel<<<dim3(static_cast<unsigned>(ceil_div64(d, cols)), batch), 256, smem, stream>>>(P, dtype == AFL_BF16 ? 1 : 0);
+    if (dtype == AFL_F16) {
+      AFL_CUDA(ensure_dyn_smem(trimmed_mean_large_kernel<true>, static_cast<int>(kLargeMaxRows) * 16, smem_attr_done_f16));
+      trimmed_mean_large_kernel<true><<<grid, 256, smem, stream>>>(P, 1);
+    } else {
+      AFL_CUDA(ensure_dyn_smem(trimmed_mean_large_kernel<false>, static_cast<int>(kLargeMaxRows) * 16, smem_attr_done));
+      trimmed_mean_large_kernel<false><<<grid, 256, smem, stream>>>(P, dtype == AFL_BF16 ? 1 : 0);
+    }
     AFL_LAUNCH_CHECK("trimmed_mean_large_kernel");
     return AFL_OK;
   }

@@ -20,8 +20,9 @@ Reference surface mirrored (file:line in /root/reference):
     `krum(..., return_index=True)` stream the matrix into the same slab-summed distance table
     (`afl_sqdist_host`), so `krum(G, n, f)` is `G[krum(G, n, f, return_index=True)]`;
     `bulyan(..., return_selection=True)` also returns the selection (`afl_bulyan_host`);
-  * a torch.cuda float32 / bfloat16 [N, D] tensor: device-resident path, returns torch tensors
-    (fp32), `krum` again returns a view `users_grads[idx]`.
+  * a torch.cuda float32 / bfloat16 / float16 [N, D] tensor: device-resident path, returns torch tensors
+    (fp32; a 16-bit matrix gives the reference's result on its values upcast to fp32), `krum` again returns a
+    view `users_grads[idx]`.
 There is no CPU implementation in this package.
 """
 from __future__ import annotations

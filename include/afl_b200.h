@@ -17,8 +17,11 @@
  *     default stream).  Device entry points only enqueue work; they never synchronise.
  *   - Matrices are row-major `[n rows = clients][d columns = parameters]`, `ld` = row pitch in
  *     ELEMENTS (server.py:35 allocates users_grads as a C-contiguous N x D fp32 array, ld == d).
- *   - dtype: AFL_F32 (the reference's only type) or AFL_BF16 (config "trimmed_mean, bf16"); outputs
- *     are always fp32.
+ *   - dtype of a device client matrix: AFL_F32 (the reference's only type), AFL_BF16 (config
+ *     "trimmed_mean, bf16") or AFL_F16 (fp16 client updates, as sent over the uplink or produced by
+ *     `.half()` models).  A 16-bit matrix computes the reference's result on its values upcast to fp32
+ *     (exact); outputs are always fp32.  Any other code is AFL_ERR_UNSUPPORTED.  The host-buffer entry
+ *     points take fp32 only.
  *   - No entry point allocates device memory; scratch comes from a caller-owned workspace whose size
  *     the matching *_workspace_bytes() function reports.
  *   - Multi-GPU: the parameter dimension D is sharded; every GPU calls the same entry points on its
@@ -47,7 +50,7 @@ typedef enum afl_status {
                              /* reference raises KeyError(-1) at defences.py:66 (`distances.pop(-1)`)  */
 } afl_status;
 
-typedef enum afl_dtype { AFL_F32 = 0, AFL_BF16 = 1 } afl_dtype;
+typedef enum afl_dtype { AFL_F32 = 0, AFL_BF16 = 1, AFL_F16 = 2 } afl_dtype;
 
 /* flags for afl_sqdist_partial */
 enum {
@@ -88,7 +91,7 @@ int afl_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out,
 /* ---- pairwise squared distances:  defences.py:16-21  _krum_create_distances ------------------- */
 /* Partial squared L2 distances over this shard's d columns, as a dense symmetric n x n float64
  * table (zero diagonal).  AFL_GRAM_AUTO: G*G^T on the tensor cores (wgmma, TMA-fed, bf16x2 or split-TF32
- * operands for fp32, bf16 as is; lower-triangular 128 x 128 tile pairs), d2_ij = s_ii + s_jj - 2 s_ij, bf16x2
+ * operands for fp32, bf16 and fp16 as they are; lower-triangular 128 x 128 tile pairs), d2_ij = s_ii + s_jj - 2 s_ij, bf16x2
  * operands centred on the mean of the last 8 clients' rows.  Partial tables of different shards
  * ADD; take the square root only after the all-reduce (afl_sqdist_to_dist). */
 size_t afl_sqdist_workspace_bytes(int n, int64_t d, int dtype, int flags);

@@ -59,6 +59,11 @@ SIGNATURES = {
                                      _vp]),
     "afl_alie_batched_each": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp,
                                    _sz, _vp]),
+    "afl_metrics_workspace_bytes": (_sz, [_i, _i, _i64, _i]),
+    "afl_attack_metrics_batched": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp,
+                                        _vp, _vp, _vp, _sz, _vp]),
+    "afl_attack_metrics_batched_each": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp,
+                                             _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 _lib = None

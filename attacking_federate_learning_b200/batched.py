@@ -13,6 +13,10 @@ per problem (C ABI `afl_defend_batched_each` / `afl_alie_batched_each`), so that
 share and z runs as one batch.  Nothing here synchronises the host except `bulyan`, which checks for a failed
 selection round as `defences.bulyan` does.
 
+`attack_metrics` turns the batch's results into the sweep's attack-success table (SURVEY 8d) in one call: each
+problem's distance from its honest mean, whether Krum picked a malicious client, and the malicious share of
+Bulyan's selection.  It has no client limit.
+
 The server's momentum step needs no batched form: `_device.momentum_step` on contiguous `[B, D]` weights,
 velocity and gradients is already the batched step (server.py:89-90 is element-wise).
 """
@@ -189,3 +193,64 @@ def _alie_rows_each(users_grads, fs, zs):
         b_idx, r_idx = (torch.from_numpy(x).pin_memory().to(dev, non_blocking=True) for x in (b_idx, r_idx))
         users_grads[b_idx, r_idx] = crafted[b_idx].to(users_grads.dtype)
     return crafted, mu, sigma
+
+
+def attack_metrics(users_grads, corrupted_count, *, aggregated=None, krum_index=None, selection=None,
+                   return_honest_mean=False):
+    """Attack-success figures of every problem (C ABI `afl_attack_metrics_batched` / `_each`), as a dict of device
+    tensors.  The malicious users are rows 0..f_b-1 (main.py:28); corrupted_count is one int or B host values.
+
+    * aggregated (fp32 [B, D]: Bulyan's, the trimmed mean's or the mean's output) or krum_index (int32 [B], what
+      `krum(..., return_index=True)` returns; the winning rows are read in place) gives `rel_deviation` [B] fp32 =
+      ||a_b - h_b|| / ||h_b|| with h_b the mean of rows f_b..N-1 (`no_defense(G[b, f_b:])` bit for bit), and
+      `deviation_sums` [B, 2] float64, the two sums of squares, which add across column shards.  At most one of the two.
+    * krum_index also gives `krum_success` [B] bool (metrics.krum_attack_success per problem).
+    * selection (int32 [B, theta], what `bulyan(..., return_selection=True)` returns; -1 and -2 entries are not
+      counted) gives `bulyan_malicious_fraction` [B] fp32 (metrics.bulyan_attack_success per problem).
+    * return_honest_mean adds `honest_mean` [B, D] fp32.
+
+    f_b >= N (no honest row) and krum_index -1 give NaN deviations.  No host synchronisation.  One problem: pass
+    `G[None]`."""
+    fs = _per_problem(corrupted_count, users_grads.shape[0], "corrupted_count", np.int32)
+    B, N, D, ld, bs = _check(users_grads)
+    dev = users_grads.device
+
+    def arg(t, name, dtype, shape):
+        if t is None:
+            return None
+        if not (isinstance(t, torch.Tensor) and t.device == dev and t.dtype == dtype and t.dim() == len(shape)
+                and all(s == (w or s) for s, w in zip(t.shape, shape))):
+            raise ValueError(f"{name}: expected a {dtype} tensor of shape {shape} on {dev}")
+        return t.contiguous()
+    if aggregated is not None and krum_index is not None:
+        raise ValueError("attack_metrics: give the aggregate as `aggregated` or as `krum_index`, not both")
+    agg = arg(aggregated, "aggregated", torch.float32, (B, D))
+    idx = arg(krum_index, "krum_index", torch.int32, (B,))
+    sel = arg(selection, "selection", torch.int32, (B, None))       # any number of rounds
+
+    def out(when, shape, dtype):
+        return torch.empty(shape, dtype=dtype, device=dev) if when else None
+    have_agg = agg is not None or idx is not None
+    rel, sums = out(have_agg, (B,), torch.float32), out(have_agg, (B, 2), torch.float64)
+    honest = out(return_honest_mean, (B, D), torch.float32)
+    hit = out(idx is not None, (B,), torch.int32)
+    mal, cnt = out(sel is not None, (B,), torch.int32), out(sel is not None, (B,), torch.int32)
+    ptrs = [None if t is None else t.data_ptr() for t in (agg, idx, sel, rel, sums, honest, hit, mal, cnt)]
+    L = nat.lib()
+    code = dtype_code(users_grads)
+    with torch.cuda.device(dev):
+        ws = Workspace.get(dev, "metrics", L.afl_metrics_workspace_bytes(B, N, D, code))
+        call, f = (L.afl_attack_metrics_batched, int(corrupted_count)) if fs is None else \
+            (L.afl_attack_metrics_batched_each, fs.ctypes.data)
+        nat.check(call(users_grads.data_ptr(), B, bs, N, D, ld, code, f, *ptrs[:3], 0 if sel is None else sel.shape[1],
+                       *ptrs[3:], ws.data_ptr(), ws.numel(), _stream_ptr(users_grads)))
+    res = {}
+    if have_agg:
+        res["rel_deviation"], res["deviation_sums"] = rel, sums
+    if hit is not None:
+        res["krum_success"] = hit.bool()
+    if sel is not None:
+        res["bulyan_malicious_fraction"] = mal.float() / cnt.clamp(min=1).float()
+    if honest is not None:
+        res["honest_mean"] = honest
+    return res

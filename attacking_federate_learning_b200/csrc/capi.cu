@@ -133,6 +133,11 @@ int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int
                cudaStream_t stream);
 int momentum_step(float* w, float* v, const float* g, int64_t d, float momentum, float lr, cudaStream_t stream);
 int alie_band(const float* mu, const float* sigma, double z, const float* x, float* out, int64_t d, cudaStream_t stream);
+int64_t deviation_tiles(int64_t d, int dtype);
+int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, int64_t ld, int dtype, int f,
+                   const ProblemParams* each, const float* agg, const int* idx, const int* sel, int sel_ld,
+                   float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count,
+                   void* partial, cudaStream_t stream);
 }
 
 __global__ void add_f64_kernel(double* __restrict__ acc, const double* __restrict__ x, size_t n, int first) {
@@ -585,14 +590,14 @@ static BatchedRule batched_rule(const char* rule) {
   return B_BAD;
 }
 
-// Shape checks shared by the batched calls, before any CUDA call.
+// Shape checks shared by the batched calls, before any CUDA call.  max_rows: one Gram tile for the defences and ALIE.
 static int check_batch(const char* who, const void* G, int batch, int64_t batch_stride, int rows, int64_t d, int64_t ld,
-                       int dtype) {
+                       int dtype, int max_rows = kBatchMaxClients) {
   if (!G || rows < 1 || d < 1 || ld < d) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
   if (batch < 1) { set_error("%s: batch must be >= 1 (got %d)", who, batch); return AFL_ERR_BAD_ARG; }
   if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
-  if (rows > kBatchMaxClients) {
-    set_error("%s: batched problems support n <= %d clients (got %d)", who, kBatchMaxClients, rows);
+  if (rows > max_rows) {
+    set_error("%s: batched problems support n <= %d clients (got %d)", who, max_rows, rows);
     return AFL_ERR_UNSUPPORTED;
   }
   if (batch > 1 && batch_stride < static_cast<int64_t>(rows - 1) * ld + d) {
@@ -745,6 +750,46 @@ static int alie_batched(const char* who, const void* G, int batch, int64_t batch
   }
   return colstats::alie_batched(G, fmax, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast_rows, bcast_ld, batch,
                                 batch_stride, d, bcast_batch_stride, stream, each);
+}
+
+// Attack-success metrics of a batch (afl_attack_metrics_batched; fs != NULL: afl_attack_metrics_batched_each).
+// Workspace: [ProblemParams table][partial sums: double2[batch][tiles]]; the scalar call leaves the table unused.
+static size_t metrics_partial_bytes(int batch, int64_t d, int dtype) {
+  return align_up(static_cast<size_t>(batch) * colstats::deviation_tiles(d, dtype) * sizeof(double2), 256);
+}
+
+static int attack_metrics(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, int f,
+                          const int* fs, const float* agg, const int* idx, const int* sel, int sel_ld, float* dev_out,
+                          double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* ws,
+                          size_t ws_bytes, cudaStream_t stream) {
+  const char* who = fs ? "afl_attack_metrics_batched_each" : "afl_attack_metrics_batched";
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
+  if (rc) return rc;
+  int fmin = f, fmax = f;
+  if (fs && (rc = check_counts(who, fs, batch, INT32_MAX, &fmin, &fmax))) return rc;
+  if (fmin < 0) { set_error("%s: corrupted_count %d is negative", who, f); return AFL_ERR_BAD_ARG; }
+  if (agg && idx) { set_error("%s: give the aggregate as agg or as idx, not both", who); return AFL_ERR_BAD_ARG; }
+  if ((dev_out || sums_out) && !agg && !idx) {
+    set_error("%s: dev_out and sums_out need an aggregate (agg or idx)", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  if (krum_hit && !idx) { set_error("%s: krum_hit needs idx", who); return AFL_ERR_BAD_ARG; }
+  if ((mal_count || sel_count) && !sel) { set_error("%s: mal_count and sel_count need sel", who); return AFL_ERR_BAD_ARG; }
+  if (sel && sel_ld < 1) { set_error("%s: sel_ld must be >= 1 (got %d)", who, sel_ld); return AFL_ERR_BAD_ARG; }
+  const bool pass = dev_out || sums_out || honest_out;          // the column pass and its partial sums
+  const size_t need = table_bytes(batch) + metrics_partial_bytes(batch, d, dtype);
+  if ((fs || pass) && (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0)) {
+    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
+    return AFL_ERR_WORKSPACE;
+  }
+  const ProblemParams* each = nullptr;
+  if (fs) {
+    rc = upload_table(who, batch, ws, ws_bytes, need, stream, [&](int b, ProblemParams& q) { q.f = fs[b]; }, &each);
+    if (rc) return rc;
+  }
+  return colstats::attack_metrics(G, batch, batch_stride, n, d, ld, dtype, f, each, agg, idx, sel, sel_ld, dev_out,
+                                  sums_out, honest_out, krum_hit, mal_count, sel_count,
+                                  static_cast<uint8_t*>(ws) + table_bytes(batch), stream);
 }
 
 }  // namespace afl
@@ -910,6 +955,34 @@ int afl_alie_batched_each(const void* G, int batch, int64_t batch_stride, int n,
   return alie_batched("afl_alie_batched_each", G, batch, batch_stride, n, d, ld, dtype, 0, 0.0, f, z, mu_out, sigma_out,
                       crafted_out, bcast_rows, bcast_batch_stride, bcast_ld, workspace, workspace_bytes,
                       static_cast<cudaStream_t>(stream));
+}
+
+size_t afl_metrics_workspace_bytes(int batch, int n, int64_t d, int dtype) {
+  if (batch < 1 || batch > kBatchMax || n < 1 || d < 1 || (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16)) return 0;
+  return table_bytes(batch) + metrics_partial_bytes(batch, d, dtype);
+}
+
+int afl_attack_metrics_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                               int corrupted_count, const float* agg, const int* idx, const int* sel, int sel_ld,
+                               float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count,
+                               int* sel_count, void* workspace, size_t workspace_bytes, void* stream) {
+  return attack_metrics(G, batch, batch_stride, n, d, ld, dtype, corrupted_count, nullptr, agg, idx, sel, sel_ld, dev_out,
+                        sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream));
+}
+
+int afl_attack_metrics_batched_each(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                    int dtype, const int* corrupted_counts, const float* agg, const int* idx,
+                                    const int* sel, int sel_ld, float* dev_out, double* sums_out, float* honest_out,
+                                    int* krum_hit, int* mal_count, int* sel_count, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  if (!corrupted_counts) {
+    set_error("afl_attack_metrics_batched_each: the per-problem corrupted counts are NULL");
+    return AFL_ERR_BAD_ARG;
+  }
+  return attack_metrics(G, batch, batch_stride, n, d, ld, dtype, 0, corrupted_counts, agg, idx, sel, sel_ld, dev_out,
+                        sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

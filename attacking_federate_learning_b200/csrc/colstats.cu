@@ -258,6 +258,146 @@ band_kernel(const float* mu, const float* sigma, float z, const float* x, float*
   }
 }
 
+// ---- attack-success metrics (metrics.py, SURVEY 8d "Attack-success (C5)"): how far an aggregate is from the mean of
+// the honest clients, ||a - h|| / ||h||, and whether a selection holds malicious clients.  The malicious clients are
+// rows 0..f-1 (main.py:28), so the honest ones are rows f..n-1, a different range per problem of a per-problem batch.
+//
+// A thread owns V adjacent columns (4 for fp32, 8 for the 16-bit formats) whatever the pitch: with an aligned base
+// and pitch (VL) it takes them with one 16-byte load per row, otherwise with V scalar loads.  A tile is the kBlock * V
+// columns of one CTA, so the tile count, and with it the order of every sum below, depends on d and the dtype only.
+template <typename T, int V, bool VL>
+__device__ __forceinline__ Pack<V> load_cols(const T* p, int64_t c0, int64_t d) {
+  if constexpr (VL) {
+    return load_pack<T, V>(p);
+  } else {
+    Pack<V> r;
+#pragma unroll
+    for (int k = 0; k < V; ++k) r.v[k] = c0 + k < d ? load_pack<T, 1>(p + k).v[0] : 0.f;
+    return r;
+  }
+}
+
+// Sums of a and b over the CTA in thread 0: lanes by butterfly, then the warps in warp order.  No atomics: the
+// order is fixed.
+__device__ __forceinline__ void cta_sum2(double& a, double& b) {
+  __shared__ double s[2][kBlock / 32];
+  a = warp_sum(a);
+  b = warp_sum(b);
+  if (lane_id() == 0) { s[0][threadIdx.x / 32] = a; s[1][threadIdx.x / 32] = b; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    a = s[0][0]; b = s[1][0];
+#pragma unroll
+    for (int w = 1; w < kBlock / 32; ++w) { a += s[0][w]; b += s[1][w]; }
+  }
+}
+
+// h = mean of rows f..n-1: mean_kernel's sequential fp32 row sum and one IEEE division on that row range, so h is
+// afl_mean of G[f:] bit for bit.  a = the aggregate: agg[b] (fp32, pitch d), or row idx[b] of G[b] upcast to fp32
+// (Krum's result, read in place).  partial[b][tile] = (sum (a - h)^2, sum h^2) over the tile's columns in float64; the
+// differences and squares are formed from the fp32 values as float64, so nothing cancels.  f >= n (no honest row)
+// reads no row and gives h = 0 / 0 = NaN; an idx outside [0, n) reads no row and gives a = NaN.  partial == NULL:
+// only honest_out is wanted.
+template <typename T, int V, bool VL>
+__global__ void __launch_bounds__(kBlock)
+honest_deviation_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, int64_t g_batch, int f,
+                        const ProblemParams* __restrict__ each, const float* __restrict__ agg,
+                        const int* __restrict__ idx, float* __restrict__ honest_out, double2* __restrict__ partial) {
+  constexpr int U = VL ? kUnroll : 2;                 // V scalar loads per row: fewer rows in flight
+  const int b = blockIdx.y;
+  if (each) f = each[b].f;
+  f = f < n ? f : n;
+  const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * V;
+  double sd = 0.0, sh = 0.0;
+  if (c0 < d) {
+    const T* p = G + b * g_batch + c0;
+    float acc[V];
+#pragma unroll
+    for (int k = 0; k < V; ++k) acc[k] = 0.f;
+    int r = f;
+    for (; r + U <= n; r += U) {
+      Pack<V> t[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) t[u] = load_cols<T, V, VL>(p + static_cast<int64_t>(r + u) * ld, c0, d);
+#pragma unroll
+      for (int u = 0; u < U; ++u)
+#pragma unroll
+        for (int k = 0; k < V; ++k) acc[k] = __fadd_rn(acc[k], t[u].v[k]);
+    }
+    for (; r < n; ++r) {
+      Pack<V> t = load_cols<T, V, VL>(p + static_cast<int64_t>(r) * ld, c0, d);
+#pragma unroll
+      for (int k = 0; k < V; ++k) acc[k] = __fadd_rn(acc[k], t.v[k]);
+    }
+    Pack<V> a;
+#pragma unroll
+    for (int k = 0; k < V; ++k) a.v[k] = __int_as_float(0x7fc00000);
+    if (idx) {
+      const int i = idx[b];
+      if (i >= 0 && i < n) a = load_cols<T, V, VL>(p + static_cast<int64_t>(i) * ld, c0, d);
+    } else if (agg) {
+#pragma unroll
+      for (int k = 0; k < V; ++k)
+        if (c0 + k < d) a.v[k] = __ldg(agg + b * d + c0 + k);
+    }
+    const float fn = static_cast<float>(n - f);
+    const int64_t o = b * d + c0;
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+      if (c0 + k < d) {
+        const float h = __fdiv_rn(acc[k], fn);
+        if (honest_out) honest_out[o + k] = h;
+        const double hd = static_cast<double>(h), df = static_cast<double>(a.v[k]) - hd;
+        sd = fma(df, df, sd);
+        sh = fma(hd, hd, sh);
+      }
+    }
+  }
+  if (!partial) return;
+  cta_sum2(sd, sh);
+  if (threadIdx.x == 0) partial[static_cast<int64_t>(b) * gridDim.x + blockIdx.x] = make_double2(sd, sh);
+}
+
+// One CTA per problem: thread t adds tiles t, t + kBlock, ... in that order, then cta_sum2.  The order depends on
+// the tile count only.  dev_out[b] = (float)sqrt(sum (a - h)^2 / sum h^2); sums_out[b] = the two float64 sums, which
+// add across column shards.
+__global__ void __launch_bounds__(kBlock)
+deviation_finish_kernel(const double2* __restrict__ partial, int tiles, float* __restrict__ dev_out,
+                        double* __restrict__ sums_out) {
+  const int b = blockIdx.x;
+  const double2* p = partial + static_cast<int64_t>(b) * tiles;
+  double sd = 0.0, sh = 0.0;
+  for (int t = threadIdx.x; t < tiles; t += kBlock) { sd += p[t].x; sh += p[t].y; }
+  cta_sum2(sd, sh);
+  if (threadIdx.x == 0) {
+    if (sums_out) { sums_out[2 * b] = sd; sums_out[2 * b + 1] = sh; }
+    if (dev_out) dev_out[b] = static_cast<float>(sqrt(sd / sh));
+  }
+}
+
+// One thread per problem.  krum_hit[b] = 0 <= idx[b] < f_b (metrics.krum_attack_success).  Over row b of sel
+// (sel_ld entries; -1 = failed round, -2 = no such round): sel_count[b] = entries >= 0, mal_count[b] = entries in
+// [0, f_b) (metrics.bulyan_attack_success is mal_count / max(1, sel_count)).
+__global__ void __launch_bounds__(kBlock)
+selection_stats_kernel(int batch, int f, const ProblemParams* __restrict__ each, const int* __restrict__ idx,
+                       const int* __restrict__ sel, int sel_ld, int* __restrict__ krum_hit, int* __restrict__ mal_count,
+                       int* __restrict__ sel_count) {
+  const int b = blockIdx.x * kBlock + threadIdx.x;
+  if (b >= batch) return;
+  if (each) f = each[b].f;
+  if (krum_hit) { const int i = idx[b]; krum_hit[b] = i >= 0 && i < f; }
+  if (sel) {
+    int mal = 0, cnt = 0;
+    for (int j = 0; j < sel_ld; ++j) {
+      const int i = sel[static_cast<int64_t>(b) * sel_ld + j];
+      cnt += i >= 0;
+      mal += i >= 0 && i < f;
+    }
+    if (mal_count) mal_count[b] = mal;
+    if (sel_count) sel_count[b] = cnt;
+  }
+}
+
 // 16-byte loads need an aligned base, pitch and (batch > 1) batch pitch
 static bool vec_ok(const void* G, int64_t ld, int dtype, int batch, int64_t g_batch) {
   const int64_t es = dtype == AFL_F32 ? 4 : 2;
@@ -344,6 +484,51 @@ int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int
     gather_row_kernel<__half><<<static_cast<unsigned>(blocks), kBlock, 0, stream>>>(static_cast<const __half*>(G), n, d, ld, idx_dev, out);
   else { set_error("afl_gather_row: dtype"); return AFL_ERR_UNSUPPORTED; }
   AFL_LAUNCH_CHECK("gather_row_kernel");
+  return AFL_OK;
+}
+
+// Column tiles of honest_deviation_kernel: kBlock threads of 4 (fp32) or 8 (bf16, fp16) columns.
+int64_t deviation_tiles(int64_t d, int dtype) { return ceil_div64(d, kBlock * (dtype == AFL_F32 ? 4 : 8)); }
+
+// The three metric kernels on `batch` problems (arguments checked by the caller, capi.cu).  The deviation pass runs
+// when dev_out, sums_out or honest_out is wanted, the finish for the first two, the selection statistics when
+// krum_hit or sel is given.  partial: double2[batch][deviation_tiles].
+int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, int64_t ld, int dtype, int f,
+                   const ProblemParams* each, const float* agg, const int* idx, const int* sel, int sel_ld,
+                   float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count,
+                   void* partial, cudaStream_t stream) {
+  const bool sums = dev_out || sums_out;
+  if (sums || honest_out) {
+    const int tiles = static_cast<int>(deviation_tiles(d, dtype));
+    const dim3 grid(tiles, batch);
+    const bool v = vec_ok(G, ld, dtype, batch, g_batch);
+    double2* part = sums ? static_cast<double2*>(partial) : nullptr;
+    {
+      ProfScope ps("honest_deviation", stream);
+#define AFL_DEV_LAUNCH(T, V, VL) honest_deviation_kernel<T, V, VL><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, g_batch, f, each, agg, idx, honest_out, part)
+      if (dtype == AFL_F32) {
+        if (v) AFL_DEV_LAUNCH(float, 4, true);
+        else AFL_DEV_LAUNCH(float, 4, false);
+      } else if (dtype == AFL_BF16) {
+        if (v) AFL_DEV_LAUNCH(__nv_bfloat16, 8, true);
+        else AFL_DEV_LAUNCH(__nv_bfloat16, 8, false);
+      } else {
+        if (v) AFL_DEV_LAUNCH(__half, 8, true);
+        else AFL_DEV_LAUNCH(__half, 8, false);
+      }
+#undef AFL_DEV_LAUNCH
+      AFL_LAUNCH_CHECK("honest_deviation_kernel");
+    }
+    if (sums) {
+      deviation_finish_kernel<<<batch, kBlock, 0, stream>>>(part, tiles, dev_out, sums_out);
+      AFL_LAUNCH_CHECK("deviation_finish_kernel");
+    }
+  }
+  if (krum_hit || sel) {
+    selection_stats_kernel<<<static_cast<unsigned>(ceil_div64(batch, kBlock)), kBlock, 0, stream>>>(
+        batch, f, each, idx, sel, sel_ld, krum_hit, mal_count, sel_count);
+    AFL_LAUNCH_CHECK("selection_stats_kernel");
+  }
   return AFL_OK;
 }
 

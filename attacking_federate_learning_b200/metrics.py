@@ -4,6 +4,11 @@ The reference itself only logs test accuracy (main.py:73-82); these follow from 
 malicious users are ids 0..f-1 (main.py:28), Krum returns one user's gradient (defences.py:42), Bulyan
 averages around the median of theta = n - 2f selected users (defences.py:57-70).  Pure bookkeeping on
 indices and on one [D] vector norm; the aggregation itself is done by `defences`.
+
+These three take one problem at a time and `relative_deviation` synchronises the host.  For a batch of problems (a
+z x malicious-share x seed grid run through `batched`), `batched.attack_metrics` gives the same three figures for
+every problem in one call on the device, with one corrupted_count per problem and no synchronisation; D-sharded:
+`sharded.ShardedAggregator.relative_deviation`.
 """
 from __future__ import annotations
 

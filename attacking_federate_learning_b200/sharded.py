@@ -28,6 +28,11 @@ class NativeKernels:
         from . import _device as dev
         return getattr(dev, name)
 
+    def deviation_sums(self, G, corrupted_count, aggregated=None, krum_index=None):
+        from . import batched
+        return batched.attack_metrics(G, corrupted_count, aggregated=aggregated,
+                                      krum_index=krum_index)["deviation_sums"]
+
 
 class ShardedAggregator:
     def __init__(self, group=None, kernels=None):
@@ -139,6 +144,15 @@ class ShardedAggregator:
         bcast = G_shard if (write_rows and G_shard.dtype == torch.float32) else None
         crafted, _, _ = self.k.alie(src, num_std, bcast)
         return crafted
+
+    def relative_deviation(self, G_shard, corrupted_count, aggregated=None, krum_index=None):
+        """batched.attack_metrics' `rel_deviation` on column shards: G_shard is this rank's [B, N, d_local] block,
+        `aggregated` its [B, d_local] slice of the aggregate (or `krum_index` the replicated int32 [B] indices).
+        Each rank takes its shard's two float64 sums of squares per problem; they add across shards, so one
+        all-reduce of the [B, 2] table and a square root give ||a - h|| / ||h|| over all D columns (fp32 [B]),
+        identical on every rank."""
+        sums = self._allreduce_table(self.k.deviation_sums(G_shard, corrupted_count, aggregated, krum_index))
+        return torch.sqrt(sums[:, 0] / sums[:, 1]).float()
 
     def exchange_name(self):
         if self.world == 1:

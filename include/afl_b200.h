@@ -79,8 +79,8 @@ uint64_t afl_launch_count(void);
 /* ---- in-library kernel timing (measurement aid for bench.py) -----------------------------------
  * While enabled, the dominant kernel of every entry point is bracketed by CUDA events on the stream it
  * is launched on.  afl_profile_read(name, ...) waits for the recorded events of kernel `name`
- * ("gram_pair", "sqdist_simt", "trimmed_mean", "alie", "mean", "krum_tail", "row_sort", "bulyan_rounds"),
- * returns their summed duration and launch count, and forgets them.  on = 1: every bracketed kernel; on = 2: only the
+ * ("gram_pair", "sqdist_simt", "trimmed_mean", "alie", "mean", "krum_tail", "row_sort", "bulyan_rounds",
+ * "honest_deviation"), returns their summed duration and launch count, and forgets them.  on = 1: every bracketed kernel; on = 2: only the
  * dominant kernel of a rule (gram_pair, sqdist_simt, trimmed_mean, mean, alie) - one pair of events per step. */
 int afl_profile_enable(int on);
 int afl_profile_read(const char* kernel, double* total_ms, int* launches);
@@ -299,6 +299,45 @@ int afl_alie_batched_each(const void* G, int batch, int64_t batch_stride, int n,
                           const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
                           float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
                           size_t workspace_bytes, void* stream);
+
+/* ---- attack-success metrics of a batch (SURVEY 8d "Attack-success (C5)") --------------------------------------
+ * The reference logs test accuracy only (main.py:73-82); what a z x malicious-share sweep reports follows from its
+ * conventions.  The malicious users are ids 0..f-1 (main.py:28), so in problem b rows f_b..n-1 are honest:
+ *   h_b     = mean of rows f_b..n-1, afl_mean's arithmetic on that row range (bit for bit afl_mean of G[b] + f_b * ld);
+ *   a_b     = the aggregate: agg + b * d (device fp32[batch][d], the output of Bulyan, TrimmedMean or NoDefense), or,
+ *             with idx (device int[batch], Krum's idx_out) instead, row idx[b] of problem b upcast to fp32, read in
+ *             place.  At most one of agg / idx; neither: selection statistics (and honest_out) only;
+ *   dev_out   (device fp32[batch])      ||a_b - h_b|| / ||h_b||, both sums of squares accumulated in float64;
+ *   sums_out  (device double[batch][2]) those two sums, (sum (a-h)^2, sum h^2): they ADD across column shards, and
+ *             dev = sqrt(sums[0] / sums[1]) after the all-reduce;
+ *   honest_out (device fp32[batch][d])  h_b;
+ *   krum_hit  (device int[batch], needs idx)  1 when 0 <= idx[b] < f_b, else 0;
+ *   mal_count, sel_count (device int[batch], need sel = device int[batch][sel_ld], Bulyan's sel_out): the entries of
+ *             row b in [0, f_b), and the entries >= 0 (-1 = failed round, -2 = no such round are not counted).  The
+ *             malicious fraction of the selection is mal_count / max(1, sel_count).
+ * Every output may be NULL.  f_b >= n (no honest row) and idx[b] outside [0, n) (Krum found no eligible user: -1) read
+ * no row and give NaN in dev_out and in the first sum of sums_out (f_b >= n: in both sums and in honest_out too).  A
+ * zero or non-finite h gives what IEEE division gives (inf or NaN).  The sums are taken per tile of 1024 (fp32) or 2048 (bf16, fp16) columns and added in
+ * a fixed order without atomics, so a result depends on the values, d and the dtype only: not on the pitch, the
+ * alignment, the batch size or the device.
+ * Device pointers; the calls only enqueue work.  There is no client limit (no distance table is built); batch <=
+ * 65535 and the stride rule are afl_defend_batched's; batch = 1 with a plain [n][d] matrix is the single-problem
+ * call.  Checked before any CUDA call: a NULL G, batch < 1, a short batch_stride, both agg and idx, an output
+ * without its input, corrupted_count < 0 -> AFL_ERR_BAD_ARG; a dtype code other than afl_dtype's ->
+ * AFL_ERR_UNSUPPORTED; a workspace smaller than afl_metrics_workspace_bytes(batch, n, d, dtype) (0 on bad arguments)
+ * or not 256-byte aligned -> AFL_ERR_WORKSPACE (the scalar call needs none for selection statistics alone).
+ * afl_attack_metrics_batched_each takes f_b = corrupted_counts[b], a HOST array of `batch` values copied to the start
+ * of the workspace as the other *_each calls do (a NULL array or f_b < 0 -> AFL_ERR_BAD_ARG). */
+size_t afl_metrics_workspace_bytes(int batch, int n, int64_t d, int dtype);
+int afl_attack_metrics_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                               int corrupted_count, const float* agg, const int* idx, const int* sel, int sel_ld,
+                               float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count,
+                               int* sel_count, void* workspace, size_t workspace_bytes, void* stream);
+int afl_attack_metrics_batched_each(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                    int dtype, const int* corrupted_counts, const float* agg, const int* idx,
+                                    const int* sel, int sel_ld, float* dev_out, double* sums_out, float* honest_out,
+                                    int* krum_hit, int* mal_count, int* sel_count, void* workspace,
+                                    size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -22,8 +22,10 @@
 //     When the target rank is inside and <= 32 slots are marked, the candidates are re-read from the tile by slot
 //     index, compacted to one per lane (shuffle scan) and sorted with a 15-stage shuffle bitonic network; otherwise
 //     the bracket is re-aimed from the measured counts (about one column in four needs a second pass).
-//   * Selection, general path (warp_select): interpolation search on counts with a min/max bisection fallback that
-//     terminates for any data (heavy ties, non-Gaussian columns); brackets of <= 32 elements are compacted by ballot
+//   * Selection, general path (warp_select): interpolation search on counts with a min/max bisection fallback on the
+//     integer image of the keys, which halves the bracket's image range per pass: at most 4 model passes + 32
+//     bisection passes for any non-NaN column (heavy ties, non-Gaussian columns, values spread over every binade),
+//     inside the loop's cap of 96; brackets of <= 32 elements are compacted by ballot
 //     and ranked on (key, row), which makes the reference's stable tie rule exact.  In the fast path a tie group that
 //     the keep boundary cuts (ALIE's f identical rows, bf16 value collisions) is resolved in row order with ballots on
 //     the register-resident column (tie_sum).
@@ -70,6 +72,9 @@ __device__ __forceinline__ float warp_max_f(float v) {
 __device__ __forceinline__ uint32_t ord_bits(float x) {
   const uint32_t b = __float_as_uint(x);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float from_ord_bits(uint32_t o) {
+  return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
 }
 
 // true row of register index ri (registers hold each 4-slot group permuted by jx, see staging)
@@ -150,7 +155,12 @@ __device__ __forceinline__ void warp_select(const float (&v)[S], int n, int r1, 
       return;
     }
     if (iter >= 4 || !model) {
-      // ---- fallback: bisect between the actual extremes of the bracket (guaranteed progress)
+      // ---- fallback: bisect the bracket's actual extremes on the order-preserving integer image (ord_bits, with
+      // -0 taken as +0 so that equal keys have one image).  The pivot is the image midpoint rounded up, so
+      // vmin < p <= vmax and either side of it spans at most half the images of [vmin, vmax]: fewer than 2^32
+      // images, so at most 32 such passes leave a single key, and 4 model passes + 32 + the closing one stay
+      // under the 96-pass cap for any non-NaN column.  (A float midpoint removes only the top binade when the
+      // bracket spans many: a column with a hundred rows one per binade ran out of passes.)
       float vmin = kInf, vmax = -kInf;
 #pragma unroll
       for (int i = 0; i < S; ++i) {
@@ -168,9 +178,8 @@ __device__ __forceinline__ void warp_select(const float (&v)[S], int n, int r1, 
         a = warp_sum(sum_lo + part);
         return;
       }
-      p = 0.5f * vmin + 0.5f * vmax;
-      if (vmin == -kInf) p = -__FLT_MAX__;          // a -inf group: the midpoint would be -inf, split the group off
-      if (!(p > vmin)) p = vmax;
+      const uint32_t olo = ord_bits(__fadd_rn(vmin, 0.f)), ohi = ord_bits(__fadd_rn(vmax, 0.f));
+      p = from_ord_bits(olo + ((ohi - olo + 1u) >> 1));
       model = false;
     }
     int c;
@@ -658,9 +667,6 @@ __device__ __forceinline__ uint32_t warp_kth_key(const uint32_t* strip, int n, i
     if (c > k) hi = mid; else lo = mid + 1;
   }
   return lo;
-}
-__device__ __forceinline__ float from_ord_bits(uint32_t o) {
-  return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
 }
 
 // bf16 != 0: 16-bit elements (bf16, or fp16 in the F16 instance)

@@ -64,6 +64,10 @@ SIGNATURES = {
                                         _vp, _vp, _vp, _sz, _vp]),
     "afl_attack_metrics_batched_each": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp,
                                              _vp, _vp, _vp, _vp, _sz, _vp]),
+    "afl_backdoor_start_batched": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp,
+                                        _sz, _vp]),
+    "afl_backdoor_finish_batched": (_i, [_i, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _vp,
+                                         _sz, _vp]),
 }
 
 _lib = None

@@ -13,6 +13,10 @@ per problem (C ABI `afl_defend_batched_each` / `afl_alie_batched_each`), so that
 share and z runs as one batch.  Nothing here synchronises the host except `bulyan`, which checks for a failed
 selection round as `defences.bulyan` does.
 
+`backdoor_rows` is the per-problem `BackdoorAttack.attack_rows`: the backdoor crafting of every problem in three
+launches, with one call of the caller's malicious-network training between the second and the third.  It has no
+client limit.
+
 `attack_metrics` turns the batch's results into the sweep's attack-success table (SURVEY 8d) in one call: each
 problem's distance from its honest mean, whether Krum picked a malicious client, and the malicious share of
 Bulyan's selection.  It has no client limit.
@@ -188,10 +192,79 @@ def _alie_rows_each(users_grads, fs, zs):
                                           fs.ctypes.data, zs.ctypes.data, mu.data_ptr(), sigma.data_ptr(),
                                           crafted.data_ptr(), None if bcast is None else bcast.data_ptr(), bs, ld,
                                           ws.data_ptr(), ws.numel(), _stream_ptr(users_grads)))
-    if write.any() and bcast is None:                    # bf16 / fp16: rows r < f_b of the problems that write, via a cast
-        b_idx, r_idx = np.nonzero(write[:, None] & (np.arange(N)[None, :] < fs[:, None]))
-        b_idx, r_idx = (torch.from_numpy(x).pin_memory().to(dev, non_blocking=True) for x in (b_idx, r_idx))
-        users_grads[b_idx, r_idx] = crafted[b_idx].to(users_grads.dtype)
+    if write.any() and bcast is None:
+        _cast_rows(users_grads, crafted, fs, write)
+    return crafted, mu, sigma
+
+
+def _cast_rows(users_grads, crafted, fs, write):
+    """bf16 / fp16 matrices: crafted[b] over rows r < f_b of the problems that write, via a cast."""
+    N = users_grads.shape[1]
+    b_idx, r_idx = np.nonzero(write[:, None] & (np.arange(N)[None, :] < fs[:, None]))
+    b_idx, r_idx = (torch.from_numpy(x).pin_memory().to(users_grads.device, non_blocking=True) for x in (b_idx, r_idx))
+    users_grads[b_idx, r_idx] = crafted[b_idx].to(users_grads.dtype)
+
+
+def backdoor_rows(users_grads, corrupted_count, num_std, original_params, learning_rate, train_malicious_network):
+    """Per problem malicious.BackdoorAttack.attack_rows (backdoor.py:52-63): the malicious users are rows 0..f_b-1 of
+    problem b.  Returns (crafted, mu, sigma), each fp32 [B, D] (mu is the malicious rows' mean), and writes crafted into
+    those rows in place (fp32 directly; bf16 and fp16 through a cast).  Any number of clients.
+
+    corrupted_count, num_std and learning_rate are each one number or B host values (as `alie_rows`), f_b <= N.
+    original_params: fp32 CUDA [D] (shared by every problem) or [B, D].  The crafting runs on the device, with one
+    call of `train_malicious_network(initial, problems)` in the middle (backdoor.py:56): `problems` is the host list of
+    the k problems that attack (f_b > 0 and z_b != 0), in order, `initial` their fp32 [k, D] starting parameters
+    w_b - lr_b * mu_b, and it returns their trained parameters as a fp32 CUDA [k, D] tensor.  With no such problem it
+    is not called.  f_b = 0 gives NaN crafted, mu and sigma; z_b = 0 the statistics only (crafted = mu); neither
+    writes a row.  Nothing here synchronises the host."""
+    if not (isinstance(original_params, torch.Tensor) and original_params.is_cuda):
+        raise TypeError("original_params: expected a torch.cuda float32 tensor of shape [D] or [B, D]")
+    B, N, D, ld, bs = _check(users_grads)
+    dev = users_grads.device
+    if original_params.dtype != torch.float32 or original_params.device != dev or \
+            tuple(original_params.shape) not in ((D,), (B, D)):
+        raise ValueError(f"original_params: expected a float32 tensor of shape ({D},) or ({B}, {D}) on {dev}")
+    w = original_params.contiguous()
+
+    def per_problem(x, name, dtype):
+        a = _per_problem(x, B, name, dtype)
+        return np.full(B, int(x) if dtype == np.int32 else float(x), dtype) if a is None else a
+    fs = per_problem(corrupted_count, "corrupted_count", np.int32)
+    zs = per_problem(num_std, "num_std", np.float64)
+    lrs = per_problem(learning_rate, "learning_rate", np.float64)
+    mu, sigma, initial, crafted = (torch.empty((B, D), dtype=torch.float32, device=dev) for _ in range(4))
+    L = nat.lib()
+    code = dtype_code(users_grads)
+    stream = _stream_ptr(users_grads)
+    with torch.cuda.device(dev):
+        ws = Workspace.get(dev, "backdoor", L.afl_batched_each_workspace_bytes(b"ALIE", B, 1, D, code))   # the table
+        nat.check(L.afl_backdoor_start_batched(users_grads.data_ptr(), B, bs, N, D, ld, code, fs.ctypes.data,
+                                               zs.ctypes.data, lrs.ctypes.data, w.data_ptr(),
+                                               w.stride(0) if w.dim() == 2 else 0, mu.data_ptr(), sigma.data_ptr(),
+                                               initial.data_ptr(), ws.data_ptr(), ws.numel(), stream))
+    write = (fs > 0) & (zs != 0)
+    problems = np.flatnonzero(write).tolist()
+    mal = initial                                        # read for the problems that attack only
+    if problems:
+        k = len(problems)
+        sel = None if k == B else torch.as_tensor(problems, device=dev)
+        out = train_malicious_network(initial if sel is None else initial[sel], problems)
+        if not (isinstance(out, torch.Tensor) and out.device == dev and out.dtype == torch.float32
+                and tuple(out.shape) == (k, D)):
+            raise ValueError(f"train_malicious_network must return a float32 tensor of shape ({k}, {D}) on {dev}")
+        if sel is None:
+            mal = out.contiguous()
+        else:
+            mal = torch.empty((B, D), dtype=torch.float32, device=dev)
+            mal[sel] = out
+    bcast = users_grads if problems and users_grads.dtype == torch.float32 else None
+    with torch.cuda.device(dev):
+        nat.check(L.afl_backdoor_finish_batched(B, D, fs.ctypes.data, zs.ctypes.data, lrs.ctypes.data, mu.data_ptr(),
+                                                sigma.data_ptr(), initial.data_ptr(), mal.data_ptr(), mal.stride(0),
+                                                crafted.data_ptr(), None if bcast is None else bcast.data_ptr(), bs,
+                                                ld, ws.data_ptr(), ws.numel(), stream))
+    if problems and bcast is None:
+        _cast_rows(users_grads, crafted, fs, write)
     return crafted, mu, sigma
 
 

@@ -66,11 +66,14 @@ struct TmShape {
 // call derives on the host from that problem's corrupted_count and z.  The table of `batch` rows sits at the start of
 // the caller's workspace; the kernels read row blockIdx.y (Bulyan's rounds: blockIdx.x) when handed a table.
 struct ProblemParams {
-  int f;                  // corrupted_count: Bulyan's first-round keep, ALIE's rows
+  int f;                  // corrupted_count: Bulyan's first-round keep, ALIE's and the backdoor's rows
   int take;               // Krum: len(sorted(...)[:users_count - f])
-  int theta;              // Bulyan: users_count - 2f rounds
-  int write;              // ALIE: crafted is written over rows 0..f-1 (f > 0 and z != 0)
-  float z;                // ALIE: (float)z
+  union {                 // a table serves either a defence or an attack, so the row keeps its 40 bytes
+    int theta;            // Bulyan: users_count - 2f rounds
+    float lr;             // backdoor: (float)learning_rate
+  };
+  int write;              // ALIE, backdoor: crafted is written over rows 0..f-1 (f > 0 and z != 0)
+  float z;                // ALIE, backdoor: (float)z
   TmShape tm;             // TrimmedMean: n rows and f; Bulyan's second stage: theta rows and 2f
 };
 

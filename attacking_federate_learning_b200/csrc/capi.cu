@@ -138,6 +138,12 @@ int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, 
                    const ProblemParams* each, const float* agg, const int* idx, const int* sel, int sel_ld,
                    float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count,
                    void* partial, cudaStream_t stream);
+int backdoor_start(const void* G, int fmax, int64_t d, int64_t ld, int dtype, int batch, int64_t g_batch,
+                   const ProblemParams* each, const float* w, int64_t w_batch, float* mu_out, float* sigma_out,
+                   float* initial_out, cudaStream_t stream);
+int backdoor_finish(int batch, int64_t d, const ProblemParams* each, const float* mu, const float* sigma,
+                    const float* initial, const float* mal, int64_t mal_batch, float* crafted_out, float* bcast,
+                    int64_t bcast_batch, int64_t bcast_ld, cudaStream_t stream);
 }
 
 __global__ void add_f64_kernel(double* __restrict__ acc, const double* __restrict__ x, size_t n, int first) {
@@ -792,6 +798,71 @@ static int attack_metrics(const void* G, int batch, int64_t batch_stride, int n,
                                   static_cast<uint8_t*>(ws) + table_bytes(batch), stream);
 }
 
+// The backdoor's per-problem values (afl_backdoor_start_batched / _finish_batched): non-NULL, counts in [0, f_cap].
+static int backdoor_values(const char* who, int batch, const int* fs, int f_cap, const double* zs, const double* lrs,
+                           int* fmax) {
+  if (!zs || !lrs) { set_error("%s: the per-problem attack strengths or learning rates are NULL", who); return AFL_ERR_BAD_ARG; }
+  int fmin = 0;
+  return check_counts(who, fs, batch, f_cap, &fmin, fmax);
+}
+
+// Their table (f, (float)z, (float)lr, write) at the start of the workspace: the calls' first CUDA call.
+static int backdoor_table(const char* who, int batch, const int* fs, const double* zs, const double* lrs, void* ws,
+                          size_t ws_bytes, cudaStream_t stream, const ProblemParams** each) {
+  return upload_table(who, batch, ws, ws_bytes, table_bytes(batch), stream, [&](int b, ProblemParams& q) {
+    q.f = fs[b];
+    q.z = static_cast<float>(zs[b]);
+    q.lr = static_cast<float>(lrs[b]);
+    q.write = fs[b] > 0 && zs[b] != 0.0;               // malicious.py:20-21: z == 0 computes the statistics only
+  }, each);
+}
+
+static int backdoor_start(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                          const int* fs, const double* zs, const double* lrs, const float* w, int64_t w_batch_stride,
+                          float* mu_out, float* sigma_out, float* initial_out, void* ws, size_t ws_bytes,
+                          cudaStream_t stream) {
+  const char* who = "afl_backdoor_start_batched";
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
+  if (rc) return rc;
+  if (!w || !mu_out || !sigma_out || !initial_out) { set_error("%s: w and every output are required", who); return AFL_ERR_BAD_ARG; }
+  if (w_batch_stride < 0 || (w_batch_stride > 0 && w_batch_stride < d)) {
+    set_error("%s: w_batch_stride %lld must be 0 (one shared w) or >= d", who, static_cast<long long>(w_batch_stride));
+    return AFL_ERR_BAD_ARG;
+  }
+  int fmax = 0;
+  if ((rc = backdoor_values(who, batch, fs, n, zs, lrs, &fmax))) return rc;
+  const ProblemParams* each = nullptr;
+  if ((rc = backdoor_table(who, batch, fs, zs, lrs, ws, ws_bytes, stream, &each))) return rc;
+  return colstats::backdoor_start(G, fmax, d, ld, dtype, batch, batch_stride, each, w, w_batch_stride, mu_out,
+                                  sigma_out, initial_out, stream);
+}
+
+static int backdoor_finish(int batch, int64_t d, const int* fs, const double* zs, const double* lrs, const float* mu,
+                           const float* sigma, const float* initial, const float* mal, int64_t mal_batch_stride,
+                           float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* ws,
+                           size_t ws_bytes, cudaStream_t stream) {
+  const char* who = "afl_backdoor_finish_batched";
+  if (!mu || !sigma || !initial || !mal || !crafted_out || d < 1) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
+  if (batch < 1) { set_error("%s: batch must be >= 1 (got %d)", who, batch); return AFL_ERR_BAD_ARG; }
+  if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
+  if (batch > 1 && mal_batch_stride < d) {
+    set_error("%s: mal_batch_stride %lld makes problems overlap", who, static_cast<long long>(mal_batch_stride));
+    return AFL_ERR_BAD_ARG;
+  }
+  int fmax = 0;
+  int rc = backdoor_values(who, batch, fs, INT32_MAX, zs, lrs, &fmax);
+  if (rc) return rc;
+  if (bcast_rows && fmax > 0 &&
+      (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(fmax - 1) * bcast_ld + d))) {
+    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  const ProblemParams* each = nullptr;
+  if ((rc = backdoor_table(who, batch, fs, zs, lrs, ws, ws_bytes, stream, &each))) return rc;
+  return colstats::backdoor_finish(batch, d, each, mu, sigma, initial, mal, mal_batch_stride, crafted_out, bcast_rows,
+                                   bcast_batch_stride, bcast_ld, stream);
+}
+
 }  // namespace afl
 
 using namespace afl;
@@ -983,6 +1054,22 @@ int afl_attack_metrics_batched_each(const void* G, int batch, int64_t batch_stri
   return attack_metrics(G, batch, batch_stride, n, d, ld, dtype, 0, corrupted_counts, agg, idx, sel, sel_ld, dev_out,
                         sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
                         static_cast<cudaStream_t>(stream));
+}
+
+int afl_backdoor_start_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                               const int* f, const double* z, const double* lr, const float* w, int64_t w_batch_stride,
+                               float* mu_out, float* sigma_out, float* initial_out, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  return backdoor_start(G, batch, batch_stride, n, d, ld, dtype, f, z, lr, w, w_batch_stride, mu_out, sigma_out,
+                        initial_out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int afl_backdoor_finish_batched(int batch, int64_t d, const int* f, const double* z, const double* lr, const float* mu,
+                                const float* sigma, const float* initial, const float* mal, int64_t mal_batch_stride,
+                                float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  return backdoor_finish(batch, d, f, z, lr, mu, sigma, initial, mal, mal_batch_stride, crafted_out, bcast_rows,
+                         bcast_batch_stride, bcast_ld, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

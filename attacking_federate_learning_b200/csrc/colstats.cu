@@ -239,10 +239,17 @@ momentum_kernel(float* __restrict__ w, float* __restrict__ v, const float* __res
   }
 }
 
+// np.clip(v, lo, hi) = minimum(maximum(v, lo), hi) with NumPy's NaN propagation (backdoor.py:62-63).
+__device__ __forceinline__ float np_clip(float v, float lo, float hi) {
+  float r = fminf(fmaxf(v, lo), hi);
+  if (v != v || lo != lo || hi != hi) r = __int_as_float(0x7fc00000);
+  return r;
+}
+
 // ALIE band: lo = mu - z*sigma, hi = mu + z*sigma (fp32 product, fp32 sum: the roundings of
 // `grads_mean -/+ num_std * grads_stdev`).  x == nullptr: out = lo (malicious.py:35, DriftAttack);
-// otherwise out = np.clip(x, lo, hi) = minimum(maximum(x, lo), hi) with NumPy's NaN propagation
-// (backdoor.py:60-61).  out may alias mu or x (each element is read before it is written).
+// otherwise out = np_clip(x, lo, hi) (backdoor.py:62-63).  out may alias mu or x (each element is read before it is
+// written).
 __global__ void __launch_bounds__(kBlock)
 band_kernel(const float* mu, const float* sigma, float z, const float* x, float* out, int64_t d) {
   for (int64_t c = static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x; c < d;
@@ -251,10 +258,55 @@ band_kernel(const float* mu, const float* sigma, float z, const float* x, float*
     const float lo = __fsub_rn(m, zs);
     if (x == nullptr) { out[c] = lo; continue; }
     const float hi = __fadd_rn(m, zs);
-    const float v = x[c];
-    float r = fminf(fmaxf(v, lo), hi);
-    if (v != v || lo != lo || hi != hi) r = __int_as_float(0x7fc00000);
-    out[c] = r;
+    out[c] = np_clip(x[c], lo, hi);
+  }
+}
+
+// ---- backdoor crafting (backdoor.py:52-63) of a batch, problem b = blockIdx.y with lr = (float)learning_rate, z and f
+// from its table row; [batch][d] fp32 vectors at b * d.  The caller's model training (backdoor.py:56) runs between
+// the two kernels, so the crafting is two element-wise passes around it.
+//
+// start: initial = w - mu * lr (backdoor.py:54), w at b * w_batch (0: one vector shared by every problem).
+__global__ void __launch_bounds__(kBlock)
+backdoor_start_kernel(const float* __restrict__ mu, const float* __restrict__ w, int64_t w_batch, int64_t d,
+                      const ProblemParams* __restrict__ each, float* __restrict__ initial) {
+  const int64_t o = static_cast<int64_t>(blockIdx.y) * d;
+  const float lr = each[blockIdx.y].lr;
+  w += blockIdx.y * w_batch;
+  for (int64_t c = static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x; c < d;
+       c += static_cast<int64_t>(gridDim.x) * kBlock)
+    initial[o + c] = __fsub_rn(w[c], __fmul_rn(mu[o + c], lr));
+}
+
+// finish, for a problem that writes (f > 0, z != 0), with mal = the trained parameters (mal + b * mal_batch):
+//   step = mu * lr; new_params = mal + step (backdoor.py:59); new_grads = (initial - new_params) / lr (backdoor.py:60,
+//   IEEE division); crafted = np_clip(new_grads, mu - z*sigma, mu + z*sigma) (backdoor.py:62-63, band_kernel's roundings)
+// and, with bcast, crafted over rows 0..f-1 of bcast + b * bcast_batch (server.py:82-83).  Any other problem reads no
+// mal and writes no row: crafted = mu (z = 0: the statistics only; f = 0: mu is NaN).
+__global__ void __launch_bounds__(kBlock)
+backdoor_finish_kernel(const float* __restrict__ mu, const float* __restrict__ sigma, const float* __restrict__ initial,
+                       const float* mal, int64_t mal_batch, int64_t d, const ProblemParams* __restrict__ each,
+                       float* __restrict__ crafted_out, float* bcast, int64_t bcast_batch, int64_t bcast_ld) {
+  const ProblemParams& q = each[blockIdx.y];
+  const int64_t o = static_cast<int64_t>(blockIdx.y) * d;
+  const bool write = q.write != 0;
+  const int f = q.f;
+  const float lr = q.lr, z = q.z;
+  mal += blockIdx.y * mal_batch;
+  if (bcast) bcast += blockIdx.y * bcast_batch;
+  for (int64_t c = static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x; c < d;
+       c += static_cast<int64_t>(gridDim.x) * kBlock) {
+    const float m = mu[o + c];
+    float r = m;
+    if (write) {
+      const float step = __fmul_rn(m, lr);
+      const float g = __fdiv_rn(__fsub_rn(initial[o + c], __fadd_rn(mal[c], step)), lr);
+      const float zs = __fmul_rn(z, sigma[o + c]);
+      r = np_clip(g, __fsub_rn(m, zs), __fadd_rn(m, zs));
+      if (bcast)
+        for (int rr = 0; rr < f; ++rr) bcast[static_cast<int64_t>(rr) * bcast_ld + c] = r;
+    }
+    crafted_out[o + c] = r;
   }
 }
 
@@ -548,6 +600,37 @@ int alie_band(const float* mu, const float* sigma, double z, const float* x, flo
   if (blocks > 132 * 16) blocks = 132 * 16;
   band_kernel<<<static_cast<unsigned>(blocks), kBlock, 0, stream>>>(mu, sigma, static_cast<float>(z), x, out, d);
   AFL_LAUNCH_CHECK("band_kernel");
+  return AFL_OK;
+}
+
+// Grid of the backdoor's element-wise passes: column blocks (capped, the kernels stride) x problems.
+static dim3 backdoor_grid(int64_t d, int batch) {
+  int64_t blocks = ceil_div64(d, kBlock);
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  return dim3(static_cast<unsigned>(blocks), batch);
+}
+
+// The backdoor's statistics (afl_alie's per-problem pass on rows 0..f_b-1, nothing crafted or written), then initial.
+// fmax: the largest f_b.  Arguments checked by the caller (capi.cu).
+int backdoor_start(const void* G, int fmax, int64_t d, int64_t ld, int dtype, int batch, int64_t g_batch,
+                   const ProblemParams* each, const float* w, int64_t w_batch, float* mu_out, float* sigma_out,
+                   float* initial_out, cudaStream_t stream) {
+  int rc = alie_batched(G, fmax, d, ld, dtype, 0.0, mu_out, sigma_out, nullptr, nullptr, 0, batch, g_batch, d, 0,
+                        stream, each);
+  if (rc) return rc;
+  ProfScope ps("backdoor_start", stream);
+  backdoor_start_kernel<<<backdoor_grid(d, batch), kBlock, 0, stream>>>(mu_out, w, w_batch, d, each, initial_out);
+  AFL_LAUNCH_CHECK("backdoor_start_kernel");
+  return AFL_OK;
+}
+
+int backdoor_finish(int batch, int64_t d, const ProblemParams* each, const float* mu, const float* sigma,
+                    const float* initial, const float* mal, int64_t mal_batch, float* crafted_out, float* bcast,
+                    int64_t bcast_batch, int64_t bcast_ld, cudaStream_t stream) {
+  ProfScope ps("backdoor_finish", stream);
+  backdoor_finish_kernel<<<backdoor_grid(d, batch), kBlock, 0, stream>>>(mu, sigma, initial, mal, mal_batch, d, each,
+                                                                          crafted_out, bcast, bcast_batch, bcast_ld);
+  AFL_LAUNCH_CHECK("backdoor_finish_kernel");
   return AFL_OK;
 }
 

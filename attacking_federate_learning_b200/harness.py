@@ -4,6 +4,10 @@ Reference behaviour mirrored (file:line in /root/reference):
     main(...)                      main.py:12-100   build users + server, epoch loop, test every 5 epochs, CSV, checkpoint
     corrupted_count, is_malicious  main.py:21,28    malicious ids are 0..int(mal_prop*N)-1
     epoch body                     main.py:64-71    dispatch_weights -> attacker.attack(mal_users) -> collect -> defend
+    attacker                       main.py:44-54    -b pattern|1|2|3: BackdoorAttack (alpha 4, 5 malicious epochs,
+                                                    main.py:139-142) with backdoor.py:13-159's training restated on
+                                                    the synthetic data (BackdoorTrainer); otherwise DriftAttack (ALIE)
+    backdoor check                 main.py:91-95    the global model tested on the backdoor data ('POST') at every test
     learning-rate fading           server.py:50-52  lr_t = lr * fading / (epoch + fading) for the CLIENT optimiser only;
                                                     the server step uses the base rate (server.py:89, reproduced)
     test                           server.py:92-112 sum of per-batch NLL / dataset size, argmax accuracy
@@ -17,6 +21,7 @@ device-resident N x D matrix (ingest.ParamLayout: user.py:17-28 order), so attac
 leave the device.  The training simulation itself is not part of the accelerated path (SURVEY 2).
 
     python -m attacking_federate_learning_b200.harness -d Krum -e 30 --users-count 10
+    python -m attacking_federate_learning_b200.harness -d Krum -e 30 -z 1.0 -b pattern
 """
 from __future__ import annotations
 
@@ -88,8 +93,62 @@ class Client:
         self.grads = out_row
 
 
+class BackdoorTrainer:
+    """backdoor.py:13-159 on the synthetic problem: the attacker's own network, trained from the starting point the
+    crafting hands it towards the backdoor, and tested on the backdoor data.  backdoor='pattern': a shard of the
+    training set with x[:, :5, :5] = 2.8 on the 28x28 view, all labelled 0; backdoor = 1, 2 or 3: the single training
+    sample backdoor - 1, labelled (y + 1) % 5."""
+
+    def __init__(self, backdoor, alpha, num_epochs, layout, x, y, device, my_print, seed=0, batch_size=200):
+        self.backdoor, self.alpha, self.num_epochs, self.layout, self.my_print = backdoor, alpha, num_epochs, layout, my_print
+        self.batch_size = batch_size
+        self.net = MnistNet().to(device)
+        if backdoor == 'pattern':                                         # backdoor.py:37-42, 47-50
+            u = max(len(x) // batch_size // 10, 1)
+            x = x[int(np.random.default_rng(seed).integers(u))::u].clone()
+            x.view(-1, 28, 28)[:, :5, :5] = 2.8
+            y = torch.zeros_like(y[:len(x)])
+        else:                                                             # backdoor.py:30-35
+            i = int(backdoor) - 1
+            x, y = x[i:i + 1], (y[i:i + 1] + 1) % 5
+        self.x, self.y = x, y
+
+    def test(self, tag, to_print=True):                                   # backdoor.py:67-102
+        loss, correct = 0.0, 0
+        with torch.no_grad():
+            for lo in range(0, len(self.x), self.batch_size):
+                out = self.net(self.x[lo:lo + self.batch_size])
+                loss += F.nll_loss(out, self.y[lo:lo + self.batch_size]).item()
+                correct += int(out.max(1)[1].eq(self.y[lo:lo + self.batch_size]).sum())
+        accuracy = 100. * correct / len(self.x)
+        if to_print:
+            self.my_print('##Test malicious net: [{}] Average loss: {:.4f}, Accuracy: {}/{} ({:.2f}%)'.format(
+                tag, loss / len(self.x), correct, len(self.x), accuracy))
+        return accuracy
+
+    def train(self, initial):                                             # backdoor.py:108-159
+        params = list(self.net.parameters())
+        self.layout.row_into_parameters(initial, params)
+        p0 = [p.detach().clone() for p in params]
+        if self.test('BEFORE', to_print=False) >= 100.:
+            return initial
+        self.net.train()
+        for _ in range(self.num_epochs):
+            for lo in range(0, len(self.x), self.batch_size):
+                opt = torch.optim.SGD(params, lr=0.1, momentum=0.9, weight_decay=0.0001)   # a new one every minibatch
+                opt.zero_grad()
+                loss = F.nll_loss(self.net(self.x[lo:lo + self.batch_size]), self.y[lo:lo + self.batch_size])
+                if self.alpha > 0:
+                    loss = loss + self.alpha * sum(F.mse_loss(p, q) for p, q in zip(params, p0))
+                loss.backward()
+                opt.step()
+        self.test(self.num_epochs - 1)
+        return self.layout.flatten(params)
+
+
 def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0.1, fading_rate=10000, momentum=0.9,
-         batch_size=83, output=None, device="cuda", out_dir=".", seed=0, train_size=20000, test_size=4000, test_step=5):
+         batch_size=83, output=None, device="cuda", out_dir=".", seed=0, train_size=20000, test_size=4000, test_step=5,
+         backdoor=False, alpha=4, mal_epochs=5):
     if output:
         def my_print(s, end='\n'):
             with open(output, 'a+') as f:
@@ -97,7 +156,7 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     else:
         my_print = print
     my_print(dict(mal_prop=mal_prop, num_std=num_std, defense=defense, users_count=users_count, epochs=epochs,
-                  learning_rate=learning_rate, dataset=SYNTH))
+                  learning_rate=learning_rate, dataset=SYNTH, backdoor=backdoor))
     torch.manual_seed(seed)
     corrupted_count = int(mal_prop * users_count)                         # main.py:21
     (xtr, ytr), (xte, yte) = synthetic_problem(train_size, test_size, device, seed)
@@ -107,7 +166,11 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
                             initial_weights=layout.flatten(list(test_net.parameters())))
     users = [Client(u, u < corrupted_count, xtr[u::users_count], ytr[u::users_count], batch_size, layout, device)
              for u in range(users_count)]                                 # DistributedSampler-style partition (user.py:50)
-    attacker = malicious.DriftAttack(num_std)
+    if backdoor:                                                          # main.py:44-54
+        trainer = BackdoorTrainer(backdoor, alpha, mal_epochs, layout, xtr, ytr, device, my_print, seed)
+        attacker = malicious.BackdoorAttack(num_std, trainer.train)
+    else:
+        attacker = malicious.DriftAttack(num_std)
     my_print("\nStarting Training...")
     criterion = nn.NLLLoss()
     accuracies, accuracies_epochs = [], []
@@ -115,7 +178,10 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
         lr_t = learning_rate * fading_rate / (epoch + fading_rate)       # server.py:50-52
         for u in users:                                                   # server.py:54-56 dispatch_weights
             u.step(srv.current_weights, lr_t, srv.users_grads[u.user_id])
-        attacker.attack_rows(srv.users_grads, corrupted_count)            # main.py:66-68 + server.py:82-83, in place
+        if backdoor:                                                      # main.py:66-68 + server.py:82-83, in place
+            attacker.attack_rows(srv.users_grads, corrupted_count, users[0].original_params, users[0].learning_rate)
+        else:
+            attacker.attack_rows(srv.users_grads, corrupted_count)
         srv.defend(defense, epoch)                                        # main.py:71
         if epoch % test_step == 0 or epoch == epochs - 1:
             layout.row_into_parameters(srv.current_weights, list(test_net.parameters()))
@@ -137,11 +203,14 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
                 os.makedirs(directory, exist_ok=True)
                 torch.save({'epoch': epoch + 1, 'state_dict': test_net.state_dict(), 'acc': accuracy},
                            os.path.join(directory, 'checkpoint.pth.tar'))
+            if backdoor:                                                  # main.py:91-95: the backdoor in the global model
+                layout.row_into_parameters(srv.current_weights, list(trainer.net.parameters()))
+                trainer.test('POST')
     my_print(datetime.datetime.now().time())
     my_print("Max accuracy: {}".format(max(accuracies)))
     os.makedirs(os.path.join(out_dir, "logs"), exist_ok=True)             # the reference needs a pre-made logs/ (readme.md:25)
     csv = os.path.join(out_dir, 'logs', '{}_stdev_{}_{}_backdoor-{}_mal_prop_{}_users_{}_alpha_{}_lr_{}.csv'.format(
-        SYNTH, num_std, defense, False, mal_prop, users_count, None, learning_rate))
+        SYNTH, num_std, defense, backdoor, mal_prop, users_count, alpha if backdoor else None, learning_rate))
     np.savetxt(csv, accuracies, delimiter=',')                            # main.py:100
     return accuracies, accuracies_epochs, csv
 
@@ -156,6 +225,8 @@ if __name__ == '__main__':
     p.add_argument('-e', '--epochs', default=300, type=int)
     p.add_argument('-l', '--learning_rate', default=0.1, type=float)
     p.add_argument('-o', '--output', type=str)
+    p.add_argument('-b', '--backdoor', default='No', choices=['No', 'pattern', '1', '2', '3'])
     a = p.parse_args()
+    bd = False if a.backdoor == 'No' else a.backdoor if a.backdoor == 'pattern' else int(a.backdoor)
     main(a.mal_prop, a.num_std, a.defense, users_count=a.users_count, epochs=a.epochs, learning_rate=a.learning_rate,
-         batch_size=a.batch_size, output=a.output)
+         batch_size=a.batch_size, output=a.output, backdoor=bd)

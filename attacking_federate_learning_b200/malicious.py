@@ -11,7 +11,9 @@ malicious user holds THE SAME array object; for DriftAttack that object is also 
 (mutated in place); `self.grads_stdev` keeps sigma.  All arithmetic runs on the GPU.  With NumPy
 gradients `attack()` streams column slabs of the users' own arrays to the device (`afl_alie_host`, within
 the host-buffer budget of `defences.py`), so no stacked f x D copy exists on the host or the device; the
-statistics come back as NumPy vectors.
+statistics come back as NumPy vectors.  `attack_rows` is the GPU-resident form for a stacked matrix whose rows 0..f-1
+are the malicious users: the fused drift kernel for DriftAttack, and for BackdoorAttack the backdoor kernels around
+one call of the training (`batched.backdoor_rows` with one problem).
 """
 from __future__ import annotations
 
@@ -156,6 +158,28 @@ class BackdoorAttack(Attack):
         new_grads = (initial - new_params) / torch.tensor(learning_rate, dtype=torch.float32, device=mu.device)   # backdoor.py:60
         out = dev.alie_band(mu, sd, self.num_std, new_grads.contiguous())            # backdoor.py:62-63
         return out if on_gpu else out.cpu().numpy()
+
+    def attack_rows(self, users_grads, corrupted_count, original_params=None, learning_rate=None):
+        """GPU-resident form of attack() (backdoor.py:52-63): the malicious users are rows 0..f-1 of the stacked
+        matrix (main.py:28); `original_params` (fp32 CUDA [D]) and `learning_rate` are what users[0] carries.  Computes
+        the statistics and the crafted vector on the device, calling `train_malicious_network` once in between with
+        a fp32 CUDA [D] vector (it must return one), and writes the crafted vector into those rows in place
+        (server.py:82-83).  Sets grads_mean and grads_stdev and returns the crafted vector; None when
+        corrupted_count <= 0, and None after the statistics when num_std == 0 (malicious.py:20-21)."""
+        if corrupted_count <= 0:                            # malicious.py:11-12: no malicious user, nothing to craft
+            return None
+        if original_params is None or learning_rate is None:
+            raise TypeError("BackdoorAttack.attack_rows needs original_params and learning_rate (backdoor.py:52)")
+        import torch
+        from . import batched
+
+        def train(initial, problems):
+            mal = self.train_malicious_network(initial[0])
+            return mal[None] if isinstance(mal, torch.Tensor) else mal
+        crafted, mu, sigma = batched.backdoor_rows(users_grads[None], corrupted_count, self.num_std, original_params,
+                                                   learning_rate, train)
+        self.grads_mean, self.grads_stdev = mu[0], sigma[0]
+        return None if self.num_std == 0 else crafted[0]
 
 
 def backdoor_clip(new_grads, grads_mean, grads_stdev, num_std):

@@ -339,6 +339,41 @@ int afl_attack_metrics_batched_each(const void* G, int batch, int64_t batch_stri
                                     int* krum_hit, int* mal_count, int* sel_count, void* workspace,
                                     size_t workspace_bytes, void* stream);
 
+/* ---- backdoor attack of a batch (backdoor.py:52-63, BackdoorAttack._attack_grads driven by malicious.py:10-27) -----
+ * The crafting calls the attacker's model training (backdoor.py:56) in the middle, so it is two calls with the
+ * caller's training between them.  Per problem b, with f_b = f[b], z_b = (float)z[b], lr_b = (float)lr[b] (HOST arrays
+ * of `batch` values, copied into a parameter table at the start of the workspace as the other per-problem calls do):
+ *   mu, sigma = afl_alie's statistics of rows 0..f_b-1 of G + b * batch_stride     malicious.py:17-18
+ *   step      = mu * lr_b;  initial = w_b - step                                      backdoor.py:54
+ *   mal       = the caller's training started from initial                          backdoor.py:56
+ *   new_g     = (initial - (mal + step)) / lr_b  (IEEE division)                     backdoor.py:59-60
+ *   crafted   = np.clip(new_g, mu - z_b*sigma, mu + z_b*sigma)  (NaN rules of afl_alie_band)   backdoor.py:62-63
+ * and crafted is written over rows 0..f_b-1 (server.py:82-83), every operation one fp32 rounding as in the reference.
+ * f_b = 0: NaN mu, sigma and crafted, no row read or written (malicious.py:11-12); z_b = 0: the statistics only,
+ * crafted = mu, no row written (malicious.py:20-21).  Negative z_b and lr_b = 0 get what NumPy gives.
+ *
+ * afl_backdoor_start_batched — problems of n rows (no client limit: the pass is column-wise), f_b <= n, dtype fp32,
+ * bf16 or fp16, batch_stride and batch <= 65535 as afl_defend_batched.  w: device fp32 params at w + b * w_batch_stride
+ * (0: one [d] vector for every problem, else >= d).  Writes mu_out, sigma_out (afl_alie_batched_each's, bit for bit) and
+ * initial_out, each device fp32[batch][d].
+ * afl_backdoor_finish_batched — mu, sigma, initial as the start call left them; mal: device fp32 trained parameters at
+ * mal + b * mal_batch_stride (>= d when batch > 1; read only for problems with f_b > 0 and z_b != 0).  Writes
+ * crafted_out (device fp32[batch][d]) and, when bcast_rows is given (an fp32 matrix: a 16-bit one is written by the
+ * caller), rows 0..f_b-1 of bcast_rows + b * bcast_batch_stride (pitch bcast_ld) of those problems.
+ * Workspace of both: the table alone, afl_batched_each_workspace_bytes("ALIE", batch, 1, d, dtype) bytes (its size
+ * depends on batch only, so any n <= 128 gives it), 256-byte aligned.  Device pointers; the calls only enqueue work.  Checked before any CUDA call: a NULL pointer
+ * (outputs included; bcast_rows may be NULL), d < 1, batch < 1, f_b < 0 (start: f_b > n), a short batch_stride,
+ * w_batch_stride, mal_batch_stride, bcast_ld or bcast_batch_stride -> AFL_ERR_BAD_ARG; batch > 65535 or another dtype
+ * code -> AFL_ERR_UNSUPPORTED; a short or misaligned workspace -> AFL_ERR_WORKSPACE. */
+int afl_backdoor_start_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                               const int* f, const double* z, const double* lr, const float* w, int64_t w_batch_stride,
+                               float* mu_out, float* sigma_out, float* initial_out, void* workspace,
+                               size_t workspace_bytes, void* stream);
+int afl_backdoor_finish_batched(int batch, int64_t d, const int* f, const double* z, const double* lr, const float* mu,
+                                const float* sigma, const float* initial, const float* mal, int64_t mal_batch_stride,
+                                float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld,
+                                void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,6 +13,12 @@ per problem (C ABI `afl_defend_batched_each` / `afl_alie_batched_each`), so that
 share and z runs as one batch.  Nothing here synchronises the host except `bulyan`, which checks for a failed
 selection round as `defences.bulyan` does.
 
+Every defence and `attack_metrics` also take `rows=` (B host ints, 1 <= rows_b <= N): a ragged batch, where problem b
+is `G[b, :rows_b]` and rows rows_b..N-1 are padding that no result depends on (C ABI `afl_defend_batched_rows` /
+`afl_attack_metrics_batched_rows`).  So a grid over the number of users (main.py:118), or rounds in which a different
+number of clients reports, runs as one batch; `users_count` may then be B values too and defaults to `rows`, the
+`len(self.users)` that `Server.defend` passes (server.py:87).
+
 `backdoor_rows` is the per-problem `BackdoorAttack.attack_rows`: the backdoor crafting of every problem in three
 launches, with one call of the caller's malicious-network training between the second and the third.  It has no
 client limit.
@@ -63,9 +69,34 @@ def _per_problem(x, B: int, name: str, dtype):
     return np.ascontiguousarray(a, dtype=dtype)
 
 
-def _defend(rule: str, G: torch.Tensor, users_count: int, corrupted_count, out=None, idx=None, sel=None):
+def _full(x, B: int, name: str):
+    """B per-problem int32 host values of x (one number or B of them)."""
+    a = _per_problem(x, B, name, np.int32)
+    return np.full(B, int(x), np.int32) if a is None else a
+
+
+def _ragged(B: int, rows, users_count, corrupted_count):
+    """(rows, users_count, corrupted_count) of a ragged batch as int32 host arrays; users_count defaults to rows."""
+    rs = _full(rows, B, "rows")
+    return rs, (rs if users_count is None else _full(users_count, B, "users_count")), \
+        _full(corrupted_count, B, "corrupted_count")
+
+
+def _defend(rule: str, G: torch.Tensor, users_count: int, corrupted_count, out=None, idx=None, sel=None, rows=None):
     B, N, D, ld, bs = _check(G)
     L = nat.lib()
+    if rows is not None:
+        rs, ucs, fs = _ragged(B, rows, users_count, corrupted_count)
+        with torch.cuda.device(G.device):
+            nbytes = L.afl_batched_rows_workspace_bytes(rule.encode(), B, N, D, dtype_code(G))
+            ws = Workspace.get(G.device, "batched", nbytes)
+            nat.check(L.afl_defend_batched_rows(rule.encode(), G.data_ptr(), B, bs, N, D, ld, dtype_code(G),
+                                                rs.ctypes.data, ucs.ctypes.data, fs.ctypes.data,
+                                                None if out is None else out.data_ptr(),
+                                                None if idx is None else idx.data_ptr(),
+                                                None if sel is None else sel.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                _stream_ptr(G)))
+        return
     fs = _per_problem(corrupted_count, B, "corrupted_count", np.int32)
     with torch.cuda.device(G.device):
         if fs is not None:
@@ -87,40 +118,56 @@ def _defend(rule: str, G: torch.Tensor, users_count: int, corrupted_count, out=N
                                        _stream_ptr(G)))
 
 
-def krum(users_grads, users_count, corrupted_count, return_index=False):
+def krum(users_grads, users_count, corrupted_count, return_index=False, *, rows=None):
     """Per problem defences.krum (corrupted_count: one int or B of them): the winning rows `G[arange(B), idx]`
     ([B, D], input dtype), or with return_index the device int32 [B] indices (-1 where no user is eligible).
+    With rows, problem b is G[b, :rows_b] and index -1 returns its row rows_b - 1 (the reference's users_grads[-1]).
     No host synchronisation."""
     B = users_grads.shape[0]
-    idx = torch.empty(B, dtype=torch.int32, device=users_grads.device)
-    _defend(DefenseTypes.Krum, users_grads, users_count, corrupted_count, idx=idx)
+    dev = users_grads.device
+    idx = torch.empty(B, dtype=torch.int32, device=dev)
+    _defend(DefenseTypes.Krum, users_grads, users_count, corrupted_count, idx=idx, rows=rows)
     if return_index:
         return idx
-    return users_grads[torch.arange(B, device=users_grads.device), idx.long()]
+    row = idx.long()
+    if rows is not None:
+        last = torch.from_numpy(_full(rows, B, "rows").astype(np.int64) - 1).pin_memory().to(dev, non_blocking=True)
+        row = torch.where(row < 0, last, row)
+    return users_grads[torch.arange(B, device=dev), row]
 
 
-def trimmed_mean(users_grads, users_count, corrupted_count):
-    """Per problem defences.trimmed_mean: fp32 [B, D]."""
+def trimmed_mean(users_grads, users_count, corrupted_count, *, rows=None):
+    """Per problem defences.trimmed_mean: fp32 [B, D].  With rows, over G[b, :rows_b]."""
     B, _, D = users_grads.shape
     out = torch.empty((B, D), dtype=torch.float32, device=users_grads.device)
-    _defend(DefenseTypes.TrimmedMean, users_grads, users_count, corrupted_count, out=out)
+    _defend(DefenseTypes.TrimmedMean, users_grads, users_count, corrupted_count, out=out, rows=rows)
     return out
 
 
-def no_defense(users_grads, users_count, corrupted_count):
-    """Per problem defences.no_defense: fp32 [B, D]."""
+def no_defense(users_grads, users_count, corrupted_count, *, rows=None):
+    """Per problem defences.no_defense: fp32 [B, D].  With rows, the mean of G[b, :rows_b]."""
     B, _, D = users_grads.shape
     out = torch.empty((B, D), dtype=torch.float32, device=users_grads.device)
-    _defend(DefenseTypes.NoDefense, users_grads, users_count, corrupted_count, out=out)
+    _defend(DefenseTypes.NoDefense, users_grads, users_count, corrupted_count, out=out, rows=rows)
     return out
 
 
-def bulyan(users_grads, users_count, corrupted_count, return_selection=False):
+def bulyan(users_grads, users_count, corrupted_count, return_selection=False, *, rows=None):
     """Per problem defences.bulyan: fp32 [B, D] and, with return_selection, the int32 [B, theta] selections.
     With one corrupted_count per problem the selections are [B, theta_max], theta_max = users_count - 2 min(f):
     problem b's theta_b = users_count - 2 f_b rounds, then -2 ("no such round").  Raises KeyError(-1) when any
-    problem's last round is -1 (a round found no eligible user), as `defences.bulyan` does for one problem."""
+    problem's last round is -1 (a round found no eligible user), as `defences.bulyan` does for one problem.
+    With rows, problem b is G[b, :rows_b] with users_count_b == rows_b, and theta_max = max_b(users_count_b - 2 f_b)."""
     B, _, D = users_grads.shape
+    if rows is not None:
+        rs, ucs, fs = _ragged(B, rows, users_count, corrupted_count)
+        theta = ucs.astype(np.int64) - 2 * fs
+        out = torch.empty((B, D), dtype=torch.float32, device=users_grads.device)
+        sel = torch.empty((B, max(int(theta.max()), 1) if B else 1), dtype=torch.int32, device=users_grads.device)
+        _defend(DefenseTypes.Bulyan, users_grads, ucs, fs, out=out, sel=sel, rows=rs)
+        if bool((sel.cpu()[torch.arange(B), torch.from_numpy(theta - 1)] < 0).any()):   # defences.py:66
+            raise KeyError(-1)
+        return (out, sel) if return_selection else out
     fs = _per_problem(corrupted_count, B, "corrupted_count", np.int32)
     if fs is None:
         assert users_count >= 4 * corrupted_count + 3
@@ -146,7 +193,8 @@ defend = {DefenseTypes.Krum: krum,
 
 def alie_rows(users_grads, corrupted_count, num_std):
     """Per problem malicious.Attack.attack_rows (DriftAttack): the malicious users are rows 0..f-1 of every
-    problem.  Returns (crafted, mu, sigma), each fp32 [B, D] (mu is the unperturbed mean), and writes crafted
+    problem.  A ragged batch (rows_b clients in problem b, as the defences' `rows=`) needs no extra argument: the
+    attack reads and writes rows 0..f_b-1 only, so f_b <= rows_b is all it asks.  Returns (crafted, mu, sigma), each fp32 [B, D] (mu is the unperturbed mean), and writes crafted
     = mu - num_std * sigma into those rows in place (fp32 directly; bf16 and fp16 through a cast, as attack_rows does).
     With num_std == 0 the rows are left alone, as attack_rows does.  None when corrupted_count <= 0.
 
@@ -207,7 +255,7 @@ def _cast_rows(users_grads, crafted, fs, write):
 
 def backdoor_rows(users_grads, corrupted_count, num_std, original_params, learning_rate, train_malicious_network):
     """Per problem malicious.BackdoorAttack.attack_rows (backdoor.py:52-63): the malicious users are rows 0..f_b-1 of
-    problem b.  Returns (crafted, mu, sigma), each fp32 [B, D] (mu is the malicious rows' mean), and writes crafted into
+    problem b (which is all a ragged batch needs: no `rows` argument, f_b <= rows_b).  Returns (crafted, mu, sigma), each fp32 [B, D] (mu is the malicious rows' mean), and writes crafted into
     those rows in place (fp32 directly; bf16 and fp16 through a cast).  Any number of clients.
 
     corrupted_count, num_std and learning_rate are each one number or B host values (as `alie_rows`), f_b <= N.
@@ -269,7 +317,7 @@ def backdoor_rows(users_grads, corrupted_count, num_std, original_params, learni
 
 
 def attack_metrics(users_grads, corrupted_count, *, aggregated=None, krum_index=None, selection=None,
-                   return_honest_mean=False):
+                   return_honest_mean=False, rows=None):
     """Attack-success figures of every problem (C ABI `afl_attack_metrics_batched` / `_each`), as a dict of device
     tensors.  The malicious users are rows 0..f_b-1 (main.py:28); corrupted_count is one int or B host values.
 
@@ -283,8 +331,11 @@ def attack_metrics(users_grads, corrupted_count, *, aggregated=None, krum_index=
     * return_honest_mean adds `honest_mean` [B, D] fp32.
 
     f_b >= N (no honest row) and krum_index -1 give NaN deviations.  No host synchronisation.  One problem: pass
-    `G[None]`."""
+    `G[None]`.  rows (B host ints, C ABI `afl_attack_metrics_batched_rows`): a ragged batch, problem b being
+    G[b, :rows_b], so its honest rows are f_b..rows_b-1."""
     fs = _per_problem(corrupted_count, users_grads.shape[0], "corrupted_count", np.int32)
+    if rows is not None:
+        rs, _, fs = _ragged(users_grads.shape[0], rows, None, corrupted_count)
     B, N, D, ld, bs = _check(users_grads)
     dev = users_grads.device
 
@@ -313,8 +364,12 @@ def attack_metrics(users_grads, corrupted_count, *, aggregated=None, krum_index=
     code = dtype_code(users_grads)
     with torch.cuda.device(dev):
         ws = Workspace.get(dev, "metrics", L.afl_metrics_workspace_bytes(B, N, D, code))
-        call, f = (L.afl_attack_metrics_batched, int(corrupted_count)) if fs is None else \
-            (L.afl_attack_metrics_batched_each, fs.ctypes.data)
+        if rows is not None:
+            call, f = (lambda *a: L.afl_attack_metrics_batched_rows(*a[:7], rs.ctypes.data, *a[7:])), fs.ctypes.data
+        elif fs is None:
+            call, f = L.afl_attack_metrics_batched, int(corrupted_count)
+        else:
+            call, f = L.afl_attack_metrics_batched_each, fs.ctypes.data
         nat.check(call(users_grads.data_ptr(), B, bs, N, D, ld, code, f, *ptrs[:3], 0 if sel is None else sel.shape[1],
                        *ptrs[3:], ws.data_ptr(), ws.numel(), _stream_ptr(users_grads)))
     res = {}

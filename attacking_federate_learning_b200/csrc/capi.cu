@@ -97,7 +97,7 @@ size_t workspace_bytes(int n, int64_t d, int dtype, int flags, int batch);
 int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, double* d2_out, void* ws, size_t ws_bytes,
                    int flags, cudaStream_t stream);
 int sqdist_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, double* d2_out,
-                   void* ws, size_t ws_bytes, int flags, cudaStream_t stream);
+                   void* ws, size_t ws_bytes, int flags, cudaStream_t stream, const ProblemParams* rows = nullptr);
 int sqdist_to_dist(const double* d2, int n, float* dist, cudaStream_t stream, int batch = 1);
 }
 namespace select {
@@ -107,9 +107,12 @@ size_t workspace_bytes(int n, int batch);
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
                 void* ws, size_t ws_bytes, cudaStream_t stream);
 int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
-                     size_t ws_bytes, cudaStream_t stream, int batch = 1, const ProblemParams* each = nullptr);
+                     size_t ws_bytes, cudaStream_t stream, int batch = 1, const ProblemParams* each = nullptr,
+                     bool rows = false);
 int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out, void* ws, size_t ws_bytes,
                   cudaStream_t stream, int batch = 1, const ProblemParams* each = nullptr);
+int bulyan_rounds(const float* dist, int n, int f, int theta, int* sel_out, void* ws, size_t ws_bytes,
+                  cudaStream_t stream, int batch, const ProblemParams* each, bool rows);
 int krum_take(int n, int users_count, int corrupted_count);
 }
 namespace tmean {
@@ -123,7 +126,7 @@ TmShape shape(int n_rows, int corrupted_count);
 namespace colstats {
 int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream);
 int mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, int batch, int64_t g_batch,
-                 int64_t out_batch, cudaStream_t stream);
+                 int64_t out_batch, cudaStream_t stream, const ProblemParams* rows = nullptr);
 int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
          float* crafted_out, float* bcast, int64_t bcast_ld, cudaStream_t stream);
 int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
@@ -137,7 +140,7 @@ int64_t deviation_tiles(int64_t d, int dtype);
 int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, int64_t ld, int dtype, int f,
                    const ProblemParams* each, const float* agg, const int* idx, const int* sel, int sel_ld,
                    float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count,
-                   void* partial, cudaStream_t stream);
+                   void* partial, cudaStream_t stream, bool rows = false);
 int backdoor_start(const void* G, int fmax, int64_t d, int64_t ld, int dtype, int batch, int64_t g_batch,
                    const ProblemParams* each, const float* w, int64_t w_batch, float* mu_out, float* sigma_out,
                    float* initial_out, cudaStream_t stream);
@@ -727,6 +730,85 @@ static int defend_batched(const char* rule, const void* G, int batch, int64_t ba
                                      stream, each);
 }
 
+// A ragged batch (afl_defend_batched_rows): problem b is rows 0..rows[b]-1 of its n-row slot, with its own users_count
+// ucs[b] and corrupted count fs[b].  Every check is the single call's, per problem and before any CUDA call; the table
+// rows come from the single call's host helpers on (rows[b], ucs[b], fs[b]), and each kernel reads the problem's row
+// count from them: tm.n_rows (the Gram centre, Krum, TrimmedMean, NoDefense), theta + 2f (Bulyan's selection, whose
+// users_count is its row count).  Bulyan's second stage needs tm = shape(theta, 2f): that table is copied over the
+// first one after the selection kernels, in stream order.  The workspace layout is afl_defend_batched_each's.
+static int defend_batched_rows(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                               int64_t ld, int dtype, const int* rows, const int* ucs, const int* fs, float* out,
+                               int* idx_out, int* sel_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  const char* who = "afl_defend_batched_rows";
+  const BatchedRule r = batched_rule(rule);
+  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
+  if (rc) return rc;
+  if (!rows || !ucs) { set_error("%s: the per-problem row counts or users counts are NULL", who); return AFL_ERR_BAD_ARG; }
+  int fmin = 0, fmax = 0;
+  if ((rc = check_counts(who, fs, batch, INT32_MAX / 4, &fmin, &fmax))) return rc;
+  for (int b = 0; b < batch; ++b)
+    if (rows[b] < 1 || rows[b] > n) {
+      set_error("%s: row count %d of problem %d is outside [1, %d]", who, rows[b], b, n);
+      return AFL_ERR_BAD_ARG;
+    }
+  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out)) {
+    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
+    return AFL_ERR_BAD_ARG;
+  }
+  int theta_max = 0;
+  for (int b = 0; b < batch; ++b) {
+    // the reference's asserts (defences.py:24-25, 56), per problem
+    const int64_t need = r == B_KRUM ? 2 * static_cast<int64_t>(fs[b]) + 1 : r == B_BULYAN ? 4 * static_cast<int64_t>(fs[b]) + 3 : 0;
+    if (ucs[b] < need) {
+      set_error("%s violated (%d, %d) in problem %d",
+                r == B_KRUM ? "krum: users_count >= 2*corrupted_count + 1" : "bulyan: users_count >= 4*corrupted_count + 3",
+                ucs[b], fs[b], b);
+      return AFL_ERR_PRECONDITION;
+    }
+    if (r == B_BULYAN && ucs[b] != rows[b]) {
+      set_error("%s: Bulyan's users_count (%d) must equal the number of rows (%d) in problem %d", who, ucs[b], rows[b], b);
+      return AFL_ERR_UNSUPPORTED;
+    }
+    const int theta = ucs[b] - 2 * fs[b];
+    theta_max = theta > theta_max ? theta : theta_max;
+  }
+  size_t gram_ws = 0, tabs = 0;
+  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  const ProblemParams* each = nullptr;
+  auto row = [&](int b, ProblemParams& q) {
+    q.f = fs[b];
+    q.take = select::krum_take(rows[b], ucs[b], fs[b]);
+    q.theta = ucs[b] - 2 * fs[b];
+    q.tm = tmean::shape(rows[b], fs[b]);
+  };
+  rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch) + rule_ws, stream, row, &each);
+  if (rc) return rc;
+  uint8_t* p = static_cast<uint8_t*>(ws) + table_bytes(batch);
+  if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, each);
+  if (r == B_TM)
+    return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, fmin, out, batch, batch_stride, 0, d, stream, each);
+  const size_t nn = static_cast<size_t>(batch) * n * n;
+  double* d2 = reinterpret_cast<double*>(p);
+  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
+  void* sel_ws = p + tabs + gram_ws;
+  const size_t sel_ws_bytes = ws_bytes - table_bytes(batch) - tabs - gram_ws;
+  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream, each);
+  if (rc) return rc;
+  if (r == B_KRUM)
+    return select::krum_from_sqdist(d2, n, 0, 0, idx_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
+  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
+  rc = select::bulyan_rounds(dist, n, fmin, theta_max, sel_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
+  if (rc) return rc;
+  rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch) + rule_ws, stream, [&](int b, ProblemParams& q) {
+    row(b, q);
+    q.tm = tmean::shape(q.theta, 2 * fs[b]);              // the trimmed mean of the theta_b selected rows with 2 f_b
+  }, &each);
+  if (rc) return rc;
+  return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, theta_max, 2 * fmin, out, batch, batch_stride, theta_max,
+                                     d, stream, each);
+}
+
 // fs == NULL: rows 0..f-1 and z in every problem of f-row problems (afl_alie_batched).  Otherwise problem b has n rows of
 // which fs[b] are malicious, and its own z (afl_alie_batched_each); the workspace holds the table.
 static int alie_batched(const char* who, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
@@ -764,15 +846,21 @@ static size_t metrics_partial_bytes(int batch, int64_t d, int dtype) {
   return align_up(static_cast<size_t>(batch) * colstats::deviation_tiles(d, dtype) * sizeof(double2), 256);
 }
 
+// rows != NULL (afl_attack_metrics_batched_rows, fs required): problem b has rows[b] rows, in [1, n].
 static int attack_metrics(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, int f,
                           const int* fs, const float* agg, const int* idx, const int* sel, int sel_ld, float* dev_out,
                           double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* ws,
-                          size_t ws_bytes, cudaStream_t stream) {
-  const char* who = fs ? "afl_attack_metrics_batched_each" : "afl_attack_metrics_batched";
+                          size_t ws_bytes, cudaStream_t stream, const int* rows = nullptr) {
+  const char* who = rows ? "afl_attack_metrics_batched_rows" : fs ? "afl_attack_metrics_batched_each" : "afl_attack_metrics_batched";
   int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
   if (rc) return rc;
   int fmin = f, fmax = f;
   if (fs && (rc = check_counts(who, fs, batch, INT32_MAX, &fmin, &fmax))) return rc;
+  for (int b = 0; rows && b < batch; ++b)
+    if (rows[b] < 1 || rows[b] > n) {
+      set_error("%s: row count %d of problem %d is outside [1, %d]", who, rows[b], b, n);
+      return AFL_ERR_BAD_ARG;
+    }
   if (fmin < 0) { set_error("%s: corrupted_count %d is negative", who, f); return AFL_ERR_BAD_ARG; }
   if (agg && idx) { set_error("%s: give the aggregate as agg or as idx, not both", who); return AFL_ERR_BAD_ARG; }
   if ((dev_out || sums_out) && !agg && !idx) {
@@ -790,12 +878,15 @@ static int attack_metrics(const void* G, int batch, int64_t batch_stride, int n,
   }
   const ProblemParams* each = nullptr;
   if (fs) {
-    rc = upload_table(who, batch, ws, ws_bytes, need, stream, [&](int b, ProblemParams& q) { q.f = fs[b]; }, &each);
+    rc = upload_table(who, batch, ws, ws_bytes, need, stream, [&](int b, ProblemParams& q) {
+      q.f = fs[b];
+      if (rows) q.tm.n_rows = rows[b];
+    }, &each);
     if (rc) return rc;
   }
   return colstats::attack_metrics(G, batch, batch_stride, n, d, ld, dtype, f, each, agg, idx, sel, sel_ld, dev_out,
                                   sums_out, honest_out, krum_hit, mal_count, sel_count,
-                                  static_cast<uint8_t*>(ws) + table_bytes(batch), stream);
+                                  static_cast<uint8_t*>(ws) + table_bytes(batch), stream, rows != nullptr);
 }
 
 // The backdoor's per-problem values (afl_backdoor_start_batched / _finish_batched): non-NULL, counts in [0, f_cap].
@@ -1028,6 +1119,19 @@ int afl_alie_batched_each(const void* G, int batch, int64_t batch_stride, int n,
                       static_cast<cudaStream_t>(stream));
 }
 
+size_t afl_batched_rows_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
+  if (batched_rule(rule) == B_BAD) return 0;
+  return afl_batched_each_workspace_bytes(rule, batch, n, d, dtype);
+}
+
+int afl_defend_batched_rows(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                            int64_t ld, int dtype, const int* rows, const int* users_counts, const int* corrupted_counts,
+                            float* out, int* idx_out, int* sel_out, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+  return defend_batched_rows(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_counts, corrupted_counts, out,
+                             idx_out, sel_out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
 size_t afl_metrics_workspace_bytes(int batch, int n, int64_t d, int dtype) {
   if (batch < 1 || batch > kBatchMax || n < 1 || d < 1 || (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16)) return 0;
   return table_bytes(batch) + metrics_partial_bytes(batch, d, dtype);
@@ -1054,6 +1158,20 @@ int afl_attack_metrics_batched_each(const void* G, int batch, int64_t batch_stri
   return attack_metrics(G, batch, batch_stride, n, d, ld, dtype, 0, corrupted_counts, agg, idx, sel, sel_ld, dev_out,
                         sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
                         static_cast<cudaStream_t>(stream));
+}
+
+int afl_attack_metrics_batched_rows(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                    int dtype, const int* rows, const int* corrupted_counts, const float* agg,
+                                    const int* idx, const int* sel, int sel_ld, float* dev_out, double* sums_out,
+                                    float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  if (!rows || !corrupted_counts) {
+    set_error("afl_attack_metrics_batched_rows: the per-problem row counts or corrupted counts are NULL");
+    return AFL_ERR_BAD_ARG;
+  }
+  return attack_metrics(G, batch, batch_stride, n, d, ld, dtype, 0, corrupted_counts, agg, idx, sel, sel_ld, dev_out,
+                        sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream), rows);
 }
 
 int afl_backdoor_start_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,

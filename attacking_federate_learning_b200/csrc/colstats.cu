@@ -98,12 +98,14 @@ __device__ __forceinline__ Pack<VEC> load_rows(const T* p) {
 
 // ---- mean: sequential fp32 row accumulation, then one IEEE division — the order NumPy uses for
 // np.mean(axis=0) on a C-contiguous array, so fp32 results are bit-identical to the reference.
-template <typename T, int VEC>
+// kRows (a ragged batch): problem b averages its rows 0..each[b].tm.n_rows-1.
+template <typename T, int VEC, bool kRows>
 __global__ void __launch_bounds__(kBlock)
 mean_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, float* __restrict__ out, int64_t g_batch,
-            int64_t out_batch) {
+            int64_t out_batch, const ProblemParams* __restrict__ each) {
   const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * VEC;
   if (c0 >= d) return;
+  if constexpr (kRows) n = each[blockIdx.y].tm.n_rows;
   G += blockIdx.y * g_batch;
   out += blockIdx.y * out_batch;
   float acc[VEC];
@@ -349,8 +351,8 @@ __device__ __forceinline__ void cta_sum2(double& a, double& b) {
 // (Krum's result, read in place).  partial[b][tile] = (sum (a - h)^2, sum h^2) over the tile's columns in float64; the
 // differences and squares are formed from the fp32 values as float64, so nothing cancels.  f >= n (no honest row)
 // reads no row and gives h = 0 / 0 = NaN; an idx outside [0, n) reads no row and gives a = NaN.  partial == NULL:
-// only honest_out is wanted.
-template <typename T, int V, bool VL>
+// only honest_out is wanted.  kRows (a ragged batch): problem b has each[b].tm.n_rows rows instead of n.
+template <typename T, int V, bool VL, bool kRows>
 __global__ void __launch_bounds__(kBlock)
 honest_deviation_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, int64_t g_batch, int f,
                         const ProblemParams* __restrict__ each, const float* __restrict__ agg,
@@ -358,6 +360,7 @@ honest_deviation_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, i
   constexpr int U = VL ? kUnroll : 2;                 // V scalar loads per row: fewer rows in flight
   const int b = blockIdx.y;
   if (each) f = each[b].f;
+  if constexpr (kRows) n = each[b].tm.n_rows;
   f = f < n ? f : n;
   const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * V;
   double sd = 0.0, sh = 0.0;
@@ -456,15 +459,20 @@ static bool vec_ok(const void* G, int64_t ld, int dtype, int batch, int64_t g_ba
   return (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0) && (batch == 1 || (g_batch * es) % 16 == 0);
 }
 
+// rows (device, may be NULL): a ragged batch, problem b averaging rows 0..rows[b].tm.n_rows-1 (at most n).
 int mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, int batch, int64_t g_batch,
-                 int64_t out_batch, cudaStream_t stream) {
+                 int64_t out_batch, cudaStream_t stream, const ProblemParams* rows) {
   if (!G || !out || n < 1 || d < 1 || ld < d) { set_error("afl_mean: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
   const bool v = vec_ok(G, ld, dtype, batch, g_batch);
   const int vec = v ? (dtype == AFL_F32 ? 4 : 8) : 1;
   const dim3 grid(static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock)), batch);
   ProfScope ps("mean", stream);
-#define AFL_MEAN_LAUNCH(T, V) mean_kernel<T, V><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, out, g_batch, out_batch)
+#define AFL_MEAN_LAUNCH(T, V)                                                                                            \
+  do {                                                                                                                   \
+    if (rows) mean_kernel<T, V, true><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, out, g_batch, out_batch, rows); \
+    else mean_kernel<T, V, false><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, out, g_batch, out_batch, nullptr); \
+  } while (0)
   if (dtype == AFL_F32) {
     if (v) AFL_MEAN_LAUNCH(float, 4);
     else AFL_MEAN_LAUNCH(float, 1);
@@ -481,7 +489,7 @@ int mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, float* 
 }
 
 int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream) {
-  return mean_batched(G, n, d, ld, dtype, out, 1, 0, 0, stream);
+  return mean_batched(G, n, d, ld, dtype, out, 1, 0, 0, stream, nullptr);
 }
 
 // `batch` problems: G + b * g_batch; mu/sigma/crafted + b * out_batch; bcast + b * bcast_batch.  each (device, may be
@@ -544,11 +552,12 @@ int64_t deviation_tiles(int64_t d, int dtype) { return ceil_div64(d, kBlock * (d
 
 // The three metric kernels on `batch` problems (arguments checked by the caller, capi.cu).  The deviation pass runs
 // when dev_out, sums_out or honest_out is wanted, the finish for the first two, the selection statistics when
-// krum_hit or sel is given.  partial: double2[batch][deviation_tiles].
+// krum_hit or sel is given.  partial: double2[batch][deviation_tiles].  rows (each required): a ragged batch, problem b
+// having each[b].tm.n_rows rows.
 int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, int64_t ld, int dtype, int f,
                    const ProblemParams* each, const float* agg, const int* idx, const int* sel, int sel_ld,
                    float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count,
-                   void* partial, cudaStream_t stream) {
+                   void* partial, cudaStream_t stream, bool rows) {
   const bool sums = dev_out || sums_out;
   if (sums || honest_out) {
     const int tiles = static_cast<int>(deviation_tiles(d, dtype));
@@ -557,7 +566,11 @@ int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, 
     double2* part = sums ? static_cast<double2*>(partial) : nullptr;
     {
       ProfScope ps("honest_deviation", stream);
-#define AFL_DEV_LAUNCH(T, V, VL) honest_deviation_kernel<T, V, VL><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, g_batch, f, each, agg, idx, honest_out, part)
+#define AFL_DEV_LAUNCH(T, V, VL)                                                                                          \
+  do {                                                                                                                   \
+    if (rows) honest_deviation_kernel<T, V, VL, true><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, g_batch, f, each, agg, idx, honest_out, part); \
+    else honest_deviation_kernel<T, V, VL, false><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), n, d, ld, g_batch, f, each, agg, idx, honest_out, part); \
+  } while (0)
       if (dtype == AFL_F32) {
         if (v) AFL_DEV_LAUNCH(float, 4, true);
         else AFL_DEV_LAUNCH(float, 4, false);

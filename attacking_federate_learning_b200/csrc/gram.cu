@@ -105,7 +105,8 @@ __global__ void sqdist_to_dist_kernel(const double* __restrict__ d2, int n, size
 size_t pair_parts_bytes(int n, int64_t d, int batch);
 size_t pair_center_bytes(int64_t d);
 int launch_pair(const void* G, int mode, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, float* parts,
-                double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream);
+                double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream,
+                const ProblemParams* rows);
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -171,9 +172,10 @@ size_t workspace_bytes(int n, int64_t d, int dtype, int flags, int batch) {
 }
 
 // `batch` problems of the same shape, problem b at G + b * batch_stride elements; d2_out: batch consecutive n x n tables.
-// One problem is batch = 1 (batch_stride unused).
+// One problem is batch = 1 (batch_stride unused).  rows (device, may be NULL): a ragged batch's table; problem b's rows
+// past rows[b].tm.n_rows then affect only the table entries that involve them.
 int sqdist_batched(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, double* d2_out,
-                   void* ws, size_t ws_bytes, int flags, cudaStream_t stream) {
+                   void* ws, size_t ws_bytes, int flags, cudaStream_t stream, const ProblemParams* rows) {
   if (!G || !d2_out || n < 1 || d < 1 || ld < d) { set_error("afl_sqdist_partial: bad argument"); return AFL_ERR_BAD_ARG; }
   if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_sqdist_partial: dtype"); return AFL_ERR_UNSUPPORTED; }
   Plan pl = make_plan(G, batch, batch_stride, n, d, ld, dtype, flags);
@@ -193,7 +195,7 @@ int sqdist_batched(const void* G, int batch, int64_t batch_stride, int n, int64_
     double* S = reinterpret_cast<double*>(static_cast<uint8_t*>(ws) + pl.parts_bytes);
     float* cvec = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + pl.parts_bytes + pl.s_bytes);
     return launch_pair(G, pl.mode, batch, batch_stride, n, d, ld, parts, S, cvec, d2_out, env_int("AFL_GRAM_FLUSH", 4),
-                       center, (flags & AFL_GRAM_SINGLE_PASS) ? 1 : 0, stream);
+                       center, (flags & AFL_GRAM_SINGLE_PASS) ? 1 : 0, stream, rows);
   } else {
     const int t32 = (n + 31) / 32;
     double* part = static_cast<double*>(ws);
@@ -221,7 +223,7 @@ size_t workspace_bytes(int n, int64_t d, int dtype, int flags) { return workspac
 
 int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, double* d2_out, void* ws, size_t ws_bytes,
                    int flags, cudaStream_t stream) {
-  return sqdist_batched(G, 1, 0, n, d, ld, dtype, d2_out, ws, ws_bytes, flags, stream);
+  return sqdist_batched(G, 1, 0, n, d, ld, dtype, d2_out, ws, ws_bytes, flags, stream, nullptr);
 }
 
 // batch consecutive n x n tables

@@ -62,6 +62,7 @@ struct PairParams {
   int single_pass;      // kModeTf32x2: hi hi^T only (plain TF32), for measurement
   const float* cvec;    // centre (mean of the last rows), padded with zeros to a multiple of 64 columns
   float* parts;         // [pairs][splits][128][128]
+  const ProblemParams* each;   // kRows: problem b's participating rows are each[b].tm.n_rows
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2_rn_p(float lo, float hi) {
@@ -123,7 +124,9 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[K]) {
 // kSymN > 0: kModeBf16x2 with one tile, the symmetric two-product form on boxes of kSymN = p.box_rows rows (N rounded
 // up to 8, 56..112), with wgmma.m64nNk16 for N = kSymN: no tensor work on columns past the box.  (A template
 // parameter: a runtime branch between the two MMA sequences makes ptxas fence every k-block's wgmma issue.)
-template <int kMode, int kSymN>
+// kRows (a ragged batch, center == 2 only): problem b's centre is the mean of its own last 8 participating rows,
+// max(m - 8, 0) .. m - 1 with m = p.each[b].tm.n_rows, instead of rows n - 8 .. n - 1 of the box.
+template <int kMode, int kSymN, bool kRows>
 __global__ void __launch_bounds__(kPThreads, 1)
 gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
   constexpr bool kSym = kSymN != 0;
@@ -211,6 +214,11 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
       };
       const int units = box_bytes / 2048u;
       constexpr float two = kSym ? 2.f : 1.f;               // kSym: the second atom is 2 b2 (exact, a power of 2)
+      int rows_b = 0, crow0_b = 0;                          // kRows: this problem's row count and first centre row
+      if constexpr (kRows) {
+        rows_b = p.each[blockIdx.y].tm.n_rows;
+        crow0_b = rows_b > kGramCenterRows ? rows_b - kGramCenterRows : 0;
+      }
       float4 cen = load_center(w);
       for (int box = w; box < nboxes; box += kConverters) {
         const int s = box % kPSlots;
@@ -223,7 +231,8 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
           float4 t[kGramCenterRows];
 #pragma unroll
           for (int r = 0; r < kGramCenterRows; ++r)
-            t[r] = lds128(base + static_cast<uint32_t>(min(p.crow0 + r, p.n - 1)) * 256u + static_cast<uint32_t>(c16) * 16u);
+            t[r] = lds128(base + static_cast<uint32_t>(min((kRows ? crow0_b : p.crow0) + r, (kRows ? rows_b : p.n) - 1)) * 256u +
+                          static_cast<uint32_t>(c16) * 16u);
           cen = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
           for (int r = 0; r < kGramCenterRows; ++r) { cen.x += t[r].x; cen.y += t[r].y; cen.z += t[r].z; cen.w += t[r].w; }
@@ -463,30 +472,32 @@ size_t pair_parts_bytes(int n, int64_t d, int batch) {
   return static_cast<size_t>(pairs) * batch * pair_splits(n, d, batch) * kPPartElems * sizeof(float);
 }
 
-template <int kMode, int kSymN>
+template <int kMode, int kSymN, bool kRows = false>
 static int launch_mode(const CUtensorMap& tmap, const PairParams& p, int batch, cudaStream_t stream) {
   const size_t smem = static_cast<size_t>(kPSlots) * kPSlotBytes + 1024;
   static int smem_attr_done[kMaxDevices] = {0};
-  AFL_CUDA(ensure_dyn_smem(gram_pair_kernel<kMode, kSymN>, static_cast<int>(smem), smem_attr_done));
+  AFL_CUDA(ensure_dyn_smem(gram_pair_kernel<kMode, kSymN, kRows>, static_cast<int>(smem), smem_attr_done));
   {
     ProfScope ps("gram_pair", stream);
-    gram_pair_kernel<kMode, kSymN><<<dim3(p.pairs * p.splits, batch), kPThreads, smem, stream>>>(tmap, p);
+    gram_pair_kernel<kMode, kSymN, kRows><<<dim3(p.pairs * p.splits, batch), kPThreads, smem, stream>>>(tmap, p);
   }
   AFL_LAUNCH_CHECK("gram_pair_kernel");
   return AFL_OK;
 }
 
-// the one-tile symmetric form: one instance per box height (gram.cu:make_plan runs it for 49 <= N <= 112)
+// the one-tile symmetric form: one instance per box height (gram.cu:make_plan runs it for 49 <= N <= 112), and per box
+// height one for a ragged batch's per-problem centre
+template <bool kRows>
 static int launch_sym(const CUtensorMap& tmap, const PairParams& p, int batch, cudaStream_t stream) {
   switch (p.box_rows) {
-    case 56: return launch_mode<kModeBf16x2, 56>(tmap, p, batch, stream);
-    case 64: return launch_mode<kModeBf16x2, 64>(tmap, p, batch, stream);
-    case 72: return launch_mode<kModeBf16x2, 72>(tmap, p, batch, stream);
-    case 80: return launch_mode<kModeBf16x2, 80>(tmap, p, batch, stream);
-    case 88: return launch_mode<kModeBf16x2, 88>(tmap, p, batch, stream);
-    case 96: return launch_mode<kModeBf16x2, 96>(tmap, p, batch, stream);
-    case 104: return launch_mode<kModeBf16x2, 104>(tmap, p, batch, stream);
-    case 112: return launch_mode<kModeBf16x2, 112>(tmap, p, batch, stream);
+    case 56: return launch_mode<kModeBf16x2, 56, kRows>(tmap, p, batch, stream);
+    case 64: return launch_mode<kModeBf16x2, 64, kRows>(tmap, p, batch, stream);
+    case 72: return launch_mode<kModeBf16x2, 72, kRows>(tmap, p, batch, stream);
+    case 80: return launch_mode<kModeBf16x2, 80, kRows>(tmap, p, batch, stream);
+    case 88: return launch_mode<kModeBf16x2, 88, kRows>(tmap, p, batch, stream);
+    case 96: return launch_mode<kModeBf16x2, 96, kRows>(tmap, p, batch, stream);
+    case 104: return launch_mode<kModeBf16x2, 104, kRows>(tmap, p, batch, stream);
+    case 112: return launch_mode<kModeBf16x2, 112, kRows>(tmap, p, batch, stream);
   }
   set_error("gram_pair_kernel: no one-tile bf16x2 instance for %d clients (49..112)", p.n);
   return AFL_ERR_UNSUPPORTED;
@@ -495,8 +506,11 @@ static int launch_sym(const CUtensorMap& tmap, const PairParams& p, int batch, c
 // G: `batch` problems of fp32 [n, d] (pitch multiple of 4 elements) or bf16 / fp16 (kModeBf16In / kModeF16In, pitch
 // multiple of 8), 16-byte aligned, problem b at G + b * batch_stride elements (batch > 1: one tile, a 16-byte multiple
 // >= n * ld).  parts: pair_parts_bytes(); S and d2_out: batch * n * n doubles; cvec: pair_center_bytes().
+// rows (device, may be NULL): a ragged batch's table, whose tm.n_rows places the one-tile form's centre per problem.  Any
+// other entry S_ij depends on rows i and j only, so the other forms need no table.
 int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, float* parts,
-                double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream) {
+                double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream,
+                const ProblemParams* rows) {
   const float* G = static_cast<const float*>(Gv);
   const bool half16 = mode == kModeBf16In || mode == kModeF16In;    // 16-bit elements
   if (batch > 1 && n > 128) { set_error("gram_pair_kernel: batched problems are one tile (n <= 128, got %d)", n); return AFL_ERR_UNSUPPORTED; }
@@ -524,6 +538,7 @@ int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n
   p.single_pass = single_pass ? 1 : 0;
   p.parts = parts;
   p.cvec = cvec;
+  p.each = rows;
   if (p.center == 1) {
     const int cref_rows = n < kGramCenterRows ? n : kGramCenterRows;
     const int64_t d_pad = (d + kPCols - 1) / kPCols * kPCols;
@@ -546,7 +561,8 @@ int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n
                    mode == kModeBf16x2 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed: %d", static_cast<int>(r)); return AFL_ERR_CUDA; }
-  int rc = sym                   ? launch_sym(tmap, p, batch, stream)
+  int rc = sym                   ? (rows && p.center == 2 ? launch_sym<true>(tmap, p, batch, stream)
+                                                          : launch_sym<false>(tmap, p, batch, stream))
          : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, 0>(tmap, p, batch, stream)
          : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, 0>(tmap, p, batch, stream)
          : mode == kModeF16In  ? launch_mode<kModeF16In, 0>(tmap, p, batch, stream)

@@ -136,7 +136,9 @@ __device__ __forceinline__ float krum_value(const KrumParams& p, size_t off, int
   else return p.dist[off + static_cast<size_t>(u) * p.n + static_cast<int>(k & 0xFFFFFFFFu)];
 }
 
-template <KrumSource kSrc>
+// kRows (a ragged batch, afl_defend_batched_rows): problem b has m = each[b].tm.n_rows participating users in its n x n
+// table (n stays the pitch).  CTAs u >= m only count themselves done, and the scores and the argmin cover users < m.
+template <KrumSource kSrc, bool kRows>
 __global__ void __launch_bounds__(256)
 krum_tail_kernel(const KrumParams p) {
   using Key = KrumKey<kSrc>;
@@ -146,23 +148,29 @@ krum_tail_kernel(const KrumParams p) {
   const int u = blockIdx.x, n = p.n, b = blockIdx.y;                     // user u of problem b
   const size_t off = static_cast<size_t>(b) * n * n;
   float* score = p.score + static_cast<size_t>(b) * n;
-  if constexpr (kSrc == kSqdist) {
+  if constexpr (kSrc == kSqdist && !kRows) {                            // (a ragged batch is never a peer exchange)
     if (p.world > 1 && !wait_flags(p.flags, p.world, p.epoch)) {
       if (threadIdx.x == 0 && u == 0) { *p.status_host = 1; *p.idx_host = -1; *p.idx_dev = -1; }
       return;
     }
   }
-  int P = 1;
-  while (P < n) P <<= 1;
-  for (int v = threadIdx.x; v < P; v += blockDim.x) keys[v] = (v < n && v != u) ? krum_key<kSrc>(p, off, u, v) : ~Key(0);
-  __syncthreads();
-  block_bitonic_sort(keys, P);
+  const int m = kRows ? p.each[b].tm.n_rows : n;
+  const bool work = !kRows || u < m;
+  if (work) {
+    int P = 1;
+    while (P < m) P <<= 1;
+    for (int v = threadIdx.x; v < P; v += blockDim.x) keys[v] = (v < m && v != u) ? krum_key<kSrc>(p, off, u, v) : ~Key(0);
+    __syncthreads();
+    block_bitonic_sort(keys, P);
+  }
   if (threadIdx.x == 0) {
-    float s = 0.f;                                                       // Python: sum() starts at int 0; ascending fp32 adds
-    const int take = p.each ? p.each[b].take : p.take;
-    for (int pos = 0; pos < take; ++pos) s = s + krum_value<kSrc>(p, off, u, keys[pos]);
-    score[u] = s;
-    __threadfence();
+    if (work) {
+      float s = 0.f;                                                     // Python: sum() starts at int 0; ascending fp32 adds
+      const int take = p.each ? p.each[b].take : p.take;
+      for (int pos = 0; pos < take; ++pos) s = s + krum_value<kSrc>(p, off, u, keys[pos]);
+      score[u] = s;
+      __threadfence();
+    }
     s_last = (atomicAdd(p.done + b, 1u) == static_cast<unsigned>(n - 1)) ? 1 : 0;
   }
   __syncthreads();
@@ -171,9 +179,9 @@ krum_tail_kernel(const KrumParams p) {
   __threadfence();
   float best = __int_as_float(0x7f800000);
   int best_pos = 0x7fffffff;
-  for (int v = threadIdx.x; v < n; v += blockDim.x) {
+  for (int v = threadIdx.x; v < m; v += blockDim.x) {
     const float s = __ldcg(score + v);
-    if (n >= 2 && static_cast<double>(s) < 1e20) argmin_combine(best, best_pos, s, visit_pos(v));   // vs the Python float 1e20
+    if (m >= 2 && static_cast<double>(s) < 1e20) argmin_combine(best, best_pos, s, visit_pos(v));   // vs the Python float 1e20
   }
   const int idx = block_argmin_user<256 / 32>(best, best_pos);
   if (threadIdx.x == 0) {
@@ -190,35 +198,41 @@ int krum_take(int n, int users_count, int corrupted_count) {
 }
 
 // Fills p.take and launches the kernel for the row source p selects, grid (n, batch).  p.done[0 .. batch) must be zero.
-int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream, int batch) {
+// rows: each problem's participating users are p.each[b].tm.n_rows (d2 tables only).
+int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream, int batch, bool rows) {
   p.take = krum_take(p.n, users_count, corrupted_count);
   int P = 1; while (P < p.n) P <<= 1;
   {
     ProfScope ps("krum_tail", stream);
     const dim3 grid(p.n, batch);
-    if (p.dist) krum_tail_kernel<kDist><<<grid, 256, static_cast<size_t>(P) * sizeof(KrumKey<kDist>), stream>>>(p);
-    else krum_tail_kernel<kSqdist><<<grid, 256, static_cast<size_t>(P) * sizeof(KrumKey<kSqdist>), stream>>>(p);
+    if (p.dist) krum_tail_kernel<kDist, false><<<grid, 256, static_cast<size_t>(P) * sizeof(KrumKey<kDist>), stream>>>(p);
+    else if (rows) krum_tail_kernel<kSqdist, true><<<grid, 256, static_cast<size_t>(P) * sizeof(KrumKey<kSqdist>), stream>>>(p);
+    else krum_tail_kernel<kSqdist, false><<<grid, 256, static_cast<size_t>(P) * sizeof(KrumKey<kSqdist>), stream>>>(p);
   }
   AFL_LAUNCH_CHECK("krum_tail_kernel");
   return AFL_OK;
 }
 
+// kRows (a ragged batch): problem b sorts the first m = theta_b + 2 f_b entries of its rows u < m (n stays the pitch).
+template <bool kRows>
 __global__ void __launch_bounds__(256)
-row_sort_kernel(const float* __restrict__ dist, int n, SortWs w) {
+row_sort_kernel(const float* __restrict__ dist, int n, SortWs w, const ProblemParams* __restrict__ each) {
   extern __shared__ unsigned long long keys[];
   const int u = blockIdx.x;
+  const int m = kRows ? each[blockIdx.y].theta + 2 * each[blockIdx.y].f : n;
+  if (kRows && u >= m) return;
   const size_t off = static_cast<size_t>(blockIdx.y) * n * n;           // problem blockIdx.y
   dist += off; w.sval += off; w.sidx += off; w.rank += off;
   int P = 1;
-  while (P < n) P <<= 1;
+  while (P < m) P <<= 1;
   for (int v = threadIdx.x; v < P; v += blockDim.x)
-    keys[v] = (v < n && v != u) ? dist_key(dist[static_cast<size_t>(u) * n + v], v) : ~0ull;
+    keys[v] = (v < m && v != u) ? dist_key(dist[static_cast<size_t>(u) * n + v], v) : ~0ull;
   __syncthreads();
   block_bitonic_sort(keys, P);
   const size_t base = static_cast<size_t>(u) * n;
-  for (int pos = threadIdx.x; pos < n; pos += blockDim.x) {
+  for (int pos = threadIdx.x; pos < m; pos += blockDim.x) {
     const unsigned long long k = keys[pos];
-    if (pos < n - 1) {
+    if (pos < m - 1) {
       const int v = static_cast<int>(k & 0xFFFFFFFFu);
       w.sval[base + pos] = dist[base + v];               // original bits (keeps a NaN a NaN)
       w.sidx[base + pos] = static_cast<uint16_t>(v);
@@ -233,6 +247,8 @@ row_sort_kernel(const float* __restrict__ dist, int n, SortWs w) {
 
 constexpr int kRowsPerThread = kMaxN / 1024;
 
+// kRows (a ragged batch): problem b's users are u < m = theta_b + 2 f_b (its users_count); n stays the table pitch.
+template <bool kRows>
 __global__ void __launch_bounds__(1024, 1)
 bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, SortWs w, int* __restrict__ sel_out,
                      const ProblemParams* __restrict__ each) {
@@ -248,17 +264,18 @@ bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, So
     for (int r = theta_b + tid; r < theta; r += 1024) sel_out[r] = -2;
     f = each[blockIdx.x].f; theta = theta_b;
   }
+  const int m = kRows ? theta + 2 * f : n;
   double score[kRowsPerThread];
   int bptr[kRowsPerThread];
 
-  for (int v = tid; v < kMaxN; v += 1024) alive[v] = (v < n) ? 1 : 0;
-  // round 0: keep0 = min(n - f, n - 1) smallest distances, summed ascending in float64
-  const int keep0 = min(n - f, n - 1);
+  for (int v = tid; v < kMaxN; v += 1024) alive[v] = (v < m) ? 1 : 0;
+  // round 0: keep0 = min(m - f, m - 1) smallest distances, summed ascending in float64
+  const int keep0 = min(m - f, m - 1);
 #pragma unroll
   for (int r = 0; r < kRowsPerThread; ++r) {
     const int u = tid + r * 1024;
     score[r] = 0.0; bptr[r] = keep0 - 1;
-    if (u < n) {
+    if (u < m) {
       const float* sv = w.sval + static_cast<size_t>(u) * n;
       double s = 0.0;
       for (int pos = 0; pos < keep0; ++pos) s += static_cast<double>(sv[pos]);
@@ -274,7 +291,7 @@ bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, So
 #pragma unroll
     for (int r = 0; r < kRowsPerThread; ++r) {
       const int u = tid + r * 1024;
-      if (u < n && alive[u] && score[r] < 1e20) argmin_combine(best, best_pos, score[r], visit_pos(u));
+      if (u < m && alive[u] && score[r] < 1e20) argmin_combine(best, best_pos, score[r], visit_pos(u));
     }
     const int idx = block_argmin_user<1024 / 32>(best, best_pos);
     if (tid == 0) {
@@ -292,7 +309,7 @@ bulyan_rounds_kernel(const float* __restrict__ dist, int n, int f, int theta, So
 #pragma unroll
     for (int r = 0; r < kRowsPerThread; ++r) {
       const int u = tid + r * 1024;
-      if (u < n && u != s && alive[u]) {
+      if (u < m && u != s && alive[u]) {
         const size_t base = static_cast<size_t>(u) * n;
         const int pos = w.rank[base + s];
         int b = bptr[r];
@@ -328,14 +345,14 @@ static int check_ws(int n, int batch, void* ws, size_t ws_bytes) {
 // Krum on a workspace: the batch counters live at its start (cleared here: workspaces are not initialised), the
 // scores behind them unless the caller wants them.
 static int krum_on_workspace(KrumParams p, int batch, int users_count, int corrupted_count, float* scores_out, void* ws,
-                             size_t ws_bytes, cudaStream_t stream) {
+                             size_t ws_bytes, cudaStream_t stream, bool rows = false) {
   int rc = check_ws(p.n, batch, ws, ws_bytes);
   if (rc) return rc;
   p.done = static_cast<unsigned int*>(ws);
   p.score = scores_out ? scores_out
                        : reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + align_up(static_cast<size_t>(batch) * 4, 256));
   AFL_CUDA(cudaMemsetAsync(p.done, 0, static_cast<size_t>(batch) * sizeof(unsigned int), stream));
-  return krum_tail(p, users_count, corrupted_count, stream, batch);
+  return krum_tail(p, users_count, corrupted_count, stream, batch, rows);
 }
 
 int krum_select(const float* dist, int n, int users_count, int corrupted_count, int* idx_out, float* scores_out,
@@ -346,14 +363,18 @@ int krum_select(const float* dist, int n, int users_count, int corrupted_count, 
   return krum_on_workspace(p, 1, users_count, corrupted_count, scores_out, ws, ws_bytes, stream);
 }
 
-// d2: batch consecutive n x n tables; idx_out[batch]; each (device, may be NULL): per-problem take
+// d2: batch consecutive n x n tables; idx_out[batch]; each (device, may be NULL): per-problem take, and with rows also
+// the problem's participating users (tm.n_rows)
 int krum_from_sqdist(const double* d2, int n, int users_count, int corrupted_count, int* idx_out, void* ws,
-                     size_t ws_bytes, cudaStream_t stream, int batch, const ProblemParams* each) {
-  if (!d2 || !idx_out || n < 1) { set_error("afl_krum_from_sqdist: bad argument"); return AFL_ERR_BAD_ARG; }
+                     size_t ws_bytes, cudaStream_t stream, int batch, const ProblemParams* each, bool rows) {
+  if (!d2 || !idx_out || n < 1 || (rows && !each)) { set_error("afl_krum_from_sqdist: bad argument"); return AFL_ERR_BAD_ARG; }
   KrumParams p{};
   p.tab[0] = d2; p.world = 1; p.n = n; p.idx_dev = idx_out; p.each = each;
-  return krum_on_workspace(p, batch, users_count, corrupted_count, nullptr, ws, ws_bytes, stream);
+  return krum_on_workspace(p, batch, users_count, corrupted_count, nullptr, ws, ws_bytes, stream, rows);
 }
+
+int bulyan_rounds(const float* dist, int n, int f, int theta, int* sel_out, void* ws, size_t ws_bytes,
+                  cudaStream_t stream, int batch, const ProblemParams* each, bool rows);
 
 // dist: batch consecutive n x n tables; sel_out[batch][theta], theta = users_count - 2f.  each (device, may be NULL):
 // per-problem f and theta; f is then the smallest problem's, so that every row of sel_out holds its problem's rounds.
@@ -368,18 +389,28 @@ int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out
     set_error("afl_bulyan_select: users_count (%d) must equal the number of rows (%d)", users_count, n);
     return AFL_ERR_UNSUPPORTED;
   }
-  const int theta = users_count - 2 * f;
+  return bulyan_rounds(dist, n, f, users_count - 2 * f, sel_out, ws, ws_bytes, stream, batch, each, false);
+}
+
+// The two Bulyan kernels on checked arguments: sel_out[batch][theta].  rows (a ragged batch, each required): problem b's
+// users are each[b].theta + 2 each[b].f of its n x n table.
+int bulyan_rounds(const float* dist, int n, int f, int theta, int* sel_out, void* ws, size_t ws_bytes,
+                  cudaStream_t stream, int batch, const ProblemParams* each, bool rows) {
   int rc = check_ws(n, batch, ws, ws_bytes);
   if (rc) return rc;
   const SortWs w = carve(ws, n, batch);
   int P = 1; while (P < n) P <<= 1;
+  const dim3 grid(n, batch);
+  const size_t smem = static_cast<size_t>(P) * sizeof(unsigned long long);
   {
     ProfScope ps("row_sort", stream);
-    row_sort_kernel<<<dim3(n, batch), 256, static_cast<size_t>(P) * sizeof(unsigned long long), stream>>>(dist, n, w);
+    if (rows) row_sort_kernel<true><<<grid, 256, smem, stream>>>(dist, n, w, each);
+    else row_sort_kernel<false><<<grid, 256, smem, stream>>>(dist, n, w, nullptr);
   }
   AFL_LAUNCH_CHECK("row_sort_kernel");
   ProfScope ps("bulyan_rounds", stream);
-  bulyan_rounds_kernel<<<batch, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out, each);
+  if (rows) bulyan_rounds_kernel<true><<<batch, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out, each);
+  else bulyan_rounds_kernel<false><<<batch, 1024, 0, stream>>>(dist, n, f, theta, w, sel_out, each);
   AFL_LAUNCH_CHECK("bulyan_rounds_kernel");
   return AFL_OK;
 }

@@ -26,7 +26,7 @@ int sqdist_partial(const void* G, int n, int64_t d, int64_t ld, int dtype, doubl
                    int flags, cudaStream_t stream);
 }
 namespace select {
-int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream, int batch = 1);
+int krum_tail(KrumParams p, int users_count, int corrupted_count, cudaStream_t stream, int batch = 1, bool rows = false);
 }
 namespace xgpu {
 

@@ -300,6 +300,39 @@ int afl_alie_batched_each(const void* G, int batch, int64_t batch_stride, int n,
                           float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
                           size_t workspace_bytes, void* stream);
 
+/* ---- ragged batches: a different number of clients per problem ---------------------------------------------------
+ * The reference's client count is a run parameter (--users-count, main.py:118), and Server.defend aggregates however many
+ * users reported (server.py:87: defend[rule](users_grads, len(self.users), corrupted_count)).  These calls run problems of
+ * different client counts, or rounds with partial participation, as one batch.  G is laid out as for
+ * afl_defend_batched_each, n <= 128 rows per problem slot; problem b is its first rows[b] rows (1 <= rows[b] <= n).  Rows
+ * rows[b]..n-1 of a slot are padding with any contents (NaN and +-inf included): no result depends on them.  rows,
+ * users_counts and corrupted_counts are HOST arrays of `batch` values; problem b's result is the single device call's on
+ * the rows[b] x d matrix G[b][:rows[b]] with users_counts[b] and corrupted_counts[b], bit for bit when both run the same
+ * Gram operand format and split count (the format is chosen once for the batch from n, d and the dtype, as for a single
+ * call of n clients; pin AFL_GRAM_SPLITS, and for fp32 AFL_GRAM_TF32X2, when comparing).  Checked before any CUDA call,
+ * with the first failing problem named: a NULL array, rows[b] outside [1, n] or corrupted_counts[b] < 0 ->
+ * AFL_ERR_BAD_ARG; the reference's asserts per problem -> AFL_ERR_PRECONDITION; a workspace that is too small or not
+ * 256-byte aligned -> AFL_ERR_WORKSPACE.  Every other argument, limit and stride rule is afl_defend_batched_each's.
+ *
+ * afl_batched_rows_workspace_bytes(rule, ...) — rule as afl_defend_batched (0 otherwise, and on bad arguments); the same
+ * bytes and layout as afl_batched_each_workspace_bytes (the parameter table, then for Krum and Bulyan the batch's n x n
+ * squared-distance tables, whose entries between participating rows are the problems' own).
+ *
+ * afl_defend_batched_rows — defences.py:73-75 defend[rule](G[b][:rows[b]], users_counts[b], corrupted_counts[b]):
+ *   "Krum"        defences.py:23-42 on rows[b] users (replaces the Python loop over server.py:87 for each client count):
+ *                 idx_out[b] in [0, rows[b]) or -1 (rows[b] = 1, or no eligible user; the reference then returns
+ *                 users_grads[-1], row rows[b] - 1).  users_counts[b] >= 2 corrupted_counts[b] + 1.
+ *   "TrimmedMean" defences.py:44-52 over rows[b] rows (users_counts[b] is not used, as in the reference).
+ *   "NoDefense"   defences.py:13-14, the mean of rows[b] rows (afl_mean's arithmetic).
+ *   "Bulyan"      defences.py:55-70 with users_counts[b] >= 4 corrupted_counts[b] + 3 and users_counts[b] == rows[b]
+ *                 (else AFL_ERR_UNSUPPORTED).  sel_out is device int[batch][theta_max], theta_max = max_b(users_counts[b]
+ *                 - 2 corrupted_counts[b]); positions past problem b's theta_b hold -2, as afl_defend_batched_each. */
+size_t afl_batched_rows_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype);
+int afl_defend_batched_rows(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                            int64_t ld, int dtype, const int* rows, const int* users_counts, const int* corrupted_counts,
+                            float* out, int* idx_out, int* sel_out, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 /* ---- attack-success metrics of a batch (SURVEY 8d "Attack-success (C5)") --------------------------------------
  * The reference logs test accuracy only (main.py:73-82); what a z x malicious-share sweep reports follows from its
  * conventions.  The malicious users are ids 0..f-1 (main.py:28), so in problem b rows f_b..n-1 are honest:
@@ -337,6 +370,15 @@ int afl_attack_metrics_batched_each(const void* G, int batch, int64_t batch_stri
                                     int dtype, const int* corrupted_counts, const float* agg, const int* idx,
                                     const int* sel, int sel_ld, float* dev_out, double* sums_out, float* honest_out,
                                     int* krum_hit, int* mal_count, int* sel_count, void* workspace,
+                                    size_t workspace_bytes, void* stream);
+/* afl_attack_metrics_batched_rows — afl_attack_metrics_batched_each on a ragged batch: problem b is its first rows[b]
+ * rows (a HOST array, 1 <= rows[b] <= n, else AFL_ERR_BAD_ARG; NULL -> AFL_ERR_BAD_ARG), so its honest rows are
+ * f_b..rows[b]-1 and h_b is afl_mean of those rows bit for bit; f_b >= rows[b] and idx[b] outside [0, rows[b]) give NaN
+ * as above.  Rows past rows[b] are never read.  Same workspace as afl_attack_metrics_batched_each. */
+int afl_attack_metrics_batched_rows(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                    int dtype, const int* rows, const int* corrupted_counts, const float* agg,
+                                    const int* idx, const int* sel, int sel_ld, float* dev_out, double* sums_out,
+                                    float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* workspace,
                                     size_t workspace_bytes, void* stream);
 
 /* ---- backdoor attack of a batch (backdoor.py:52-63, BackdoorAttack._attack_grads driven by malicious.py:10-27) -----

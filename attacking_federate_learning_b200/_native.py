@@ -69,6 +69,11 @@ SIGNATURES = {
                                      _sz, _vp]),
     "afl_attack_metrics_batched_rows": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
                                              _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "afl_batched_large_workspace_bytes": (_sz, [C.c_char_p, _i, _i, _i64, _i]),
+    "afl_defend_batched_large": (_i, [C.c_char_p, _vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                      _sz, _vp]),
+    "afl_alie_batched_large": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp,
+                                    _sz, _vp]),
     "afl_backdoor_start_batched": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp,
                                         _sz, _vp]),
     "afl_backdoor_finish_batched": (_i, [_i, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _vp,

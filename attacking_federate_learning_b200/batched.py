@@ -6,8 +6,8 @@ Every problem keeps the reference's semantics exactly: problem b's result is wha
 (`defences.krum` / `bulyan` / `trimmed_mean` / `no_defense`, `malicious.Attack.attack_rows`) returns for
 `G[b]`, bit for bit (C ABI `afl_defend_batched` / `afl_alie_batched`).
 
-Inputs are torch.cuda float32 / bfloat16 / float16 tensors `[B, N, D]` with `stride(2) == 1` and N <= 128 clients (one
-Gram tile); every problem shares N, D and `users_count`.  `corrupted_count` (and `alie_rows`' `num_std`) is
+Inputs are torch.cuda float32 / bfloat16 / float16 tensors `[B, N, D]` with `stride(2) == 1` and N <= 1024 clients;
+every problem shares N, D and `users_count`.  `corrupted_count` (and `alie_rows`' `num_std`) is
 either one number for every problem or a host sequence of B values (list, tuple, NumPy array, CPU tensor), one
 per problem (C ABI `afl_defend_batched_each` / `afl_alie_batched_each`), so that a grid over the malicious
 share and z runs as one batch.  Nothing here synchronises the host except `bulyan`, which checks for a failed
@@ -18,6 +18,12 @@ is `G[b, :rows_b]` and rows rows_b..N-1 are padding that no result depends on (C
 `afl_attack_metrics_batched_rows`).  So a grid over the number of users (main.py:118), or rounds in which a different
 number of clients reports, runs as one batch; `users_count` may then be B values too and defaults to `rows`, the
 `len(self.users)` that `Server.defend` passes (server.py:87).
+
+N <= 128 (one Gram tile) runs the calls above.  128 < N <= 1024 (the N = 500 and N = 1000 runs, f = 240 at N = 1000)
+runs `afl_defend_batched_large`, the ragged call with the larger limit: without `rows`, every problem has N rows and
+scalar counts apply to every problem.  Results and return shapes are the same as at N <= 128; every problem's trimmed
+mean runs the kernel its own row count selects.  N > 1024 raises NotImplementedError.  `alie_rows` takes any N: a
+scalar f > 128, or per-problem counts with N > 128, run `afl_alie_batched_large`.
 
 `backdoor_rows` is the per-problem `BackdoorAttack.attack_rows`: the backdoor crafting of every problem in three
 launches, with one call of the caller's malicious-network training between the second and the third.  It has no
@@ -82,20 +88,27 @@ def _ragged(B: int, rows, users_count, corrupted_count):
         _full(corrupted_count, B, "corrupted_count")
 
 
+MAX_CLIENTS = 1024          # clients per problem of the batched defences (afl_defend_batched_large)
+ONE_TILE = 128              # the calls for one Gram tile (afl_defend_batched, _each, _rows)
+
+
 def _defend(rule: str, G: torch.Tensor, users_count: int, corrupted_count, out=None, idx=None, sel=None, rows=None):
     B, N, D, ld, bs = _check(G)
+    if N > MAX_CLIENTS:
+        raise NotImplementedError(f"batched defences support N <= {MAX_CLIENTS} clients per problem (got {N})")
     L = nat.lib()
-    if rows is not None:
-        rs, ucs, fs = _ragged(B, rows, users_count, corrupted_count)
+    if rows is not None or N > ONE_TILE:
+        rs, ucs, fs = _ragged(B, N if rows is None else rows, users_count, corrupted_count)
+        ws_bytes, call = ((L.afl_batched_rows_workspace_bytes, L.afl_defend_batched_rows) if N <= ONE_TILE
+                          else (L.afl_batched_large_workspace_bytes, L.afl_defend_batched_large))
         with torch.cuda.device(G.device):
-            nbytes = L.afl_batched_rows_workspace_bytes(rule.encode(), B, N, D, dtype_code(G))
-            ws = Workspace.get(G.device, "batched", nbytes)
-            nat.check(L.afl_defend_batched_rows(rule.encode(), G.data_ptr(), B, bs, N, D, ld, dtype_code(G),
-                                                rs.ctypes.data, ucs.ctypes.data, fs.ctypes.data,
-                                                None if out is None else out.data_ptr(),
-                                                None if idx is None else idx.data_ptr(),
-                                                None if sel is None else sel.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                _stream_ptr(G)))
+            ws = Workspace.get(G.device, "batched", ws_bytes(rule.encode(), B, N, D, dtype_code(G)))
+            nat.check(call(rule.encode(), G.data_ptr(), B, bs, N, D, ld, dtype_code(G),
+                           rs.ctypes.data, ucs.ctypes.data, fs.ctypes.data,
+                           None if out is None else out.data_ptr(),
+                           None if idx is None else idx.data_ptr(),
+                           None if sel is None else sel.data_ptr(), ws.data_ptr(), ws.numel(),
+                           _stream_ptr(G)))
         return
     fs = _per_problem(corrupted_count, B, "corrupted_count", np.int32)
     with torch.cuda.device(G.device):
@@ -209,6 +222,8 @@ def alie_rows(users_grads, corrupted_count, num_std):
     f = int(corrupted_count)
     if f <= 0:
         return None
+    if f > ONE_TILE:                                     # afl_alie_batched takes f-row problems of one tile
+        return _alie_rows_each(users_grads, f, num_std)
     B, _, D, ld, bs = _check(users_grads)
     dev = users_grads.device
     mu, sigma, crafted = (torch.empty((B, D), dtype=torch.float32, device=dev) for _ in range(3))
@@ -233,13 +248,14 @@ def _alie_rows_each(users_grads, fs, zs):
     write = (fs > 0) & (zs != 0)
     bcast = users_grads if write.any() and users_grads.dtype == torch.float32 else None
     L = nat.lib()
+    call = L.afl_alie_batched_each if N <= ONE_TILE else L.afl_alie_batched_large
     with torch.cuda.device(dev):
-        nbytes = L.afl_batched_each_workspace_bytes(b"ALIE", B, N, D, dtype_code(users_grads))
+        nbytes = L.afl_batched_each_workspace_bytes(b"ALIE", B, min(N, ONE_TILE), D, dtype_code(users_grads))
         ws = Workspace.get(dev, "batched_alie", nbytes)
-        nat.check(L.afl_alie_batched_each(users_grads.data_ptr(), B, bs, N, D, ld, dtype_code(users_grads),
-                                          fs.ctypes.data, zs.ctypes.data, mu.data_ptr(), sigma.data_ptr(),
-                                          crafted.data_ptr(), None if bcast is None else bcast.data_ptr(), bs, ld,
-                                          ws.data_ptr(), ws.numel(), _stream_ptr(users_grads)))
+        nat.check(call(users_grads.data_ptr(), B, bs, N, D, ld, dtype_code(users_grads),
+                       fs.ctypes.data, zs.ctypes.data, mu.data_ptr(), sigma.data_ptr(),
+                       crafted.data_ptr(), None if bcast is None else bcast.data_ptr(), bs, ld,
+                       ws.data_ptr(), ws.numel(), _stream_ptr(users_grads)))
     if write.any() and bcast is None:
         _cast_rows(users_grads, crafted, fs, write)
     return crafted, mu, sigma

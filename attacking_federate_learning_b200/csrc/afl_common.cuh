@@ -61,6 +61,8 @@ struct TmShape {
   float key_q;            // Gaussian guess of the |dev| threshold in sigmas
   float key_density;      // 2 * phi(key_q) * n_rows (ranks per unit |dev| at that threshold, unit sigma)
 };
+// Register-resident trimmed-mean kernels: S = 4, 8, ..., 32 slots per lane for up to 128, 256, ..., 1024 rows.
+constexpr int kSlotClasses = 8;
 
 // One problem of a per-problem batched call (afl_defend_batched_each, afl_alie_batched_each): the values the single
 // call derives on the host from that problem's corrupted_count and z.  The table of `batch` rows sits at the start of

@@ -121,6 +121,10 @@ int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const i
 int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
                          int corrupted_count, float* out, int batch, int64_t g_batch, int ri_batch, int64_t out_batch,
                          cudaStream_t stream, const ProblemParams* each = nullptr);
+int trimmed_mean_classes(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, float* out,
+                         int batch, int64_t g_batch, int ri_batch, int64_t out_batch, cudaStream_t stream,
+                         const ProblemParams* each, const int* perm, const int* counts);
+int slot_class(int n_rows);
 TmShape shape(int n_rows, int corrupted_count);
 }
 namespace colstats {
@@ -585,8 +589,11 @@ static int alie_host(const float* const* rows, int f, int64_t d, double z, float
 // ProblemParams row per problem, built here with the single call's own host code (krum_take, tmean::shape) and copied
 // to the start of the workspace; the scalar call's layout follows it.  The scalar calls pass no table and run as they
 // always have.
+// The large calls (afl_defend_batched_large) take up to 1024 clients per problem: every Gram form is batched for any
+// tile count, and the register-resident trimmed-mean kernels end at 1024 rows.
 // ------------------------------------------------------------------------------------------------
 constexpr int kBatchMaxClients = 128;            // one Gram tile
+constexpr int kBatchLargeMaxClients = 1024;      // the largest register-resident trimmed-mean kernel (S = 32)
 constexpr int kBatchMax = 65535;                 // grid y / z limit
 
 enum BatchedRule { B_BAD, B_MEAN, B_KRUM, B_TM, B_BULYAN };
@@ -634,6 +641,12 @@ static int check_counts(const char* who, const int* fs, int batch, int f_cap, in
 }
 
 static size_t table_bytes(int batch) { return align_up(static_cast<size_t>(batch) * sizeof(ProblemParams), 256); }
+// The table of a batch with more than kBatchMaxClients rows per slot: ProblemParams[batch], then int perm[batch], the
+// problems grouped by trimmed-mean slot class (tmean::trimmed_mean_classes).
+static size_t class_table_bytes(int batch, int n) {
+  if (n <= kBatchMaxClients) return table_bytes(batch);
+  return align_up(static_cast<size_t>(batch) * (sizeof(ProblemParams) + sizeof(int)), 256);
+}
 
 // The rule's scratch after the table (0: the rule needs none).
 static size_t batched_ws_parts(BatchedRule r, int batch, int n, int64_t d, int dtype, size_t* gram_ws, size_t* tabs) {
@@ -658,6 +671,36 @@ static int upload_table(const char* who, int batch, void* ws, size_t ws_bytes, s
   for (int b = 0; b < batch; ++b) row(b, host[b]);
   AFL_CUDA(cudaMemcpyAsync(ws, host.data(), host.size() * sizeof(ProblemParams), cudaMemcpyHostToDevice, stream));
   *table = static_cast<const ProblemParams*>(ws);
+  return AFL_OK;
+}
+
+// upload_table followed by the problems grouped by the trimmed-mean slot class of their tm.n_rows, in one copy: the
+// device permutation in *perm, the class sizes in counts[kSlotClasses] (host).
+template <typename Row>
+static int upload_class_table(const char* who, int batch, void* ws, size_t ws_bytes, size_t need, cudaStream_t stream,
+                              Row row, const ProblemParams** table, const int** perm, int* counts) {
+  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
+    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
+    return AFL_ERR_WORKSPACE;
+  }
+  const size_t nb = static_cast<size_t>(batch);
+  std::vector<ProblemParams> host(nb);
+  std::vector<int> cls(nb), order(nb);
+  for (int c = 0; c < kSlotClasses; ++c) counts[c] = 0;
+  for (int b = 0; b < batch; ++b) {
+    row(b, host[b]);
+    cls[b] = tmean::slot_class(host[b].tm.n_rows);
+    ++counts[cls[b]];
+  }
+  int start[kSlotClasses];
+  for (int c = 0, s = 0; c < kSlotClasses; s += counts[c], ++c) start[c] = s;
+  for (int b = 0; b < batch; ++b) order[start[cls[b]]++] = b;          // problems in order within a class
+  std::vector<uint8_t> bytes(nb * (sizeof(ProblemParams) + sizeof(int)));
+  memcpy(bytes.data(), host.data(), nb * sizeof(ProblemParams));
+  memcpy(bytes.data() + nb * sizeof(ProblemParams), order.data(), nb * sizeof(int));
+  AFL_CUDA(cudaMemcpyAsync(ws, bytes.data(), bytes.size(), cudaMemcpyHostToDevice, stream));
+  *table = static_cast<const ProblemParams*>(ws);
+  *perm = reinterpret_cast<const int*>(static_cast<const uint8_t*>(ws) + nb * sizeof(ProblemParams));
   return AFL_OK;
 }
 
@@ -736,13 +779,16 @@ static int defend_batched(const char* rule, const void* G, int batch, int64_t ba
 // count from them: tm.n_rows (the Gram centre, Krum, TrimmedMean, NoDefense), theta + 2f (Bulyan's selection, whose
 // users_count is its row count).  Bulyan's second stage needs tm = shape(theta, 2f): that table is copied over the
 // first one after the selection kernels, in stream order.  The workspace layout is afl_defend_batched_each's.
-static int defend_batched_rows(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
-                               int64_t ld, int dtype, const int* rows, const int* ucs, const int* fs, float* out,
-                               int* idx_out, int* sel_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  const char* who = "afl_defend_batched_rows";
+// max_clients: kBatchMaxClients (afl_defend_batched_rows) or kBatchLargeMaxClients (afl_defend_batched_large).  Slots of
+// more than kBatchMaxClients rows append the problems' trimmed-mean class permutation to the table
+// (class_table_bytes), and the trimmed mean runs one launch per class (tmean::trimmed_mean_classes).
+static int defend_batched_rows(const char* who, int max_clients, const char* rule, const void* G, int batch,
+                               int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, const int* rows,
+                               const int* ucs, const int* fs, float* out, int* idx_out, int* sel_out, void* ws,
+                               size_t ws_bytes, cudaStream_t stream) {
   const BatchedRule r = batched_rule(rule);
   if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
-  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, max_clients);
   if (rc) return rc;
   if (!rows || !ucs) { set_error("%s: the per-problem row counts or users counts are NULL", who); return AFL_ERR_BAD_ARG; }
   int fmin = 0, fmax = 0;
@@ -775,24 +821,32 @@ static int defend_batched_rows(const char* rule, const void* G, int batch, int64
   }
   size_t gram_ws = 0, tabs = 0;
   const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  const bool classes = n > kBatchMaxClients;
+  const size_t tab_bytes = class_table_bytes(batch, n);
   const ProblemParams* each = nullptr;
+  const int* perm = nullptr;
+  int counts[kSlotClasses];
   auto row = [&](int b, ProblemParams& q) {
     q.f = fs[b];
     q.take = select::krum_take(rows[b], ucs[b], fs[b]);
     q.theta = ucs[b] - 2 * fs[b];
     q.tm = tmean::shape(rows[b], fs[b]);
   };
-  rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch) + rule_ws, stream, row, &each);
+  rc = classes ? upload_class_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row, &each, &perm, counts)
+               : upload_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row, &each);
   if (rc) return rc;
-  uint8_t* p = static_cast<uint8_t*>(ws) + table_bytes(batch);
+  uint8_t* p = static_cast<uint8_t*>(ws) + tab_bytes;
   if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, each);
+  if (r == B_TM && classes)
+    return tmean::trimmed_mean_classes(G, n, d, ld, dtype, nullptr, out, batch, batch_stride, 0, d, stream, each, perm,
+                                       counts);
   if (r == B_TM)
     return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, fmin, out, batch, batch_stride, 0, d, stream, each);
   const size_t nn = static_cast<size_t>(batch) * n * n;
   double* d2 = reinterpret_cast<double*>(p);
   float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
   void* sel_ws = p + tabs + gram_ws;
-  const size_t sel_ws_bytes = ws_bytes - table_bytes(batch) - tabs - gram_ws;
+  const size_t sel_ws_bytes = ws_bytes - tab_bytes - tabs - gram_ws;
   rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream, each);
   if (rc) return rc;
   if (r == B_KRUM)
@@ -800,10 +854,17 @@ static int defend_batched_rows(const char* rule, const void* G, int batch, int64
   rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
   rc = select::bulyan_rounds(dist, n, fmin, theta_max, sel_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
   if (rc) return rc;
-  rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch) + rule_ws, stream, [&](int b, ProblemParams& q) {
+  auto row2 = [&](int b, ProblemParams& q) {
     row(b, q);
     q.tm = tmean::shape(q.theta, 2 * fs[b]);              // the trimmed mean of the theta_b selected rows with 2 f_b
-  }, &each);
+  };
+  if (classes) {
+    rc = upload_class_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row2, &each, &perm, counts);
+    if (rc) return rc;
+    return tmean::trimmed_mean_classes(G, n, d, ld, dtype, sel_out, out, batch, batch_stride, theta_max, d, stream, each,
+                                       perm, counts);
+  }
+  rc = upload_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row2, &each);
   if (rc) return rc;
   return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, theta_max, 2 * fmin, out, batch, batch_stride, theta_max,
                                      d, stream, each);
@@ -811,11 +872,12 @@ static int defend_batched_rows(const char* rule, const void* G, int batch, int64
 
 // fs == NULL: rows 0..f-1 and z in every problem of f-row problems (afl_alie_batched).  Otherwise problem b has n rows of
 // which fs[b] are malicious, and its own z (afl_alie_batched_each); the workspace holds the table.
+// max_rows: kBatchMaxClients, or no limit for afl_alie_batched_large (a column pass, as the backdoor's).
 static int alie_batched(const char* who, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
                         int dtype, int f, double z, const int* fs, const double* zs, float* mu_out, float* sigma_out,
                         float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* ws,
-                        size_t ws_bytes, cudaStream_t stream) {
-  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
+                        size_t ws_bytes, cudaStream_t stream, int max_rows = kBatchMaxClients) {
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, max_rows);
   if (rc) return rc;
   int fmin = f, fmax = f;
   if (fs) {
@@ -1128,8 +1190,42 @@ int afl_defend_batched_rows(const char* rule, const void* G, int batch, int64_t 
                             int64_t ld, int dtype, const int* rows, const int* users_counts, const int* corrupted_counts,
                             float* out, int* idx_out, int* sel_out, void* workspace, size_t workspace_bytes,
                             void* stream) {
-  return defend_batched_rows(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_counts, corrupted_counts, out,
-                             idx_out, sel_out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  return defend_batched_rows("afl_defend_batched_rows", kBatchMaxClients, rule, G, batch, batch_stride, n, d, ld, dtype,
+                             rows, users_counts, corrupted_counts, out, idx_out, sel_out, workspace, workspace_bytes,
+                             static_cast<cudaStream_t>(stream));
+}
+
+size_t afl_batched_large_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
+  const BatchedRule r = batched_rule(rule);
+  if (r == B_BAD || n < 1 || n > kBatchLargeMaxClients) return 0;
+  if (n <= kBatchMaxClients) return afl_batched_rows_workspace_bytes(rule, batch, n, d, dtype);
+  if (batch < 1 || batch > kBatchMax || d < 1 || (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16)) return 0;
+  size_t gram_ws = 0, tabs = 0;
+  return class_table_bytes(batch, n) + batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+}
+
+int afl_defend_batched_large(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                             int64_t ld, int dtype, const int* rows, const int* users_counts,
+                             const int* corrupted_counts, float* out, int* idx_out, int* sel_out, void* workspace,
+                             size_t workspace_bytes, void* stream) {
+  std::vector<int> all;                                 // rows == NULL: n rows in every problem
+  if (!rows && batch >= 1 && batch <= kBatchMax) {
+    all.assign(static_cast<size_t>(batch), n);
+    rows = all.data();
+  }
+  return defend_batched_rows("afl_defend_batched_large", kBatchLargeMaxClients, rule, G, batch, batch_stride, n, d, ld,
+                             dtype, rows, users_counts, corrupted_counts, out, idx_out, sel_out, workspace,
+                             workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int afl_alie_batched_large(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                           const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
+                           float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                           size_t workspace_bytes, void* stream) {
+  if (!f) { set_error("afl_alie_batched_large: the per-problem corrupted counts are NULL"); return AFL_ERR_BAD_ARG; }
+  return alie_batched("afl_alie_batched_large", G, batch, batch_stride, n, d, ld, dtype, 0, 0.0, f, z, mu_out, sigma_out,
+                      crafted_out, bcast_rows, bcast_batch_stride, bcast_ld, workspace, workspace_bytes,
+                      static_cast<cudaStream_t>(stream), INT32_MAX);
 }
 
 size_t afl_metrics_workspace_bytes(int batch, int n, int64_t d, int dtype) {

@@ -103,7 +103,7 @@ __global__ void sqdist_to_dist_kernel(const double* __restrict__ d2, int n, size
 
 // tensor-core tile-pair kernel (gram_pair.cu)
 size_t pair_parts_bytes(int n, int64_t d, int batch);
-size_t pair_center_bytes(int64_t d);
+size_t pair_center_bytes(int64_t d, int batch);
 int launch_pair(const void* G, int mode, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, float* parts,
                 double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream,
                 const ProblemParams* rows);
@@ -135,7 +135,8 @@ static bool tensor_eligible(const void* G, int batch, int64_t batch_stride, int 
 // D >= 32768); elsewhere, and with AFL_GRAM_TF32X2 / AFL_GRAM_SINGLE_PASS, to the split-TF32 operands (smaller
 // uniform bias, no centring).  bf16 and fp16 clients are the operands themselves (kModeBf16In, kModeF16In); the fp32
 // operand flags do not apply to them.  A batch chooses like one problem of its shape; its split counts see batch times
-// the CTAs of one problem, and AFL_GRAM_SPLITS overrides both paths' split count.
+// the CTAs of one problem, and AFL_GRAM_SPLITS overrides both paths' split count.  A multi-tile bf16x2 batch holds one
+// centre vector per problem.
 static Plan make_plan(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, int flags) {
   Plan pl{};
   pl.tensor = !(flags & AFL_GRAM_FORCE_SIMT) && tensor_eligible(G, batch, batch_stride, n, d, ld, dtype);
@@ -149,7 +150,7 @@ static Plan make_plan(const void* G, int batch, int64_t batch_stride, int n, int
     else pl.mode = kModeBf16x2;
     pl.parts_bytes = pair_parts_bytes(n, d, batch);
     pl.s_bytes = align_up(static_cast<size_t>(batch) * n * n * sizeof(double), 256);
-    pl.total = pl.parts_bytes + pl.s_bytes + pair_center_bytes(d);
+    pl.total = pl.parts_bytes + pl.s_bytes + pair_center_bytes(d, pl.mode == kModeBf16x2 && n > 128 ? batch : 1);
   } else {
     const int t32 = (n + 31) / 32;
     int64_t chunks = (d + 31) / 32;

@@ -3,8 +3,9 @@
 //
 //   * The N x N table is cut into T = ceil(N/128) row tiles; only the T(T+1)/2 pairs (I >= J) are computed.
 //     CTA = (pair, K split); split s owns the k-blocks s, s+S, s+2S, ... and writes its partial S tile to a private
-//     slot, which pair_reduce_kernel sums in a fixed order in float64 (bit-reproducible).  A batch of same-shape one-tile
-//     problems adds grid dimension y = problem (a 3-D tensor map {d, n, batch}), with one private slot per (problem, split).
+//     slot, which pair_reduce_kernel sums in a fixed order in float64 (bit-reproducible).  A batch of same-shape
+//     problems adds grid dimension y = problem (a 3-D tensor map {d, n, batch}), with one private slot per (problem,
+//     pair, split); with more than one tile each problem's bf16x2 centre is its own row of a [batch][d_pad] buffer.
 //   * One TMA box {k-block columns x 128 rows} per tile and k-block lands in a 7-slot ring of 32 KB slots (rows past
 //     N and columns past D are zero-filled).  Three operand formats (`kMode`):
 //       kModeBf16x2  fp32 clients, 64-column k-blocks.  A converter warp rewrites the slot IN PLACE: every 8-row
@@ -126,10 +127,13 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[K]) {
 // parameter: a runtime branch between the two MMA sequences makes ptxas fence every k-block's wgmma issue.)
 // kRows (a ragged batch, center == 2 only): problem b's centre is the mean of its own last 8 participating rows,
 // max(m - 8, 0) .. m - 1 with m = p.each[b].tm.n_rows, instead of rows n - 8 .. n - 1 of the box.
+// kRows without kSym (kModeBf16x2 with more than one tile, batch > 1): problem b's centre is row b of the
+// [batch][kblocks * 64] cvec buffer that pair_center_kernel wrote (its own last rows, ragged or not).
 template <int kMode, int kSymN, bool kRows>
 __global__ void __launch_bounds__(kPThreads, 1)
 gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
   constexpr bool kSym = kSymN != 0;
+  constexpr bool kEachCen = kRows && !kSym;                 // per-problem centre vector
   static_assert(!kSym || (kMode == kModeBf16x2 && kSymN % 8 == 0 && kSymN >= 56 && kSymN <= 112),
                 "the symmetric form is a bf16x2 form on 8-row units, and warpgroup 2's rows 64.. must exist");
   constexpr int kAcc = kSym ? kSymN / 2 : 64;               // accumulators per thread (m64nN: N / 2)
@@ -210,12 +214,14 @@ gram_pair_kernel(const __grid_constant__ CUtensorMap tmap, const PairParams p) {
       auto load_center = [&](int box) -> float4 {
         if (!(p.center == 1 && box < nboxes)) return make_float4(0.f, 0.f, 0.f, 0.f);
         const int64_t col = static_cast<int64_t>(split + (box / nbx) * p.splits) * kPCols + c16 * 4;
+        if constexpr (kEachCen)
+          return __ldg(reinterpret_cast<const float4*>(p.cvec + static_cast<int64_t>(blockIdx.y) * p.kblocks * kPCols + col));
         return __ldg(reinterpret_cast<const float4*>(p.cvec + col));
       };
       const int units = box_bytes / 2048u;
       constexpr float two = kSym ? 2.f : 1.f;               // kSym: the second atom is 2 b2 (exact, a power of 2)
       int rows_b = 0, crow0_b = 0;                          // kRows: this problem's row count and first centre row
-      if constexpr (kRows) {
+      if constexpr (kRows && kSym) {
         rows_b = p.each[blockIdx.y].tm.n_rows;
         crow0_b = rows_b > kGramCenterRows ? rows_b - kGramCenterRows : 0;
       }
@@ -431,13 +437,18 @@ __global__ void pair_to_sqdist_kernel(const double* __restrict__ S, int n, int s
   d2[static_cast<size_t>(i) * n + j] = v;
 }
 
-// centre vector: mean of the last `rows` clients, zero past d (the k-blocks are 64 columns wide)
+// centre vectors, grid y = problem: problem b's is the mean of its last min(m, 8) clients, rows max(m - 8, 0) .. m - 1
+// of G + b * batch_stride with m = each[b].tm.n_rows (a ragged batch) or n, zero past d (the k-blocks are 64 columns
+// wide), at cvec + b * d_pad.  gram_center's arithmetic: problem b's centre is a single call's on its m rows.
 __global__ void __launch_bounds__(256)
-pair_center_kernel(const float* __restrict__ cref, int rows, int64_t ld, int64_t d, int64_t d_pad, float* __restrict__ cvec) {
+pair_center_kernel(const float* __restrict__ G, int n, int64_t ld, int64_t batch_stride, int64_t d, int64_t d_pad,
+                   const ProblemParams* __restrict__ each, float* __restrict__ cvec) {
   const int64_t col = (static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x) * 4;
   if (col >= d_pad) return;
-  const float4 c = gram_center(cref, rows, ld, col, d);
-  *reinterpret_cast<float4*>(cvec + col) = c;
+  const int m = each ? each[blockIdx.y].tm.n_rows : n;
+  const int rows = m < kGramCenterRows ? m : kGramCenterRows;
+  const float4 c = gram_center(G + blockIdx.y * batch_stride + static_cast<int64_t>(m - rows) * ld, rows, ld, col, d);
+  *reinterpret_cast<float4*>(cvec + blockIdx.y * d_pad + col) = c;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -466,7 +477,10 @@ int pair_splits(int n, int64_t d, int batch) {
   if (s > kblocks) s = static_cast<int>(kblocks);
   return s < 1 ? 1 : s;
 }
-size_t pair_center_bytes(int64_t d) { return align_up(static_cast<size_t>((d + kPCols - 1) / kPCols * kPCols) * sizeof(float), 256); }
+// one centre vector per problem (only the multi-tile bf16x2 form of a batch uses more than the first)
+size_t pair_center_bytes(int64_t d, int batch) {
+  return static_cast<size_t>(batch) * align_up(static_cast<size_t>((d + kPCols - 1) / kPCols * kPCols) * sizeof(float), 256);
+}
 size_t pair_parts_bytes(int n, int64_t d, int batch) {
   const int tiles = (n + 127) / 128, pairs = tiles * (tiles + 1) / 2;
   return static_cast<size_t>(pairs) * batch * pair_splits(n, d, batch) * kPPartElems * sizeof(float);
@@ -504,16 +518,16 @@ static int launch_sym(const CUtensorMap& tmap, const PairParams& p, int batch, c
 }
 
 // G: `batch` problems of fp32 [n, d] (pitch multiple of 4 elements) or bf16 / fp16 (kModeBf16In / kModeF16In, pitch
-// multiple of 8), 16-byte aligned, problem b at G + b * batch_stride elements (batch > 1: one tile, a 16-byte multiple
-// >= n * ld).  parts: pair_parts_bytes(); S and d2_out: batch * n * n doubles; cvec: pair_center_bytes().
-// rows (device, may be NULL): a ragged batch's table, whose tm.n_rows places the one-tile form's centre per problem.  Any
-// other entry S_ij depends on rows i and j only, so the other forms need no table.
+// multiple of 8), 16-byte aligned, problem b at G + b * batch_stride elements (batch > 1: a 16-byte multiple >= n * ld).
+// parts: pair_parts_bytes(); S and d2_out: batch * n * n doubles; cvec: pair_center_bytes(d, batch) with more than one
+// tile, else pair_center_bytes(d, 1).  rows (device, may be NULL): a ragged batch's table, whose tm.n_rows places each
+// problem's centre in the bf16x2 forms.  Any other entry S_ij depends on rows i and j only, so the other forms need no
+// table.
 int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, float* parts,
                 double* S, float* cvec, double* d2_out, int flush, int center, int single_pass, cudaStream_t stream,
                 const ProblemParams* rows) {
   const float* G = static_cast<const float*>(Gv);
   const bool half16 = mode == kModeBf16In || mode == kModeF16In;    // 16-bit elements
-  if (batch > 1 && n > 128) { set_error("gram_pair_kernel: batched problems are one tile (n <= 128, got %d)", n); return AFL_ERR_UNSUPPORTED; }
   static EncodeTiledFn enc = nullptr;
   if (!enc) {
     void* fp = nullptr;
@@ -540,10 +554,9 @@ int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n
   p.cvec = cvec;
   p.each = rows;
   if (p.center == 1) {
-    const int cref_rows = n < kGramCenterRows ? n : kGramCenterRows;
     const int64_t d_pad = (d + kPCols - 1) / kPCols * kPCols;
-    pair_center_kernel<<<static_cast<unsigned>((d_pad / 4 + 255) / 256), 256, 0, stream>>>(
-        G + static_cast<int64_t>(n - cref_rows) * ld, cref_rows, ld, d, d_pad, cvec);
+    pair_center_kernel<<<dim3(static_cast<unsigned>((d_pad / 4 + 255) / 256), batch), 256, 0, stream>>>(
+        G, n, ld, batch > 1 ? batch_stride : 0, d, d_pad, rows, cvec);
     AFL_LAUNCH_CHECK("pair_center_kernel");
   }
   CUtensorMap tmap;
@@ -563,7 +576,8 @@ int launch_pair(const void* Gv, int mode, int batch, int64_t batch_stride, int n
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed: %d", static_cast<int>(r)); return AFL_ERR_CUDA; }
   int rc = sym                   ? (rows && p.center == 2 ? launch_sym<true>(tmap, p, batch, stream)
                                                           : launch_sym<false>(tmap, p, batch, stream))
-         : mode == kModeBf16x2 ? launch_mode<kModeBf16x2, 0>(tmap, p, batch, stream)
+         : mode == kModeBf16x2 ? (batch > 1 ? launch_mode<kModeBf16x2, 0, true>(tmap, p, batch, stream)
+                                            : launch_mode<kModeBf16x2, 0>(tmap, p, batch, stream))
          : mode == kModeTf32x2 ? launch_mode<kModeTf32x2, 0>(tmap, p, batch, stream)
          : mode == kModeF16In  ? launch_mode<kModeF16In, 0>(tmap, p, batch, stream)
                                : launch_mode<kModeBf16In, 0>(tmap, p, batch, stream);

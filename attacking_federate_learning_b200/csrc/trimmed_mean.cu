@@ -31,8 +31,12 @@
 //     the register-resident column (tie_sum).
 //   * More than 1024 rows: trimmed_mean_large_kernel (shared-memory strip, bisection on the integer image of the keys).
 //   * A batch (grid y) may carry a ProblemParams table: problem b then has its own participating rows, keep and pivot
-//     constants (tm).  Batches have n <= 128 rows, so only S = 4 has instances that read it (EACH); rows past a
-//     problem's n_rows are staged as +inf like the rows past n_rows of a single call.
+//     constants (tm); rows past a problem's n_rows are staged as +inf like the rows past n_rows of a single call.  With
+//     n <= 128 rows every problem runs trimmed_mean_kernel<4, DT, EACH> over grid y = problem.  Larger batches
+//     (trimmed_mean_classes) run every problem in the instance that its own n_rows selects, as its single call does: one
+//     launch per slot class present, grid y = the class's problems, problem P.perm[blockIdx.y] (CLASS).
+#include <type_traits>
+
 #include "afl_common.cuh"
 
 namespace afl {
@@ -55,6 +59,12 @@ struct Params {
   int ri_batch;
   int vec_ok;
 };
+// A class launch's arguments (trimmed_mean_kernel<S, DT, true, true>): Params and the class's problems (device).  A type
+// of its own, so that Params and the kernels that take it keep their layout.
+struct ClassParams : Params {
+  const int* perm;
+};
+template <bool CLASS> using KernelParams = std::conditional_t<CLASS, ClassParams, Params>;
 
 __device__ __forceinline__ int warp_sum_i(int v) { return __reduce_add_sync(0xffffffffu, v); }
 __device__ __forceinline__ float warp_min_f(float v) {
@@ -424,7 +434,14 @@ __device__ __forceinline__ bool select_fast(const float (&v)[S], const ColRef& c
 // Thread t loads the 16-byte chunk j = t&3 of row (it*64 + t>>2) in iteration `it`.  Row r lives in
 // slot r>>5 of lane r&31; slot-group m = slot>>2 and the XOR-ed slot position are compile-time
 // functions of `it`, so every store below has an immediate offset from one of two per-thread bases.
-template <int S, int DT>
+// The problem a CTA works on: blockIdx.y, or for a class launch (CLASS) the class's blockIdx.y-th problem.
+template <bool CLASS>
+__device__ __forceinline__ unsigned problem_of(const Params& P) {
+  if constexpr (CLASS) return static_cast<unsigned>(static_cast<const ClassParams&>(P).perm[blockIdx.y]);
+  else return blockIdx.y;
+}
+
+template <int S, int DT, bool CLASS>
 __device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, uint32_t* tile, int64_t col0) {
   constexpr int kGroups = S / 4;
   constexpr bool W16 = DT != AFL_F32;                   // two 16-bit columns per word
@@ -432,8 +449,16 @@ __device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, u
   const int es = W16 ? 2 : 4;
   const int cols_per_tile = W16 ? 32 : 16;
   const uint32_t sentinel = DT == AFL_F16 ? 0x7C007C00u : DT == AFL_BF16 ? 0x7F807F80u : 0x7F800000u;   // +inf
-  const uint8_t* base = static_cast<const uint8_t*>(P.G) + static_cast<int64_t>(blockIdx.y) * P.g_batch * es;
-  const int* row_index = P.row_index ? P.row_index + static_cast<int64_t>(blockIdx.y) * P.ri_batch : nullptr;
+  const uint8_t* base;
+  const int* row_index;
+  if constexpr (CLASS) {
+    const int64_t b = problem_of<CLASS>(P);
+    base = static_cast<const uint8_t*>(P.G) + b * P.g_batch * es;
+    row_index = P.row_index ? P.row_index + b * P.ri_batch : nullptr;
+  } else {
+    base = static_cast<const uint8_t*>(P.G) + static_cast<int64_t>(blockIdx.y) * P.g_batch * es;
+    row_index = P.row_index ? P.row_index + static_cast<int64_t>(blockIdx.y) * P.ri_batch : nullptr;
+  }
   constexpr int kIters = (32 * S * 4) / kThreads;      // S/2
   const bool full_tile = P.vec_ok && (col0 + cols_per_tile <= P.d);
   const int rowq = tid >> 2, j = tid & 3, l = rowq & 31, hi2 = tid >> 7;
@@ -598,12 +623,17 @@ constexpr int kScratchWords = 96;              // per warp: dense candidate list
 
 // S <= 20 (up to 640 rows: Bulyan's second stage at N = 500 and N = 1000) leaves room for four CTAs per SM in shared memory; ask
 // the compiler for 64 registers there (resident warps are what hides the shuffle chains of the scans and sorts).
-// EACH: problem blockIdx.y's constants come from the per-problem table P.each (batches only, so S = 4).  A separate instance:
+// EACH: problem blockIdx.y's constants come from the per-problem table P.each (batches only).  A separate instance:
 // holding them in registers instead of reading the constant bank takes the fp32 kernel from 48 to 54 registers, which
-// would cost the single calls a fifth CTA per SM.
-template <int S, int DT, bool EACH>
-__global__ void __launch_bounds__(kThreads, (S <= 20 ? 4 : 3))      // (S = 24 fits 4 CTAs in shared memory too, but the fp32 instance spills at 64 registers)
-trimmed_mean_kernel(const Params P) {
+// would cost the single calls a fifth CTA per SM.  CLASS (with EACH): a class launch, problem P.perm[blockIdx.y].
+// The class instances hold the table constants and the problem index in registers too: they would spill from S = 16 on
+// at the single calls' bounds, so they ask for fewer CTAs per SM: 3 at S = 16 (80 registers), 2 from S = 20 (128; the
+// 16-bit S = 20 instances still spill at 80).
+template <int S, int DT, bool EACH, bool CLASS = false>
+__global__ void __launch_bounds__(kThreads, CLASS ? (S <= 12 ? 4 : S <= 16 ? 3 : 2)
+                                                  : (S <= 20 ? 4 : 3))      // (S = 24 fits 4 CTAs in shared memory too, but the fp32 instance spills at 64 registers)
+trimmed_mean_kernel(const KernelParams<CLASS> P) {
+  static_assert(EACH || !CLASS, "a class launch reads the table");
   extern __shared__ __align__(1024) uint32_t tile[];     // [16 word-cols][S/4 groups][32 lanes][4 slots] + scratch
   constexpr int kGroups = S / 4;
   constexpr bool W16 = DT != AFL_F32;                    // bf16 / fp16: two columns per word-column
@@ -611,8 +641,9 @@ trimmed_mean_kernel(const Params P) {
   const int cols_per_tile = W16 ? 32 : 16;
   const int64_t col0 = static_cast<int64_t>(blockIdx.x) * cols_per_tile;
   TmShape sh = P.tm;
-  if constexpr (EACH) sh = P.each[blockIdx.y].tm;
-  stage_tile<S, DT>(P, sh, tile, col0);
+  if constexpr (CLASS) sh = P.each[problem_of<CLASS>(P)].tm;
+  else if constexpr (EACH) sh = P.each[blockIdx.y].tm;
+  stage_tile<S, DT, CLASS>(P, sh, tile, col0);
   // read once, after staging: `volatile` keeps ptxas from re-reading the special register (S2R, ~50 cycles of
   // latency) in front of every scan and sort of the per-column code to save one register
   int lane = tid & 31, warp_o = warp;
@@ -629,7 +660,11 @@ trimmed_mean_kernel(const Params P) {
       const int64_t col = col0 + (W16 ? 2 * cw + half : cw);
       if (col >= P.d) break;                         // warp-uniform
       const float res = general_column_impl<S, DT>(sh, tile, cw, half, scratch, lane);
-      if (lane == 0) P.out[static_cast<int64_t>(blockIdx.y) * P.out_batch + col] = res;
+      if constexpr (CLASS) {
+        if (lane == 0) P.out[static_cast<int64_t>(problem_of<CLASS>(P)) * P.out_batch + col] = res;
+      } else {
+        if (lane == 0) P.out[static_cast<int64_t>(blockIdx.y) * P.out_batch + col] = res;
+      }
     }
   }
 }
@@ -765,27 +800,36 @@ static double norm_ppf(double pr) {   // Acklam's rational approximation, |error
          (((((b[0] * r + b[1]) * r + b[2]) * r + b[3]) * r + b[4]) * r + 1.0);
 }
 
+// perm != NULL: a class launch over `batch` problems perm[0 .. batch) (trimmed_mean_classes)
 template <int S>
-static int launch(const Params& P, int dtype, int batch, cudaStream_t stream) {
+static int launch(const Params& P, int dtype, int batch, cudaStream_t stream, const int* perm = nullptr) {
   const size_t smem = static_cast<size_t>(S) * 2048 + kWarps * kScratchWords * 4;
   const int cols = dtype != AFL_F32 ? 32 : 16;
   const dim3 grid(static_cast<unsigned>(ceil_div64(P.d, cols)), batch);
   ProfScope ps("trimmed_mean", stream);
-  auto go = [&](auto kernel) -> int {
+  auto go = [&](auto kernel, const auto& args) -> int {
     AFL_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    kernel<<<grid, kThreads, smem, stream>>>(P);
+    kernel<<<grid, kThreads, smem, stream>>>(args);
     AFL_LAUNCH_CHECK("trimmed_mean_kernel");
     return AFL_OK;
   };
+  if (perm) {
+    ClassParams C{};
+    static_cast<Params&>(C) = P;
+    C.perm = perm;
+    return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, true, true>, C)
+           : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, true, true>, C)
+                              : go(trimmed_mean_kernel<S, AFL_F32, true, true>, C);
+  }
   if constexpr (S == 4) {
     if (P.each)
-      return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, true>)
-             : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, true>)
-                                : go(trimmed_mean_kernel<S, AFL_F32, true>);
+      return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, true>, P)
+             : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, true>, P)
+                                : go(trimmed_mean_kernel<S, AFL_F32, true>, P);
   }
-  return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, false>)
-         : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, false>)
-                            : go(trimmed_mean_kernel<S, AFL_F32, false>);
+  return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, false>, P)
+         : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, false>, P)
+                            : go(trimmed_mean_kernel<S, AFL_F32, false>, P);
 }
 
 // The constants of n_rows participating rows and corrupted_count: number_to_consider = rows - f - 1 with Python slice
@@ -846,6 +890,47 @@ int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype,
   if (n_rows <= 768) return launch<24>(P, dtype, batch, stream);
   if (n_rows <= 896) return launch<28>(P, dtype, batch, stream);
   return launch<32>(P, dtype, batch, stream);
+}
+
+// The slot class of n_rows <= 1024 participating rows: c = 0 .. kSlotClasses - 1 for the kernel with S = 4 (c + 1)
+// slots per lane, the instance that trimmed_mean_batched launches for them.
+int slot_class(int n_rows) { return n_rows <= 128 ? 0 : (n_rows - 1) / 128; }
+
+// A batch with a table whose problems have up to 1024 participating rows each (each[b].tm.n_rows): problem b runs the
+// instance that its own row count selects, so its result is its single call's bit for bit.  perm (device, `batch`
+// entries) lists the problems class by class, counts[c] (host, kSlotClasses entries) how many have class c; one launch
+// per class present, over its problems only.
+int trimmed_mean_classes(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, float* out,
+                         int batch, int64_t g_batch, int ri_batch, int64_t out_batch, cudaStream_t stream,
+                         const ProblemParams* each, const int* perm, const int* counts) {
+  if (!G || !out || !each || !perm || !counts || n < 1 || d < 1 || ld < d || batch < 1) {
+    set_error("afl_trimmed_mean: bad argument");
+    return AFL_ERR_BAD_ARG;
+  }
+  if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_trimmed_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
+  Params P{};
+  P.G = G; P.row_index = row_index; P.out = out; P.d = d; P.ld = ld; P.n_total = n;
+  P.each = each; P.g_batch = g_batch; P.out_batch = out_batch; P.ri_batch = ri_batch;
+  const int64_t es = dtype == AFL_F32 ? 4 : 2;
+  P.vec_ok = (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0) && (batch == 1 || (g_batch * es) % 16 == 0);
+  int first = 0;
+  for (int c = 0; c < kSlotClasses; first += counts[c], ++c) {
+    if (counts[c] < 1) continue;
+    const int* pc = perm + first;
+    int rc = AFL_OK;
+    switch (c) {
+      case 0: rc = launch<4>(P, dtype, counts[c], stream, pc); break;
+      case 1: rc = launch<8>(P, dtype, counts[c], stream, pc); break;
+      case 2: rc = launch<12>(P, dtype, counts[c], stream, pc); break;
+      case 3: rc = launch<16>(P, dtype, counts[c], stream, pc); break;
+      case 4: rc = launch<20>(P, dtype, counts[c], stream, pc); break;
+      case 5: rc = launch<24>(P, dtype, counts[c], stream, pc); break;
+      case 6: rc = launch<28>(P, dtype, counts[c], stream, pc); break;
+      default: rc = launch<32>(P, dtype, counts[c], stream, pc); break;
+    }
+    if (rc) return rc;
+  }
+  return AFL_OK;
 }
 
 int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,

@@ -333,6 +333,33 @@ int afl_defend_batched_rows(const char* rule, const void* G, int batch, int64_t 
                             float* out, int* idx_out, int* sel_out, void* workspace, size_t workspace_bytes,
                             void* stream);
 
+/* ---- large batches: up to 1024 clients per problem ----------------------------------------------------------------
+ * The reference's larger runs have N = 500 and N = 1000 users (f = 240 at N = 1000).  These calls take the batches of
+ * the calls above with 1 <= n <= 1024 rows per problem slot; n > 1024 -> AFL_ERR_UNSUPPORTED ("n <= 1024").
+ *
+ * afl_batched_large_workspace_bytes(rule, ...) — rule as afl_defend_batched; 0 on bad arguments and for n > 1024.  For
+ * n <= 128 exactly afl_batched_rows_workspace_bytes.  For n > 128 the parameter table is followed by `batch` ints (the
+ * problems grouped by trimmed-mean size class), then the layout of afl_batched_rows_workspace_bytes.
+ *
+ * afl_defend_batched_large — afl_defend_batched_rows with 1 <= n <= 1024: the same semantics, error codes, per-problem
+ * error messages and output layouts (sel_out [batch][theta_max], -2 past theta_b).  rows may be NULL: n rows in every
+ * problem.  rows, users_counts and corrupted_counts are HOST arrays.  Problem b's result is the single device call's
+ * on G[b][:rows[b]] bit for bit when both run the same Gram operand format and split count (the format is chosen from
+ * n, d and the dtype; for fp32 a single call at rows[b] > 128 runs the format a slot of n > 128 rows runs).  The
+ * trimmed mean (TrimmedMean, Bulyan's second stage) of every problem runs the kernel its own row count selects.
+ *
+ * afl_alie_batched_large — afl_alie_batched_each without the client limit: f_b <= n for any n (ALIE is a column pass,
+ * as afl_backdoor_start_batched).  Workspace: afl_batched_each_workspace_bytes("ALIE", batch, 1, d, dtype). */
+size_t afl_batched_large_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype);
+int afl_defend_batched_large(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                             int64_t ld, int dtype, const int* rows, const int* users_counts,
+                             const int* corrupted_counts, float* out, int* idx_out, int* sel_out, void* workspace,
+                             size_t workspace_bytes, void* stream);
+int afl_alie_batched_large(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                           const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
+                           float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                           size_t workspace_bytes, void* stream);
+
 /* ---- attack-success metrics of a batch (SURVEY 8d "Attack-success (C5)") --------------------------------------
  * The reference logs test accuracy only (main.py:73-82); what a z x malicious-share sweep reports follows from its
  * conventions.  The malicious users are ids 0..f-1 (main.py:28), so in problem b rows f_b..n-1 are honest:

@@ -3,8 +3,8 @@
 //
 // Tensor-core path (fp32, bf16 or fp16 input, 16-byte aligned rows): d2_ij = s_ii + s_jj - 2 s_ij with S = G G^T on the
 // Hopper warpgroup MMAs (csrc/gram_pair.cu), fp32 split into two bf16 or two TF32 terms, 16-bit clients as they are, K split over CTAs and the
-// partial tiles summed in a fixed order in float64 -> bit-reproducible, and identical rows give bit-identical
-// table rows (Krum's [1,0,2,...] tie-break relies on this).
+// partial tiles summed in a fixed order in float64 -> bit-reproducible, and identical rows give exact zeros and
+// bit-identical table rows outside the rows between them (Krum's [1,0,2,...] tie-break relies on this; DESIGN 2.1).
 //
 // SIMT path (any pitch, fp32, bf16 or fp16): direct sum of squared fp32 differences, float64 accumulation.
 // Used for misaligned pitches and as an independent check of the tensor path in the tests.

@@ -30,7 +30,9 @@
 //                    fp32 too).
 //     With more than one tile EVERY pair - diagonal ones too - issues the same sequence on the same K partition, so two
 //     clients with identical rows get bit-identical s_ii, s_jj and s_ij wherever their tiles are, and their distance is
-//     exactly 0 (ALIE makes rows 0..f-1 one array; Krum's [1, 0, 2, ...] tie-break depends on it).  The one-tile
+//     exactly 0 (ALIE makes rows 0..f-1 one array; Krum's [1, 0, 2, ...] tie-break depends on it).  Their distances to
+//     a third client j are identical unless j lies between them: the higher row of a pair is the I operand, so the two
+//     cross products of (j, i) and (k, j), i < j < k, are added in opposite orders (DESIGN 2.1).  The one-tile
 //     symmetric form keeps this: identical rows i, k give M_ik = M_ki = M_ii = M_kk bit for bit, and M_ij + M_ji =
 //     M_kj + M_jk.  (Across tiles an off-diagonal pair would need all three products to match the diagonal ones.)
 //   * Two consumer warpgroups own rows 0..63 and 64..127 of the I tile and issue wgmma.m64n128 with both operands

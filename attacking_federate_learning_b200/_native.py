@@ -78,6 +78,13 @@ SIGNATURES = {
                                         _sz, _vp]),
     "afl_backdoor_finish_batched": (_i, [_i, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _vp,
                                          _sz, _vp]),
+    "afl_batched_table_dev": (_i, [C.c_char_p, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "afl_defend_batched_dev": (_i, [C.c_char_p, _vp, _i, _i64, _i, _i64, _i64, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i,
+                                    _vp, _sz, _vp, _vp]),
+    "afl_alie_batched_dev": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _sz,
+                                  _vp, _vp]),
+    "afl_attack_metrics_batched_dev": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
+                                            _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
 }
 
 _lib = None

@@ -33,6 +33,12 @@ client limit.
 problem's distance from its honest mean, whether Krum picked a malicious client, and the malicious share of
 Bulyan's selection.  It has no client limit.
 
+`DeviceRound` runs the same calls with `f`, `z`, `rows` and `users_count` held as device tensors that the caller
+refills in place (C ABI `afl_*_dev`): its methods never synchronise, so after one eager warm-up a whole round can be
+captured with `torch.cuda.graph` and replayed.  Per-problem checks run on the device and land in `DeviceRound.status`;
+`raise_for_status` raises what the host-parameter call would.  The functions above do not change and keep refusing
+CUDA tensors for their per-problem values.
+
 The server's momentum step needs no batched form: `_device.momentum_step` on contiguous `[B, D]` weights,
 velocity and gradients is already the batched step (server.py:89-90 is element-wise).
 """
@@ -398,3 +404,185 @@ def attack_metrics(users_grads, corrupted_count, *, aggregated=None, krum_index=
     if honest is not None:
         res["honest_mean"] = honest
     return res
+
+
+_STATUS_ERRORS = {nat.AFL_ERR_BAD_ARG: (ValueError, "a corrupted count or row count is out of range"),
+                  nat.AFL_ERR_PRECONDITION: (AssertionError, "the reference's assert users_count >= 2*corrupted_count"
+                                             " + 1 (Krum) or >= 4*corrupted_count + 3 (Bulyan) is violated"),
+                  nat.AFL_ERR_UNSUPPORTED: (NotImplementedError, "Bulyan's users_count must equal its number of rows")}
+
+
+class DeviceRound:
+    """One lock-step round of a batch whose per-problem parameters live on the device (C ABI `afl_*_dev`).
+
+    The module-level functions take corrupted counts, strengths, row counts and users counts as host values and refuse
+    CUDA tensors, since reading one would synchronise.  A DeviceRound holds them as device tensors instead, which the
+    caller refills in place between rounds: `f` (int32 [B]), `z` (float64 [B]), `rows` (int32 [B], with rows=True) and
+    `users_count` (int32 [B], with rows=True and per_problem_users_count=True; otherwise it follows `rows`).  `G` is the
+    caller's [B, N, D] client tensor, also refilled in place.  Every method only enqueues work on the current stream
+    into outputs and a workspace sized once here (attack_metrics' small outputs are allocated per call, which a
+    captured graph serves from its own pool), so after one eager warm-up a whole round (your own training, then
+    `alie`, a defence, `attack_metrics` and `_device.momentum_step`) can be captured with `torch.cuda.graph` and
+    replayed.  Each method's result is the host-parameter call's on the same values, bit for bit.
+
+    Per-problem checks run on the device.  A problem that fails one gets its first error code in `status` (int32 [B],
+    sticky until `clear_status`) and runs on a safe row (rows_b = N, users_count_b = N, f_b = 0), so its outputs are
+    not the reference's; `raise_for_status` (the one call that synchronises) raises what the host-parameter call would:
+    ValueError, AssertionError, NotImplementedError, or KeyError(-1) for a Bulyan round with no eligible user.
+
+    users_count: one int for every problem without rows (default N).  rules: the defences this round runs (their
+    workspace is sized here); any of them needs N <= 128."""
+
+    def __init__(self, users_grads, users_count=None, *, rows=False, per_problem_users_count=False,
+                 rules=(DefenseTypes.Krum, DefenseTypes.Bulyan, DefenseTypes.TrimmedMean, DefenseTypes.NoDefense)):
+        if not isinstance(users_grads, torch.Tensor):
+            raise TypeError("users_grads: expected a torch.cuda tensor")
+        if users_grads.dim() != 3 or users_grads.stride(2) != 1:
+            raise ValueError("users_grads must be a [problems, clients, params] tensor with stride(2) == 1")
+        B, N, D = users_grads.shape
+        rules = tuple(rules)
+        for r in rules:
+            if r not in defend:
+                raise ValueError(f"DeviceRound: unknown rule {r!r}")
+        if rules and N > ONE_TILE:
+            raise NotImplementedError(f"DeviceRound defences support N <= {ONE_TILE} clients per problem (got {N})")
+        if per_problem_users_count and not rows:
+            raise ValueError("DeviceRound: per-problem users counts need rows=True")
+        if rows and users_count is not None:
+            raise ValueError("DeviceRound: with rows, users_count follows rows or is per problem")
+        if B < 1 or N < 1 or D < 1:
+            raise ValueError(f"DeviceRound: empty batch {tuple(users_grads.shape)}")
+        code = dtype_code(users_grads)
+        if not users_grads.is_cuda:
+            raise TypeError("users_grads: expected a torch.cuda tensor")
+        _, _, _, self._ld, self._bs = _check(users_grads)
+        self.G, self.B, self.N, self.D, self._code, self.rules = users_grads, B, N, D, code, rules
+        self.users_count_scalar = N if users_count is None else int(users_count)
+        dev = self.device = users_grads.device
+        self.f = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.z = torch.zeros(B, dtype=torch.float64, device=dev)
+        self.rows = torch.full((B,), N, dtype=torch.int32, device=dev) if rows else None
+        self.users_count = torch.full((B,), N, dtype=torch.int32, device=dev) if per_problem_users_count else None
+        self.status = torch.zeros(B, dtype=torch.int32, device=dev)
+        L = nat.lib()
+        nbytes = max([L.afl_batched_rows_workspace_bytes(r.encode(), B, N, D, code) for r in rules] +
+                     [L.afl_batched_each_workspace_bytes(b"ALIE", B, 1, D, code),
+                      L.afl_metrics_workspace_bytes(B, N, D, code)])
+        self._ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)     # one round's calls run in stream order
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.mu, self.sigma, self.crafted = (torch.empty((B, D), **f32) for _ in range(3))
+        self.out = {r: torch.empty((B, D), **f32) for r in rules if r != DefenseTypes.Krum}
+        self.krum_index = torch.empty(B, dtype=torch.int32, device=dev)
+        self.krum_rows = torch.empty((B, D), dtype=users_grads.dtype, device=dev)
+        self.selection = torch.empty((B, N), dtype=torch.int32, device=dev)
+        self._problems = torch.arange(B, dtype=torch.int64, device=dev)
+
+    @staticmethod
+    def _ptr(t):
+        return None if t is None else t.data_ptr()
+
+    def _call(self, fn, *args):
+        with torch.cuda.device(self.device):
+            nat.check(fn(*args))
+
+    def _defend(self, rule, out=None, idx=None, sel=None):
+        if rule not in self.rules:
+            raise ValueError(f"DeviceRound: {rule} was not among the rules given at construction")
+        self._call(nat.lib().afl_defend_batched_dev, rule.encode(), self.G.data_ptr(), self.B, self._bs, self.N, self.D,
+                   self._ld, self._code, self._ptr(self.rows), self.users_count_scalar, self._ptr(self.users_count),
+                   self.f.data_ptr(), self._ptr(out), self._ptr(idx), self._ptr(sel), self.N, self._ws.data_ptr(),
+                   self._ws.numel(), self.status.data_ptr(), _stream_ptr(self.G))
+
+    def alie(self):
+        """alie_rows with the device f and z: returns (crafted, mu, sigma), fp32 [B, D], and writes crafted over rows
+        0..f_b-1 of the problems with f_b > 0 and z_b != 0, in G's dtype (bf16 and fp16 rounded to nearest even)."""
+        self._call(nat.lib().afl_alie_batched_dev, self.G.data_ptr(), self.B, self._bs, self.N, self.D, self._ld,
+                   self._code, self.f.data_ptr(), self.z.data_ptr(), self.mu.data_ptr(), self.sigma.data_ptr(),
+                   self.crafted.data_ptr(), self.G.data_ptr(), self._bs, self._ld, self._ws.data_ptr(), self._ws.numel(),
+                   self.status.data_ptr(), _stream_ptr(self.G))
+        return self.crafted, self.mu, self.sigma
+
+    def krum(self, return_index=False):
+        """`krum`: the device int32 [B] indices, or the winning rows [B, D] in G's dtype.  Index -1 (no eligible user)
+        selects row rows_b - 1 (N - 1 without rows), the reference's users_grads[-1]."""
+        self._defend(DefenseTypes.Krum, idx=self.krum_index)
+        if return_index:
+            return self.krum_index
+        idx = self.krum_index.long()
+        last = self.N - 1 if self.rows is None else self.rows.long() - 1
+        row = torch.where(idx < 0, last, idx)
+        self.krum_rows.copy_(self.G[self._problems, row])
+        return self.krum_rows
+
+    def bulyan(self, return_selection=False):
+        """`bulyan`: fp32 [B, D] and, with return_selection, the int32 [B, N] selections (theta_b rounds, then -2; -1
+        from a failed round on).  A failed round flags its problem with KeyError(-1) in `status`."""
+        out = self.out[DefenseTypes.Bulyan] if DefenseTypes.Bulyan in self.out else None
+        self._defend(DefenseTypes.Bulyan, out=out, sel=self.selection)
+        return (out, self.selection) if return_selection else out
+
+    def trimmed_mean(self):
+        """`trimmed_mean`: fp32 [B, D]."""
+        out = self.out.get(DefenseTypes.TrimmedMean)
+        self._defend(DefenseTypes.TrimmedMean, out=out)
+        return out
+
+    def no_defense(self):
+        """`no_defense`: fp32 [B, D]."""
+        out = self.out.get(DefenseTypes.NoDefense)
+        self._defend(DefenseTypes.NoDefense, out=out)
+        return out
+
+    def attack_metrics(self, *, aggregated=None, krum_index=None, selection=None, return_honest_mean=False):
+        """`attack_metrics` with the device f (and rows): the same dict of device tensors."""
+        if aggregated is not None and krum_index is not None:
+            raise ValueError("attack_metrics: give the aggregate as `aggregated` or as `krum_index`, not both")
+        for t, name, dtype, shape in ((aggregated, "aggregated", torch.float32, (self.B, self.D)),
+                                      (krum_index, "krum_index", torch.int32, (self.B,)),
+                                      (selection, "selection", torch.int32, None)):
+            if t is not None and not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == dtype
+                                      and t.is_contiguous() and (t.shape == shape if shape else
+                                                                 (t.dim() == 2 and t.shape[0] == self.B))):
+                raise ValueError(f"{name}: expected a contiguous {dtype} tensor for {self.B} problems on {self.device}")
+        def out(when, shape, dtype):                     # fresh outputs: two calls in one round keep both results
+            return torch.empty(shape, dtype=dtype, device=self.device) if when else None
+        have_agg = aggregated is not None or krum_index is not None
+        rel, sums = out(have_agg, (self.B,), torch.float32), out(have_agg, (self.B, 2), torch.float64)
+        honest = out(return_honest_mean, (self.B, self.D), torch.float32)
+        hit = out(krum_index is not None, (self.B,), torch.int32)
+        mal, cnt = (out(selection is not None, (self.B,), torch.int32) for _ in range(2))
+        self._call(nat.lib().afl_attack_metrics_batched_dev, self.G.data_ptr(), self.B, self._bs, self.N, self.D,
+                   self._ld, self._code, self._ptr(self.rows), self.f.data_ptr(), self._ptr(aggregated),
+                   self._ptr(krum_index), self._ptr(selection), 0 if selection is None else selection.shape[1],
+                   *(self._ptr(t) for t in (rel, sums, honest, hit, mal, cnt)), self._ws.data_ptr(), self._ws.numel(),
+                   self.status.data_ptr(), _stream_ptr(self.G))
+        res = {}
+        if have_agg:
+            res["rel_deviation"], res["deviation_sums"] = rel, sums
+        if hit is not None:
+            res["krum_success"] = hit.bool()
+        if mal is not None:
+            res["bulyan_malicious_fraction"] = mal.float() / cnt.clamp(min=1).float()
+        if honest is not None:
+            res["honest_mean"] = honest
+        return res
+
+    def clear_status(self):
+        """Zero `status` (enqueued)."""
+        self.status.zero_()
+
+    def raise_for_status(self):
+        """Synchronise and raise for the first flagged problem, as the host-parameter call raises for it."""
+        st = self.status.cpu().numpy()
+        bad = np.flatnonzero(st)
+        if not bad.size:
+            return
+        b, code = int(bad[0]), int(st[bad[0]])
+        if code == nat.AFL_ERR_NO_WINNER:
+            e = KeyError(-1)
+            e.add_note(f"problem {b}: a Bulyan selection round found no eligible user (defences.py:66)")
+            raise e
+        exc, what = _STATUS_ERRORS.get(code, (nat.NativeError, None))
+        if what is None:
+            raise nat.NativeError(code, f"problem {b}")
+        raise exc(f"problem {b}: {what}")

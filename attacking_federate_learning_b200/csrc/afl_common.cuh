@@ -53,7 +53,7 @@ static inline cudaError_t ensure_dyn_smem(K kernel, int bytes, int (&done)[kMaxD
 
 constexpr int kMaxWorld = 16;            // ranks of one peer-exchange context (csrc/xgpu.cu)
 
-// Trimmed-mean constants (csrc/trimmed_mean.cu, tmean::shape) of `n_rows` participating rows and a corrupted count.
+// Trimmed-mean constants (tmean::shape below, read by csrc/trimmed_mean.cu) of `n_rows` participating rows and a corrupted count.
 struct TmShape {
   int n_rows;             // participating rows
   int keep;               // effective number of kept devs (python slice semantics applied), >= 0
@@ -78,6 +78,65 @@ struct ProblemParams {
   float z;                // ALIE, backdoor: (float)z
   TmShape tm;             // TrimmedMean: n rows and f; Bulyan's second stage: theta rows and 2f
 };
+
+// The row values the host builds for a table (capi.cu) and problem_table_kernel builds on the device: one definition
+// for both, so a device-built row is the host's.
+namespace select {
+__host__ __device__ inline int python_slice_take(int m, int len) {   // len(errors[:m])
+  if (m >= 0) return m < len ? m : len;
+  const int t = len + m;
+  return t > 0 ? t : 0;
+}
+// Krum's score length for n clients: len(sorted(errors)[:users_count - corrupted_count]) over n - 1 distances.
+__host__ __device__ inline int krum_take(int n, int users_count, int corrupted_count) {
+  return python_slice_take(users_count - corrupted_count, n - 1);
+}
+}  // namespace select
+
+namespace tmean {
+__host__ __device__ inline double norm_ppf(double pr) {   // Acklam's rational approximation, |error| < 1.2e-9
+  const double a[] = {-3.969683028665376e+01, 2.209460984245205e+02, -2.759285104469687e+02,
+                      1.383577518672690e+02, -3.066479806614716e+01, 2.506628277459239e+00};
+  const double b[] = {-5.447609879822406e+01, 1.615858368580409e+02, -1.556989798598866e+02,
+                      6.680131188771972e+01, -1.328068155288572e+01};
+  const double c[] = {-7.784894002430293e-03, -3.223964580411365e-01, -2.400758277161838e+00,
+                      -2.549732539343734e+00, 4.374664141464968e+00, 2.938163982698783e+00};
+  const double dd[] = {7.784695709041462e-03, 3.224671290700398e-01, 2.445134137142996e+00,
+                       3.754408661907416e+00};
+  if (pr <= 0.0) return -8.0;
+  if (pr >= 1.0) return 8.0;
+  if (pr < 0.02425) {
+    const double q = sqrt(-2.0 * log(pr));
+    return (((((c[0] * q + c[1]) * q + c[2]) * q + c[3]) * q + c[4]) * q + c[5]) /
+           ((((dd[0] * q + dd[1]) * q + dd[2]) * q + dd[3]) * q + 1.0);
+  }
+  if (pr > 1.0 - 0.02425) {
+    const double q = sqrt(-2.0 * log(1.0 - pr));
+    return -(((((c[0] * q + c[1]) * q + c[2]) * q + c[3]) * q + c[4]) * q + c[5]) /
+           ((((dd[0] * q + dd[1]) * q + dd[2]) * q + dd[3]) * q + 1.0);
+  }
+  const double q = pr - 0.5, r = q * q;
+  return (((((a[0] * r + a[1]) * r + a[2]) * r + a[3]) * r + a[4]) * r + a[5]) * q /
+         (((((b[0] * r + b[1]) * r + b[2]) * r + b[3]) * r + b[4]) * r + 1.0);
+}
+
+// The constants of n_rows participating rows and corrupted_count: number_to_consider = rows - f - 1 with Python slice
+// semantics for sorted(...)[:k] (defences.py:45,50), and the pivot model's Gaussian guesses.  The integer fields are
+// exact on both sides; the three floats come from the host's or the device's exp / log / sqrt, and only steer the
+// kernel's first pivot (csrc/trimmed_mean.cu), never its result.
+__host__ __device__ inline TmShape shape(int n_rows, int corrupted_count) {
+  TmShape t{};
+  const int k = n_rows - corrupted_count - 1;
+  t.n_rows = n_rows;
+  t.keep = k >= 0 ? (k < n_rows ? k : n_rows) : (n_rows + k > 0 ? n_rows + k : 0);
+  t.med_density = 0.3989422804f * static_cast<float>(n_rows);
+  const double frac = t.keep > 0 ? (static_cast<double>(t.keep) - 0.5) / n_rows : 0.5;
+  const double q = norm_ppf(0.5 * (1.0 + (frac < 0.999999 ? frac : 0.999999)));
+  t.key_q = static_cast<float>(q);
+  t.key_density = static_cast<float>(2.0 * 0.3989422804014327 * exp(-0.5 * q * q) * n_rows);
+  return t;
+}
+}  // namespace tmean
 
 // Arguments of the Krum kernel (csrc/select.cu).  The row of distances comes from `dist` (a caller's fp32 table) when
 // it is set, otherwise from the float64 d2 tables tab[0..world), summed in rank order; with world > 1 the kernel first

@@ -113,7 +113,6 @@ int bulyan_select(const float* dist, int n, int users_count, int f, int* sel_out
                   cudaStream_t stream, int batch = 1, const ProblemParams* each = nullptr);
 int bulyan_rounds(const float* dist, int n, int f, int theta, int* sel_out, void* ws, size_t ws_bytes,
                   cudaStream_t stream, int batch, const ProblemParams* each, bool rows);
-int krum_take(int n, int users_count, int corrupted_count);
 }
 namespace tmean {
 int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
@@ -125,7 +124,6 @@ int trimmed_mean_classes(const void* G, int n, int64_t d, int64_t ld, int dtype,
                          int batch, int64_t g_batch, int ri_batch, int64_t out_batch, cudaStream_t stream,
                          const ProblemParams* each, const int* perm, const int* counts);
 int slot_class(int n_rows);
-TmShape shape(int n_rows, int corrupted_count);
 }
 namespace colstats {
 int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream);
@@ -136,6 +134,9 @@ int alie(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float
 int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double z, float* mu_out, float* sigma_out,
                  float* crafted_out, float* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
                  int64_t bcast_batch, cudaStream_t stream, const ProblemParams* each = nullptr);
+int alie_batched_dev(const void* G, int f_bound, int64_t d, int64_t ld, int dtype, float* mu_out, float* sigma_out,
+                     float* crafted_out, void* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
+                     int64_t bcast_batch, cudaStream_t stream, const ProblemParams* each);
 int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* idx_dev, float* out,
                cudaStream_t stream);
 int momentum_step(float* w, float* v, const float* g, int64_t d, float momentum, float lr, cudaStream_t stream);
@@ -1016,6 +1017,202 @@ static int backdoor_finish(int batch, int64_t d, const int* fs, const double* zs
                                    bcast_batch_stride, bcast_ld, stream);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Device-parameter calls (afl_*_dev): the per-problem arrays are device memory, so a call never reads them on the host.
+// problem_table_kernel builds the table the host calls above build, one thread per problem, and runs their per-problem
+// checks in the same order.  A problem that fails a check gets its first code in the caller's sticky status[b] and
+// the safe row of rows_b = n, users_count_b = n, f_b = 0, which keeps every kernel inside its slot; its outputs are
+// then not the reference's, and only status says so.  After the host checks of shapes, pointers and the workspace,
+// a call makes no host copy, synchronisation or allocation, so it can be captured into a CUDA graph.
+// ------------------------------------------------------------------------------------------------
+enum TableRule { T_ALIE = B_BULYAN + 1, T_METRICS };
+
+struct TableArgs {
+  int rule;                   // BatchedRule, T_ALIE or T_METRICS
+  int batch, n;
+  const int* rows;            // NULL: n rows in every problem
+  const int* ucs;             // NULL: users_count without rows, rows with them
+  int users_count;
+  const int* fs;
+  const double* zs;           // ALIE only
+  ProblemParams* table;
+  int* status;
+  const int* sel;             // Bulyan's second stage: rows of sel_ld entries, sel[b][theta_b - 1] < 0 = failed round
+  int sel_ld;
+};
+
+// The first code of the host calls' checks for one problem: afl_defend_batched_rows / _each (rows = n),
+// afl_alie_batched_each, afl_attack_metrics_batched_rows / _each.
+__device__ int problem_code(int rule, int n, bool ragged, int m, int uc, int f) {
+  if (rule == T_ALIE) return f < 0 || f > n ? AFL_ERR_BAD_ARG : AFL_OK;
+  if (f < 0 || (rule != T_METRICS && f > INT32_MAX / 4)) return AFL_ERR_BAD_ARG;
+  if (ragged && (m < 1 || m > n)) return AFL_ERR_BAD_ARG;
+  if (rule == B_KRUM && uc < 2 * static_cast<int64_t>(f) + 1) return AFL_ERR_PRECONDITION;
+  if (rule == B_BULYAN && uc < 4 * static_cast<int64_t>(f) + 3) return AFL_ERR_PRECONDITION;
+  if (rule == B_BULYAN && uc != m) return AFL_ERR_UNSUPPORTED;
+  return AFL_OK;
+}
+
+__global__ void __launch_bounds__(128) problem_table_kernel(const TableArgs a) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= a.batch) return;
+  int f = a.fs[b];
+  int m = a.rows ? a.rows[b] : a.n;
+  int uc = a.ucs ? a.ucs[b] : a.rows ? m : a.users_count;
+  const int code = problem_code(a.rule, a.n, a.rows != nullptr, m, uc, f);
+  if (code != AFL_OK) { m = a.n; uc = a.n; f = 0; }
+  ProblemParams q{};
+  q.f = f;
+  if (a.rule == T_ALIE) {
+    q.z = static_cast<float>(a.zs[b]);
+    q.write = f > 0 && a.zs[b] != 0.0;                  // malicious.py:20-21: z == 0 computes the statistics only
+  } else if (a.rule == T_METRICS) {
+    if (a.rows) q.tm.n_rows = m;
+  } else {
+    q.take = select::krum_take(m, uc, f);
+    q.theta = uc - 2 * f;
+    // Bulyan's second stage: the trimmed mean of the theta_b selected rows with 2 f_b (the whole-slot call's only table)
+    q.tm = a.rule == B_BULYAN && (a.sel || !a.rows) ? tmean::shape(q.theta, 2 * f) : tmean::shape(m, f);
+  }
+  a.table[b] = q;
+  int st = code;
+  if (st == AFL_OK && a.sel && a.sel[static_cast<int64_t>(b) * a.sel_ld + q.theta - 1] < 0) st = AFL_ERR_NO_WINNER;
+  if (st != AFL_OK && a.status[b] == AFL_OK) a.status[b] = st;
+}
+
+static int launch_table(const TableArgs& a, cudaStream_t stream) {
+  problem_table_kernel<<<static_cast<unsigned>((a.batch + 127) / 128), 128, 0, stream>>>(a);
+  AFL_LAUNCH_CHECK("problem_table_kernel");
+  return AFL_OK;
+}
+
+// Host checks shared by the _dev calls: the per-problem arrays and the status are non-NULL, and the workspace holds
+// `need` bytes at a 256-byte boundary.
+static int check_dev(const char* who, const int* fs, const int* status, void* ws, size_t ws_bytes, size_t need) {
+  if (!fs || !status) { set_error("%s: the per-problem corrupted counts or the status array are NULL", who); return AFL_ERR_BAD_ARG; }
+  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
+    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
+    return AFL_ERR_WORKSPACE;
+  }
+  return AFL_OK;
+}
+
+static int table_dev(const char* rule, int batch, int n, const int* rows, int users_count, const int* ucs,
+                     const int* fs, const double* zs, void* ws, size_t ws_bytes, int* status, cudaStream_t stream) {
+  const char* who = "afl_batched_table_dev";
+  const bool alie = rule && !strcmp(rule, "ALIE"), metrics = rule && !strcmp(rule, "AttackMetrics");
+  const BatchedRule r = batched_rule(rule);
+  if (r == B_BAD && !alie && !metrics) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
+  if (batch < 1 || n < 1) { set_error("%s: batch and n must be >= 1 (got %d, %d)", who, batch, n); return AFL_ERR_BAD_ARG; }
+  if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
+  if (alie && !zs) { set_error("%s: the per-problem attack strengths are NULL", who); return AFL_ERR_BAD_ARG; }
+  int rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch));
+  if (rc) return rc;
+  TableArgs a{};
+  a.rule = alie ? static_cast<int>(T_ALIE) : metrics ? static_cast<int>(T_METRICS) : static_cast<int>(r);
+  a.batch = batch; a.n = n; a.rows = alie ? nullptr : rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
+  a.fs = fs; a.zs = zs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
+  return launch_table(a, stream);
+}
+
+// afl_defend_batched_rows (rows != NULL) or afl_defend_batched_each (rows == NULL, n rows and users_count in every
+// problem) with device arrays: the same kernels on a device-built table.  Host scalars of those calls become bounds
+// that hold for every accepted value: Bulyan's selection width is the caller's sel_ld >= n >= theta_b (the host calls
+// use theta_max), and the corrupted counts and users counts that only fill fields a table overrides are passed as 0.
+static int defend_batched_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                              int64_t ld, int dtype, const int* rows, int users_count, const int* ucs, const int* fs,
+                              float* out, int* idx_out, int* sel_out, int sel_ld, void* ws, size_t ws_bytes,
+                              int* status, cudaStream_t stream) {
+  const char* who = "afl_defend_batched_dev";
+  const BatchedRule r = batched_rule(rule);
+  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
+  if (rc) return rc;
+  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out)) {
+    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
+    return AFL_ERR_BAD_ARG;
+  }
+  if (r == B_BULYAN && sel_ld < n) {
+    set_error("%s: Bulyan's selection width sel_ld (%d) must be at least n (%d)", who, sel_ld, n);
+    return AFL_ERR_BAD_ARG;
+  }
+  size_t gram_ws = 0, tabs = 0;
+  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  if ((rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch) + rule_ws))) return rc;
+
+  TableArgs a{};
+  a.rule = r; a.batch = batch; a.n = n; a.rows = rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
+  a.fs = fs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
+  if ((rc = launch_table(a, stream))) return rc;
+  const ProblemParams* each = a.table;
+  const ProblemParams* ragged = rows ? each : nullptr;
+  if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, ragged);
+  if (r == B_TM) return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, 0, out, batch, batch_stride, 0, d, stream, each);
+  uint8_t* p = static_cast<uint8_t*>(ws) + table_bytes(batch);
+  const size_t nn = static_cast<size_t>(batch) * n * n;
+  double* d2 = reinterpret_cast<double*>(p);
+  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
+  void* sel_ws = p + tabs + gram_ws;
+  const size_t sel_ws_bytes = ws_bytes - table_bytes(batch) - tabs - gram_ws;
+  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream, ragged);
+  if (rc) return rc;
+  if (r == B_KRUM) return select::krum_from_sqdist(d2, n, 0, 0, idx_out, sel_ws, sel_ws_bytes, stream, batch, each, rows != nullptr);
+  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
+  rc = select::bulyan_rounds(dist, n, 0, sel_ld, sel_out, sel_ws, sel_ws_bytes, stream, batch, each, rows != nullptr);
+  if (rc) return rc;
+  a.sel = sel_out; a.sel_ld = sel_ld;                    // second stage's table, and a failed round's status
+  if ((rc = launch_table(a, stream))) return rc;
+  return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, n, 0, out, batch, batch_stride, sel_ld, d, stream, each);
+}
+
+// afl_alie_batched_each / _large with device arrays; bcast_rows in G's dtype (a 16-bit matrix is written in the kernel).
+static int alie_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                            const int* fs, const double* zs, float* mu_out, float* sigma_out, float* crafted_out,
+                            void* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* ws, size_t ws_bytes,
+                            int* status, cudaStream_t stream) {
+  const char* who = "afl_alie_batched_dev";
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
+  if (rc) return rc;
+  if (!zs) { set_error("%s: the per-problem attack strengths are NULL", who); return AFL_ERR_BAD_ARG; }
+  if (bcast_rows && (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(n - 1) * bcast_ld + d))) {
+    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  if ((rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch)))) return rc;
+  TableArgs a{};
+  a.rule = T_ALIE; a.batch = batch; a.n = n; a.fs = fs; a.zs = zs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
+  if ((rc = launch_table(a, stream))) return rc;
+  return colstats::alie_batched_dev(G, n, d, ld, dtype, mu_out, sigma_out, crafted_out, bcast_rows, bcast_ld, batch,
+                                    batch_stride, d, bcast_batch_stride, stream, a.table);
+}
+
+// afl_attack_metrics_batched_rows (rows != NULL) or _each with device arrays.
+static int attack_metrics_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                              const int* rows, const int* fs, const float* agg, const int* idx, const int* sel,
+                              int sel_ld, float* dev_out, double* sums_out, float* honest_out, int* krum_hit,
+                              int* mal_count, int* sel_count, void* ws, size_t ws_bytes, int* status,
+                              cudaStream_t stream) {
+  const char* who = "afl_attack_metrics_batched_dev";
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
+  if (rc) return rc;
+  if (agg && idx) { set_error("%s: give the aggregate as agg or as idx, not both", who); return AFL_ERR_BAD_ARG; }
+  if ((dev_out || sums_out) && !agg && !idx) {
+    set_error("%s: dev_out and sums_out need an aggregate (agg or idx)", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  if (krum_hit && !idx) { set_error("%s: krum_hit needs idx", who); return AFL_ERR_BAD_ARG; }
+  if ((mal_count || sel_count) && !sel) { set_error("%s: mal_count and sel_count need sel", who); return AFL_ERR_BAD_ARG; }
+  if (sel && sel_ld < 1) { set_error("%s: sel_ld must be >= 1 (got %d)", who, sel_ld); return AFL_ERR_BAD_ARG; }
+  if ((rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch) + metrics_partial_bytes(batch, d, dtype)))) return rc;
+  TableArgs a{};
+  a.rule = T_METRICS; a.batch = batch; a.n = n; a.rows = rows; a.fs = fs; a.table = static_cast<ProblemParams*>(ws);
+  a.status = status;
+  if ((rc = launch_table(a, stream))) return rc;
+  return colstats::attack_metrics(G, batch, batch_stride, n, d, ld, dtype, 0, a.table, agg, idx, sel, sel_ld, dev_out,
+                                  sums_out, honest_out, krum_hit, mal_count, sel_count,
+                                  static_cast<uint8_t*>(ws) + table_bytes(batch), stream, rows != nullptr);
+}
+
 }  // namespace afl
 
 using namespace afl;
@@ -1284,6 +1481,41 @@ int afl_backdoor_finish_batched(int batch, int64_t d, const int* f, const double
                                 void* workspace, size_t workspace_bytes, void* stream) {
   return backdoor_finish(batch, d, f, z, lr, mu, sigma, initial, mal, mal_batch_stride, crafted_out, bcast_rows,
                          bcast_batch_stride, bcast_ld, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int afl_batched_table_dev(const char* rule, int batch, int n, const int* rows, int users_count, const int* users_counts,
+                          const int* corrupted_counts, const double* z, void* workspace, size_t workspace_bytes,
+                          int* status, void* stream) {
+  return table_dev(rule, batch, n, rows, users_count, users_counts, corrupted_counts, z, workspace, workspace_bytes,
+                   status, static_cast<cudaStream_t>(stream));
+}
+
+int afl_defend_batched_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                           int dtype, const int* rows, int users_count, const int* users_counts,
+                           const int* corrupted_counts, float* out, int* idx_out, int* sel_out, int sel_ld,
+                           void* workspace, size_t workspace_bytes, int* status, void* stream) {
+  return defend_batched_dev(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_count, users_counts,
+                            corrupted_counts, out, idx_out, sel_out, sel_ld, workspace, workspace_bytes, status,
+                            static_cast<cudaStream_t>(stream));
+}
+
+int afl_alie_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                         const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
+                         void* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                         size_t workspace_bytes, int* status, void* stream) {
+  return alie_batched_dev(G, batch, batch_stride, n, d, ld, dtype, f, z, mu_out, sigma_out, crafted_out, bcast_rows,
+                          bcast_batch_stride, bcast_ld, workspace, workspace_bytes, status,
+                          static_cast<cudaStream_t>(stream));
+}
+
+int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                   int dtype, const int* rows, const int* corrupted_counts, const float* agg,
+                                   const int* idx, const int* sel, int sel_ld, float* dev_out, double* sums_out,
+                                   float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* workspace,
+                                   size_t workspace_bytes, int* status, void* stream) {
+  return attack_metrics_dev(G, batch, batch_stride, n, d, ld, dtype, rows, corrupted_counts, agg, idx, sel, sel_ld,
+                            dev_out, sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
+                            status, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

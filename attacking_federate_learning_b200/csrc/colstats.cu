@@ -140,11 +140,20 @@ mean_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, float* __rest
 // variance); crafted = mu - z*sigma with the same two fp32 roundings as `grads_mean[:] -= num_std * grads_stdev[:]`.
 // With a table (each != NULL) problem b uses its own f, z and write flag; f = 0 reads and writes no row and gives NaN
 // statistics (the reference returns before computing any, malicious.py:11-12).
-template <typename T, int VEC, bool COHERENT>
-__global__ void __launch_bounds__(kBlock)
-alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict__ mu_out,
-            float* __restrict__ sigma_out, float* __restrict__ crafted_out, float* bcast, int64_t bcast_ld,
-            int64_t g_batch, int64_t out_batch, int64_t bcast_batch, const ProblemParams* __restrict__ each) {
+// W: the element type of bcast, float (every existing caller) or T (alie_write16_kernel: a 16-bit matrix written in its
+// own dtype, rounded to nearest even as torch's .to(dtype) does on the device).
+template <typename W> __device__ __forceinline__ W from_f32(float x);
+template <> __device__ __forceinline__ float from_f32<float>(float x) { return x; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+template <> __device__ __forceinline__ __half from_f32<__half>(float x) { return __float2half_rn(x); }
+__device__ __forceinline__ uint32_t bits16(__nv_bfloat16 x) { return __bfloat16_as_ushort(x); }
+__device__ __forceinline__ uint32_t bits16(__half x) { return __half_as_ushort(x); }
+
+template <typename T, int VEC, bool COHERENT, typename W>
+__device__ __forceinline__ void alie_body(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict__ mu_out,
+                                          float* __restrict__ sigma_out, float* __restrict__ crafted_out, W* bcast,
+                                          int64_t bcast_ld, int64_t g_batch, int64_t out_batch, int64_t bcast_batch,
+                                          const ProblemParams* __restrict__ each) {
   const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * VEC;
   if (c0 >= d) return;
   if (each) {
@@ -201,19 +210,55 @@ alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict
     bcast += blockIdx.y * bcast_batch;
     // server.py:82-83 copies the one aliased array into every malicious row: f row segments of VEC floats,
     // written as 16-byte stores when the destination allows it (all of this thread's reads are done)
-    const bool v16 = (VEC % 4 == 0) && (c0 + VEC <= d) && (bcast_ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(bcast) & 15) == 0);
+    constexpr int kPer16 = 16 / sizeof(W);               // elements of one 16-byte store
+    const bool v16 = (VEC % kPer16 == 0) && (c0 + VEC <= d) && (bcast_ld % kPer16 == 0) && ((reinterpret_cast<uintptr_t>(bcast) & 15) == 0);
     for (int rr = 0; rr < f; ++rr) {
-      float* dst = bcast + static_cast<int64_t>(rr) * bcast_ld + c0;
-      if (v16) {
+      W* dst = bcast + static_cast<int64_t>(rr) * bcast_ld + c0;
+      if constexpr (sizeof(W) == 4) {
+        if (v16) {
 #pragma unroll
-        for (int k = 0; k + 4 <= VEC; k += 4) *reinterpret_cast<float4*>(dst + k) = make_float4(crafted[k], crafted[k + 1], crafted[k + 2], crafted[k + 3]);
+          for (int k = 0; k + 4 <= VEC; k += 4) *reinterpret_cast<float4*>(dst + k) = make_float4(crafted[k], crafted[k + 1], crafted[k + 2], crafted[k + 3]);
+        } else {
+#pragma unroll
+          for (int k = 0; k < VEC; ++k)
+            if (c0 + k < d) dst[k] = crafted[k];
+        }
       } else {
+        if (v16) {
+          uint32_t w[VEC / 2 > 0 ? VEC / 2 : 1];
 #pragma unroll
-        for (int k = 0; k < VEC; ++k)
-          if (c0 + k < d) dst[k] = crafted[k];
+          for (int k = 0; k + 1 < VEC; k += 2) w[k / 2] = bits16(from_f32<W>(crafted[k])) | (bits16(from_f32<W>(crafted[k + 1])) << 16);
+#pragma unroll
+          for (int k = 0; k + 8 <= VEC; k += 8)
+            *reinterpret_cast<uint4*>(dst + k) = make_uint4(w[k / 2], w[k / 2 + 1], w[k / 2 + 2], w[k / 2 + 3]);
+        } else {
+#pragma unroll
+          for (int k = 0; k < VEC; ++k)
+            if (c0 + k < d) dst[k] = from_f32<W>(crafted[k]);
+        }
       }
     }
   }
+}
+
+template <typename T, int VEC, bool COHERENT>
+__global__ void __launch_bounds__(kBlock)
+alie_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict__ mu_out,
+            float* __restrict__ sigma_out, float* __restrict__ crafted_out, float* bcast, int64_t bcast_ld,
+            int64_t g_batch, int64_t out_batch, int64_t bcast_batch, const ProblemParams* __restrict__ each) {
+  alie_body<T, VEC, COHERENT, float>(G, f, d, ld, z, mu_out, sigma_out, crafted_out, bcast, bcast_ld, g_batch, out_batch,
+                                     bcast_batch, each);
+}
+
+// ALIE of a 16-bit matrix whose crafted vector is written back into that matrix (afl_alie_batched_dev): the same
+// statistics as alie_kernel, and the rows written in T.
+template <typename T, int VEC, bool COHERENT>
+__global__ void __launch_bounds__(kBlock)
+alie_write16_kernel(const T* G, int f, int64_t d, int64_t ld, float z, float* __restrict__ mu_out,
+                    float* __restrict__ sigma_out, float* __restrict__ crafted_out, T* bcast, int64_t bcast_ld,
+                    int64_t g_batch, int64_t out_batch, int64_t bcast_batch, const ProblemParams* __restrict__ each) {
+  alie_body<T, VEC, COHERENT, T>(G, f, d, ld, z, mu_out, sigma_out, crafted_out, bcast, bcast_ld, g_batch, out_batch,
+                                 bcast_batch, each);
 }
 
 template <typename T>
@@ -523,6 +568,37 @@ int alie_batched(const void* G, int f, int64_t d, int64_t ld, int dtype, double 
   }
 #undef AFL_ALIE_LAUNCH
   AFL_LAUNCH_CHECK("alie_kernel");
+  return AFL_OK;
+}
+
+// alie_batched with a table (each required) and bcast in G's dtype (afl_alie_batched_dev).  f_bound >= every f_b (the
+// slot's row count): it only widens the overlap test that picks coherent loads, which changes no value.
+int alie_batched_dev(const void* G, int f_bound, int64_t d, int64_t ld, int dtype, float* mu_out, float* sigma_out,
+                     float* crafted_out, void* bcast, int64_t bcast_ld, int batch, int64_t g_batch, int64_t out_batch,
+                     int64_t bcast_batch, cudaStream_t stream, const ProblemParams* each) {
+  if (dtype == AFL_F32 || !bcast)
+    return alie_batched(G, f_bound, d, ld, dtype, 0.0, mu_out, sigma_out, crafted_out, static_cast<float*>(bcast),
+                        bcast_ld, batch, g_batch, out_batch, bcast_batch, stream, each);
+  if (!G || !each || f_bound < 0 || d < 1 || ld < d || bcast_ld < d) { set_error("afl_alie: bad argument"); return AFL_ERR_BAD_ARG; }
+  if (dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_alie: dtype"); return AFL_ERR_UNSUPPORTED; }
+  const bool v = vec_ok(G, ld, dtype, batch, g_batch);
+  const int vec = v ? 8 : 1;
+  const dim3 grid(static_cast<unsigned>(ceil_div64(ceil_div64(d, vec), kBlock)), batch);
+  ProfScope ps("alie", stream);
+  const int64_t last = static_cast<int64_t>(batch - 1);
+  const uintptr_t g0 = reinterpret_cast<uintptr_t>(G), g1 = g0 + static_cast<uintptr_t>((last * g_batch + static_cast<int64_t>(f_bound - 1) * ld + d) * 2);
+  const uintptr_t b0 = reinterpret_cast<uintptr_t>(bcast), b1 = b0 + static_cast<uintptr_t>((last * bcast_batch + static_cast<int64_t>(f_bound - 1) * bcast_ld + d) * 2);
+  const bool coh = f_bound > 0 && b0 < g1 && g0 < b1;
+#define AFL_ALIE16_LAUNCH(T, V, C) alie_write16_kernel<T, V, C><<<grid, kBlock, 0, stream>>>(static_cast<const T*>(G), f_bound, d, ld, 0.f, mu_out, sigma_out, crafted_out, static_cast<T*>(bcast), bcast_ld, g_batch, out_batch, bcast_batch, each)
+  if (dtype == AFL_BF16) {
+    if (v) { if (coh) AFL_ALIE16_LAUNCH(__nv_bfloat16, 8, true); else AFL_ALIE16_LAUNCH(__nv_bfloat16, 8, false); }
+    else { if (coh) AFL_ALIE16_LAUNCH(__nv_bfloat16, 1, true); else AFL_ALIE16_LAUNCH(__nv_bfloat16, 1, false); }
+  } else {
+    if (v) { if (coh) AFL_ALIE16_LAUNCH(__half, 8, true); else AFL_ALIE16_LAUNCH(__half, 8, false); }
+    else { if (coh) AFL_ALIE16_LAUNCH(__half, 1, true); else AFL_ALIE16_LAUNCH(__half, 1, false); }
+  }
+#undef AFL_ALIE16_LAUNCH
+  AFL_LAUNCH_CHECK("alie_write16_kernel");
   return AFL_OK;
 }
 

@@ -104,12 +104,6 @@ __device__ __forceinline__ unsigned long long dist_key(float d, int v) {
   return (static_cast<unsigned long long>(__float_as_uint(d) & 0x7FFFFFFFu) << 32) | static_cast<unsigned>(v);
 }
 
-static int python_slice_take(int m, int len) {   // len(errors[:m])
-  if (m >= 0) return m < len ? m : len;
-  const int t = len + m;
-  return t > 0 ? t : 0;
-}
-
 enum KrumSource { kSqdist, kDist };
 template <KrumSource kSrc>
 using KrumKey = typename std::conditional<kSrc == kSqdist, uint32_t, unsigned long long>::type;
@@ -190,11 +184,6 @@ krum_tail_kernel(const KrumParams p) {
     p.done[b] = 0u;                                                      // ready for the next step
     __threadfence_system();
   }
-}
-
-// Krum's score length for n clients: len(sorted(errors)[:users_count - corrupted_count]) over n - 1 distances.
-int krum_take(int n, int users_count, int corrupted_count) {
-  return python_slice_take(users_count - corrupted_count, n - 1);
 }
 
 // Fills p.take and launches the kernel for the row source p selects, grid (n, batch).  p.done[0 .. batch) must be zero.

@@ -774,32 +774,6 @@ trimmed_mean_large_kernel(const Params P, int bf16) {
   }
 }
 
-static double norm_ppf(double pr) {   // Acklam's rational approximation, |error| < 1.2e-9
-  static const double a[] = {-3.969683028665376e+01, 2.209460984245205e+02, -2.759285104469687e+02,
-                             1.383577518672690e+02, -3.066479806614716e+01, 2.506628277459239e+00};
-  static const double b[] = {-5.447609879822406e+01, 1.615858368580409e+02, -1.556989798598866e+02,
-                             6.680131188771972e+01, -1.328068155288572e+01};
-  static const double c[] = {-7.784894002430293e-03, -3.223964580411365e-01, -2.400758277161838e+00,
-                             -2.549732539343734e+00, 4.374664141464968e+00, 2.938163982698783e+00};
-  static const double dd[] = {7.784695709041462e-03, 3.224671290700398e-01, 2.445134137142996e+00,
-                              3.754408661907416e+00};
-  if (pr <= 0.0) return -8.0;
-  if (pr >= 1.0) return 8.0;
-  if (pr < 0.02425) {
-    const double q = sqrt(-2.0 * log(pr));
-    return (((((c[0] * q + c[1]) * q + c[2]) * q + c[3]) * q + c[4]) * q + c[5]) /
-           ((((dd[0] * q + dd[1]) * q + dd[2]) * q + dd[3]) * q + 1.0);
-  }
-  if (pr > 1.0 - 0.02425) {
-    const double q = sqrt(-2.0 * log(1.0 - pr));
-    return -(((((c[0] * q + c[1]) * q + c[2]) * q + c[3]) * q + c[4]) * q + c[5]) /
-           ((((dd[0] * q + dd[1]) * q + dd[2]) * q + dd[3]) * q + 1.0);
-  }
-  const double q = pr - 0.5, r = q * q;
-  return (((((a[0] * r + a[1]) * r + a[2]) * r + a[3]) * r + a[4]) * r + a[5]) * q /
-         (((((b[0] * r + b[1]) * r + b[2]) * r + b[3]) * r + b[4]) * r + 1.0);
-}
-
 // perm != NULL: a class launch over `batch` problems perm[0 .. batch) (trimmed_mean_classes)
 template <int S>
 static int launch(const Params& P, int dtype, int batch, cudaStream_t stream, const int* perm = nullptr) {
@@ -830,21 +804,6 @@ static int launch(const Params& P, int dtype, int batch, cudaStream_t stream, co
   return dtype == AFL_BF16  ? go(trimmed_mean_kernel<S, AFL_BF16, false>, P)
          : dtype == AFL_F16 ? go(trimmed_mean_kernel<S, AFL_F16, false>, P)
                             : go(trimmed_mean_kernel<S, AFL_F32, false>, P);
-}
-
-// The constants of n_rows participating rows and corrupted_count: number_to_consider = rows - f - 1 with Python slice
-// semantics for sorted(...)[:k] (defences.py:45,50), and the pivot model's Gaussian guesses.
-TmShape shape(int n_rows, int corrupted_count) {
-  TmShape t{};
-  const int k = n_rows - corrupted_count - 1;
-  t.n_rows = n_rows;
-  t.keep = k >= 0 ? (k < n_rows ? k : n_rows) : (n_rows + k > 0 ? n_rows + k : 0);
-  t.med_density = 0.3989422804f * static_cast<float>(n_rows);
-  const double frac = t.keep > 0 ? (static_cast<double>(t.keep) - 0.5) / n_rows : 0.5;
-  const double q = norm_ppf(0.5 * (1.0 + (frac < 0.999999 ? frac : 0.999999)));
-  t.key_q = static_cast<float>(q);
-  t.key_density = static_cast<float>(2.0 * 0.3989422804014327 * exp(-0.5 * q * q) * n_rows);
-  return t;
 }
 
 // `batch` problems (grid y): problem b reads G + b * g_batch and row_index + b * ri_batch, and writes out + b * out_batch.

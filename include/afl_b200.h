@@ -443,6 +443,60 @@ int afl_backdoor_finish_batched(int batch, int64_t d, const int* f, const double
                                 float* crafted_out, float* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld,
                                 void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- device-parameter batched calls: per-problem arrays in device memory, capturable into a CUDA graph ---------
+ * The per-problem calls above take their arrays on the host and build the parameter table there.  These take
+ * rows, users_counts and corrupted_counts as DEVICE int32 arrays of `batch` values and z as a DEVICE float64 array,
+ * build the table on the device (the host calls' row, field for field) and run the same kernels on it, so a result
+ * is the host-parameter call's on the same values, bit for bit.  After the host checks below no call copies,
+ * synchronises or allocates: every call only enqueues work and can be captured into a CUDA graph, whose replays read
+ * whatever the arrays hold at that time.
+ *
+ * Per-problem checks run on the device, in the host calls' order: corrupted_counts[b] < 0 (or above the host
+ * call's cap) or rows[b] outside [1, n] -> AFL_ERR_BAD_ARG; the reference's asserts (users_count >= 2f + 1 for Krum,
+ * >= 4f + 3 for Bulyan) -> AFL_ERR_PRECONDITION; Bulyan's users_counts[b] != rows[b] -> AFL_ERR_UNSUPPORTED; and, after
+ * Bulyan's selection, a failed round (sel_out[b][theta_b - 1] < 0) -> AFL_ERR_NO_WINNER.  The first code of problem b
+ * is written to status[b] (DEVICE int32[batch], the caller's, left alone once nonzero: clear it to start again).  A
+ * flagged problem runs with rows_b = n, users_count_b = n and f_b = 0 instead, which keeps every kernel inside its
+ * slot; its outputs are then not the reference's, and only status says so.  The other problems are unaffected.
+ *
+ * Arguments follow the host calls: rows == NULL means n rows in every problem; users_counts == NULL means the scalar
+ * users_count without rows, or rows with them.  Checked on the host before any CUDA call: NULL pointers, batch, the
+ * stride rule, dtype and the workspace exactly as the host-parameter calls (status and corrupted_counts NULL ->
+ * AFL_ERR_BAD_ARG).
+ *
+ * afl_batched_table_dev — writes only the table (ProblemParams[batch], 40 bytes a row, at the workspace start) and
+ * status for rule "Krum", "Bulyan", "TrimmedMean", "NoDefense", "ALIE" (z required, rows ignored) or "AttackMetrics".
+ * Workspace: afl_batched_each_workspace_bytes("ALIE", batch, 1, 1, 0) bytes or more.
+ *
+ * afl_defend_batched_dev — afl_defend_batched_rows (rows != NULL) or afl_defend_batched_each (rows == NULL) with
+ * device arrays, n <= 128 (larger n -> AFL_ERR_UNSUPPORTED: the per-class trimmed-mean launches of larger slots need
+ * the classes on the host).  Bulyan's sel_out is [batch][sel_ld] with sel_ld >= n (else AFL_ERR_BAD_ARG): theta_b
+ * entries, then -2.  Workspace and layout: afl_batched_rows_workspace_bytes(rule, ...).
+ *
+ * afl_alie_batched_dev — afl_alie_batched_each / _large with device arrays, any n, f_b <= n.  bcast_rows (may be NULL)
+ * has G's dtype: a bf16 or fp16 matrix is written in the kernel, rounded to nearest even (what torch's .to(dtype)
+ * gives).  bcast_batch_stride >= (n - 1) * bcast_ld + d when batch > 1.  Workspace:
+ * afl_batched_each_workspace_bytes("ALIE", batch, 1, d, dtype).
+ *
+ * afl_attack_metrics_batched_dev — afl_attack_metrics_batched_rows (rows != NULL) or _each with device arrays, any n.
+ * Workspace: afl_metrics_workspace_bytes. */
+int afl_batched_table_dev(const char* rule, int batch, int n, const int* rows, int users_count, const int* users_counts,
+                          const int* corrupted_counts, const double* z, void* workspace, size_t workspace_bytes,
+                          int* status, void* stream);
+int afl_defend_batched_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                           int dtype, const int* rows, int users_count, const int* users_counts,
+                           const int* corrupted_counts, float* out, int* idx_out, int* sel_out, int sel_ld,
+                           void* workspace, size_t workspace_bytes, int* status, void* stream);
+int afl_alie_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                         const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
+                         void* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                         size_t workspace_bytes, int* status, void* stream);
+int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                   int dtype, const int* rows, const int* corrupted_counts, const float* agg,
+                                   const int* idx, const int* sel, int sel_ld, float* dev_out, double* sums_out,
+                                   float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* workspace,
+                                   size_t workspace_bytes, int* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

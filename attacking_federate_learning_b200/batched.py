@@ -412,6 +412,20 @@ _STATUS_ERRORS = {nat.AFL_ERR_BAD_ARG: (ValueError, "a corrupted count or row co
                   nat.AFL_ERR_UNSUPPORTED: (NotImplementedError, "Bulyan's users_count must equal its number of rows")}
 
 
+def krum_gather_rows(idx, rows, N):
+    """The row DeviceRound.krum gathers per problem (int64, same device as idx): idx_b for an index >= 0, and for
+    -1 (no eligible user) the last row the problem ran with, rows_b - 1 when rows_b lies in [1, N] and N - 1 otherwise
+    (the safe row of a problem flagged for its row count).  rows: int32 [B] or None (N rows in every problem).  For
+    kernel indices in [-1, N) the result is in [0, N) whatever int32 rows holds."""
+    idx = idx.long()
+    if rows is None:
+        last = N - 1
+    else:
+        rows = rows.long()
+        last = torch.where((rows >= 1) & (rows <= N), rows - 1, N - 1)
+    return torch.where(idx < 0, last, idx)
+
+
 class DeviceRound:
     """One lock-step round of a batch whose per-problem parameters live on the device (C ABI `afl_*_dev`).
 
@@ -504,14 +518,13 @@ class DeviceRound:
 
     def krum(self, return_index=False):
         """`krum`: the device int32 [B] indices, or the winning rows [B, D] in G's dtype.  Index -1 (no eligible user)
-        selects row rows_b - 1 (N - 1 without rows), the reference's users_grads[-1]."""
+        selects the last row the problem ran with, the reference's users_grads[-1]: row rows_b - 1 (N - 1 without
+        rows), and N - 1 for a problem whose rows_b lies outside [1, N], which ran on the safe row (see
+        `krum_gather_rows`)."""
         self._defend(DefenseTypes.Krum, idx=self.krum_index)
         if return_index:
             return self.krum_index
-        idx = self.krum_index.long()
-        last = self.N - 1 if self.rows is None else self.rows.long() - 1
-        row = torch.where(idx < 0, last, idx)
-        self.krum_rows.copy_(self.G[self._problems, row])
+        self.krum_rows.copy_(self.G[self._problems, krum_gather_rows(self.krum_index, self.rows, self.N)])
         return self.krum_rows
 
     def bulyan(self, return_selection=False):

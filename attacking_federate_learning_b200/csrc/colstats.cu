@@ -139,7 +139,8 @@ mean_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, float* __rest
 // round-1 version shifted by the first row in fp32 and lost ~1e-5 relative there).  sigma = sqrt(population
 // variance); crafted = mu - z*sigma with the same two fp32 roundings as `grads_mean[:] -= num_std * grads_stdev[:]`.
 // With a table (each != NULL) problem b uses its own f, z and write flag; f = 0 reads and writes no row and gives NaN
-// statistics (the reference returns before computing any, malicious.py:11-12).
+// statistics (the reference returns before computing any, malicious.py:11-12).  A column holding an inf has mu = +-inf
+// (NaN with both signs) and, as np.var's inf - inf, sigma = NaN, so its crafted value is NaN.
 // W: the element type of bcast, float (every existing caller) or T (alie_write16_kernel: a 16-bit matrix written in its
 // own dtype, rounded to nearest even as torch's .to(dtype) does on the device).
 template <typename W> __device__ __forceinline__ W from_f32(float x);
@@ -196,7 +197,7 @@ __device__ __forceinline__ void alie_body(const T* G, int f, int64_t d, int64_t 
   for (int k = 0; k < VEC; ++k) {
     const double m = s1[k] * inv;
     double var = fma(-m, m, s2[k] * inv);
-    var = var > 0.0 ? var : (f > 0 ? 0.0 : m);      // f = 0: m is NaN
+    var = var < 0.0 ? 0.0 : var;                    // NaN stays NaN: f = 0, or an inf or NaN in the column (np.var)
     const float mu = static_cast<float>(m);
     const float sigma = static_cast<float>(sqrt(var));
     crafted[k] = __fsub_rn(mu, __fmul_rn(z, sigma));

@@ -36,8 +36,10 @@ Bulyan's selection.  It has no client limit.
 `DeviceRound` runs the same calls with `f`, `z`, `rows` and `users_count` held as device tensors that the caller
 refills in place (C ABI `afl_*_dev`): its methods never synchronise, so after one eager warm-up a whole round can be
 captured with `torch.cuda.graph` and replayed.  Per-problem checks run on the device and land in `DeviceRound.status`;
-`raise_for_status` raises what the host-parameter call would.  The functions above do not change and keep refusing
-CUDA tensors for their per-problem values.
+`raise_for_status` raises what the host-parameter call would.  Its defences take N <= 128, or N <= 1024 with
+`large=True` (C ABI `afl_defend_batched_large_dev`, which groups the problems by trimmed-mean slot class on the
+device), so the N = 500 and N = 1000 sweeps run as captured rounds too.  The functions above do not change and keep
+refusing CUDA tensors for their per-problem values.
 
 The server's momentum step needs no batched form: `_device.momentum_step` on contiguous `[B, D]` weights,
 velocity and gradients is already the batched step (server.py:89-90 is element-wise).
@@ -445,10 +447,13 @@ class DeviceRound:
     ValueError, AssertionError, NotImplementedError, or KeyError(-1) for a Bulyan round with no eligible user.
 
     users_count: one int for every problem without rows (default N).  rules: the defences this round runs (their
-    workspace is sized here); any of them needs N <= 128."""
+    workspace is sized here); any of them needs N <= 128, or N <= 1024 with large=True.  large=True runs the defences
+    through `afl_defend_batched_large_dev` (at N <= 128 the same call as without it); each result is then the
+    host-parameter call's (`afl_defend_batched_large` above 128 clients) bit for bit."""
 
     def __init__(self, users_grads, users_count=None, *, rows=False, per_problem_users_count=False,
-                 rules=(DefenseTypes.Krum, DefenseTypes.Bulyan, DefenseTypes.TrimmedMean, DefenseTypes.NoDefense)):
+                 rules=(DefenseTypes.Krum, DefenseTypes.Bulyan, DefenseTypes.TrimmedMean, DefenseTypes.NoDefense),
+                 large=False):
         if not isinstance(users_grads, torch.Tensor):
             raise TypeError("users_grads: expected a torch.cuda tensor")
         if users_grads.dim() != 3 or users_grads.stride(2) != 1:
@@ -458,8 +463,10 @@ class DeviceRound:
         for r in rules:
             if r not in defend:
                 raise ValueError(f"DeviceRound: unknown rule {r!r}")
-        if rules and N > ONE_TILE:
-            raise NotImplementedError(f"DeviceRound defences support N <= {ONE_TILE} clients per problem (got {N})")
+        limit = MAX_CLIENTS if large else ONE_TILE
+        if rules and N > limit:
+            hint = "" if large else f"; large=True takes up to {MAX_CLIENTS}"
+            raise NotImplementedError(f"DeviceRound defences support N <= {limit} clients per problem (got {N}){hint}")
         if per_problem_users_count and not rows:
             raise ValueError("DeviceRound: per-problem users counts need rows=True")
         if rows and users_count is not None:
@@ -470,7 +477,7 @@ class DeviceRound:
         if not users_grads.is_cuda:
             raise TypeError("users_grads: expected a torch.cuda tensor")
         _, _, _, self._ld, self._bs = _check(users_grads)
-        self.G, self.B, self.N, self.D, self._code, self.rules = users_grads, B, N, D, code, rules
+        self.G, self.B, self.N, self.D, self._code, self.rules, self.large = users_grads, B, N, D, code, rules, large
         self.users_count_scalar = N if users_count is None else int(users_count)
         dev = self.device = users_grads.device
         self.f = torch.zeros(B, dtype=torch.int32, device=dev)
@@ -479,7 +486,8 @@ class DeviceRound:
         self.users_count = torch.full((B,), N, dtype=torch.int32, device=dev) if per_problem_users_count else None
         self.status = torch.zeros(B, dtype=torch.int32, device=dev)
         L = nat.lib()
-        nbytes = max([L.afl_batched_rows_workspace_bytes(r.encode(), B, N, D, code) for r in rules] +
+        rule_bytes = L.afl_batched_large_dev_workspace_bytes if large else L.afl_batched_rows_workspace_bytes
+        nbytes = max([rule_bytes(r.encode(), B, N, D, code) for r in rules] +
                      [L.afl_batched_each_workspace_bytes(b"ALIE", B, 1, D, code),
                       L.afl_metrics_workspace_bytes(B, N, D, code)])
         self._ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)     # one round's calls run in stream order
@@ -502,7 +510,9 @@ class DeviceRound:
     def _defend(self, rule, out=None, idx=None, sel=None):
         if rule not in self.rules:
             raise ValueError(f"DeviceRound: {rule} was not among the rules given at construction")
-        self._call(nat.lib().afl_defend_batched_dev, rule.encode(), self.G.data_ptr(), self.B, self._bs, self.N, self.D,
+        L = nat.lib()
+        call = L.afl_defend_batched_large_dev if self.large else L.afl_defend_batched_dev
+        self._call(call, rule.encode(), self.G.data_ptr(), self.B, self._bs, self.N, self.D,
                    self._ld, self._code, self._ptr(self.rows), self.users_count_scalar, self._ptr(self.users_count),
                    self.f.data_ptr(), self._ptr(out), self._ptr(idx), self._ptr(sel), self.N, self._ws.data_ptr(),
                    self._ws.numel(), self.status.data_ptr(), _stream_ptr(self.G))

@@ -123,7 +123,9 @@ int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype,
 int trimmed_mean_classes(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, float* out,
                          int batch, int64_t g_batch, int ri_batch, int64_t out_batch, cudaStream_t stream,
                          const ProblemParams* each, const int* perm, const int* counts);
-int slot_class(int n_rows);
+int trimmed_mean_classes_dev(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, float* out,
+                             int batch, int64_t g_batch, int ri_batch, int64_t out_batch, cudaStream_t stream,
+                             const ProblemParams* each, const int* perm, const int* start);
 }
 namespace colstats {
 int mean(const void* G, int n, int64_t d, int64_t ld, int dtype, float* out, cudaStream_t stream);
@@ -1086,6 +1088,78 @@ static int launch_table(const TableArgs& a, cudaStream_t stream) {
   return AFL_OK;
 }
 
+// The problems of a table grouped by the trimmed-mean slot class of their tm.n_rows, on the device: perm[batch] lists
+// them class by class and in problem order within a class (upload_class_table's order), and start[kSlotClasses + 1]
+// holds the offset of each class in perm.  One CTA walks the problems in chunks of its size: a first pass counts the
+// classes (__syncthreads_count), a second places each problem at its class's running offset plus its rank in the
+// chunk (warp ballots, then the counts of the warps before it).  No atomics and no waits between CTAs, so the order is
+// stable and deterministic.  A flagged problem carries the safe row and falls into the class of its row count.
+constexpr int kPermThreads = 1024;
+constexpr size_t kClassStartBytes = 256;         // start[kSlotClasses + 1] at the end of a large _dev workspace
+
+__device__ __forceinline__ int class_of(const ProblemParams* table, int b) {
+  const int c = tmean::slot_class(table[b].tm.n_rows);
+  return c < 0 ? 0 : c >= kSlotClasses ? kSlotClasses - 1 : c;
+}
+
+__global__ void __launch_bounds__(kPermThreads) class_perm_kernel(const ProblemParams* table, int batch, int* perm,
+                                                                  int* start) {
+  __shared__ int base[kSlotClasses];
+  __shared__ int wcount[kPermThreads / 32][kSlotClasses];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int count = 0;                                        // thread c < kSlotClasses: the size of class c
+  for (int b0 = 0; b0 < batch; b0 += kPermThreads) {
+    const int c = b0 + tid < batch ? class_of(table, b0 + tid) : -1;
+#pragma unroll
+    for (int k = 0; k < kSlotClasses; ++k) {
+      const int n = __syncthreads_count(c == k);
+      if (tid == k) count += n;
+    }
+  }
+  if (tid < kSlotClasses) base[tid] = count;
+  __syncthreads();
+  if (tid == 0) {
+    int s = 0;
+    for (int k = 0; k < kSlotClasses; ++k) {
+      const int n = base[k];
+      base[k] = s; start[k] = s;
+      s += n;
+    }
+    start[kSlotClasses] = s;
+  }
+  __syncthreads();
+  for (int b0 = 0; b0 < batch; b0 += kPermThreads) {
+    const int b = b0 + tid;
+    const int c = b < batch ? class_of(table, b) : -1;
+    int rank = 0;
+#pragma unroll
+    for (int k = 0; k < kSlotClasses; ++k) {
+      const unsigned m = __ballot_sync(0xffffffffu, c == k);
+      if (lane == 0) wcount[warp][k] = __popc(m);
+      if (c == k) rank = __popc(m & ((1u << lane) - 1u));
+    }
+    __syncthreads();
+    if (c >= 0) {
+      int pos = base[c] + rank;
+      for (int w = 0; w < warp; ++w) pos += wcount[w][c];
+      perm[pos] = b;
+    }
+    __syncthreads();                                    // base and wcount read before they change
+    if (tid < kSlotClasses) {
+      int t = 0;
+      for (int w = 0; w < kPermThreads / 32; ++w) t += wcount[w][tid];
+      base[tid] += t;
+    }
+    __syncthreads();
+  }
+}
+
+static int launch_class_perm(const ProblemParams* table, int batch, int* perm, int* start, cudaStream_t stream) {
+  class_perm_kernel<<<1, kPermThreads, 0, stream>>>(table, batch, perm, start);
+  AFL_LAUNCH_CHECK("class_perm_kernel");
+  return AFL_OK;
+}
+
 // Host checks shared by the _dev calls: the per-problem arrays and the status are non-NULL, and the workspace holds
 // `need` bytes at a 256-byte boundary.
 static int check_dev(const char* who, const int* fs, const int* status, void* ws, size_t ws_bytes, size_t need) {
@@ -1163,6 +1237,70 @@ static int defend_batched_dev(const char* rule, const void* G, int batch, int64_
   a.sel = sel_out; a.sel_ld = sel_ld;                    // second stage's table, and a failed round's status
   if ((rc = launch_table(a, stream))) return rc;
   return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, n, 0, out, batch, batch_stride, sel_ld, d, stream, each);
+}
+
+// afl_defend_batched_large with device arrays (afl_defend_batched_large_dev): n <= 128 is afl_defend_batched_dev.  Above,
+// the workspace is the large call's (ProblemParams[batch], perm[batch], then the rule's scratch) followed by one
+// kClassStartBytes block for start[].  After each table launch class_perm_kernel groups the problems on the device, and
+// the trimmed mean runs one device-count launch per class (tmean::trimmed_mean_classes_dev).  Every kernel reads the
+// table as afl_defend_batched_large does, except the Gram without rows: with n rows in every problem its multi-tile
+// centre is the same without the table, and the table of a whole-slot Bulyan holds the second stage's tm already.
+static int defend_batched_large_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                                    int64_t ld, int dtype, const int* rows, int users_count, const int* ucs,
+                                    const int* fs, float* out, int* idx_out, int* sel_out, int sel_ld, void* ws,
+                                    size_t ws_bytes, int* status, cudaStream_t stream) {
+  const char* who = "afl_defend_batched_large_dev";
+  const BatchedRule r = batched_rule(rule);
+  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, kBatchLargeMaxClients);
+  if (rc) return rc;
+  if (n <= kBatchMaxClients)
+    return defend_batched_dev(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_count, ucs, fs, out, idx_out,
+                              sel_out, sel_ld, ws, ws_bytes, status, stream);
+  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out)) {
+    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
+    return AFL_ERR_BAD_ARG;
+  }
+  if (r == B_BULYAN && sel_ld < n) {
+    set_error("%s: Bulyan's selection width sel_ld (%d) must be at least n (%d)", who, sel_ld, n);
+    return AFL_ERR_BAD_ARG;
+  }
+  size_t gram_ws = 0, tabs = 0;
+  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  const size_t tab_bytes = class_table_bytes(batch, n);
+  if ((rc = check_dev(who, fs, status, ws, ws_bytes, tab_bytes + rule_ws + kClassStartBytes))) return rc;
+
+  TableArgs a{};
+  a.rule = r; a.batch = batch; a.n = n; a.rows = rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
+  a.fs = fs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
+  const ProblemParams* each = a.table;
+  uint8_t* p = static_cast<uint8_t*>(ws) + tab_bytes;
+  int* perm = reinterpret_cast<int*>(static_cast<uint8_t*>(ws) + static_cast<size_t>(batch) * sizeof(ProblemParams));
+  int* start = reinterpret_cast<int*>(p + rule_ws);
+  if ((rc = launch_table(a, stream))) return rc;
+  if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, each);
+  if (r == B_TM) {
+    if ((rc = launch_class_perm(each, batch, perm, start, stream))) return rc;
+    return tmean::trimmed_mean_classes_dev(G, n, d, ld, dtype, nullptr, out, batch, batch_stride, 0, d, stream, each,
+                                           perm, start);
+  }
+  const size_t nn = static_cast<size_t>(batch) * n * n;
+  double* d2 = reinterpret_cast<double*>(p);
+  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
+  void* sel_ws = p + tabs + gram_ws;
+  const size_t sel_ws_bytes = rule_ws - tabs - gram_ws;
+  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream,
+                            rows ? each : nullptr);
+  if (rc) return rc;
+  if (r == B_KRUM) return select::krum_from_sqdist(d2, n, 0, 0, idx_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
+  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
+  rc = select::bulyan_rounds(dist, n, 0, sel_ld, sel_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
+  if (rc) return rc;
+  a.sel = sel_out; a.sel_ld = sel_ld;                    // second stage's table (theta_b classes), and a failed round's status
+  if ((rc = launch_table(a, stream))) return rc;
+  if ((rc = launch_class_perm(each, batch, perm, start, stream))) return rc;
+  return tmean::trimmed_mean_classes_dev(G, n, d, ld, dtype, sel_out, out, batch, batch_stride, sel_ld, d, stream, each,
+                                         perm, start);
 }
 
 // afl_alie_batched_each / _large with device arrays; bcast_rows in G's dtype (a 16-bit matrix is written in the kernel).
@@ -1497,6 +1635,21 @@ int afl_defend_batched_dev(const char* rule, const void* G, int batch, int64_t b
   return defend_batched_dev(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_count, users_counts,
                             corrupted_counts, out, idx_out, sel_out, sel_ld, workspace, workspace_bytes, status,
                             static_cast<cudaStream_t>(stream));
+}
+
+size_t afl_batched_large_dev_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
+  const size_t large = afl_batched_large_workspace_bytes(rule, batch, n, d, dtype);
+  if (!large || n <= kBatchMaxClients) return large;
+  return large + kClassStartBytes;
+}
+
+int afl_defend_batched_large_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                                 int64_t ld, int dtype, const int* rows, int users_count, const int* users_counts,
+                                 const int* corrupted_counts, float* out, int* idx_out, int* sel_out, int sel_ld,
+                                 void* workspace, size_t workspace_bytes, int* status, void* stream) {
+  return defend_batched_large_dev(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_count, users_counts,
+                                  corrupted_counts, out, idx_out, sel_out, sel_ld, workspace, workspace_bytes, status,
+                                  static_cast<cudaStream_t>(stream));
 }
 
 int afl_alie_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,

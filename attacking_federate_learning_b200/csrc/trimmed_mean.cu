@@ -34,7 +34,9 @@
 //     constants (tm); rows past a problem's n_rows are staged as +inf like the rows past n_rows of a single call.  With
 //     n <= 128 rows every problem runs trimmed_mean_kernel<4, DT, EACH> over grid y = problem.  Larger batches
 //     (trimmed_mean_classes) run every problem in the instance that its own n_rows selects, as its single call does: one
-//     launch per slot class present, grid y = the class's problems, problem P.perm[blockIdx.y] (CLASS).
+//     launch per slot class present, grid y = the class's problems, problem P.perm[blockIdx.y] (CLASS).  The device-
+//     parameter calls (trimmed_mean_classes_dev) read the class sizes from device memory instead: one persistent-grid
+//     launch per class, every class, whose CTAs stride over the class's (problem, column tile) items (DEV).
 #include <type_traits>
 
 #include "afl_common.cuh"
@@ -441,24 +443,16 @@ __device__ __forceinline__ unsigned problem_of(const Params& P) {
   else return blockIdx.y;
 }
 
-template <int S, int DT, bool CLASS>
-__device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, uint32_t* tile, int64_t col0) {
+// The tile of one problem: its matrix at `base`, its row_index (may be NULL) and its participating rows sh.n_rows.
+template <int S, int DT>
+__device__ __forceinline__ void stage_rows(const Params& P, const TmShape& sh, uint32_t* tile, int64_t col0,
+                                           const uint8_t* base, const int* row_index) {
   constexpr int kGroups = S / 4;
   constexpr bool W16 = DT != AFL_F32;                   // two 16-bit columns per word
   const int tid = threadIdx.x;
   const int es = W16 ? 2 : 4;
   const int cols_per_tile = W16 ? 32 : 16;
   const uint32_t sentinel = DT == AFL_F16 ? 0x7C007C00u : DT == AFL_BF16 ? 0x7F807F80u : 0x7F800000u;   // +inf
-  const uint8_t* base;
-  const int* row_index;
-  if constexpr (CLASS) {
-    const int64_t b = problem_of<CLASS>(P);
-    base = static_cast<const uint8_t*>(P.G) + b * P.g_batch * es;
-    row_index = P.row_index ? P.row_index + b * P.ri_batch : nullptr;
-  } else {
-    base = static_cast<const uint8_t*>(P.G) + static_cast<int64_t>(blockIdx.y) * P.g_batch * es;
-    row_index = P.row_index ? P.row_index + static_cast<int64_t>(blockIdx.y) * P.ri_batch : nullptr;
-  }
   constexpr int kIters = (32 * S * 4) / kThreads;      // S/2
   const bool full_tile = P.vec_ok && (col0 + cols_per_tile <= P.d);
   const int rowq = tid >> 2, j = tid & 3, l = rowq & 31, hi2 = tid >> 7;
@@ -527,6 +521,22 @@ __device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, u
     b[(2 * kGroups) * 128] = w[2];
     b[(3 * kGroups) * 128] = w[3];
   }
+}
+
+template <int S, int DT, bool CLASS>
+__device__ __forceinline__ void stage_tile(const Params& P, const TmShape& sh, uint32_t* tile, int64_t col0) {
+  const int es = DT != AFL_F32 ? 2 : 4;
+  const uint8_t* base;
+  const int* row_index;
+  if constexpr (CLASS) {
+    const int64_t b = problem_of<CLASS>(P);
+    base = static_cast<const uint8_t*>(P.G) + b * P.g_batch * es;
+    row_index = P.row_index ? P.row_index + b * P.ri_batch : nullptr;
+  } else {
+    base = static_cast<const uint8_t*>(P.G) + static_cast<int64_t>(blockIdx.y) * P.g_batch * es;
+    row_index = P.row_index ? P.row_index + static_cast<int64_t>(blockIdx.y) * P.ri_batch : nullptr;
+  }
+  stage_rows<S, DT>(P, sh, tile, col0, base, row_index);
 }
 
 // ---------------- general per-column path (any data): one warp, one column ----------------
@@ -669,6 +679,89 @@ trimmed_mean_kernel(const KernelParams<CLASS> P) {
   }
 }
 
+// A device-count class launch's arguments (trimmed_mean_dev_kernel): Params, and the class's problems perm[start[cls] ..
+// start[cls + 1]), device values that class_perm_kernel (capi.cu) wrote.
+struct DevClassParams : Params {
+  const int* perm;
+  const int* start;       // kSlotClasses + 1 offsets into perm
+  int cls, batch;
+  int tiles;              // column tiles per problem, < 2^31
+  int step_p, step_t;     // gridDim.x as (problems, tiles): gridDim.x = step_p * tiles + step_t
+};
+
+// Device-count class launch: a persistent grid whose size the host knows without the class's size strides over the
+// class's work items i in [0, count * tiles), item i being problem perm[start[cls] + i / tiles] and column tile
+// i % tiles.  So the launch needs no class size on the host, and an absent class costs one wave of CTAs that read a
+// zero count.  Per column it runs the CLASS instance's stage_rows and general_column_impl with the same S, so a
+// column's result does not depend on which CTA computed it: the outputs are the host-count launch's bit for bit.
+// Launch bounds: the CLASS instances' for fp32.  The 16-bit instances spill at those (the per-item loop keeps a few
+// more values live than a CLASS CTA's single problem), so they ask for fewer CTAs per SM from S = 8 on: 80 registers
+// at S = 8, 128 at S = 12 to 24, and one CTA per SM at S = 28 and 32.
+template <int DT, int S>
+constexpr int dev_min_ctas() {
+  if (DT == AFL_F32) return S <= 12 ? 4 : S <= 16 ? 3 : 2;
+  return S <= 4 ? 4 : S <= 8 ? 3 : S <= 24 ? 2 : 1;
+}
+template <int S, int DT>
+__global__ void __launch_bounds__(kThreads, dev_min_ctas<DT, S>())
+trimmed_mean_dev_kernel(const DevClassParams P) {
+  extern __shared__ __align__(1024) uint32_t tile[];     // trimmed_mean_kernel's layout
+  constexpr int kGroups = S / 4;
+  constexpr bool W16 = DT != AFL_F32;
+  const int es = W16 ? 2 : 4;
+  const int cols_per_tile = W16 ? 32 : 16;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  // The item (p, t) = (i / tiles, i % tiles) and the class's span live in shared memory: the column code needs every
+  // register it had in the CLASS instance, and loop state held in registers across it made the 16-bit instances
+  // spill.  Thread 0 writes the next item into the other slot of `item`; the barrier at the end of an item orders
+  // that write before every read of it, and after every read of the slot's previous contents.
+  __shared__ int item[2][2];
+  __shared__ int span[2];                              // first, count: the offsets clamped to [0, batch]
+  if (tid == 0) {
+    const int first = min(max(P.start[P.cls], 0), P.batch);
+    span[0] = first;
+    span[1] = min(max(P.start[P.cls + 1], first), P.batch) - first;
+    item[0][0] = static_cast<int>(blockIdx.x / static_cast<unsigned>(P.tiles));
+    item[0][1] = static_cast<int>(blockIdx.x % static_cast<unsigned>(P.tiles));
+  }
+  __syncthreads();
+#pragma unroll 1
+  for (int k = 0;; k ^= 1) {
+    const int p = item[k][0], t = item[k][1];
+    if (p >= span[1]) break;                         // CTA-uniform; p grows every item, so the loop ends
+    if (tid == 0) {                                  // i + gridDim.x without a division
+      unsigned nt = static_cast<unsigned>(t) + P.step_t;
+      int np = p + P.step_p;
+      if (nt >= static_cast<unsigned>(P.tiles)) { nt -= P.tiles; ++np; }
+      item[k ^ 1][0] = np;
+      item[k ^ 1][1] = static_cast<int>(nt);
+    }
+    const int64_t b = P.perm[span[0] + p];
+    const int64_t col0 = static_cast<int64_t>(t) * cols_per_tile;
+    const TmShape sh = P.each[b].tm;
+    stage_rows<S, DT>(P, sh, tile, col0, static_cast<const uint8_t*>(P.G) + b * P.g_batch * es,
+                      P.row_index ? P.row_index + b * P.ri_batch : nullptr);
+    int lane = tid & 31, warp_o = warp;
+    if (W16 || S < 32) {      // as trimmed_mean_kernel
+      asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+      asm volatile("mov.u32 %0, %1;" : "=r"(warp_o) : "r"(warp));
+    }
+    __syncthreads();
+    uint32_t* scratch = tile + kWordCols * kGroups * 128 + warp_o * kScratchWords;
+#pragma unroll 1
+    for (int cw = warp_o; cw < kWordCols; cw += kWarps) {
+#pragma unroll 1
+      for (int half = 0; half < (W16 ? 2 : 1); ++half) {
+        const int64_t col = col0 + (W16 ? 2 * cw + half : cw);
+        if (col >= P.d) break;                         // warp-uniform
+        const float res = general_column_impl<S, DT>(sh, tile, cw, half, scratch, lane);
+        if (lane == 0) P.out[b * P.out_batch + col] = res;
+      }
+    }
+    __syncthreads();          // every warp is done with the tile before the next item re-stages it
+  }
+}
+
 // ---------------- more than 1024 participating rows: shared-memory bisection kernel (any n that fits) ----------------
 // The register-resident kernels above hold ceil(n/32) <= 32 values per lane.  Beyond that a CTA stages a 16-byte-wide
 // column strip of ALL rows in shared memory ([row][4 words], up to kLargeMaxRows rows) and one warp per column finds
@@ -806,6 +899,41 @@ static int launch(const Params& P, int dtype, int batch, cudaStream_t stream, co
                             : go(trimmed_mean_kernel<S, AFL_F32, false>, P);
 }
 
+// One device-count class launch (trimmed_mean_dev_kernel) of class cls over a batch of `batch` problems.  Grid:
+// min(resident CTAs of the instance x SMs, tiles x batch), the occupancy cached per device and instance.
+template <int S>
+static int launch_dev(const Params& P, int dtype, int batch, cudaStream_t stream, const int* perm, const int* start,
+                      int cls) {
+  const size_t smem = static_cast<size_t>(S) * 2048 + kWarps * kScratchWords * 4;
+  const int cols = dtype != AFL_F32 ? 32 : 16;
+  const int64_t tiles = ceil_div64(P.d, cols);
+  if (tiles > INT32_MAX) { set_error("afl_trimmed_mean: d = %lld is too wide", static_cast<long long>(P.d)); return AFL_ERR_UNSUPPORTED; }
+  DevClassParams C{};
+  static_cast<Params&>(C) = P;
+  C.perm = perm; C.start = start; C.cls = cls; C.batch = batch; C.tiles = static_cast<int>(tiles);
+  ProfScope ps("trimmed_mean", stream);
+  auto go = [&](auto kernel, int (&smem_done)[kMaxDevices], int (&resident)[kMaxDevices]) -> int {
+    AFL_CUDA(ensure_dyn_smem(kernel, static_cast<int>(smem), smem_done));
+    const int dev = current_device();
+    if (!resident[dev]) {
+      int r = 0;
+      AFL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kernel, kThreads, smem));
+      resident[dev] = r > 0 ? r : 1;
+    }
+    const int64_t work = tiles * batch, wave = static_cast<int64_t>(resident[dev]) * sm_count();
+    const int grid = static_cast<int>(work < wave ? work : wave);
+    C.step_p = grid / C.tiles;
+    C.step_t = grid % C.tiles;
+    kernel<<<grid, kThreads, smem, stream>>>(C);
+    AFL_LAUNCH_CHECK("trimmed_mean_dev_kernel");
+    return AFL_OK;
+  };
+  static int smem_done[3][kMaxDevices], resident[3][kMaxDevices];
+  return dtype == AFL_BF16  ? go(trimmed_mean_dev_kernel<S, AFL_BF16>, smem_done[1], resident[1])
+         : dtype == AFL_F16 ? go(trimmed_mean_dev_kernel<S, AFL_F16>, smem_done[2], resident[2])
+                            : go(trimmed_mean_dev_kernel<S, AFL_F32>, smem_done[0], resident[0]);
+}
+
 // `batch` problems (grid y): problem b reads G + b * g_batch and row_index + b * ri_batch, and writes out + b * out_batch.
 // each (device, may be NULL; n_rows <= 128): problem b's participating rows and constants are each[b].tm, at most n_rows.
 int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,
@@ -851,10 +979,6 @@ int trimmed_mean_batched(const void* G, int n, int64_t d, int64_t ld, int dtype,
   return launch<32>(P, dtype, batch, stream);
 }
 
-// The slot class of n_rows <= 1024 participating rows: c = 0 .. kSlotClasses - 1 for the kernel with S = 4 (c + 1)
-// slots per lane, the instance that trimmed_mean_batched launches for them.
-int slot_class(int n_rows) { return n_rows <= 128 ? 0 : (n_rows - 1) / 128; }
-
 // A batch with a table whose problems have up to 1024 participating rows each (each[b].tm.n_rows): problem b runs the
 // instance that its own row count selects, so its result is its single call's bit for bit.  perm (device, `batch`
 // entries) lists the problems class by class, counts[c] (host, kSlotClasses entries) how many have class c; one launch
@@ -890,6 +1014,33 @@ int trimmed_mean_classes(const void* G, int n, int64_t d, int64_t ld, int dtype,
     if (rc) return rc;
   }
   return AFL_OK;
+}
+
+// trimmed_mean_classes with the class sizes in device memory: perm as there, start[kSlotClasses + 1] (device) the offset
+// of each class in perm.  One device-count launch per class, all kSlotClasses of them whether a class is present or
+// not, so the host reads nothing and the launches can be captured into a CUDA graph.
+int trimmed_mean_classes_dev(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, float* out,
+                             int batch, int64_t g_batch, int ri_batch, int64_t out_batch, cudaStream_t stream,
+                             const ProblemParams* each, const int* perm, const int* start) {
+  if (!G || !out || !each || !perm || !start || n < 1 || d < 1 || ld < d || batch < 1) {
+    set_error("afl_trimmed_mean: bad argument");
+    return AFL_ERR_BAD_ARG;
+  }
+  if (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16) { set_error("afl_trimmed_mean: dtype"); return AFL_ERR_UNSUPPORTED; }
+  Params P{};
+  P.G = G; P.row_index = row_index; P.out = out; P.d = d; P.ld = ld; P.n_total = n;
+  P.each = each; P.g_batch = g_batch; P.out_batch = out_batch; P.ri_batch = ri_batch;
+  const int64_t es = dtype == AFL_F32 ? 4 : 2;
+  P.vec_ok = (reinterpret_cast<uintptr_t>(G) % 16 == 0) && ((ld * es) % 16 == 0) && (batch == 1 || (g_batch * es) % 16 == 0);
+  int rc = AFL_OK;
+  if ((rc = launch_dev<4>(P, dtype, batch, stream, perm, start, 0))) return rc;
+  if ((rc = launch_dev<8>(P, dtype, batch, stream, perm, start, 1))) return rc;
+  if ((rc = launch_dev<12>(P, dtype, batch, stream, perm, start, 2))) return rc;
+  if ((rc = launch_dev<16>(P, dtype, batch, stream, perm, start, 3))) return rc;
+  if ((rc = launch_dev<20>(P, dtype, batch, stream, perm, start, 4))) return rc;
+  if ((rc = launch_dev<24>(P, dtype, batch, stream, perm, start, 5))) return rc;
+  if ((rc = launch_dev<28>(P, dtype, batch, stream, perm, start, 6))) return rc;
+  return launch_dev<32>(P, dtype, batch, stream, perm, start, 7);
 }
 
 int trimmed_mean(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* row_index, int n_rows,

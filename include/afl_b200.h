@@ -469,8 +469,8 @@ int afl_backdoor_finish_batched(int batch, int64_t d, const int* f, const double
  * Workspace: afl_batched_each_workspace_bytes("ALIE", batch, 1, 1, 0) bytes or more.
  *
  * afl_defend_batched_dev — afl_defend_batched_rows (rows != NULL) or afl_defend_batched_each (rows == NULL) with
- * device arrays, n <= 128 (larger n -> AFL_ERR_UNSUPPORTED: the per-class trimmed-mean launches of larger slots need
- * the classes on the host).  Bulyan's sel_out is [batch][sel_ld] with sel_ld >= n (else AFL_ERR_BAD_ARG): theta_b
+ * device arrays, n <= 128 (larger n -> AFL_ERR_UNSUPPORTED; afl_defend_batched_large_dev takes up to 1024).
+ * Bulyan's sel_out is [batch][sel_ld] with sel_ld >= n (else AFL_ERR_BAD_ARG): theta_b
  * entries, then -2.  Workspace and layout: afl_batched_rows_workspace_bytes(rule, ...).
  *
  * afl_alie_batched_dev — afl_alie_batched_each / _large with device arrays, any n, f_b <= n.  bcast_rows (may be NULL)
@@ -479,7 +479,16 @@ int afl_backdoor_finish_batched(int batch, int64_t d, const int* f, const double
  * afl_batched_each_workspace_bytes("ALIE", batch, 1, d, dtype).
  *
  * afl_attack_metrics_batched_dev — afl_attack_metrics_batched_rows (rows != NULL) or _each with device arrays, any n.
- * Workspace: afl_metrics_workspace_bytes. */
+ * Workspace: afl_metrics_workspace_bytes.
+ *
+ * afl_defend_batched_large_dev — afl_defend_batched_large with device arrays: the arguments of afl_defend_batched_dev
+ * and 1 <= n <= 1024 (larger n -> AFL_ERR_UNSUPPORTED).  For n <= 128 it is afl_defend_batched_dev.  Above, the
+ * per-problem checks, codes and safe row are afl_defend_batched_dev's, and the problems are grouped by trimmed-mean slot
+ * class on the device, so the call still makes no host copy, synchronisation or allocation after its host checks.
+ * Workspace: afl_batched_large_dev_workspace_bytes(rule, ...) — 0 on bad arguments and for n > 1024; for n <= 128
+ * afl_batched_rows_workspace_bytes; above, afl_batched_large_workspace_bytes plus one 256-byte block at the end that
+ * holds the class offsets, so every offset of the large call's layout (the table, perm, d2, dist, the Gram workspace
+ * and the selection scratch) holds for this call too. */
 int afl_batched_table_dev(const char* rule, int batch, int n, const int* rows, int users_count, const int* users_counts,
                           const int* corrupted_counts, const double* z, void* workspace, size_t workspace_bytes,
                           int* status, void* stream);
@@ -491,6 +500,11 @@ int afl_alie_batched_dev(const void* G, int batch, int64_t batch_stride, int n, 
                          const int* f, const double* z, float* mu_out, float* sigma_out, float* crafted_out,
                          void* bcast_rows, int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
                          size_t workspace_bytes, int* status, void* stream);
+size_t afl_batched_large_dev_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype);
+int afl_defend_batched_large_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
+                                 int64_t ld, int dtype, const int* rows, int users_count, const int* users_counts,
+                                 const int* corrupted_counts, float* out, int* idx_out, int* sel_out, int sel_ld,
+                                 void* workspace, size_t workspace_bytes, int* status, void* stream);
 int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
                                    int dtype, const int* rows, const int* corrupted_counts, const float* agg,
                                    const int* idx, const int* sel, int sel_ld, float* dev_out, double* sums_out,

@@ -88,6 +88,9 @@ SIGNATURES = {
     "afl_batched_large_dev_workspace_bytes": (_sz, [C.c_char_p, _i, _i, _i64, _i]),
     "afl_defend_batched_large_dev": (_i, [C.c_char_p, _vp, _i, _i64, _i, _i64, _i64, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp,
                                           _i, _vp, _sz, _vp, _vp]),
+    "afl_mnist_client_grads": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i64, _i64, _vp]),
+    "afl_mnist_evaluate_workspace_bytes": (_sz, [_i, _i, _i]),
+    "afl_mnist_evaluate": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }
 
 _lib = None

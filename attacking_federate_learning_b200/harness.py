@@ -22,6 +22,10 @@ leave the device.  The training simulation itself is not part of the accelerated
 
     python -m attacking_federate_learning_b200.harness -d Krum -e 30 --users-count 10
     python -m attacking_federate_learning_b200.harness -d Krum -e 30 -z 1.0 -b pattern
+
+A grid of these experiments (defence x z x malicious share x users x seed) runs as one batch in `sweep.run` / `python -m
+attacking_federate_learning_b200.sweep`: each experiment starts from `experiment_setup`'s data and weights, as here,
+and the client gradients of every experiment come from one CUDA kernel instead of this file's per-client autograd.
 """
 from __future__ import annotations
 
@@ -62,6 +66,20 @@ def synthetic_problem(n_train, n_test, device, seed=0):
         x = protos[y] + 2.5 * torch.randn(n, 28 * 28, generator=g)
         return x.to(device), y.to(device)
     return draw(n_train), draw(n_test)
+
+
+def experiment_setup(seed, train_size, test_size, device):
+    """The seeded start of an experiment: torch.manual_seed(seed), the synthetic train and test sets and the test
+    network, whose parameters are the initial global weights.  ((xtr, ytr), (xte, yte), test_net)."""
+    torch.manual_seed(seed)
+    train, test = synthetic_problem(train_size, test_size, device, seed)
+    return train, test, MnistNet().to(device)
+
+
+def csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate):
+    """main.py:100's accuracy log name (without the logs/ directory)."""
+    return '{}_stdev_{}_{}_backdoor-{}_mal_prop_{}_users_{}_alpha_{}_lr_{}.csv'.format(
+        SYNTH, num_std, defense, backdoor, mal_prop, users_count, alpha if backdoor else None, learning_rate)
 
 
 class Client:
@@ -157,10 +175,8 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
         my_print = print
     my_print(dict(mal_prop=mal_prop, num_std=num_std, defense=defense, users_count=users_count, epochs=epochs,
                   learning_rate=learning_rate, dataset=SYNTH, backdoor=backdoor))
-    torch.manual_seed(seed)
     corrupted_count = int(mal_prop * users_count)                         # main.py:21
-    (xtr, ytr), (xte, yte) = synthetic_problem(train_size, test_size, device, seed)
-    test_net = MnistNet().to(device)
+    (xtr, ytr), (xte, yte), test_net = experiment_setup(seed, train_size, test_size, device)
     layout = ParamLayout(test_net.parameters())
     srv = AggregationServer(users_count, layout.dim, mal_prop, learning_rate, momentum, device=device,
                             initial_weights=layout.flatten(list(test_net.parameters())))
@@ -209,8 +225,7 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     my_print(datetime.datetime.now().time())
     my_print("Max accuracy: {}".format(max(accuracies)))
     os.makedirs(os.path.join(out_dir, "logs"), exist_ok=True)             # the reference needs a pre-made logs/ (readme.md:25)
-    csv = os.path.join(out_dir, 'logs', '{}_stdev_{}_{}_backdoor-{}_mal_prop_{}_users_{}_alpha_{}_lr_{}.csv'.format(
-        SYNTH, num_std, defense, backdoor, mal_prop, users_count, alpha if backdoor else None, learning_rate))
+    csv = os.path.join(out_dir, 'logs', csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate))
     np.savetxt(csv, accuracies, delimiter=',')                            # main.py:100
     return accuracies, accuracies_epochs, csv
 

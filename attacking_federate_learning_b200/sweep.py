@@ -1,0 +1,330 @@
+"""Training sweeps: a grid of `harness.main` experiments trained side by side as one batch on the GPU.
+
+An experiment is `(defense, mal_prop, num_std, users_count, seed)`, what main.py:104-131 takes (without the backdoor).
+Experiment b starts from exactly the data and weights `harness.main(mal_prop, num_std, defense, users_count,
+seed=seed)` starts from (`harness.experiment_setup`) and runs main.py's epoch loop (main.py:64-71, server.py:86-90):
+
+  1. every client's MnistNet gradient on its minibatch (user.py:76-92), for every experiment in one launch of the
+     client-gradient kernel (C ABI `afl_mnist_client_grads`), written straight into the experiment's rows of one
+     [B, N_max, ld] client matrix;
+  2. per defence, on the contiguous slice of experiments that use it (`batched.DeviceRound` with the experiments' own
+     f_b = int(mal_prop * n_b), z_b and row counts): ALIE on rows 0..f_b-1, the rule, and the server's momentum step on
+     the slice's [B_r, D] weights at the base learning rate (server.py:89);
+  3. the device epoch counter advances (the kernel reads it, so a replayed graph moves every client's minibatch on);
+  4. every `test_step` epochs and at the last epoch, every experiment's test loss and accuracy (`afl_mnist_evaluate`,
+     harness.main's test loop) into the next slot of a device table.
+
+Nothing synchronises the host until the run ends.  With capture=True epoch 0 runs eagerly and the later epochs replay
+a captured training epoch and test epoch; both paths give the same bits.  A client's gradient depends only on its own
+weights and rows, so an experiment's trajectory does not depend on which other experiments share its batch (the
+Krum and Bulyan distance tables aside, whose split count follows the batch unless AFL_GRAM_SPLITS pins it).  A
+failure that only the data can show (a Bulyan round with no eligible user) lands in the rule's `DeviceRound.status`:
+that experiment is reported as failed with the error `raise_for_status` gives, and the others complete.
+
+Outputs per experiment: the accuracy list and the CSV `harness.main` writes (np.savetxt(..., delimiter=',') in
+out_dir/logs, with `_seed_<s>` before `.csv` so that seeds do not overwrite one another), and one summary CSV with the
+parameters, max and final accuracy and status.  No checkpoint is written: main.py's checkpoint path has no experiment
+key, so the experiments of a batch would overwrite one file.
+
+    python -m attacking_federate_learning_b200.sweep -d Krum TrimmedMean -z 0.5 1.5 -m 0.1 0.24 -n 10 --seeds 0 1 -e 30
+"""
+from __future__ import annotations
+
+import argparse
+import csv as _csv
+import itertools
+import os
+from typing import NamedTuple
+
+import numpy as np
+import torch
+
+from . import _native as nat
+from . import batched
+from . import harness
+from ._device import momentum_step
+from .defences import DefenseTypes
+
+RULES = (DefenseTypes.Krum, DefenseTypes.Bulyan, DefenseTypes.TrimmedMean, DefenseTypes.NoDefense)
+MAX_USERS = batched.MAX_CLIENTS          # clients per experiment (DeviceRound with large=True)
+MAX_BATCH_SIZE = 128                     # minibatch rows of the client-gradient kernel
+SUMMARY = 'sweep_summary.csv'
+
+
+class Experiment(NamedTuple):
+    defense: str
+    mal_prop: float
+    num_std: float
+    users_count: int
+    seed: int
+
+    @property
+    def corrupted_count(self):
+        return int(self.mal_prop * self.users_count)                      # main.py:21
+
+
+def minibatch(n_train, users_count, user, batch_size, epoch):
+    """Shard positions [lo, hi) of `user`'s minibatch at `epoch`: harness.Client.step's cycling position in closed form
+    (the kernel computes the same).  The shard is training rows user, user + n, ...; row = user + n * position."""
+    length = (n_train - user + users_count - 1) // users_count
+    k = epoch % ((length + batch_size - 1) // batch_size)
+    return k * batch_size, min(k * batch_size + batch_size, length)
+
+
+def check(exp, batch_size=83, train_size=20000):
+    """Raise what main.py would raise for this experiment at its first `defend` (AssertionError for the reference's
+    asserts), or for what the sweep's kernels do not take.  Returns the normalised Experiment."""
+    exp = Experiment(str(exp[0]), float(exp[1]), float(exp[2]), int(exp[3]), int(exp[4]))
+    if exp.defense not in RULES:
+        raise KeyError(f"{exp}: unknown defence {exp.defense!r} (expected one of {', '.join(RULES)})")
+    if not 1 <= exp.users_count <= MAX_USERS:
+        raise (ValueError if exp.users_count < 1 else NotImplementedError)(
+            f"{exp}: users_count must lie in 1..{MAX_USERS}")
+    if exp.users_count > train_size:
+        raise ValueError(f"{exp}: {exp.users_count} users need at least as many training samples (got {train_size})")
+    n, f = exp.users_count, exp.corrupted_count
+    if exp.defense == DefenseTypes.Krum and not n >= 2 * f + 1:           # defences.py:24
+        raise AssertionError(f"{exp}: Krum needs users_count >= 2 * corrupted_count + 1 ({n}, {f})")
+    if exp.defense == DefenseTypes.Bulyan and not n >= 4 * f + 3:         # defences.py:56
+        raise AssertionError(f"{exp}: Bulyan needs users_count >= 4 * corrupted_count + 3 ({n}, {f})")
+    if not 1 <= batch_size <= MAX_BATCH_SIZE:
+        raise (ValueError if batch_size < 1 else NotImplementedError)(
+            f"batch_size must lie in 1..{MAX_BATCH_SIZE} (got {batch_size})")
+    return exp
+
+
+def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000):
+    """The Cartesian grid (defence-major) as (kept experiments, [(experiment, rejection), ...]): a cell main.py
+    would reject is dropped with the exception `check` raises for it."""
+    kept, dropped = [], []
+    for cell in itertools.product(defenses, mal_props, num_stds, users_counts, seeds):
+        try:
+            kept.append(check(cell, batch_size, train_size))
+        except (AssertionError, KeyError, ValueError, NotImplementedError) as e:
+            dropped.append((cell, e))
+    return kept, dropped
+
+
+def csv_name(exp, learning_rate):
+    """harness.main's log name for this experiment, with `_seed_<s>` before `.csv`."""
+    name = harness.csv_name(exp.num_std, exp.defense, False, exp.mal_prop, exp.users_count, 4, learning_rate)
+    return name[:-len('.csv')] + f'_seed_{exp.seed}.csv'
+
+
+def test_epochs(epochs, test_step):
+    return [e for e in range(epochs) if e % test_step == 0 or e == epochs - 1]
+
+
+def status_error(code, name):
+    """The exception DeviceRound.raise_for_status raises for a status code, naming the experiment."""
+    if code == nat.AFL_ERR_NO_WINNER:
+        e = KeyError(-1)
+        e.add_note(f"{name}: a Bulyan selection round found no eligible user (defences.py:66)")
+        return e
+    exc, what = batched._STATUS_ERRORS.get(code, (nat.NativeError, None))
+    return nat.NativeError(code, name) if what is None else exc(f"{name}: {what}")
+
+
+class Sweep:
+    """The device state of a batch of experiments and its epoch.  `run` drives it; tests and tools may drive it
+    directly: `train_epoch()` and `test_epoch()` enqueue one epoch's work, `step(epoch)` runs epoch `epoch` (captured
+    after epoch 0 when capture=True), `results()` synchronises and reads the tables back.
+
+    Batch order: experiments grouped by defence in RULES order, each group in the given order; `order[i]` is the
+    position in `experiments` of batch problem i.  W, V: fp32 [B, D] weights and velocity; G: the [B, N_max, ld]
+    client matrix (ld a multiple of 32, as AggregationServer pads); `rounds`: {defence: (slice, DeviceRound)}."""
+
+    def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000,
+                 test_size=4000, test_step=5, capture=True, device='cuda'):
+        exps = [check(e, batch_size, train_size) for e in experiments]
+        if not exps:
+            raise ValueError("sweep: no experiment")
+        if epochs < 1 or test_step < 1 or test_size < 1:
+            raise ValueError(f"sweep: epochs, test_step and test_size must be >= 1 (got {epochs}, {test_step}, "
+                             f"{test_size})")
+        self.order = [i for r in RULES for i, e in enumerate(exps) if e.defense == r]
+        self.experiments = [exps[i] for i in self.order]
+        self.epochs, self.learning_rate, self.momentum = epochs, learning_rate, momentum
+        self.batch_size, self.train_size, self.test_size, self.test_step = batch_size, train_size, test_size, test_step
+        self.capture = capture
+        dev = self.device = torch.device(device)
+        seeds = list(dict.fromkeys(e.seed for e in self.experiments))
+        xtr, ytr, xte, yte, w0 = [], [], [], [], {}
+        for s in seeds:                                                   # harness.main's start, seed by seed
+            (a, b), (c, d), net = harness.experiment_setup(s, train_size, test_size, dev)
+            xtr.append(a); ytr.append(b); xte.append(c); yte.append(d)
+            w0[s] = harness.ParamLayout(net.parameters()).flatten(list(net.parameters()))
+        self.x_train, self.y_train = torch.stack(xtr).contiguous(), torch.stack(ytr).contiguous()
+        self.x_test, self.y_test = torch.stack(xte).contiguous(), torch.stack(yte).contiguous()
+        B, self.D = len(self.experiments), w0[seeds[0]].numel()
+        self.B = B
+        self.N = max(e.users_count for e in self.experiments)
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.data_index = torch.tensor([seeds.index(e.seed) for e in self.experiments], **i32)
+        self.rows = torch.tensor([e.users_count for e in self.experiments], **i32)
+        self.W = torch.stack([w0[e.seed] for e in self.experiments]).contiguous()
+        self.V = torch.zeros_like(self.W)
+        ld = (self.D + 31) // 32 * 32
+        self._storage = torch.zeros((B, self.N, ld), dtype=torch.float32, device=dev)
+        self.G = self._storage[:, :, :self.D]
+        self.epoch_counter = torch.zeros(1, **i32)                       # the kernel's epoch
+        self.test_slot = torch.zeros(1, **i32)                           # the next row of the test tables
+        self.n_tests = len(test_epochs(epochs, test_step))
+        self.loss_sum = torch.zeros((self.n_tests, B), dtype=torch.float64, device=dev)
+        self.correct = torch.zeros((self.n_tests, B), **i32)
+        L = nat.lib()
+        self._eval_ws = torch.empty(max(L.afl_mnist_evaluate_workspace_bytes(B, test_size, batch_size), 256),
+                                    dtype=torch.uint8, device=dev)
+        self.rounds = {}
+        for r in RULES:
+            idx = [i for i, e in enumerate(self.experiments) if e.defense == r]
+            if not idx:
+                continue
+            sl = slice(idx[0], idx[-1] + 1)
+            rnd = batched.DeviceRound(self.G[sl], rows=True, rules=(r,), large=self.N > batched.ONE_TILE)
+            sub = self.experiments[sl]
+            rnd.f.copy_(torch.tensor([e.corrupted_count for e in sub], dtype=torch.int32))
+            rnd.z.copy_(torch.tensor([e.num_std for e in sub], dtype=torch.float64))
+            rnd.rows.copy_(torch.tensor([e.users_count for e in sub], dtype=torch.int32))
+            self.rounds[r] = (sl, rnd)
+        self._graphs = None
+
+    def client_grads(self):
+        """Step 1: every client's gradient into G at the current device epoch."""
+        G = self._storage
+        with torch.cuda.device(self.device):
+            nat.check(nat.lib().afl_mnist_client_grads(
+                self.W.data_ptr(), self.B, self.D, self.x_train.data_ptr(), self.y_train.data_ptr(),
+                self.x_train.shape[0], self.train_size, self.data_index.data_ptr(), self.rows.data_ptr(), self.N,
+                self.batch_size, self.epoch_counter.data_ptr(), G.data_ptr(), G.stride(0), G.stride(1),
+                torch.cuda.current_stream(self.device).cuda_stream))
+
+    def aggregate(self, rule=None):
+        """Step 2 for one defence (every defence when rule is None): ALIE, the rule and the momentum step."""
+        for r, (sl, rnd) in self.rounds.items():
+            if rule is not None and r != rule:
+                continue
+            rnd.alie()
+            agg = {DefenseTypes.Krum: rnd.krum, DefenseTypes.Bulyan: rnd.bulyan,
+                   DefenseTypes.TrimmedMean: rnd.trimmed_mean, DefenseTypes.NoDefense: rnd.no_defense}[r]()
+            momentum_step(self.W[sl], self.V[sl], agg, self.momentum, self.learning_rate)
+
+    def train_epoch(self):
+        self.client_grads()
+        self.aggregate()
+        self.epoch_counter.add_(1)
+
+    def test_epoch(self):
+        """Step 4: every experiment's test loss sum and correct count into the next slot of the tables."""
+        with torch.cuda.device(self.device):
+            nat.check(nat.lib().afl_mnist_evaluate(
+                self.W.data_ptr(), self.B, self.D, self.x_test.data_ptr(), self.y_test.data_ptr(),
+                self.x_test.shape[0], self.test_size, self.data_index.data_ptr(), self.batch_size,
+                self.test_slot.data_ptr(), self.n_tests, self.loss_sum.data_ptr(), self.correct.data_ptr(),
+                self._eval_ws.data_ptr(), self._eval_ws.numel(), torch.cuda.current_stream(self.device).cuda_stream))
+        self.test_slot.add_(1)
+
+    def is_test_epoch(self, epoch):
+        return epoch % self.test_step == 0 or epoch == self.epochs - 1
+
+    def step(self, epoch):
+        """Epoch `epoch` (host bookkeeping only: the device counters advance on their own).  With capture, epoch 0 runs
+        eagerly and captures the training and test epochs, which every later epoch replays."""
+        if not self.capture or self._graphs is None:
+            self.train_epoch()
+            if self.is_test_epoch(epoch):
+                self.test_epoch()
+            if self.capture:
+                self._graphs = (torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph())
+                with torch.cuda.device(self.device):
+                    with torch.cuda.graph(self._graphs[0]):
+                        self.train_epoch()
+                    with torch.cuda.graph(self._graphs[1]):
+                        self.test_epoch()
+            return
+        self._graphs[0].replay()
+        if self.is_test_epoch(epoch):
+            self._graphs[1].replay()
+
+    def status(self):
+        """Per batch problem: 0, or the first error code its rule's DeviceRound flagged (synchronises)."""
+        st = torch.zeros(self.B, dtype=torch.int32, device=self.device)
+        for sl, rnd in self.rounds.values():
+            st[sl] = rnd.status
+        return st.cpu().numpy()
+
+    def results(self):
+        """Synchronise and return, in the order of `experiments` as given, one dict per experiment: experiment,
+        accuracies, accuracies_epochs, losses (harness.main's test loss), error (None, or the exception)."""
+        st = self.status()
+        correct = self.correct.cpu().numpy()
+        loss = self.loss_sum.cpu().numpy()
+        epochs = test_epochs(self.epochs, self.test_step)
+        out = [None] * self.B
+        for i, (pos, e) in enumerate(zip(self.order, self.experiments)):
+            acc = [100. * float(correct[t, i]) / self.test_size for t in range(self.n_tests)]
+            err = status_error(int(st[i]), f"experiment {tuple(e)}") if st[i] else None
+            out[pos] = dict(experiment=e, accuracies=acc, accuracies_epochs=epochs,
+                            losses=[float(loss[t, i]) / self.test_size for t in range(self.n_tests)], error=err)
+        return out
+
+
+def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000, test_size=4000,
+        test_step=5, out_dir='.', capture=True, device='cuda'):
+    """Train every experiment for `epochs` epochs as one batch; write each one's accuracy CSV and the summary CSV under
+    out_dir/logs.  Returns `Sweep.results()` with `csv` (None for a failed experiment) added to each dict.  Raises
+    before any GPU work for an experiment main.py would reject (see `check`)."""
+    sw = Sweep(experiments, epochs, learning_rate, momentum, batch_size, train_size, test_size, test_step, capture,
+               device)
+    with torch.cuda.device(sw.device):
+        for epoch in range(epochs):
+            sw.step(epoch)
+    res = sw.results()
+    logs = os.path.join(out_dir, 'logs')
+    os.makedirs(logs, exist_ok=True)
+    with open(os.path.join(logs, SUMMARY), 'w', newline='') as fh:
+        w = _csv.writer(fh)
+        w.writerow(list(Experiment._fields) + ['max_accuracy', 'final_accuracy', 'status'])
+        for r in res:
+            e = r['experiment']
+            r['csv'] = None
+            if r['error'] is None:
+                r['csv'] = os.path.join(logs, csv_name(e, learning_rate))
+                np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
+                w.writerow(list(e) + [max(r['accuracies']), r['accuracies'][-1], 'ok'])
+            else:
+                w.writerow(list(e) + ['', '', f"failed: {type(r['error']).__name__}: {r['error']}"])
+    return res
+
+
+def main(argv=None):
+    p = argparse.ArgumentParser(description="A grid of main.py experiments as one batched training run.")
+    p.add_argument('-d', '--defense', nargs='+', default=['NoDefense'], choices=list(RULES))
+    p.add_argument('-z', '--num_std', nargs='+', type=float, default=[1.5])
+    p.add_argument('-m', '--mal-prop', nargs='+', type=float, default=[0.24])
+    p.add_argument('-n', '--users-count', nargs='+', type=int, default=[10])
+    p.add_argument('--seeds', nargs='+', type=int, default=[0])
+    p.add_argument('-e', '--epochs', type=int, default=300)
+    p.add_argument('-c', '--batch_size', type=int, default=83)
+    p.add_argument('-l', '--learning_rate', type=float, default=0.1)
+    p.add_argument('--out-dir', default='.')
+    p.add_argument('--no-capture', action='store_true')
+    a = p.parse_args(argv)
+    kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size)
+    for cell, e in dropped:
+        print(f"skipped {cell}: {type(e).__name__}: {e}")
+    if not kept:
+        print("no experiment left to run")
+        return []
+    res = run(kept, a.epochs, a.learning_rate, batch_size=a.batch_size, out_dir=a.out_dir, capture=not a.no_capture)
+    for r in res:
+        e = r['experiment']
+        if r['error'] is None:
+            print(f"{tuple(e)}: max accuracy {max(r['accuracies']):.2f}, final {r['accuracies'][-1]:.2f} -> {r['csv']}")
+        else:
+            print(f"{tuple(e)}: failed: {type(r['error']).__name__}: {r['error']}")
+    return res
+
+
+if __name__ == '__main__':
+    main()

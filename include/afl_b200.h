@@ -511,6 +511,40 @@ int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_strid
                                    float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* workspace,
                                    size_t workspace_bytes, int* status, void* stream);
 
+/* ---- MnistNet client gradients and evaluation (csrc/client_grad.cu): the training half of a sweep epoch ----------
+ * The model is the harness's MnistNet (data_sets.py:13-24), log_softmax(fc2(relu(fc1(x)))), its d = 79,510 parameters
+ * in ParamLayout order (fc1.weight [100][784], fc1.bias, fc2.weight [10][100], fc2.bias).  weights: device fp32
+ * [batch][d], problem b's model.  x: device fp32 [n_sets][set_size][784] and y: device int64 [n_sets][set_size], one
+ * data set per seed; data_index (device int32 [batch]) picks problem b's set (outside [0, n_sets): the problem is
+ * skipped).  fp32 FFMA throughout, no atomics and every sum in a fixed order, so each result depends only on its
+ * problem's weights, rows and m, never on batch, n or the other problems.  The calls only enqueue work on `stream`
+ * (no allocation, copy or synchronisation), so they can be captured in a CUDA graph.  Checked before any CUDA call: a
+ * NULL pointer, batch / n_sets / set size / m < 1 -> AFL_ERR_BAD_ARG; d != 79,510, m > 128 or batch > 65535 ->
+ * AFL_ERR_UNSUPPORTED.
+ *
+ * afl_mnist_client_grads — user.py:76-92 for every client of every problem: client u < n_b = min(rows[b], n) (rows:
+ * device int32 [batch]) computes the gradient of NLLLoss(mean) on its minibatch at problem b's weights and writes it
+ * to columns [0, d) of row u of problem b, G + b * batch_stride + u * ld (fp32).  Nothing else of G is written.  Client
+ * u's shard is training rows u, u + n_b, u + 2 n_b, ... (L = ceil((n_train - u) / n_b) of them); at epoch e = *epoch
+ * (device int32, read when the kernel runs) it takes shard positions [k m, min(k m + m, L)), k = e mod ceil(L / m):
+ * harness.Client.step's cycling position.  1 <= n <= 1024 clients and n <= n_train, else AFL_ERR_BAD_ARG /
+ * AFL_ERR_UNSUPPORTED; ld >= d and (batch > 1) batch_stride >= (n - 1) * ld + d, else AFL_ERR_BAD_ARG.
+ *
+ * afl_mnist_evaluate — server.py:92-112 / harness.main's test loop for every problem: test batches of m rows (the last
+ * one shorter), each batch's mean NLL in fp32, summed over the batches in order in float64 into
+ * loss_sum[slot][b] (divide by n_test for the reported loss), and correct[slot][b] = the number of rows whose argmax
+ * (the first maximum of the log-probabilities) is the label.  slot = *slot_index (device int32, read when the kernel
+ * runs); a slot outside [0, n_slots) writes nothing.  loss_sum: device float64 [n_slots][batch], correct: device int32
+ * [n_slots][batch].  Workspace: afl_mnist_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned (else
+ * AFL_ERR_WORKSPACE); 0 on bad arguments.  More than 65535 test batches -> AFL_ERR_UNSUPPORTED. */
+int afl_mnist_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                           int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
+                           float* G, int64_t batch_stride, int64_t ld, void* stream);
+size_t afl_mnist_evaluate_workspace_bytes(int batch, int n_test, int m);
+int afl_mnist_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                       int n_test, const int* data_index, int m, const int* slot_index, int n_slots, double* loss_sum,
+                       int* correct, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

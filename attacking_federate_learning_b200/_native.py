@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libafl_b200.so")
 
 AFL_OK, AFL_ERR_BAD_ARG, AFL_ERR_PRECONDITION, AFL_ERR_CUDA, AFL_ERR_UNSUPPORTED, AFL_ERR_WORKSPACE, AFL_ERR_NO_WINNER = range(7)
+AFL_ERR_NAN_LOSS, AFL_ERR_NAN_DIST_LOSS = 7, 8
 AFL_F32, AFL_BF16, AFL_F16 = 0, 1, 2
 GRAM_AUTO, GRAM_FORCE_SIMT, GRAM_FORCE_TCGEN05, GRAM_SINGLE_PASS, GRAM_REWRITE_HI = 0, 1, 2, 4, 8
 GRAM_TF32X2 = 16
@@ -91,6 +92,12 @@ SIGNATURES = {
     "afl_mnist_client_grads": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i64, _i64, _vp]),
     "afl_mnist_evaluate_workspace_bytes": (_sz, [_i, _i, _i]),
     "afl_mnist_evaluate": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "afl_backdoor_start_batched_dev": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp,
+                                            _vp, _sz, _vp, _vp]),
+    "afl_backdoor_finish_batched_dev": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
+                                             _i64, _vp, _sz, _vp, _vp]),
+    "afl_mnist_backdoor_train": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _d, _i, _i, _vp]),
+    "afl_mnist_backdoor_test": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
 }
 
 _lib = None

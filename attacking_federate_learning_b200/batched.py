@@ -441,6 +441,10 @@ class DeviceRound:
     `alie`, a defence, `attack_metrics` and `_device.momentum_step`) can be captured with `torch.cuda.graph` and
     replayed.  Each method's result is the host-parameter call's on the same values, bit for bit.
 
+    `lr` (float64 [B]) is the backdoor crafting's per-problem client learning rate: `backdoor_start` and
+    `backdoor_finish` are `backdoor_rows` around the caller's training of the malicious networks (in a sweep,
+    `afl_mnist_backdoor_train`), with f, z and lr read on the device.
+
     Per-problem checks run on the device.  A problem that fails one gets its first error code in `status` (int32 [B],
     sticky until `clear_status`) and runs on a safe row (rows_b = N, users_count_b = N, f_b = 0), so its outputs are
     not the reference's; `raise_for_status` (the one call that synchronises) raises what the host-parameter call would:
@@ -484,6 +488,7 @@ class DeviceRound:
         self.z = torch.zeros(B, dtype=torch.float64, device=dev)
         self.rows = torch.full((B,), N, dtype=torch.int32, device=dev) if rows else None
         self.users_count = torch.full((B,), N, dtype=torch.int32, device=dev) if per_problem_users_count else None
+        self.lr = torch.zeros(B, dtype=torch.float64, device=dev)
         self.status = torch.zeros(B, dtype=torch.int32, device=dev)
         L = nat.lib()
         rule_bytes = L.afl_batched_large_dev_workspace_bytes if large else L.afl_batched_rows_workspace_bytes
@@ -498,6 +503,8 @@ class DeviceRound:
         self.krum_rows = torch.empty((B, D), dtype=users_grads.dtype, device=dev)
         self.selection = torch.empty((B, N), dtype=torch.int32, device=dev)
         self._problems = torch.arange(B, dtype=torch.int64, device=dev)
+        self.initial = None                              # backdoor_start's [B, D], allocated by its first call
+        self._initial_used = None                        # the initial the last backdoor_start wrote
 
     @staticmethod
     def _ptr(t):
@@ -525,6 +532,52 @@ class DeviceRound:
                    self.crafted.data_ptr(), self.G.data_ptr(), self._bs, self._ld, self._ws.data_ptr(), self._ws.numel(),
                    self.status.data_ptr(), _stream_ptr(self.G))
         return self.crafted, self.mu, self.sigma
+
+    def backdoor_start(self, original_params, initial=None):
+        """`backdoor_rows` up to the training, with the device f, z and lr (float64 [B]): returns (mu, sigma, initial),
+        fp32 [B, D], initial_b = w_b - lr_b * mu_b (w: original_params, fp32 CUDA [D] or [B, D]).  `initial` (fp32 [B, D],
+        contiguous) receives it when given; otherwise `self.initial` does.  A problem with f_b < 0 or f_b > N is flagged
+        (ValueError) and runs with f_b = 0.  The problems that attack, f_b > 0 and z_b != 0 with a clear status, are
+        the ones `afl_mnist_backdoor_train` trains."""
+        w = original_params
+        if not (isinstance(w, torch.Tensor) and w.device == self.device and w.dtype == torch.float32
+                and tuple(w.shape) in ((self.D,), (self.B, self.D)) and w.stride(-1) == 1
+                and (w.dim() == 1 or w.stride(0) >= self.D)):
+            raise ValueError(f"original_params: expected a float32 tensor of shape ({self.D},) or ({self.B}, {self.D}) "
+                             f"with unit column stride on {self.device}")
+        if initial is None:
+            if self.initial is None:
+                self.initial = torch.empty((self.B, self.D), dtype=torch.float32, device=self.device)
+            initial = self.initial
+        elif not (initial.device == self.device and initial.dtype == torch.float32 and initial.is_contiguous()
+                  and tuple(initial.shape) == (self.B, self.D)):
+            raise ValueError(f"initial: expected a contiguous float32 tensor of shape ({self.B}, {self.D})")
+        self._call(nat.lib().afl_backdoor_start_batched_dev, self.G.data_ptr(), self.B, self._bs, self.N, self.D,
+                   self._ld, self._code, self.f.data_ptr(), self.z.data_ptr(), self.lr.data_ptr(), w.data_ptr(),
+                   w.stride(0) if w.dim() == 2 else 0, self.mu.data_ptr(), self.sigma.data_ptr(), initial.data_ptr(),
+                   self._ws.data_ptr(), self._ws.numel(), self.status.data_ptr(), _stream_ptr(self.G))
+        self._initial_used = initial
+        return self.mu, self.sigma, initial
+
+    def backdoor_finish(self, mal):
+        """`backdoor_rows` after the training: returns crafted (fp32 [B, D]) from the last backdoor_start's mu, sigma
+        and initial and the trained parameters `mal` (fp32 [B, D], rows read only for the problems that attack), and
+        writes it over rows 0..f_b-1 of those problems.  Takes the f, z and lr backdoor_start took.  fp32 client
+        matrices only (a 16-bit one needs the host-parameter `backdoor_rows`)."""
+        if self._initial_used is None:
+            raise RuntimeError("DeviceRound.backdoor_finish: call backdoor_start first")
+        if self.G.dtype != torch.float32:
+            raise TypeError("DeviceRound.backdoor_finish writes fp32 client matrices only")
+        if not (isinstance(mal, torch.Tensor) and mal.device == self.device and mal.dtype == torch.float32
+                and tuple(mal.shape) == (self.B, self.D) and mal.stride(1) == 1
+                and (self.B == 1 or mal.stride(0) >= self.D)):
+            raise ValueError(f"mal: expected a float32 tensor of shape ({self.B}, {self.D}) on {self.device}")
+        self._call(nat.lib().afl_backdoor_finish_batched_dev, self.B, self.N, self.D, self.f.data_ptr(),
+                   self.z.data_ptr(), self.lr.data_ptr(), self.mu.data_ptr(), self.sigma.data_ptr(),
+                   self._initial_used.data_ptr(), mal.data_ptr(), mal.stride(0), self.crafted.data_ptr(),
+                   self.G.data_ptr(), self._bs, self._ld, self._ws.data_ptr(), self._ws.numel(), self.status.data_ptr(),
+                   _stream_ptr(self.G))
+        return self.crafted
 
     def krum(self, return_index=False):
         """`krum`: the device int32 [B] indices, or the winning rows [B, D] in G's dtype.  Index -1 (no eligible user)

@@ -1324,6 +1324,77 @@ static int alie_batched_dev(const void* G, int batch, int64_t batch_stride, int 
                                     batch_stride, d, bcast_batch_stride, stream, a.table);
 }
 
+// The backdoor crafting's table from device arrays (afl_backdoor_start_batched_dev / _finish_batched_dev): backdoor_table's
+// row, with the host calls' count check per problem (f_b < 0 or f_b > n -> AFL_ERR_BAD_ARG, and the safe f_b = 0).
+__global__ void __launch_bounds__(128) backdoor_table_kernel(int batch, int n, const int* fs, const double* zs,
+                                                             const double* lrs, ProblemParams* table, int* status) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  int f = fs[b];
+  const int code = f < 0 || f > n ? AFL_ERR_BAD_ARG : AFL_OK;
+  if (code != AFL_OK) f = 0;
+  ProblemParams q{};
+  q.f = f;
+  q.z = static_cast<float>(zs[b]);
+  q.lr = static_cast<float>(lrs[b]);
+  q.write = f > 0 && zs[b] != 0.0;                      // malicious.py:20-21: z == 0 computes the statistics only
+  table[b] = q;
+  if (code != AFL_OK && status[b] == AFL_OK) status[b] = code;
+}
+
+static int backdoor_table_dev(const char* who, int batch, int n, const int* fs, const double* zs, const double* lrs,
+                              void* ws, size_t ws_bytes, int* status, cudaStream_t stream) {
+  if (!zs || !lrs) { set_error("%s: the per-problem attack strengths or learning rates are NULL", who); return AFL_ERR_BAD_ARG; }
+  int rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch));
+  if (rc) return rc;
+  backdoor_table_kernel<<<static_cast<unsigned>((batch + 127) / 128), 128, 0, stream>>>(
+      batch, n, fs, zs, lrs, static_cast<ProblemParams*>(ws), status);
+  AFL_LAUNCH_CHECK("backdoor_table_kernel");
+  return AFL_OK;
+}
+
+// afl_backdoor_start_batched with device arrays: n bounds every f_b (the host call's fmax).
+static int backdoor_start_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
+                              const int* fs, const double* zs, const double* lrs, const float* w, int64_t w_batch_stride,
+                              float* mu_out, float* sigma_out, float* initial_out, void* ws, size_t ws_bytes,
+                              int* status, cudaStream_t stream) {
+  const char* who = "afl_backdoor_start_batched_dev";
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
+  if (rc) return rc;
+  if (!w || !mu_out || !sigma_out || !initial_out) { set_error("%s: w and every output are required", who); return AFL_ERR_BAD_ARG; }
+  if (w_batch_stride < 0 || (w_batch_stride > 0 && w_batch_stride < d)) {
+    set_error("%s: w_batch_stride %lld must be 0 (one shared w) or >= d", who, static_cast<long long>(w_batch_stride));
+    return AFL_ERR_BAD_ARG;
+  }
+  if ((rc = backdoor_table_dev(who, batch, n, fs, zs, lrs, ws, ws_bytes, status, stream))) return rc;
+  return colstats::backdoor_start(G, n, d, ld, dtype, batch, batch_stride, static_cast<const ProblemParams*>(ws), w,
+                                  w_batch_stride, mu_out, sigma_out, initial_out, stream);
+}
+
+// afl_backdoor_finish_batched with device arrays; n bounds every f_b, so it also bounds the rows bcast_rows receives.
+static int backdoor_finish_dev(int batch, int n, int64_t d, const int* fs, const double* zs, const double* lrs,
+                               const float* mu, const float* sigma, const float* initial, const float* mal,
+                               int64_t mal_batch_stride, float* crafted_out, float* bcast_rows,
+                               int64_t bcast_batch_stride, int64_t bcast_ld, void* ws, size_t ws_bytes, int* status,
+                               cudaStream_t stream) {
+  const char* who = "afl_backdoor_finish_batched_dev";
+  if (!mu || !sigma || !initial || !mal || !crafted_out || d < 1 || n < 1) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
+  if (batch < 1) { set_error("%s: batch must be >= 1 (got %d)", who, batch); return AFL_ERR_BAD_ARG; }
+  if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
+  if (batch > 1 && mal_batch_stride < d) {
+    set_error("%s: mal_batch_stride %lld makes problems overlap", who, static_cast<long long>(mal_batch_stride));
+    return AFL_ERR_BAD_ARG;
+  }
+  if (bcast_rows && (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(n - 1) * bcast_ld + d))) {
+    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  int rc = backdoor_table_dev(who, batch, n, fs, zs, lrs, ws, ws_bytes, status, stream);
+  if (rc) return rc;
+  return colstats::backdoor_finish(batch, d, static_cast<const ProblemParams*>(ws), mu, sigma, initial, mal,
+                                   mal_batch_stride, crafted_out, bcast_rows, bcast_batch_stride, bcast_ld, stream);
+}
+
 // afl_attack_metrics_batched_rows (rows != NULL) or _each with device arrays.
 static int attack_metrics_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
                               const int* rows, const int* fs, const float* agg, const int* idx, const int* sel,
@@ -1669,6 +1740,24 @@ int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_strid
   return attack_metrics_dev(G, batch, batch_stride, n, d, ld, dtype, rows, corrupted_counts, agg, idx, sel, sel_ld,
                             dev_out, sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
                             status, static_cast<cudaStream_t>(stream));
+}
+
+int afl_backdoor_start_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                   int dtype, const int* f, const double* z, const double* lr, const float* w,
+                                   int64_t w_batch_stride, float* mu_out, float* sigma_out, float* initial_out,
+                                   void* workspace, size_t workspace_bytes, int* status, void* stream) {
+  return backdoor_start_dev(G, batch, batch_stride, n, d, ld, dtype, f, z, lr, w, w_batch_stride, mu_out, sigma_out,
+                            initial_out, workspace, workspace_bytes, status, static_cast<cudaStream_t>(stream));
+}
+
+int afl_backdoor_finish_batched_dev(int batch, int n, int64_t d, const int* f, const double* z, const double* lr,
+                                    const float* mu, const float* sigma, const float* initial, const float* mal,
+                                    int64_t mal_batch_stride, float* crafted_out, float* bcast_rows,
+                                    int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                                    size_t workspace_bytes, int* status, void* stream) {
+  return backdoor_finish_dev(batch, n, d, f, z, lr, mu, sigma, initial, mal, mal_batch_stride, crafted_out, bcast_rows,
+                             bcast_batch_stride, bcast_ld, workspace, workspace_bytes, status,
+                             static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -25,7 +25,8 @@ leave the device.  The training simulation itself is not part of the accelerated
 
 A grid of these experiments (defence x z x malicious share x users x seed) runs as one batch in `sweep.run` / `python -m
 attacking_federate_learning_b200.sweep`: each experiment starts from `experiment_setup`'s data and weights, as here,
-and the client gradients of every experiment come from one CUDA kernel instead of this file's per-client autograd.
+and the client gradients of every experiment come from one CUDA kernel instead of this file's per-client autograd (and,
+with -b, the attacker's training of every backdoor experiment from another, on `backdoor_set`'s data).
 """
 from __future__ import annotations
 
@@ -111,6 +112,20 @@ class Client:
         self.grads = out_row
 
 
+def backdoor_set(backdoor, x, y, seed=0, batch_size=200):
+    """BackdoorTrainer's backdoor data (x, y) from the training set (x, y).  backdoor='pattern' (backdoor.py:37-42,
+    47-50): rows r::u with u = max(len(x) // batch_size // 10, 1) and r = default_rng(seed).integers(u), the 5x5 corner
+    of the 28x28 view set to 2.8, every label 0; backdoor = 1, 2 or 3 (backdoor.py:30-35): training row backdoor - 1,
+    labelled (y + 1) % 5."""
+    if backdoor == 'pattern':
+        u = max(len(x) // batch_size // 10, 1)
+        x = x[int(np.random.default_rng(seed).integers(u))::u].clone()
+        x.view(-1, 28, 28)[:, :5, :5] = 2.8
+        return x, torch.zeros_like(y[:len(x)])
+    i = int(backdoor) - 1
+    return x[i:i + 1], (y[i:i + 1] + 1) % 5
+
+
 class BackdoorTrainer:
     """backdoor.py:13-159 on the synthetic problem: the attacker's own network, trained from the starting point the
     crafting hands it towards the backdoor, and tested on the backdoor data.  backdoor='pattern': a shard of the
@@ -121,15 +136,7 @@ class BackdoorTrainer:
         self.backdoor, self.alpha, self.num_epochs, self.layout, self.my_print = backdoor, alpha, num_epochs, layout, my_print
         self.batch_size = batch_size
         self.net = MnistNet().to(device)
-        if backdoor == 'pattern':                                         # backdoor.py:37-42, 47-50
-            u = max(len(x) // batch_size // 10, 1)
-            x = x[int(np.random.default_rng(seed).integers(u))::u].clone()
-            x.view(-1, 28, 28)[:, :5, :5] = 2.8
-            y = torch.zeros_like(y[:len(x)])
-        else:                                                             # backdoor.py:30-35
-            i = int(backdoor) - 1
-            x, y = x[i:i + 1], (y[i:i + 1] + 1) % 5
-        self.x, self.y = x, y
+        self.x, self.y = backdoor_set(backdoor, x, y, seed, batch_size)
 
     def test(self, tag, to_print=True):                                   # backdoor.py:67-102
         loss, correct = 0.0, 0

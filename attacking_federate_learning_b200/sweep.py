@@ -1,32 +1,42 @@
 """Training sweeps: a grid of `harness.main` experiments trained side by side as one batch on the GPU.
 
-An experiment is `(defense, mal_prop, num_std, users_count, seed)`, what main.py:104-131 takes (without the backdoor).
-Experiment b starts from exactly the data and weights `harness.main(mal_prop, num_std, defense, users_count,
-seed=seed)` starts from (`harness.experiment_setup`) and runs main.py's epoch loop (main.py:64-71, server.py:86-90):
+An experiment is `(defense, mal_prop, num_std, users_count, seed[, backdoor])`, what main.py:104-131 takes: a drift
+experiment (ALIE) is the 5-tuple, a backdoor experiment (`-b pattern|1|2|3`) adds 'pattern', 1, 2 or 3.  Experiment b
+starts from exactly the data and weights `harness.main(mal_prop, num_std, defense, users_count, seed=seed,
+backdoor=backdoor)` starts from (`harness.experiment_setup`) and runs main.py's epoch loop (main.py:64-71,
+server.py:86-90):
 
   1. every client's MnistNet gradient on its minibatch (user.py:76-92), for every experiment in one launch of the
      client-gradient kernel (C ABI `afl_mnist_client_grads`), written straight into the experiment's rows of one
      [B, N_max, ld] client matrix;
-  2. per defence, on the contiguous slice of experiments that use it (`batched.DeviceRound` with the experiments' own
-     f_b = int(mal_prop * n_b), z_b and row counts): ALIE on rows 0..f_b-1, the rule, and the server's momentum step on
-     the slice's [B_r, D] weights at the base learning rate (server.py:89);
+  2. per (defence, attack), on the contiguous slice of experiments that use it (`batched.DeviceRound` with the
+     experiments' own f_b = int(mal_prop * n_b), z_b and row counts): the attack on rows 0..f_b-1, the rule, and the
+     server's momentum step on the slice's [B_r, D] weights at the base learning rate (server.py:89).  The drift attack
+     is ALIE.  The backdoor attack is `DeviceRound.backdoor_start` at lr_t = learning_rate * fading_rate / (epoch +
+     fading_rate) (server.py:50-52, float64 on the device from the epoch counter), then one launch of the trainer
+     kernel (C ABI `afl_mnist_backdoor_train`, harness.BackdoorTrainer.train) for every backdoor experiment of the
+     batch, then `DeviceRound.backdoor_finish`;
   3. the device epoch counter advances (the kernel reads it, so a replayed graph moves every client's minibatch on);
   4. every `test_step` epochs and at the last epoch, every experiment's test loss and accuracy (`afl_mnist_evaluate`,
-     harness.main's test loop) into the next slot of a device table.
+     harness.main's test loop) into the next slot of a device table, and every backdoor experiment's backdoor test
+     (`afl_mnist_backdoor_test`, main.py:91-95's 'POST') into the same slot of its own tables.
 
 Nothing synchronises the host until the run ends.  With capture=True epoch 0 runs eagerly and the later epochs replay
 a captured training epoch and test epoch; both paths give the same bits.  A client's gradient depends only on its own
 weights and rows, so an experiment's trajectory does not depend on which other experiments share its batch (the
 Krum and Bulyan distance tables aside, whose split count follows the batch unless AFL_GRAM_SPLITS pins it).  A
 failure that only the data can show (a Bulyan round with no eligible user) lands in the rule's `DeviceRound.status`:
-that experiment is reported as failed with the error `raise_for_status` gives, and the others complete.
+that experiment is reported as failed with the error `raise_for_status` gives, and the others complete.  So is a
+backdoor experiment whose malicious training meets a NaN loss: Exception('...: Got nan loss'), as backdoor.py raises.
 
 Outputs per experiment: the accuracy list and the CSV `harness.main` writes (np.savetxt(..., delimiter=',') in
 out_dir/logs, with `_seed_<s>` before `.csv` so that seeds do not overwrite one another), and one summary CSV with the
-parameters, max and final accuracy and status.  No checkpoint is written: main.py's checkpoint path has no experiment
+parameters, max and final accuracy and status (and, when the run has a backdoor experiment, the backdoor and its max
+and final backdoor accuracy).  No checkpoint is written: main.py's checkpoint path has no experiment
 key, so the experiments of a batch would overwrite one file.
 
     python -m attacking_federate_learning_b200.sweep -d Krum TrimmedMean -z 0.5 1.5 -m 0.1 0.24 -n 10 --seeds 0 1 -e 30
+    python -m attacking_federate_learning_b200.sweep -d Krum NoDefense -z 1.0 -b No pattern 1 --seeds 0 1 -e 30
 """
 from __future__ import annotations
 
@@ -34,7 +44,7 @@ import argparse
 import csv as _csv
 import itertools
 import os
-from typing import NamedTuple
+from operator import itemgetter
 
 import numpy as np
 import torch
@@ -48,19 +58,47 @@ from .defences import DefenseTypes
 RULES = (DefenseTypes.Krum, DefenseTypes.Bulyan, DefenseTypes.TrimmedMean, DefenseTypes.NoDefense)
 MAX_USERS = batched.MAX_CLIENTS          # clients per experiment (DeviceRound with large=True)
 MAX_BATCH_SIZE = 128                     # minibatch rows of the client-gradient kernel
+BACKDOOR_BATCH = 200                     # BackdoorTrainer's minibatch and test batch (the trainer kernel's limit)
 SUMMARY = 'sweep_summary.csv'
 
 
-class Experiment(NamedTuple):
-    defense: str
-    mal_prop: float
-    num_std: float
-    users_count: int
-    seed: int
+class Experiment(tuple):
+    """(defense, mal_prop, num_std, users_count, seed[, backdoor]): a drift experiment (backdoor False) is the 5-tuple,
+    so it equals, prints and writes as before; a backdoor experiment carries 'pattern', 1, 2 or 3 as a sixth element."""
+    __slots__ = ()
+    _fields = ('defense', 'mal_prop', 'num_std', 'users_count', 'seed')     # a drift experiment's
+
+    def __new__(cls, defense, mal_prop, num_std, users_count, seed, backdoor=False):
+        t = (defense, mal_prop, num_std, users_count, seed)
+        return tuple.__new__(cls, t if backdoor is False else t + (backdoor,))
+
+    def __getnewargs__(self):
+        return tuple(self)
+
+    def __repr__(self):
+        return 'Experiment(' + ', '.join(f'{n}={v!r}' for n, v in zip(self._fields + ('backdoor',), self)) + ')'
+
+    defense, mal_prop, num_std, users_count, seed = (property(itemgetter(i)) for i in range(5))
+
+    @property
+    def backdoor(self):
+        return self[5] if len(self) > 5 else False
 
     @property
     def corrupted_count(self):
         return int(self.mal_prop * self.users_count)                      # main.py:21
+
+
+def normalise_backdoor(bd):
+    """main.py's -b value as harness.main takes it: False (also 'No'), 'pattern' or the sample 1, 2 or 3 (also '1'..'3').
+    Raises ValueError for anything else."""
+    if bd is False or (isinstance(bd, str) and bd == 'No'):
+        return False
+    if isinstance(bd, str) and bd == 'pattern':
+        return bd
+    if isinstance(bd, (str, int, np.integer)) and not isinstance(bd, bool) and str(bd) in ('1', '2', '3'):
+        return int(bd)
+    raise ValueError(f"unknown backdoor {bd!r} (expected False, 'pattern', 1, 2 or 3)")
 
 
 def minibatch(n_train, users_count, user, batch_size, epoch):
@@ -74,7 +112,12 @@ def minibatch(n_train, users_count, user, batch_size, epoch):
 def check(exp, batch_size=83, train_size=20000):
     """Raise what main.py would raise for this experiment at its first `defend` (AssertionError for the reference's
     asserts), or for what the sweep's kernels do not take.  Returns the normalised Experiment."""
-    exp = Experiment(str(exp[0]), float(exp[1]), float(exp[2]), int(exp[3]), int(exp[4]))
+    if len(exp) not in (5, 6):
+        raise ValueError(f"{exp}: an experiment has 5 or 6 elements")
+    exp = Experiment(str(exp[0]), float(exp[1]), float(exp[2]), int(exp[3]), int(exp[4]),
+                     normalise_backdoor(exp[5]) if len(exp) == 6 else False)
+    if exp.backdoor not in (False, 'pattern') and exp.backdoor > train_size:
+        raise ValueError(f"{exp}: backdoor sample {exp.backdoor} lies past the training set ({train_size} rows)")
     if exp.defense not in RULES:
         raise KeyError(f"{exp}: unknown defence {exp.defense!r} (expected one of {', '.join(RULES)})")
     if not 1 <= exp.users_count <= MAX_USERS:
@@ -93,11 +136,14 @@ def check(exp, batch_size=83, train_size=20000):
     return exp
 
 
-def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000):
-    """The Cartesian grid (defence-major) as (kept experiments, [(experiment, rejection), ...]): a cell main.py
-    would reject is dropped with the exception `check` raises for it."""
+def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000, backdoors=(False,)):
+    """The Cartesian grid (defence-major, backdoor-minor) as (kept experiments, [(experiment, rejection), ...]): a cell
+    main.py would reject is dropped with the exception `check` raises for it.  A drift cell (backdoor False) has 5
+    elements, a backdoor cell 6."""
     kept, dropped = [], []
-    for cell in itertools.product(defenses, mal_props, num_stds, users_counts, seeds):
+    for cell in itertools.product(defenses, mal_props, num_stds, users_counts, seeds, backdoors):
+        if cell[5] is False:
+            cell = cell[:5]
         try:
             kept.append(check(cell, batch_size, train_size))
         except (AssertionError, KeyError, ValueError, NotImplementedError) as e:
@@ -105,9 +151,9 @@ def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, trai
     return kept, dropped
 
 
-def csv_name(exp, learning_rate):
+def csv_name(exp, learning_rate, alpha=4):
     """harness.main's log name for this experiment, with `_seed_<s>` before `.csv`."""
-    name = harness.csv_name(exp.num_std, exp.defense, False, exp.mal_prop, exp.users_count, 4, learning_rate)
+    name = harness.csv_name(exp.num_std, exp.defense, exp.backdoor, exp.mal_prop, exp.users_count, alpha, learning_rate)
     return name[:-len('.csv')] + f'_seed_{exp.seed}.csv'
 
 
@@ -115,8 +161,40 @@ def test_epochs(epochs, test_step):
     return [e for e in range(epochs) if e % test_step == 0 or e == epochs - 1]
 
 
+def fading_lr(epoch, learning_rate, fading_rate):
+    """harness.main's client learning rate lr_t = learning_rate * fading_rate / (epoch + fading_rate) (server.py:50-52)
+    as float64 tensor arithmetic on `epoch` (an integer tensor), in the Python expression's order: one product, one
+    sum and one IEEE division, so each value is the harness's Python double."""
+    num = torch.full(epoch.shape, learning_rate * fading_rate, dtype=torch.float64, device=epoch.device)
+    return torch.div(num, epoch.to(torch.float64) + fading_rate)
+
+
+def backdoor_sets(specs):
+    """The trainer kernel's backdoor sets from [(backdoor, x_train, y_train, seed), ...]: harness.backdoor_set (what
+    BackdoorTrainer trains and tests on) per spec, as x fp32 [n_sets, max_len, 784] and y int64 [n_sets, max_len], each
+    set zero-padded to the longest, and set_len int32 [n_sets], on the training sets' device."""
+    sets = [harness.backdoor_set(bd, x, y, seed, BACKDOOR_BATCH) for bd, x, y, seed in specs]
+    dev, max_len = sets[0][0].device, max(len(x) for x, _ in sets)
+    xs = torch.zeros((len(sets), max_len, sets[0][0].shape[-1]), dtype=torch.float32, device=dev)
+    ys = torch.zeros((len(sets), max_len), dtype=torch.int64, device=dev)
+    for k, (x, y) in enumerate(sets):
+        xs[k, :len(x)] = x
+        ys[k, :len(y)] = y
+    return xs, ys, torch.tensor([len(x) for x, _ in sets], dtype=torch.int32, device=dev)
+
+
+def summary_header(with_backdoor):
+    """The summary CSV's columns; the backdoor ones only when the run has a backdoor experiment."""
+    bd = with_backdoor
+    return list(Experiment._fields) + (['backdoor'] if bd else []) + ['max_accuracy', 'final_accuracy'] + \
+        (['max_backdoor_accuracy', 'final_backdoor_accuracy'] if bd else []) + ['status']
+
+
 def status_error(code, name):
-    """The exception DeviceRound.raise_for_status raises for a status code, naming the experiment."""
+    """The exception DeviceRound.raise_for_status raises for a status code, naming the experiment; for the backdoor
+    trainer's NaN codes, the Exception backdoor.py raises."""
+    if code in (nat.AFL_ERR_NAN_LOSS, nat.AFL_ERR_NAN_DIST_LOSS):
+        return Exception(f"{name}: Got nan {'dist loss' if code == nat.AFL_ERR_NAN_DIST_LOSS else 'loss'}")
     if code == nat.AFL_ERR_NO_WINNER:
         e = KeyError(-1)
         e.add_note(f"{name}: a Bulyan selection round found no eligible user (defences.py:66)")
@@ -130,22 +208,29 @@ class Sweep:
     directly: `train_epoch()` and `test_epoch()` enqueue one epoch's work, `step(epoch)` runs epoch `epoch` (captured
     after epoch 0 when capture=True), `results()` synchronises and reads the tables back.
 
-    Batch order: experiments grouped by defence in RULES order, each group in the given order; `order[i]` is the
-    position in `experiments` of batch problem i.  W, V: fp32 [B, D] weights and velocity; G: the [B, N_max, ld]
-    client matrix (ld a multiple of 32, as AggregationServer pads); `rounds`: {defence: (slice, DeviceRound)}."""
+    Batch order: the drift experiments grouped by defence in RULES order, then the backdoor experiments grouped the
+    same way, each group in the given order; `order[i]` is the position in `experiments` of batch problem i.  W, V:
+    fp32 [B, D] weights and velocity; G: the [B, N_max, ld] client matrix (ld a multiple of 32, as AggregationServer
+    pads); `rounds`: {defence: (slice, DeviceRound)} of the drift groups, `backdoor_rounds` the same for the backdoor
+    groups, which occupy batch problems `bd0`..B-1.  Their DeviceRounds hold views of one f, z, lr and status over
+    those problems, so the trainer reads every backdoor experiment in one launch."""
 
     def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000,
-                 test_size=4000, test_step=5, capture=True, device='cuda'):
+                 test_size=4000, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000):
         exps = [check(e, batch_size, train_size) for e in experiments]
         if not exps:
             raise ValueError("sweep: no experiment")
         if epochs < 1 or test_step < 1 or test_size < 1:
             raise ValueError(f"sweep: epochs, test_step and test_size must be >= 1 (got {epochs}, {test_step}, "
                              f"{test_size})")
-        self.order = [i for r in RULES for i, e in enumerate(exps) if e.defense == r]
+        if mal_epochs < 0 or fading_rate <= 0:
+            raise ValueError(f"sweep: mal_epochs must be >= 0 and fading_rate > 0 (got {mal_epochs}, {fading_rate})")
+        self.order = [i for bd in (False, True) for r in RULES for i, e in enumerate(exps)
+                      if e.defense == r and (e.backdoor is not False) == bd]
         self.experiments = [exps[i] for i in self.order]
         self.epochs, self.learning_rate, self.momentum = epochs, learning_rate, momentum
         self.batch_size, self.train_size, self.test_size, self.test_step = batch_size, train_size, test_size, test_step
+        self.alpha, self.mal_epochs, self.fading_rate = alpha, mal_epochs, fading_rate
         self.capture = capture
         dev = self.device = torch.device(device)
         seeds = list(dict.fromkeys(e.seed for e in self.experiments))
@@ -175,19 +260,46 @@ class Sweep:
         L = nat.lib()
         self._eval_ws = torch.empty(max(L.afl_mnist_evaluate_workspace_bytes(B, test_size, batch_size), 256),
                                     dtype=torch.uint8, device=dev)
-        self.rounds = {}
+        self.bd0 = sum(e.backdoor is False for e in self.experiments)
+        self._setup_backdoor(xtr, ytr, seeds)
+        self.rounds, self.backdoor_rounds = {}, {}
         for r in RULES:
-            idx = [i for i, e in enumerate(self.experiments) if e.defense == r]
-            if not idx:
-                continue
-            sl = slice(idx[0], idx[-1] + 1)
-            rnd = batched.DeviceRound(self.G[sl], rows=True, rules=(r,), large=self.N > batched.ONE_TILE)
-            sub = self.experiments[sl]
-            rnd.f.copy_(torch.tensor([e.corrupted_count for e in sub], dtype=torch.int32))
-            rnd.z.copy_(torch.tensor([e.num_std for e in sub], dtype=torch.float64))
-            rnd.rows.copy_(torch.tensor([e.users_count for e in sub], dtype=torch.int32))
-            self.rounds[r] = (sl, rnd)
+            for bd, rounds in ((False, self.rounds), (True, self.backdoor_rounds)):
+                idx = [i for i, e in enumerate(self.experiments) if e.defense == r and (e.backdoor is not False) == bd]
+                if not idx:
+                    continue
+                sl = slice(idx[0], idx[-1] + 1)
+                rnd = batched.DeviceRound(self.G[sl], rows=True, rules=(r,), large=self.N > batched.ONE_TILE)
+                if bd:                                                    # views of the batch-wide backdoor arrays
+                    k = slice(sl.start - self.bd0, sl.stop - self.bd0)
+                    rnd.f, rnd.z, rnd.lr, rnd.status = self._bd_f[k], self._bd_z[k], self._bd_lr[k], self._bd_status[k]
+                sub = self.experiments[sl]
+                rnd.f.copy_(torch.tensor([e.corrupted_count for e in sub], dtype=torch.int32))
+                rnd.z.copy_(torch.tensor([e.num_std for e in sub], dtype=torch.float64))
+                rnd.rows.copy_(torch.tensor([e.users_count for e in sub], dtype=torch.int32))
+                rounds[r] = (sl, rnd)
         self._graphs = None
+
+    def _setup_backdoor(self, xtr, ytr, seeds):
+        """The backdoor experiments' sets (harness.backdoor_set, one per (backdoor, seed), padded to the longest),
+        their trainer state and their backdoor-test tables."""
+        bds = self.experiments[self.bd0:]
+        self.n_backdoor = nb = len(bds)
+        if not nb:
+            return
+        dev, i32 = self.device, dict(dtype=torch.int32, device=self.device)
+        keys = list(dict.fromkeys((e.backdoor, e.seed) for e in bds))
+        self.bd_x, self.bd_y, self.bd_len = backdoor_sets(
+            [(bd, xtr[seeds.index(s)], ytr[seeds.index(s)], s) for bd, s in keys])
+        self.bd_index = torch.tensor([keys.index((e.backdoor, e.seed)) for e in bds], **i32)
+        self._bd_f = torch.zeros(nb, **i32)
+        self._bd_z = torch.zeros(nb, dtype=torch.float64, device=dev)
+        self._bd_lr = torch.zeros(nb, dtype=torch.float64, device=dev)
+        self._bd_status = torch.zeros(nb, **i32)
+        self.bd_initial = torch.empty((nb, self.D), dtype=torch.float32, device=dev)
+        self.bd_mal = torch.empty((nb, self.D), dtype=torch.float32, device=dev)
+        self.bd_loss_sum = torch.zeros((self.n_tests, nb), dtype=torch.float64, device=dev)
+        self.bd_correct = torch.zeros((self.n_tests, nb), **i32)
 
     def client_grads(self):
         """Step 1: every client's gradient into G at the current device epoch."""
@@ -199,15 +311,40 @@ class Sweep:
                 self.batch_size, self.epoch_counter.data_ptr(), G.data_ptr(), G.stride(0), G.stride(1),
                 torch.cuda.current_stream(self.device).cuda_stream))
 
+    def backdoor_train(self, k=None):
+        """The malicious networks of the backdoor experiments bd0 + k (all of them by default) in one launch
+        (BackdoorTrainer.train), from bd_initial[k] into bd_mal[k]."""
+        k = slice(0, self.n_backdoor) if k is None else k
+        with torch.cuda.device(self.device):
+            nat.check(nat.lib().afl_mnist_backdoor_train(
+                self.bd_initial[k].data_ptr(), self.bd_mal[k].data_ptr(), k.stop - k.start, self.D,
+                self.bd_x.data_ptr(), self.bd_y.data_ptr(), self.bd_x.shape[0], self.bd_x.shape[1],
+                self.bd_len.data_ptr(), self.bd_index[k].data_ptr(), self._bd_f[k].data_ptr(), self._bd_z[k].data_ptr(),
+                self._bd_status[k].data_ptr(), float(self.alpha), self.mal_epochs, BACKDOOR_BATCH,
+                torch.cuda.current_stream(self.device).cuda_stream))
+
+    def _defend(self, r, sl, rnd):
+        agg = {DefenseTypes.Krum: rnd.krum, DefenseTypes.Bulyan: rnd.bulyan,
+               DefenseTypes.TrimmedMean: rnd.trimmed_mean, DefenseTypes.NoDefense: rnd.no_defense}[r]()
+        momentum_step(self.W[sl], self.V[sl], agg, self.momentum, self.learning_rate)
+
     def aggregate(self, rule=None):
-        """Step 2 for one defence (every defence when rule is None): ALIE, the rule and the momentum step."""
+        """Step 2 for one defence (every defence when rule is None): the attack, the rule and the momentum step."""
         for r, (sl, rnd) in self.rounds.items():
             if rule is not None and r != rule:
                 continue
             rnd.alie()
-            agg = {DefenseTypes.Krum: rnd.krum, DefenseTypes.Bulyan: rnd.bulyan,
-                   DefenseTypes.TrimmedMean: rnd.trimmed_mean, DefenseTypes.NoDefense: rnd.no_defense}[r]()
-            momentum_step(self.W[sl], self.V[sl], agg, self.momentum, self.learning_rate)
+            self._defend(r, sl, rnd)
+        bd = [(r, sl, rnd) for r, (sl, rnd) in self.backdoor_rounds.items() if rule is None or r == rule]
+        if not bd:
+            return
+        self._bd_lr.copy_(fading_lr(self.epoch_counter, self.learning_rate, self.fading_rate).expand(self.n_backdoor))
+        for r, sl, rnd in bd:
+            rnd.backdoor_start(self.W[sl], initial=self.bd_initial[sl.start - self.bd0:sl.stop - self.bd0])
+        self.backdoor_train(None if rule is None else slice(bd[0][1].start - self.bd0, bd[0][1].stop - self.bd0))
+        for r, sl, rnd in bd:
+            rnd.backdoor_finish(self.bd_mal[sl.start - self.bd0:sl.stop - self.bd0])
+            self._defend(r, sl, rnd)
 
     def train_epoch(self):
         self.client_grads()
@@ -215,13 +352,21 @@ class Sweep:
         self.epoch_counter.add_(1)
 
     def test_epoch(self):
-        """Step 4: every experiment's test loss sum and correct count into the next slot of the tables."""
+        """Step 4: every experiment's test loss sum and correct count into the next slot of the tables, and every
+        backdoor experiment's backdoor test into the same slot of its tables."""
+        stream = torch.cuda.current_stream(self.device).cuda_stream
         with torch.cuda.device(self.device):
             nat.check(nat.lib().afl_mnist_evaluate(
                 self.W.data_ptr(), self.B, self.D, self.x_test.data_ptr(), self.y_test.data_ptr(),
                 self.x_test.shape[0], self.test_size, self.data_index.data_ptr(), self.batch_size,
                 self.test_slot.data_ptr(), self.n_tests, self.loss_sum.data_ptr(), self.correct.data_ptr(),
-                self._eval_ws.data_ptr(), self._eval_ws.numel(), torch.cuda.current_stream(self.device).cuda_stream))
+                self._eval_ws.data_ptr(), self._eval_ws.numel(), stream))
+            if self.n_backdoor:
+                nat.check(nat.lib().afl_mnist_backdoor_test(
+                    self.W[self.bd0:].data_ptr(), self.n_backdoor, self.D, self.bd_x.data_ptr(), self.bd_y.data_ptr(),
+                    self.bd_x.shape[0], self.bd_x.shape[1], self.bd_len.data_ptr(), self.bd_index.data_ptr(),
+                    BACKDOOR_BATCH, self.test_slot.data_ptr(), self.n_tests, self.bd_loss_sum.data_ptr(),
+                    self.bd_correct.data_ptr(), stream))
         self.test_slot.add_(1)
 
     def is_test_epoch(self, epoch):
@@ -247,18 +392,24 @@ class Sweep:
             self._graphs[1].replay()
 
     def status(self):
-        """Per batch problem: 0, or the first error code its rule's DeviceRound flagged (synchronises)."""
+        """Per batch problem: 0, or the first error code its rule's DeviceRound flagged or the backdoor trainer set
+        (synchronises)."""
         st = torch.zeros(self.B, dtype=torch.int32, device=self.device)
-        for sl, rnd in self.rounds.values():
+        for sl, rnd in list(self.rounds.values()) + list(self.backdoor_rounds.values()):
             st[sl] = rnd.status
         return st.cpu().numpy()
 
     def results(self):
         """Synchronise and return, in the order of `experiments` as given, one dict per experiment: experiment,
-        accuracies, accuracies_epochs, losses (harness.main's test loss), error (None, or the exception)."""
+        accuracies, accuracies_epochs, losses (harness.main's test loss), error (None, or the exception), and for a
+        backdoor experiment backdoor_accuracies and backdoor_losses (BackdoorTrainer.test('POST') at each test epoch)."""
         st = self.status()
         correct = self.correct.cpu().numpy()
         loss = self.loss_sum.cpu().numpy()
+        if self.n_backdoor:
+            bd_correct, bd_loss = self.bd_correct.cpu().numpy(), self.bd_loss_sum.cpu().numpy()
+            bd_len = self.bd_len.cpu().numpy()
+            bd_index = self.bd_index.cpu().numpy()
         epochs = test_epochs(self.epochs, self.test_step)
         out = [None] * self.B
         for i, (pos, e) in enumerate(zip(self.order, self.experiments)):
@@ -266,34 +417,45 @@ class Sweep:
             err = status_error(int(st[i]), f"experiment {tuple(e)}") if st[i] else None
             out[pos] = dict(experiment=e, accuracies=acc, accuracies_epochs=epochs,
                             losses=[float(loss[t, i]) / self.test_size for t in range(self.n_tests)], error=err)
+            if i >= self.bd0:
+                k = i - self.bd0
+                n = int(bd_len[bd_index[k]])
+                out[pos]['backdoor_accuracies'] = [100. * int(bd_correct[t, k]) / n for t in range(self.n_tests)]
+                out[pos]['backdoor_losses'] = [float(bd_loss[t, k]) / n for t in range(self.n_tests)]
         return out
 
 
 def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000, test_size=4000,
-        test_step=5, out_dir='.', capture=True, device='cuda'):
+        test_step=5, out_dir='.', capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000):
     """Train every experiment for `epochs` epochs as one batch; write each one's accuracy CSV and the summary CSV under
     out_dir/logs.  Returns `Sweep.results()` with `csv` (None for a failed experiment) added to each dict.  Raises
-    before any GPU work for an experiment main.py would reject (see `check`)."""
+    before any GPU work for an experiment main.py would reject (see `check`).  alpha, mal_epochs and fading_rate are
+    harness.main's (the backdoor experiments' malicious training and client learning rate)."""
     sw = Sweep(experiments, epochs, learning_rate, momentum, batch_size, train_size, test_size, test_step, capture,
-               device)
+               device, alpha, mal_epochs, fading_rate)
     with torch.cuda.device(sw.device):
         for epoch in range(epochs):
             sw.step(epoch)
     res = sw.results()
     logs = os.path.join(out_dir, 'logs')
     os.makedirs(logs, exist_ok=True)
+    with_bd = sw.n_backdoor > 0
     with open(os.path.join(logs, SUMMARY), 'w', newline='') as fh:
         w = _csv.writer(fh)
-        w.writerow(list(Experiment._fields) + ['max_accuracy', 'final_accuracy', 'status'])
+        w.writerow(summary_header(with_bd))
         for r in res:
             e = r['experiment']
             r['csv'] = None
+            head = list(e[:5]) + ([e.backdoor] if with_bd else [])
             if r['error'] is None:
-                r['csv'] = os.path.join(logs, csv_name(e, learning_rate))
+                r['csv'] = os.path.join(logs, csv_name(e, learning_rate, alpha))
                 np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
-                w.writerow(list(e) + [max(r['accuracies']), r['accuracies'][-1], 'ok'])
+                bd = r.get('backdoor_accuracies')
+                tail = ([max(bd), bd[-1]] if bd else ['', '']) if with_bd else []
+                w.writerow(head + [max(r['accuracies']), r['accuracies'][-1]] + tail + ['ok'])
             else:
-                w.writerow(list(e) + ['', '', f"failed: {type(r['error']).__name__}: {r['error']}"])
+                w.writerow(head + ['', ''] + (['', ''] if with_bd else []) +
+                           [f"failed: {type(r['error']).__name__}: {r['error']}"])
     return res
 
 
@@ -304,13 +466,15 @@ def main(argv=None):
     p.add_argument('-m', '--mal-prop', nargs='+', type=float, default=[0.24])
     p.add_argument('-n', '--users-count', nargs='+', type=int, default=[10])
     p.add_argument('--seeds', nargs='+', type=int, default=[0])
+    p.add_argument('-b', '--backdoor', nargs='+', default=['No'], choices=['No', 'pattern', '1', '2', '3'])
     p.add_argument('-e', '--epochs', type=int, default=300)
     p.add_argument('-c', '--batch_size', type=int, default=83)
     p.add_argument('-l', '--learning_rate', type=float, default=0.1)
     p.add_argument('--out-dir', default='.')
     p.add_argument('--no-capture', action='store_true')
     a = p.parse_args(argv)
-    kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size)
+    kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size,
+                         backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)])
     for cell, e in dropped:
         print(f"skipped {cell}: {type(e).__name__}: {e}")
     if not kept:
@@ -320,7 +484,10 @@ def main(argv=None):
     for r in res:
         e = r['experiment']
         if r['error'] is None:
-            print(f"{tuple(e)}: max accuracy {max(r['accuracies']):.2f}, final {r['accuracies'][-1]:.2f} -> {r['csv']}")
+            bd = r.get('backdoor_accuracies')
+            extra = f", backdoor max {max(bd):.2f}, final {bd[-1]:.2f}" if bd else ""
+            print(f"{tuple(e)}: max accuracy {max(r['accuracies']):.2f}, final {r['accuracies'][-1]:.2f}{extra} -> "
+                  f"{r['csv']}")
         else:
             print(f"{tuple(e)}: failed: {type(r['error']).__name__}: {r['error']}")
     return res

@@ -46,8 +46,10 @@ typedef enum afl_status {
   AFL_ERR_CUDA = 3,          /* a CUDA call failed; see afl_last_error()                          */
   AFL_ERR_UNSUPPORTED = 4,   /* dtype / size outside what the kernels implement                   */
   AFL_ERR_WORKSPACE = 5,     /* workspace too small                                               */
-  AFL_ERR_NO_WINNER = 6      /* a Bulyan round found no eligible user (NaN / >= 1e20 scores): the      */
+  AFL_ERR_NO_WINNER = 6,     /* a Bulyan round found no eligible user (NaN / >= 1e20 scores): the      */
                              /* reference raises KeyError(-1) at defences.py:66 (`distances.pop(-1)`)  */
+  AFL_ERR_NAN_LOSS = 7,      /* backdoor training: the minibatch loss is NaN ("Got nan loss")         */
+  AFL_ERR_NAN_DIST_LOSS = 8  /* backdoor training: the distance loss is NaN ("Got nan dist loss")     */
 } afl_status;
 
 typedef enum afl_dtype { AFL_F32 = 0, AFL_BF16 = 1, AFL_F16 = 2 } afl_dtype;
@@ -511,6 +513,24 @@ int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_strid
                                    float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* workspace,
                                    size_t workspace_bytes, int* status, void* stream);
 
+/* ---- device-parameter backdoor crafting: afl_backdoor_start_batched / _finish_batched with f (int32), z and lr
+ * (float64) as DEVICE arrays of `batch` values and a status array, as the other _dev calls take them.  The table is
+ * built on the device, the host calls' row field for field, so on the same values each result equals the host call's
+ * bit for bit.  n is the rows of a problem slot and bounds every f_b: f_b < 0 or f_b > n flags the problem with
+ * AFL_ERR_BAD_ARG in status[b] and runs it with f_b = 0 (NaN mu, sigma and crafted; no row read or written).  For the
+ * finish call n also bounds the rows bcast_rows receives: bcast_batch_stride >= (n - 1) * bcast_ld + d when batch > 1.
+ * Workspace: afl_batched_each_workspace_bytes("ALIE", batch, 1, d, dtype) bytes, 256-byte aligned.  Every host check
+ * is the host call's, plus status and f non-NULL; after them no call copies, synchronises or allocates. */
+int afl_backdoor_start_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                                   int dtype, const int* f, const double* z, const double* lr, const float* w,
+                                   int64_t w_batch_stride, float* mu_out, float* sigma_out, float* initial_out,
+                                   void* workspace, size_t workspace_bytes, int* status, void* stream);
+int afl_backdoor_finish_batched_dev(int batch, int n, int64_t d, const int* f, const double* z, const double* lr,
+                                    const float* mu, const float* sigma, const float* initial, const float* mal,
+                                    int64_t mal_batch_stride, float* crafted_out, float* bcast_rows,
+                                    int64_t bcast_batch_stride, int64_t bcast_ld, void* workspace,
+                                    size_t workspace_bytes, int* status, void* stream);
+
 /* ---- MnistNet client gradients and evaluation (csrc/client_grad.cu): the training half of a sweep epoch ----------
  * The model is the harness's MnistNet (data_sets.py:13-24), log_softmax(fc2(relu(fc1(x)))), its d = 79,510 parameters
  * in ParamLayout order (fc1.weight [100][784], fc1.bias, fc2.weight [10][100], fc2.bias).  weights: device fp32
@@ -544,6 +564,39 @@ size_t afl_mnist_evaluate_workspace_bytes(int batch, int n_test, int m);
 int afl_mnist_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                        int n_test, const int* data_index, int m, const int* slot_index, int n_slots, double* loss_sum,
                        int* correct, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- the backdoor attacker's MnistNet (csrc/backdoor_train.cu): the model half of a backdoor sweep epoch ----------
+ * Backdoor sets: x device fp32 [n_sets][max_len][784], y device int64 [n_sets][max_len], set_len device int32 [n_sets]
+ * (set s is its first set_len[s] rows); data_index (device int32 [batch]) picks problem b's set.  Minibatches and test
+ * batches are m rows (the last one shorter), 1 <= m <= 200.  One CTA per problem, fp32 FFMA throughout, no atomics and
+ * every sum in a fixed order, so a problem's result depends only on its own inputs, never on batch or the other
+ * problems.  The calls take no workspace and only enqueue work (no allocation, copy or synchronisation), so they can
+ * be captured in a CUDA graph.  Checked before any CUDA call: a NULL pointer, batch / n_sets / max_len / m < 1 ->
+ * AFL_ERR_BAD_ARG; d != 79,510, m > 200 or batch > 65535 -> AFL_ERR_UNSUPPORTED.
+ *
+ * afl_mnist_backdoor_train — harness.BackdoorTrainer.train (backdoor.py:108-159) for every problem that attacks:
+ * f[b] > 0, z[b] != 0 and status[b] == 0 (device arrays, read when the kernel runs; batched.backdoor_rows' condition).
+ * From p = p0 = initial[b] (device fp32 [batch][d]): if every row of the set is classified correctly (the BEFORE test),
+ * out[b] = initial[b] bit for bit; otherwise mal_epochs passes over the set, one SGD step per minibatch from a fresh
+ * optimiser: p <- p - 0.1 (g + 1e-4 p), g the gradient of NLLLoss(mean) + alpha * sum over the four tensors of
+ * MSELoss(p, p0) (the MSE term only when alpha > 0).  The trained vector goes to out[b] (device fp32 [batch][d], must
+ * not overlap initial).  A NaN distance loss (alpha > 0) or a NaN loss before a step sets status[b] to
+ * AFL_ERR_NAN_DIST_LOSS or AFL_ERR_NAN_LOSS and stops that problem (out[b] then holds the last step's parameters); a set
+ * index outside [0, n_sets) or a set length outside [1, max_len] sets AFL_ERR_BAD_ARG.  Any other problem's out[b] is
+ * neither read nor written.  mal_epochs < 0 or a NaN alpha -> AFL_ERR_BAD_ARG.
+ *
+ * afl_mnist_backdoor_test — BackdoorTrainer.test (backdoor.py:67-102; main.py:91-95's 'POST') at weights[b] (device
+ * fp32 [batch][d]) for every problem: loss_sum[slot][b] = the float64 sum of the batches' fp32 mean NLL (divide by the
+ * set length for the reported loss) and correct[slot][b] = the rows whose argmax (torch's: the first NaN, else the
+ * first maximum) is the label.  slot = *slot_index (device int32, read when the kernel runs); a slot outside
+ * [0, n_slots), or a problem whose set index or length is out of range, writes nothing.  loss_sum: device float64
+ * [n_slots][batch], correct: device int32 [n_slots][batch]; n_slots < 1 -> AFL_ERR_BAD_ARG. */
+int afl_mnist_backdoor_train(const float* initial, float* out, int batch, int64_t d, const float* x, const int64_t* y,
+                             int n_sets, int max_len, const int* set_len, const int* data_index, const int* f,
+                             const double* z, int* status, double alpha, int mal_epochs, int m, void* stream);
+int afl_mnist_backdoor_test(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                            int max_len, const int* set_len, const int* data_index, int m, const int* slot_index,
+                            int n_slots, double* loss_sum, int* correct, void* stream);
 
 #ifdef __cplusplus
 }

@@ -43,7 +43,10 @@ __device__ __forceinline__ Smem carve(float* base) {
   return s;
 }
 
-// Forward through relu(fc1): A[i][j] = max(sum_k X[row_i][k] W1[j][k] + b1[j], 0) for i < mb, j < 100.  Thread (tx, ty)
+// torch.relu: NaN stays NaN (fmaxf would turn it into 0).
+__device__ __forceinline__ float relu(float v) { return v > 0.f || v != v ? v : 0.f; }
+
+// Forward through relu(fc1): A[i][j] = relu(sum_k X[row_i][k] W1[j][k] + b1[j]) for i < mb, j < 100.  Thread (tx, ty)
 // owns hidden units tx + 16c and rows ty + 16r; each of its sums runs k = 0..783 in order, then adds the bias.
 template <int RT>
 __device__ __forceinline__ void forward_hidden(const float* __restrict__ xs, const float* __restrict__ w, int mb,
@@ -88,7 +91,7 @@ __device__ __forceinline__ void forward_hidden(const float* __restrict__ xs, con
 #pragma unroll
     for (int r = 0; r < RT; ++r) {
       const int i = ty + 16 * r;
-      if (i < mb) s.A[i * kLdA + j] = fmaxf(acc[r][c] + bj, 0.f);
+      if (i < mb) s.A[i * kLdA + j] = relu(acc[r][c] + bj);
     }
   }
 }
@@ -187,13 +190,14 @@ client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ 
     }
   }
   __syncthreads();
-  // delta1 = (delta2 W2) * (A > 0), in place of A (threshold_backward: zero where the pre-activation is <= 0)
+  // delta1 = delta2 W2 where A is not <= 0, in place of A (threshold_backward: zero where the ReLU output is <= 0, the
+  // gradient elsewhere, a NaN output included)
   for (int idx = threadIdx.x; idx < mb * kHid; idx += kThreads) {
     const int i = idx / kHid, j = idx % kHid;
     float d = 0.f;
 #pragma unroll
     for (int c = 0; c < kOut; ++c) d = fmaf(s.P[i * kOut + c], s.W2[c * kHid + j], d);
-    s.A[i * kLdA + j] = s.A[i * kLdA + j] > 0.f ? d : 0.f;
+    s.A[i * kLdA + j] = s.A[i * kLdA + j] <= 0.f ? 0.f : d;
   }
   __syncthreads();
   for (int j = threadIdx.x; j < kHid; j += kThreads) {

@@ -16,7 +16,8 @@ Reference behaviour mirrored (file:line in /root/reference):
 
 What differs, on purpose: (i) the datasets need a download (data_sets.py:30) that is impossible offline, so the clients
 train on a seeded synthetic 10-class 28x28 problem with the reference's MnistNet architecture (data_sets.py:13-24,
-D = 79,510); (ii) clients are evaluated on the GPU and write their flat gradients straight into their row of the
+D = 79,510), or with -s CIFAR10 on a seeded synthetic [3, 32, 32] problem with Cifar10Net (data_sets.py:33-52,
+D = 117,706); (ii) clients are evaluated on the GPU and write their flat gradients straight into their row of the
 device-resident N x D matrix (ingest.ParamLayout: user.py:17-28 order), so attack, defence and the server step never
 leave the device.  The training simulation itself is not part of the accelerated path (SURVEY 2).
 
@@ -44,6 +45,8 @@ from .ingest import ParamLayout
 from .server import AggregationServer
 
 SYNTH = 'SYNTH-MNIST'
+SYNTH_CIFAR10 = 'SYNTH-CIFAR10'
+DATASETS = ('MNIST', 'CIFAR10')                  # main.py -s
 
 
 class MnistNet(nn.Module):                       # data_sets.py:13-24
@@ -55,6 +58,26 @@ class MnistNet(nn.Module):                       # data_sets.py:13-24
 
     def forward(self, x):
         return F.log_softmax(self.fc2(F.relu(self.fc1(x))), dim=1)
+
+
+class Cifar10Net(nn.Module):                     # data_sets.py:33-52
+    def __init__(self):
+        super().__init__()
+        self.conv1 = nn.Conv2d(3, 16, 3)
+        torch.nn.init.xavier_uniform_(self.conv1.weight)
+        self.pool1 = nn.MaxPool2d(3)
+        self.conv2 = nn.Conv2d(16, 64, 4)
+        self.pool2 = nn.MaxPool2d(4)
+        self.fc1 = nn.Linear(64, 384)
+        self.fc2 = nn.Linear(384, 192)
+        self.fc3 = nn.Linear(192, 10)
+
+    def forward(self, x):
+        x = self.pool1(F.relu(self.conv1(x)))
+        x = self.pool2(F.relu(self.conv2(x)))
+        x = F.relu(self.fc1(x.view(x.size(0), -1)))
+        x = F.relu(self.fc2(x))
+        return F.log_softmax(self.fc3(x), dim=1)
 
 
 def synthetic_problem(n_train, n_test, device, seed=0):
@@ -69,27 +92,67 @@ def synthetic_problem(n_train, n_test, device, seed=0):
     return draw(n_train), draw(n_test)
 
 
-def experiment_setup(seed, train_size, test_size, device):
+def synthetic_cifar_problem(n_train, n_test, device, seed=0):
+    """The CIFAR10 stand-in for Cifar10Net: [n, 3, 32, 32] images of 10 classes, x = 0.5 * proto[y] + 0.5 * noise.
+    Each prototype is a random [3, 2, 2] grid upsampled bilinearly to 32x32 and scaled to unit standard deviation: a
+    smooth colour gradient, so the class shows in every 3x3 patch of the 23x23 corner the net's pools read.
+
+    main.py's rates (lr 0.1, momentum 0.9) train Cifar10Net unstably on every construction tried (per-pixel and smooth
+    prototypes, 2x2 to 8x8 grids, scales 0.25 to 1, noise 0.25 to 2.5): accuracy climbs, collapses and recovers.  This
+    one learned best: a CPU run of harness.main (NoDefense, no attacker, 10 users, m = 83, 20,000 training and 4,000
+    test rows, tested every 10 epochs) reached 100.0 % (seed 0) and 79.8 % (seed 1) at best and ended at 100.0 % and
+    56.9 % at epoch 99.  The learnability bar is therefore a best test accuracy of at least 40 % within 100 epochs."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    protos = F.interpolate(torch.randn(10, 3, 2, 2, generator=g), size=(32, 32), mode='bilinear', align_corners=False)
+    protos = 0.5 * protos / protos.std(dim=(1, 2, 3), keepdim=True)
+
+    def draw(n):
+        y = torch.randint(0, 10, (n,), generator=g)
+        x = protos[y] + 0.5 * torch.randn(n, 3, 32, 32, generator=g)
+        return x.to(device), y.to(device)
+    return draw(n_train), draw(n_test)
+
+
+def check_dataset(dataset):
+    if dataset not in DATASETS:
+        raise ValueError(f"unknown dataset {dataset!r} (expected one of {', '.join(DATASETS)})")
+    return dataset
+
+
+def model(dataset='MNIST'):
+    """The network main.py -s selects for the users, the server and the attacker (main.py:144-145, user.py:41-44,
+    server.py:24-29, backdoor.py:23-26)."""
+    return Cifar10Net() if check_dataset(dataset) == 'CIFAR10' else MnistNet()
+
+
+def synth_name(dataset='MNIST'):
+    return SYNTH_CIFAR10 if check_dataset(dataset) == 'CIFAR10' else SYNTH
+
+
+def experiment_setup(seed, train_size, test_size, device, dataset='MNIST'):
     """The seeded start of an experiment: torch.manual_seed(seed), the synthetic train and test sets and the test
-    network, whose parameters are the initial global weights.  ((xtr, ytr), (xte, yte), test_net)."""
+    network, whose parameters are the initial global weights.  ((xtr, ytr), (xte, yte), test_net).  dataset='CIFAR10':
+    synthetic_cifar_problem's [n, 3, 32, 32] images and a Cifar10Net."""
+    problem = synthetic_cifar_problem if check_dataset(dataset) == 'CIFAR10' else synthetic_problem
     torch.manual_seed(seed)
-    train, test = synthetic_problem(train_size, test_size, device, seed)
-    return train, test, MnistNet().to(device)
+    train, test = problem(train_size, test_size, device, seed)
+    return train, test, model(dataset).to(device)
 
 
-def csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate):
+def csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate, dataset='MNIST'):
     """main.py:100's accuracy log name (without the logs/ directory)."""
     return '{}_stdev_{}_{}_backdoor-{}_mal_prop_{}_users_{}_alpha_{}_lr_{}.csv'.format(
-        SYNTH, num_std, defense, backdoor, mal_prop, users_count, alpha if backdoor else None, learning_rate)
+        synth_name(dataset), num_std, defense, backdoor, mal_prop, users_count, alpha if backdoor else None,
+        learning_rate)
 
 
 class Client:
     """user.py:33-92 without the data loader machinery: one minibatch forward/backward per round, flat gradient out."""
 
-    def __init__(self, user_id, is_malicious, x, y, batch_size, layout, device):
+    def __init__(self, user_id, is_malicious, x, y, batch_size, layout, device, dataset='MNIST'):
         self.user_id, self.is_malicious = user_id, is_malicious
         self.x, self.y, self.batch_size, self.pos = x, y, batch_size, 0
-        self.net = MnistNet().to(device)
+        self.net = model(dataset).to(device)
         self.layout = layout
         self.criterion = nn.NLLLoss()
         self.grads = None
@@ -115,12 +178,15 @@ class Client:
 def backdoor_set(backdoor, x, y, seed=0, batch_size=200):
     """BackdoorTrainer's backdoor data (x, y) from the training set (x, y).  backdoor='pattern' (backdoor.py:37-42,
     47-50): rows r::u with u = max(len(x) // batch_size // 10, 1) and r = default_rng(seed).integers(u), the 5x5 corner
-    of the 28x28 view set to 2.8, every label 0; backdoor = 1, 2 or 3 (backdoor.py:30-35): training row backdoor - 1,
-    labelled (y + 1) % 5."""
+    of the 28x28 view (of every channel of a [3, 32, 32] image) set to 2.8, every label 0; backdoor = 1, 2 or 3
+    (backdoor.py:30-35): training row backdoor - 1, labelled (y + 1) % 5."""
     if backdoor == 'pattern':
         u = max(len(x) // batch_size // 10, 1)
         x = x[int(np.random.default_rng(seed).integers(u))::u].clone()
-        x.view(-1, 28, 28)[:, :5, :5] = 2.8
+        if x.dim() == 4:                                                  # add_pattern on a CHW image
+            x[:, :, :5, :5] = 2.8
+        else:
+            x.view(-1, 28, 28)[:, :5, :5] = 2.8
         return x, torch.zeros_like(y[:len(x)])
     i = int(backdoor) - 1
     return x[i:i + 1], (y[i:i + 1] + 1) % 5
@@ -130,12 +196,13 @@ class BackdoorTrainer:
     """backdoor.py:13-159 on the synthetic problem: the attacker's own network, trained from the starting point the
     crafting hands it towards the backdoor, and tested on the backdoor data.  backdoor='pattern': a shard of the
     training set with x[:, :5, :5] = 2.8 on the 28x28 view, all labelled 0; backdoor = 1, 2 or 3: the single training
-    sample backdoor - 1, labelled (y + 1) % 5."""
+    sample backdoor - 1, labelled (y + 1) % 5.  dataset='CIFAR10' trains a Cifar10Net, with the pattern on every channel."""
 
-    def __init__(self, backdoor, alpha, num_epochs, layout, x, y, device, my_print, seed=0, batch_size=200):
+    def __init__(self, backdoor, alpha, num_epochs, layout, x, y, device, my_print, seed=0, batch_size=200,
+                 dataset='MNIST'):
         self.backdoor, self.alpha, self.num_epochs, self.layout, self.my_print = backdoor, alpha, num_epochs, layout, my_print
         self.batch_size = batch_size
-        self.net = MnistNet().to(device)
+        self.net = model(dataset).to(device)
         self.x, self.y = backdoor_set(backdoor, x, y, seed, batch_size)
 
     def test(self, tag, to_print=True):                                   # backdoor.py:67-102
@@ -173,7 +240,8 @@ class BackdoorTrainer:
 
 def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0.1, fading_rate=10000, momentum=0.9,
          batch_size=83, output=None, device="cuda", out_dir=".", seed=0, train_size=20000, test_size=4000, test_step=5,
-         backdoor=False, alpha=4, mal_epochs=5):
+         backdoor=False, alpha=4, mal_epochs=5, dataset='MNIST'):
+    synth = synth_name(dataset)
     if output:
         def my_print(s, end='\n'):
             with open(output, 'a+') as f:
@@ -181,16 +249,16 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     else:
         my_print = print
     my_print(dict(mal_prop=mal_prop, num_std=num_std, defense=defense, users_count=users_count, epochs=epochs,
-                  learning_rate=learning_rate, dataset=SYNTH, backdoor=backdoor))
+                  learning_rate=learning_rate, dataset=synth, backdoor=backdoor))
     corrupted_count = int(mal_prop * users_count)                         # main.py:21
-    (xtr, ytr), (xte, yte), test_net = experiment_setup(seed, train_size, test_size, device)
+    (xtr, ytr), (xte, yte), test_net = experiment_setup(seed, train_size, test_size, device, dataset)
     layout = ParamLayout(test_net.parameters())
     srv = AggregationServer(users_count, layout.dim, mal_prop, learning_rate, momentum, device=device,
                             initial_weights=layout.flatten(list(test_net.parameters())))
-    users = [Client(u, u < corrupted_count, xtr[u::users_count], ytr[u::users_count], batch_size, layout, device)
-             for u in range(users_count)]                                 # DistributedSampler-style partition (user.py:50)
+    users = [Client(u, u < corrupted_count, xtr[u::users_count], ytr[u::users_count], batch_size, layout, device,
+                    dataset) for u in range(users_count)]                                 # DistributedSampler-style partition (user.py:50)
     if backdoor:                                                          # main.py:44-54
-        trainer = BackdoorTrainer(backdoor, alpha, mal_epochs, layout, xtr, ytr, device, my_print, seed)
+        trainer = BackdoorTrainer(backdoor, alpha, mal_epochs, layout, xtr, ytr, device, my_print, seed, dataset=dataset)
         attacker = malicious.BackdoorAttack(num_std, trainer.train)
     else:
         attacker = malicious.DriftAttack(num_std)
@@ -222,7 +290,7 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
             accuracies.append(accuracy)
             accuracies_epochs.append(epoch)
             if accuracy > 70.:                                            # main.py:84-89, server.py:40-46
-                directory = os.path.join(out_dir, "runs", SYNTH)
+                directory = os.path.join(out_dir, "runs", synth)
                 os.makedirs(directory, exist_ok=True)
                 torch.save({'epoch': epoch + 1, 'state_dict': test_net.state_dict(), 'acc': accuracy},
                            os.path.join(directory, 'checkpoint.pth.tar'))
@@ -232,7 +300,8 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     my_print(datetime.datetime.now().time())
     my_print("Max accuracy: {}".format(max(accuracies)))
     os.makedirs(os.path.join(out_dir, "logs"), exist_ok=True)             # the reference needs a pre-made logs/ (readme.md:25)
-    csv = os.path.join(out_dir, 'logs', csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate))
+    csv = os.path.join(out_dir, 'logs', csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate,
+                                                 dataset))
     np.savetxt(csv, accuracies, delimiter=',')                            # main.py:100
     return accuracies, accuracies_epochs, csv
 
@@ -248,7 +317,9 @@ if __name__ == '__main__':
     p.add_argument('-l', '--learning_rate', default=0.1, type=float)
     p.add_argument('-o', '--output', type=str)
     p.add_argument('-b', '--backdoor', default='No', choices=['No', 'pattern', '1', '2', '3'])
+    p.add_argument('-s', '--dataset', default='MNIST', choices=list(DATASETS))
     a = p.parse_args()
     bd = False if a.backdoor == 'No' else a.backdoor if a.backdoor == 'pattern' else int(a.backdoor)
     main(a.mal_prop, a.num_std, a.defense, users_count=a.users_count, epochs=a.epochs, learning_rate=a.learning_rate,
-         batch_size=a.batch_size, output=a.output, backdoor=bd)
+         batch_size=a.batch_size, output=a.output, backdoor=bd, dataset=a.dataset,
+         fading_rate=2000 if a.dataset == 'CIFAR10' else 10000)                 # main.py:144-147

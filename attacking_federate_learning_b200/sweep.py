@@ -37,6 +37,12 @@ key, so the experiments of a batch would overwrite one file.
 
     python -m attacking_federate_learning_b200.sweep -d Krum TrimmedMean -z 0.5 1.5 -m 0.1 0.24 -n 10 --seeds 0 1 -e 30
     python -m attacking_federate_learning_b200.sweep -d Krum NoDefense -z 1.0 -b No pattern 1 --seeds 0 1 -e 30
+    python -m attacking_federate_learning_b200.sweep -s CIFAR10 -d Krum TrimmedMean -z 0.5 1.5 --seeds 0 1 -e 30
+
+dataset='CIFAR10' (main.py -s CIFAR10) runs the same loop on harness.Cifar10Net and `synthetic_cifar_problem`, with
+the CIFAR10 kernels (C ABI `afl_cifar10_client_grads` and `afl_cifar10_evaluate`) in steps 1 and 4 and SYNTH-CIFAR10
+log names.  A batch holds one dataset: the two models have different D.  CIFAR10 backdoor experiments are not batched
+(the trainer kernel is MnistNet's); `check` raises NotImplementedError for them and `harness.main` runs them.
 """
 from __future__ import annotations
 
@@ -60,6 +66,7 @@ MAX_USERS = batched.MAX_CLIENTS          # clients per experiment (DeviceRound w
 MAX_BATCH_SIZE = 128                     # minibatch rows of the client-gradient kernel
 BACKDOOR_BATCH = 200                     # BackdoorTrainer's minibatch and test batch (the trainer kernel's limit)
 SUMMARY = 'sweep_summary.csv'
+FADING_RATE = {'MNIST': 10000, 'CIFAR10': 2000}         # main.py:144-147
 
 
 class Experiment(tuple):
@@ -109,13 +116,15 @@ def minibatch(n_train, users_count, user, batch_size, epoch):
     return k * batch_size, min(k * batch_size + batch_size, length)
 
 
-def check(exp, batch_size=83, train_size=20000):
+def check(exp, batch_size=83, train_size=20000, dataset='MNIST'):
     """Raise what main.py would raise for this experiment at its first `defend` (AssertionError for the reference's
     asserts), or for what the sweep's kernels do not take.  Returns the normalised Experiment."""
     if len(exp) not in (5, 6):
         raise ValueError(f"{exp}: an experiment has 5 or 6 elements")
     exp = Experiment(str(exp[0]), float(exp[1]), float(exp[2]), int(exp[3]), int(exp[4]),
                      normalise_backdoor(exp[5]) if len(exp) == 6 else False)
+    if harness.check_dataset(dataset) == 'CIFAR10' and exp.backdoor is not False:
+        raise NotImplementedError(f"{exp}: the sweep trains no CIFAR10 backdoor attacker (harness.main runs it)")
     if exp.backdoor not in (False, 'pattern') and exp.backdoor > train_size:
         raise ValueError(f"{exp}: backdoor sample {exp.backdoor} lies past the training set ({train_size} rows)")
     if exp.defense not in RULES:
@@ -136,7 +145,8 @@ def check(exp, batch_size=83, train_size=20000):
     return exp
 
 
-def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000, backdoors=(False,)):
+def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000, backdoors=(False,),
+         dataset='MNIST'):
     """The Cartesian grid (defence-major, backdoor-minor) as (kept experiments, [(experiment, rejection), ...]): a cell
     main.py would reject is dropped with the exception `check` raises for it.  A drift cell (backdoor False) has 5
     elements, a backdoor cell 6."""
@@ -145,15 +155,16 @@ def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, trai
         if cell[5] is False:
             cell = cell[:5]
         try:
-            kept.append(check(cell, batch_size, train_size))
+            kept.append(check(cell, batch_size, train_size, dataset))
         except (AssertionError, KeyError, ValueError, NotImplementedError) as e:
             dropped.append((cell, e))
     return kept, dropped
 
 
-def csv_name(exp, learning_rate, alpha=4):
+def csv_name(exp, learning_rate, alpha=4, dataset='MNIST'):
     """harness.main's log name for this experiment, with `_seed_<s>` before `.csv`."""
-    name = harness.csv_name(exp.num_std, exp.defense, exp.backdoor, exp.mal_prop, exp.users_count, alpha, learning_rate)
+    name = harness.csv_name(exp.num_std, exp.defense, exp.backdoor, exp.mal_prop, exp.users_count, alpha, learning_rate,
+                            dataset)
     return name[:-len('.csv')] + f'_seed_{exp.seed}.csv'
 
 
@@ -213,11 +224,14 @@ class Sweep:
     fp32 [B, D] weights and velocity; G: the [B, N_max, ld] client matrix (ld a multiple of 32, as AggregationServer
     pads); `rounds`: {defence: (slice, DeviceRound)} of the drift groups, `backdoor_rounds` the same for the backdoor
     groups, which occupy batch problems `bd0`..B-1.  Their DeviceRounds hold views of one f, z, lr and status over
-    those problems, so the trainer reads every backdoor experiment in one launch."""
+    those problems, so the trainer reads every backdoor experiment in one launch.  `dataset` picks the model, the data
+    and the kernels: x_train and x_test are [n_seeds, n, 784] for MNIST and [n_seeds, n, 3, 32, 32] for CIFAR10."""
 
     def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000,
-                 test_size=4000, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000):
-        exps = [check(e, batch_size, train_size) for e in experiments]
+                 test_size=4000, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000,
+                 dataset='MNIST'):
+        self.dataset = harness.check_dataset(dataset)
+        exps = [check(e, batch_size, train_size, dataset) for e in experiments]
         if not exps:
             raise ValueError("sweep: no experiment")
         if epochs < 1 or test_step < 1 or test_size < 1:
@@ -236,7 +250,7 @@ class Sweep:
         seeds = list(dict.fromkeys(e.seed for e in self.experiments))
         xtr, ytr, xte, yte, w0 = [], [], [], [], {}
         for s in seeds:                                                   # harness.main's start, seed by seed
-            (a, b), (c, d), net = harness.experiment_setup(s, train_size, test_size, dev)
+            (a, b), (c, d), net = harness.experiment_setup(s, train_size, test_size, dev, dataset)
             xtr.append(a); ytr.append(b); xte.append(c); yte.append(d)
             w0[s] = harness.ParamLayout(net.parameters()).flatten(list(net.parameters()))
         self.x_train, self.y_train = torch.stack(xtr).contiguous(), torch.stack(ytr).contiguous()
@@ -258,7 +272,11 @@ class Sweep:
         self.loss_sum = torch.zeros((self.n_tests, B), dtype=torch.float64, device=dev)
         self.correct = torch.zeros((self.n_tests, B), **i32)
         L = nat.lib()
-        self._eval_ws = torch.empty(max(L.afl_mnist_evaluate_workspace_bytes(B, test_size, batch_size), 256),
+        cifar = self.dataset == 'CIFAR10'
+        self._grads_fn = L.afl_cifar10_client_grads if cifar else L.afl_mnist_client_grads
+        self._evaluate_fn = L.afl_cifar10_evaluate if cifar else L.afl_mnist_evaluate
+        ws_bytes = (L.afl_cifar10_evaluate_workspace_bytes if cifar else L.afl_mnist_evaluate_workspace_bytes)
+        self._eval_ws = torch.empty(max(ws_bytes(B, test_size, batch_size), 256),
                                     dtype=torch.uint8, device=dev)
         self.bd0 = sum(e.backdoor is False for e in self.experiments)
         self._setup_backdoor(xtr, ytr, seeds)
@@ -305,7 +323,7 @@ class Sweep:
         """Step 1: every client's gradient into G at the current device epoch."""
         G = self._storage
         with torch.cuda.device(self.device):
-            nat.check(nat.lib().afl_mnist_client_grads(
+            nat.check(self._grads_fn(
                 self.W.data_ptr(), self.B, self.D, self.x_train.data_ptr(), self.y_train.data_ptr(),
                 self.x_train.shape[0], self.train_size, self.data_index.data_ptr(), self.rows.data_ptr(), self.N,
                 self.batch_size, self.epoch_counter.data_ptr(), G.data_ptr(), G.stride(0), G.stride(1),
@@ -356,7 +374,7 @@ class Sweep:
         backdoor experiment's backdoor test into the same slot of its tables."""
         stream = torch.cuda.current_stream(self.device).cuda_stream
         with torch.cuda.device(self.device):
-            nat.check(nat.lib().afl_mnist_evaluate(
+            nat.check(self._evaluate_fn(
                 self.W.data_ptr(), self.B, self.D, self.x_test.data_ptr(), self.y_test.data_ptr(),
                 self.x_test.shape[0], self.test_size, self.data_index.data_ptr(), self.batch_size,
                 self.test_slot.data_ptr(), self.n_tests, self.loss_sum.data_ptr(), self.correct.data_ptr(),
@@ -426,13 +444,14 @@ class Sweep:
 
 
 def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000, test_size=4000,
-        test_step=5, out_dir='.', capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000):
+        test_step=5, out_dir='.', capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000, dataset='MNIST'):
     """Train every experiment for `epochs` epochs as one batch; write each one's accuracy CSV and the summary CSV under
     out_dir/logs.  Returns `Sweep.results()` with `csv` (None for a failed experiment) added to each dict.  Raises
     before any GPU work for an experiment main.py would reject (see `check`).  alpha, mal_epochs and fading_rate are
-    harness.main's (the backdoor experiments' malicious training and client learning rate)."""
+    harness.main's (the backdoor experiments' malicious training and client learning rate), and so is dataset ('MNIST'
+    or 'CIFAR10', main.py -s)."""
     sw = Sweep(experiments, epochs, learning_rate, momentum, batch_size, train_size, test_size, test_step, capture,
-               device, alpha, mal_epochs, fading_rate)
+               device, alpha, mal_epochs, fading_rate, dataset)
     with torch.cuda.device(sw.device):
         for epoch in range(epochs):
             sw.step(epoch)
@@ -448,7 +467,7 @@ def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, tra
             r['csv'] = None
             head = list(e[:5]) + ([e.backdoor] if with_bd else [])
             if r['error'] is None:
-                r['csv'] = os.path.join(logs, csv_name(e, learning_rate, alpha))
+                r['csv'] = os.path.join(logs, csv_name(e, learning_rate, alpha, sw.dataset))
                 np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
                 bd = r.get('backdoor_accuracies')
                 tail = ([max(bd), bd[-1]] if bd else ['', '']) if with_bd else []
@@ -467,6 +486,7 @@ def main(argv=None):
     p.add_argument('-n', '--users-count', nargs='+', type=int, default=[10])
     p.add_argument('--seeds', nargs='+', type=int, default=[0])
     p.add_argument('-b', '--backdoor', nargs='+', default=['No'], choices=['No', 'pattern', '1', '2', '3'])
+    p.add_argument('-s', '--dataset', default='MNIST', choices=list(harness.DATASETS))
     p.add_argument('-e', '--epochs', type=int, default=300)
     p.add_argument('-c', '--batch_size', type=int, default=83)
     p.add_argument('-l', '--learning_rate', type=float, default=0.1)
@@ -474,13 +494,14 @@ def main(argv=None):
     p.add_argument('--no-capture', action='store_true')
     a = p.parse_args(argv)
     kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size,
-                         backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)])
+                         backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)], dataset=a.dataset)
     for cell, e in dropped:
         print(f"skipped {cell}: {type(e).__name__}: {e}")
     if not kept:
         print("no experiment left to run")
         return []
-    res = run(kept, a.epochs, a.learning_rate, batch_size=a.batch_size, out_dir=a.out_dir, capture=not a.no_capture)
+    res = run(kept, a.epochs, a.learning_rate, batch_size=a.batch_size, out_dir=a.out_dir, capture=not a.no_capture,
+              fading_rate=FADING_RATE[a.dataset], dataset=a.dataset)
     for r in res:
         e = r['experiment']
         if r['error'] is None:

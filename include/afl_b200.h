@@ -598,6 +598,33 @@ int afl_mnist_backdoor_test(const float* weights, int batch, int64_t d, const fl
                             int max_len, const int* set_len, const int* data_index, int m, const int* slot_index,
                             int n_slots, double* loss_sum, int* correct, void* stream);
 
+/* ---- Cifar10Net training sweeps (csrc/cifar_grad.cu): the model half of a CIFAR10 sweep epoch ----------------------
+ * harness.Cifar10Net (data_sets.py:33-52): conv1 3->16 k3, relu, maxpool 3, conv2 16->64 k4, relu, maxpool 4, fc1
+ * 64->384, relu, fc2 384->192, relu, fc3 192->10, log_softmax; parameters in ParamLayout order (user.py:17-28),
+ * D = 117,706.  The arguments are the afl_mnist_* ones above; x is device fp32 [n_sets][n_rows][3072], the NCHW
+ * [3, 32, 32] images flattened.  The pools use floor mode, so only each image's 23x23 top-left corner reaches the loss,
+ * and only it is computed; on finite values everything else contributes exact zeros (DESIGN 2.9).  MaxPool follows
+ * torch's max_pool2d (first maximum, a NaN takes the index, the gradient goes to that index alone).  Same rules as the
+ * MnistNet entries: fp32 FFMA only, no atomics, every sum in a fixed order, so a client's gradient depends only on its
+ * weights, its rows and m; no allocation, copy or synchronisation, so the calls can be captured in a CUDA graph.
+ * Checked before any CUDA call: a NULL pointer, batch / n_sets / set size / m < 1 -> AFL_ERR_BAD_ARG; d != 117,706,
+ * m > 128 or batch > 65535 -> AFL_ERR_UNSUPPORTED.
+ *
+ * afl_cifar10_client_grads — user.py:76-92 with Cifar10Net for every client of every problem: afl_mnist_client_grads'
+ * clients, shards, minibatches (from *epoch) and limits on n, ld and batch_stride.  Only columns [0, d) of rows u <
+ * min(rows[b], n) of each problem are written.  No workspace: the kernel accumulates the weight gradients in the row.
+ *
+ * afl_cifar10_evaluate — server.py:92-112 / harness.main's test loop with Cifar10Net: afl_mnist_evaluate's batches,
+ * float64 loss sums, first-maximum correct counts, NaN loss for a label outside 0..9, slot rule and workspace
+ * (afl_cifar10_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned). */
+int afl_cifar10_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                             int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
+                             float* G, int64_t batch_stride, int64_t ld, void* stream);
+size_t afl_cifar10_evaluate_workspace_bytes(int batch, int n_test, int m);
+int afl_cifar10_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                         int n_test, const int* data_index, int m, const int* slot_index, int n_slots,
+                         double* loss_sum, int* correct, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

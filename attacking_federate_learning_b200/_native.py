@@ -90,6 +90,8 @@ SIGNATURES = {
     "afl_defend_batched_large_dev": (_i, [C.c_char_p, _vp, _i, _i64, _i, _i64, _i64, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp,
                                           _i, _vp, _sz, _vp, _vp]),
     "afl_mnist_client_grads": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i64, _i64, _vp]),
+    "afl_mnist_client_grads_sets": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _i64, _i64,
+                                         _vp]),
     "afl_mnist_evaluate_workspace_bytes": (_sz, [_i, _i, _i]),
     "afl_mnist_evaluate": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
     "afl_backdoor_start_batched_dev": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp,
@@ -99,6 +101,8 @@ SIGNATURES = {
     "afl_mnist_backdoor_train": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _d, _i, _i, _vp]),
     "afl_mnist_backdoor_test": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "afl_cifar10_client_grads": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i64, _i64, _vp]),
+    "afl_cifar10_client_grads_sets": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _i64,
+                                           _i64, _vp]),
     "afl_cifar10_evaluate_workspace_bytes": (_sz, [_i, _i, _i]),
     "afl_cifar10_evaluate": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }

@@ -403,17 +403,20 @@ __device__ __forceinline__ void stage_conv1(const float* __restrict__ w, const S
 
 __global__ void __launch_bounds__(kThreads, 2)
 client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ x, const int64_t* __restrict__ y,
-                   int n_sets, int n_train, const int* __restrict__ data_index, const int* __restrict__ rows, int n_max,
-                   int m, const int* __restrict__ epoch, float* __restrict__ G, int64_t batch_stride, int64_t ld) {
+                   int n_sets, int n_rows, const int* __restrict__ set_len, const int* __restrict__ data_index,
+                   const int* __restrict__ rows, int n_max, int m, const int* __restrict__ epoch, float* __restrict__ G,
+                   int64_t batch_stride, int64_t ld) {
   const int u = blockIdx.x, b = blockIdx.y;
   const int n = min(rows[b], n_max);
   const int set = data_index[b];
   if (u >= n || set < 0 || set >= n_sets) return;                 // block-uniform, before any barrier
+  const int n_train = set_len ? set_len[set] : n_rows;            // no set_len: every set is n_rows long
+  if (n_train < n || n_train > n_rows) return;
   extern __shared__ float smem[];
   const Smem s = carve(smem);
   const float* w = weights + int64_t(b) * kD;
-  const float* xs = x + int64_t(set) * n_train * kImg;
-  const int64_t* ys = y + int64_t(set) * n_train;
+  const float* xs = x + int64_t(set) * n_rows * kImg;
+  const int64_t* ys = y + int64_t(set) * n_rows;
   int mb;
   const int lo = batch_start(n_train, n, u, m, *epoch, &mb);
   for (int i = threadIdx.x; i < mb; i += kThreads) {
@@ -521,6 +524,29 @@ static int check_common(const char* who, int batch, int64_t d, int n_sets, int n
   return AFL_OK;
 }
 
+static int client_grads(const char* who, const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                        int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows, int n, int m,
+                        const int* epoch, float* G, int64_t batch_stride, int64_t ld, void* stream) {
+  if (!weights || !x || !y || !data_index || !rows || !epoch || !G) {
+    set_error("%s: a pointer argument is NULL", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  if (int rc = check_common(who, batch, d, n_sets, n_rows, m)) return rc;
+  if (n < 1 || n > 1024) { set_error("%s: 1 <= n <= 1024 clients per problem (got %d)", who, n); return n < 1 ? AFL_ERR_BAD_ARG : AFL_ERR_UNSUPPORTED; }
+  if (n > n_rows) { set_error("%s: n (%d) exceeds the training set size (%d)", who, n, n_rows); return AFL_ERR_BAD_ARG; }
+  if (ld < d || (batch > 1 && batch_stride < (n - 1) * ld + d)) {
+    set_error("%s: ld (%lld) < d or batch_stride (%lld) makes problems overlap", who, static_cast<long long>(ld),
+              static_cast<long long>(batch_stride));
+    return AFL_ERR_BAD_ARG;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  AFL_CUDA(ensure_dyn_smem(client_grad_kernel, static_cast<int>(kSmemBytes), smem_done_grad));
+  client_grad_kernel<<<dim3(n, batch), kThreads, kSmemBytes, st>>>(
+      weights, x, y, n_sets, n_rows, set_len, data_index, rows, n, m, epoch, G, batch_stride, ld);
+  AFL_LAUNCH_CHECK("cifar_client_grad_kernel");
+  return AFL_OK;
+}
+
 static int64_t eval_batches(int n_test, int m) { return (int64_t(n_test) + m - 1) / m; }
 
 }  // namespace cifar
@@ -533,25 +559,17 @@ extern "C" {
 int afl_cifar10_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                              int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
                              float* G, int64_t batch_stride, int64_t ld, void* stream) {
-  const char* who = "afl_cifar10_client_grads";
-  if (!weights || !x || !y || !data_index || !rows || !epoch || !G) {
-    set_error("%s: a pointer argument is NULL", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  if (int rc = cifar::check_common(who, batch, d, n_sets, n_train, m)) return rc;
-  if (n < 1 || n > 1024) { set_error("%s: 1 <= n <= 1024 clients per problem (got %d)", who, n); return n < 1 ? AFL_ERR_BAD_ARG : AFL_ERR_UNSUPPORTED; }
-  if (n > n_train) { set_error("%s: n (%d) exceeds the training set size (%d)", who, n, n_train); return AFL_ERR_BAD_ARG; }
-  if (ld < d || (batch > 1 && batch_stride < (n - 1) * ld + d)) {
-    set_error("%s: ld (%lld) < d or batch_stride (%lld) makes problems overlap", who, static_cast<long long>(ld),
-              static_cast<long long>(batch_stride));
-    return AFL_ERR_BAD_ARG;
-  }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  AFL_CUDA(ensure_dyn_smem(cifar::client_grad_kernel, static_cast<int>(cifar::kSmemBytes), cifar::smem_done_grad));
-  cifar::client_grad_kernel<<<dim3(n, batch), cifar::kThreads, cifar::kSmemBytes, st>>>(
-      weights, x, y, n_sets, n_train, data_index, rows, n, m, epoch, G, batch_stride, ld);
-  AFL_LAUNCH_CHECK("cifar_client_grad_kernel");
-  return AFL_OK;
+  return cifar::client_grads("afl_cifar10_client_grads", weights, batch, d, x, y, n_sets, n_train, nullptr, data_index,
+                             rows, n, m, epoch, G, batch_stride, ld, stream);
+}
+
+int afl_cifar10_client_grads_sets(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                                  int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
+                                  int n, int m, const int* epoch, float* G, int64_t batch_stride, int64_t ld,
+                                  void* stream) {
+  if (!set_len) { set_error("afl_cifar10_client_grads_sets: a pointer argument is NULL"); return AFL_ERR_BAD_ARG; }
+  return cifar::client_grads("afl_cifar10_client_grads_sets", weights, batch, d, x, y, n_sets, n_rows, set_len,
+                             data_index, rows, n, m, epoch, G, batch_stride, ld, stream);
 }
 
 size_t afl_cifar10_evaluate_workspace_bytes(int batch, int n_test, int m) {

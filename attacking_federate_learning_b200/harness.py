@@ -14,11 +14,15 @@ Reference behaviour mirrored (file:line in /root/reference):
     outputs                        main.py:85-89    torch.save({'epoch','state_dict','acc'}) to runs/<dataset>/checkpoint.pth.tar
                                    main.py:100      np.savetxt('logs/<...>.csv', accuracies, delimiter=',')
 
-What differs, on purpose: (i) the datasets need a download (data_sets.py:30) that is impossible offline, so the clients
-train on a seeded synthetic 10-class 28x28 problem with the reference's MnistNet architecture (data_sets.py:13-24,
-D = 79,510), or with -s CIFAR10 on a seeded synthetic [3, 32, 32] problem with Cifar10Net (data_sets.py:33-52,
-D = 117,706); (ii) clients are evaluated on the GPU and write their flat gradients straight into their row of the
-device-resident N x D matrix (ingest.ParamLayout: user.py:17-28 order), so attack, defence and the server step never
+What differs, on purpose: (i) the reference downloads its datasets (data_sets.py:30, 60), which is impossible offline,
+so without data_dir the clients train on a seeded synthetic 10-class 28x28 problem with the reference's MnistNet
+architecture (data_sets.py:13-24, D = 79,510), or with -s CIFAR10 on a seeded synthetic [3, 32, 32] problem with
+Cifar10Net (data_sets.py:33-52, D = 117,706), each user holding rows u, u + n, ... of it.  With data_dir (--data-dir:
+the directory that holds torchvision's files, e.g. the reference's ./mnist_data or ./cifar10_data) they train on the
+real MNIST or CIFAR10 through the reference's transforms (data.load), each user holding its DistributedSampler shard
+(user.py:49-54, data.sampler_order) and the attacker its backdoor.py loader's rows (data.backdoor_indices), under the
+reference's log and checkpoint names; (ii) clients are evaluated on the GPU and write their flat gradients straight
+into their row of the device-resident N x D matrix (ingest.ParamLayout: user.py:17-28 order), so attack, defence and the server step never
 leave the device.  The training simulation itself is not part of the accelerated path (SURVEY 2).
 
     python -m attacking_federate_learning_b200.harness -d Krum -e 30 --users-count 10
@@ -40,6 +44,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import data as _data
 from . import malicious
 from .ingest import ParamLayout
 from .server import AggregationServer
@@ -129,20 +134,41 @@ def synth_name(dataset='MNIST'):
     return SYNTH_CIFAR10 if check_dataset(dataset) == 'CIFAR10' else SYNTH
 
 
-def experiment_setup(seed, train_size, test_size, device, dataset='MNIST'):
+def dataset_name(dataset='MNIST', data_dir=None):
+    """The dataset's name in logs, checkpoint paths and prints: main.py's ('MNIST', 'CIFAR10') when the data come from
+    data_dir, SYNTH-MNIST / SYNTH-CIFAR10 for the synthetic stand-ins."""
+    return check_dataset(dataset) if data_dir is not None else synth_name(dataset)
+
+
+def real_sizes(dataset, data_dir, train_size=None, test_size=None):
+    """data.load(dataset, data_dir) and its (train, test) row counts; an explicit size that differs raises ValueError."""
+    (xtr, ytr), (xte, yte) = loaded = _data.load(check_dataset(dataset), data_dir)
+    for what, want, got in (('train_size', train_size, len(xtr)), ('test_size', test_size, len(xte))):
+        if want is not None and want != got:
+            raise ValueError(f"{what}={want}, but the {dataset} files under {data_dir} hold {got} rows")
+    return loaded
+
+
+def experiment_setup(seed, train_size, test_size, device, dataset='MNIST', data_dir=None):
     """The seeded start of an experiment: torch.manual_seed(seed), the synthetic train and test sets and the test
     network, whose parameters are the initial global weights.  ((xtr, ytr), (xte, yte), test_net).  dataset='CIFAR10':
-    synthetic_cifar_problem's [n, 3, 32, 32] images and a Cifar10Net."""
+    synthetic_cifar_problem's [n, 3, 32, 32] images and a Cifar10Net.  With data_dir the sets are data.load's, in
+    file order (train_size and test_size: None, or the files' row counts), and the test net is the same seed's."""
+    if data_dir is not None:
+        (xtr, ytr), (xte, yte) = real_sizes(dataset, data_dir, train_size, test_size)
+        torch.manual_seed(seed)
+        return (xtr.to(device), ytr.to(device)), (xte.to(device), yte.to(device)), model(dataset).to(device)
     problem = synthetic_cifar_problem if check_dataset(dataset) == 'CIFAR10' else synthetic_problem
     torch.manual_seed(seed)
-    train, test = problem(train_size, test_size, device, seed)
+    train, test = problem(20000 if train_size is None else train_size, 4000 if test_size is None else test_size,
+                          device, seed)
     return train, test, model(dataset).to(device)
 
 
-def csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate, dataset='MNIST'):
+def csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate, dataset='MNIST', data_dir=None):
     """main.py:100's accuracy log name (without the logs/ directory)."""
     return '{}_stdev_{}_{}_backdoor-{}_mal_prop_{}_users_{}_alpha_{}_lr_{}.csv'.format(
-        synth_name(dataset), num_std, defense, backdoor, mal_prop, users_count, alpha if backdoor else None,
+        dataset_name(dataset, data_dir), num_std, defense, backdoor, mal_prop, users_count, alpha if backdoor else None,
         learning_rate)
 
 
@@ -175,35 +201,42 @@ class Client:
         self.grads = out_row
 
 
-def backdoor_set(backdoor, x, y, seed=0, batch_size=200):
+def backdoor_set(backdoor, x, y, seed=0, batch_size=200, sampled=False):
     """BackdoorTrainer's backdoor data (x, y) from the training set (x, y).  backdoor='pattern' (backdoor.py:37-42,
     47-50): rows r::u with u = max(len(x) // batch_size // 10, 1) and r = default_rng(seed).integers(u), the 5x5 corner
     of the 28x28 view (of every channel of a [3, 32, 32] image) set to 2.8, every label 0; backdoor = 1, 2 or 3
-    (backdoor.py:30-35): training row backdoor - 1, labelled (y + 1) % 5."""
-    if backdoor == 'pattern':
+    (backdoor.py:30-35): training row backdoor - 1, labelled (y + 1) % 5.  sampled=True takes the rows the reference's
+    DistributedSampler loader yields instead (data.backdoor_indices), with the same pattern and labels."""
+    if sampled:
+        i = _data.backdoor_indices(backdoor, len(x), seed, batch_size).to(x.device)
+    elif backdoor == 'pattern':
         u = max(len(x) // batch_size // 10, 1)
-        x = x[int(np.random.default_rng(seed).integers(u))::u].clone()
-        if x.dim() == 4:                                                  # add_pattern on a CHW image
-            x[:, :, :5, :5] = 2.8
-        else:
-            x.view(-1, 28, 28)[:, :5, :5] = 2.8
-        return x, torch.zeros_like(y[:len(x)])
-    i = int(backdoor) - 1
-    return x[i:i + 1], (y[i:i + 1] + 1) % 5
+        i = slice(int(np.random.default_rng(seed).integers(u)), None, u)
+    else:
+        i = slice(int(backdoor) - 1, int(backdoor))
+    if backdoor != 'pattern':
+        return x[i], (y[i] + 1) % 5
+    x = x[i].clone()
+    if x.dim() == 4:                                                      # add_pattern on a CHW image
+        x[:, :, :5, :5] = 2.8
+    else:
+        x.view(-1, 28, 28)[:, :5, :5] = 2.8
+    return x, torch.zeros_like(y[:len(x)])
 
 
 class BackdoorTrainer:
     """backdoor.py:13-159 on the synthetic problem: the attacker's own network, trained from the starting point the
     crafting hands it towards the backdoor, and tested on the backdoor data.  backdoor='pattern': a shard of the
     training set with x[:, :5, :5] = 2.8 on the 28x28 view, all labelled 0; backdoor = 1, 2 or 3: the single training
-    sample backdoor - 1, labelled (y + 1) % 5.  dataset='CIFAR10' trains a Cifar10Net, with the pattern on every channel."""
+    sample backdoor - 1, labelled (y + 1) % 5.  dataset='CIFAR10' trains a Cifar10Net, with the pattern on every channel.
+    sampled=True: the rows of backdoor.py's DistributedSampler loader (backdoor_set)."""
 
     def __init__(self, backdoor, alpha, num_epochs, layout, x, y, device, my_print, seed=0, batch_size=200,
-                 dataset='MNIST'):
+                 dataset='MNIST', sampled=False):
         self.backdoor, self.alpha, self.num_epochs, self.layout, self.my_print = backdoor, alpha, num_epochs, layout, my_print
         self.batch_size = batch_size
         self.net = model(dataset).to(device)
-        self.x, self.y = backdoor_set(backdoor, x, y, seed, batch_size)
+        self.x, self.y = backdoor_set(backdoor, x, y, seed, batch_size, sampled)
 
     def test(self, tag, to_print=True):                                   # backdoor.py:67-102
         loss, correct = 0.0, 0
@@ -239,9 +272,12 @@ class BackdoorTrainer:
 
 
 def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0.1, fading_rate=10000, momentum=0.9,
-         batch_size=83, output=None, device="cuda", out_dir=".", seed=0, train_size=20000, test_size=4000, test_step=5,
-         backdoor=False, alpha=4, mal_epochs=5, dataset='MNIST'):
-    synth = synth_name(dataset)
+         batch_size=83, output=None, device="cuda", out_dir=".", seed=0, train_size=None, test_size=None, test_step=5,
+         backdoor=False, alpha=4, mal_epochs=5, dataset='MNIST', data_dir=None):
+    """main.py's experiment.  train_size and test_size (None: 20,000 and 4,000) size the synthetic problem; with
+    data_dir the data are the real dataset's files there (see the module docstring) and the sizes, when given, must
+    be the files' row counts."""
+    synth = dataset_name(dataset, data_dir)
     if output:
         def my_print(s, end='\n'):
             with open(output, 'a+') as f:
@@ -251,14 +287,19 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     my_print(dict(mal_prop=mal_prop, num_std=num_std, defense=defense, users_count=users_count, epochs=epochs,
                   learning_rate=learning_rate, dataset=synth, backdoor=backdoor))
     corrupted_count = int(mal_prop * users_count)                         # main.py:21
-    (xtr, ytr), (xte, yte), test_net = experiment_setup(seed, train_size, test_size, device, dataset)
+    (xtr, ytr), (xte, yte), test_net = experiment_setup(seed, train_size, test_size, device, dataset, data_dir)
     layout = ParamLayout(test_net.parameters())
     srv = AggregationServer(users_count, layout.dim, mal_prop, learning_rate, momentum, device=device,
                             initial_weights=layout.flatten(list(test_net.parameters())))
-    users = [Client(u, u < corrupted_count, xtr[u::users_count], ytr[u::users_count], batch_size, layout, device,
+    xs, ys = xtr, ytr
+    if data_dir is not None:                                              # DistributedSampler's padded order (user.py:50)
+        order = _data.sampler_order(len(xtr), users_count).to(xtr.device)
+        xs, ys = xtr[order], ytr[order]
+    users = [Client(u, u < corrupted_count, xs[u::users_count], ys[u::users_count], batch_size, layout, device,
                     dataset) for u in range(users_count)]                                 # DistributedSampler-style partition (user.py:50)
     if backdoor:                                                          # main.py:44-54
-        trainer = BackdoorTrainer(backdoor, alpha, mal_epochs, layout, xtr, ytr, device, my_print, seed, dataset=dataset)
+        trainer = BackdoorTrainer(backdoor, alpha, mal_epochs, layout, xtr, ytr, device, my_print, seed, dataset=dataset,
+                                  sampled=data_dir is not None)
         attacker = malicious.BackdoorAttack(num_std, trainer.train)
     else:
         attacker = malicious.DriftAttack(num_std)
@@ -301,7 +342,7 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     my_print("Max accuracy: {}".format(max(accuracies)))
     os.makedirs(os.path.join(out_dir, "logs"), exist_ok=True)             # the reference needs a pre-made logs/ (readme.md:25)
     csv = os.path.join(out_dir, 'logs', csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate,
-                                                 dataset))
+                                                 dataset, data_dir))
     np.savetxt(csv, accuracies, delimiter=',')                            # main.py:100
     return accuracies, accuracies_epochs, csv
 
@@ -318,8 +359,10 @@ if __name__ == '__main__':
     p.add_argument('-o', '--output', type=str)
     p.add_argument('-b', '--backdoor', default='No', choices=['No', 'pattern', '1', '2', '3'])
     p.add_argument('-s', '--dataset', default='MNIST', choices=list(DATASETS))
+    p.add_argument('--data-dir', default=None, help="the directory holding torchvision's MNIST or CIFAR10 files "
+                   "(the reference's ./mnist_data or ./cifar10_data); without it a synthetic stand-in is trained")
     a = p.parse_args()
     bd = False if a.backdoor == 'No' else a.backdoor if a.backdoor == 'pattern' else int(a.backdoor)
     main(a.mal_prop, a.num_std, a.defense, users_count=a.users_count, epochs=a.epochs, learning_rate=a.learning_rate,
-         batch_size=a.batch_size, output=a.output, backdoor=bd, dataset=a.dataset,
+         batch_size=a.batch_size, output=a.output, backdoor=bd, dataset=a.dataset, data_dir=a.data_dir,
          fading_rate=2000 if a.dataset == 'CIFAR10' else 10000)                 # main.py:144-147

@@ -43,6 +43,14 @@ dataset='CIFAR10' (main.py -s CIFAR10) runs the same loop on harness.Cifar10Net 
 the CIFAR10 kernels (C ABI `afl_cifar10_client_grads` and `afl_cifar10_evaluate`) in steps 1 and 4 and SYNTH-CIFAR10
 log names.  A batch holds one dataset: the two models have different D.  CIFAR10 backdoor experiments are not batched
 (the trainer kernel is MnistNet's); `check` raises NotImplementedError for them and `harness.main` runs them.
+
+data_dir (--data-dir) trains on the real dataset's files there, as `harness.main(..., data_dir=...)` does: data.load's
+rows, each client's DistributedSampler shard (user.py:49-54) and the backdoor loaders' rows (backdoor.py:30-42), with
+main.py's log names (MNIST_..., CIFAR10_...).  The training data are one sampler-ordered copy per distinct padded
+length ceil(N / n) * n (users counts 10, 100, 250, 500 and 1000 share the 60,000 rows of MNIST), and the kernel reads
+each problem's set length from the device (C ABI `afl_*_client_grads_sets`); the test set is one copy for all seeds.
+
+    python -m attacking_federate_learning_b200.sweep --data-dir ./mnist_data -d Krum NoDefense -z 1.0 -n 10 51 -e 30
 """
 from __future__ import annotations
 
@@ -57,6 +65,7 @@ import torch
 
 from . import _native as nat
 from . import batched
+from . import data as _data
 from . import harness
 from ._device import momentum_step
 from .defences import DefenseTypes
@@ -161,10 +170,10 @@ def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, trai
     return kept, dropped
 
 
-def csv_name(exp, learning_rate, alpha=4, dataset='MNIST'):
+def csv_name(exp, learning_rate, alpha=4, dataset='MNIST', data_dir=None):
     """harness.main's log name for this experiment, with `_seed_<s>` before `.csv`."""
     name = harness.csv_name(exp.num_std, exp.defense, exp.backdoor, exp.mal_prop, exp.users_count, alpha, learning_rate,
-                            dataset)
+                            dataset, data_dir)
     return name[:-len('.csv')] + f'_seed_{exp.seed}.csv'
 
 
@@ -180,11 +189,12 @@ def fading_lr(epoch, learning_rate, fading_rate):
     return torch.div(num, epoch.to(torch.float64) + fading_rate)
 
 
-def backdoor_sets(specs):
+def backdoor_sets(specs, sampled=False):
     """The trainer kernel's backdoor sets from [(backdoor, x_train, y_train, seed), ...]: harness.backdoor_set (what
-    BackdoorTrainer trains and tests on) per spec, as x fp32 [n_sets, max_len, 784] and y int64 [n_sets, max_len], each
-    set zero-padded to the longest, and set_len int32 [n_sets], on the training sets' device."""
-    sets = [harness.backdoor_set(bd, x, y, seed, BACKDOOR_BATCH) for bd, x, y, seed in specs]
+    BackdoorTrainer trains and tests on, from the reference's sampler rows when sampled) per spec, as x fp32
+    [n_sets, max_len, 784] and y int64 [n_sets, max_len], each set zero-padded to the longest, and set_len int32
+    [n_sets], on the training sets' device."""
+    sets = [harness.backdoor_set(bd, x, y, seed, BACKDOOR_BATCH, sampled) for bd, x, y, seed in specs]
     dev, max_len = sets[0][0].device, max(len(x) for x, _ in sets)
     xs = torch.zeros((len(sets), max_len, sets[0][0].shape[-1]), dtype=torch.float32, device=dev)
     ys = torch.zeros((len(sets), max_len), dtype=torch.int64, device=dev)
@@ -225,12 +235,23 @@ class Sweep:
     pads); `rounds`: {defence: (slice, DeviceRound)} of the drift groups, `backdoor_rounds` the same for the backdoor
     groups, which occupy batch problems `bd0`..B-1.  Their DeviceRounds hold views of one f, z, lr and status over
     those problems, so the trainer reads every backdoor experiment in one launch.  `dataset` picks the model, the data
-    and the kernels: x_train and x_test are [n_seeds, n, 784] for MNIST and [n_seeds, n, 3, 32, 32] for CIFAR10."""
+    and the kernels: x_train and x_test are [n_sets, n, 784] for MNIST and [n_sets, n, 3, 32, 32] for CIFAR10.
+    Problem b trains on the first set_len[data_index[b]] rows of x_train[data_index[b]] and is tested on
+    x_test[test_index[b]]: one set per seed for the synthetic data; with data_dir one training set per padded length
+    (data.sampler_order) and one test set.  train_size and test_size: None (20,000 and 4,000 synthetic rows, or the
+    files' row counts), or those sizes."""
 
-    def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000,
-                 test_size=4000, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000,
-                 dataset='MNIST'):
+    def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None,
+                 test_size=None, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000,
+                 dataset='MNIST', data_dir=None):
         self.dataset = harness.check_dataset(dataset)
+        self.data_dir = data_dir
+        real = None
+        if data_dir is not None:
+            real = harness.real_sizes(dataset, data_dir, train_size, test_size)
+            train_size, test_size = len(real[0][0]), len(real[1][0])
+        train_size = 20000 if train_size is None else train_size
+        test_size = 4000 if test_size is None else test_size
         exps = [check(e, batch_size, train_size, dataset) for e in experiments]
         if not exps:
             raise ValueError("sweep: no experiment")
@@ -248,18 +269,43 @@ class Sweep:
         self.capture = capture
         dev = self.device = torch.device(device)
         seeds = list(dict.fromkeys(e.seed for e in self.experiments))
+        i32 = dict(dtype=torch.int32, device=dev)
         xtr, ytr, xte, yte, w0 = [], [], [], [], {}
         for s in seeds:                                                   # harness.main's start, seed by seed
-            (a, b), (c, d), net = harness.experiment_setup(s, train_size, test_size, dev, dataset)
-            xtr.append(a); ytr.append(b); xte.append(c); yte.append(d)
+            if real is None:
+                (a, b), (c, d), net = harness.experiment_setup(s, train_size, test_size, dev, dataset)
+                xtr.append(a); ytr.append(b); xte.append(c); yte.append(d)
+            else:                                                         # experiment_setup's weights, data loaded once
+                torch.manual_seed(s)
+                net = harness.model(dataset).to(dev)
             w0[s] = harness.ParamLayout(net.parameters()).flatten(list(net.parameters()))
-        self.x_train, self.y_train = torch.stack(xtr).contiguous(), torch.stack(ytr).contiguous()
-        self.x_test, self.y_test = torch.stack(xte).contiguous(), torch.stack(yte).contiguous()
+        if real is None:
+            self.x_train, self.y_train = torch.stack(xtr).contiguous(), torch.stack(ytr).contiguous()
+            self.x_test, self.y_test = torch.stack(xte).contiguous(), torch.stack(yte).contiguous()
+            self.set_len = torch.full((len(seeds),), train_size, **i32)
+            self.data_index = torch.tensor([seeds.index(e.seed) for e in self.experiments], **i32)
+            self.test_index = self.data_index
+        else:
+            (a, b), (c, d) = real
+            a, b = a.to(dev), b.to(dev)
+            xtr, ytr = [a] * len(seeds), [b] * len(seeds)                 # the backdoor sets' source, per seed
+            users = {}                                                    # padded length -> a users count with it
+            for e in self.experiments:
+                users.setdefault(_data.padded_length(train_size, e.users_count), e.users_count)
+            lengths = list(users)
+            self.x_train = torch.zeros((len(lengths), max(lengths)) + tuple(a.shape[1:]), dtype=a.dtype, device=dev)
+            self.y_train = torch.zeros((len(lengths), max(lengths)), dtype=b.dtype, device=dev)
+            for k, T in enumerate(lengths):
+                order = _data.sampler_order(train_size, users[T]).to(dev)
+                self.x_train[k, :T], self.y_train[k, :T] = a[order], b[order]
+            self.x_test, self.y_test = c.to(dev)[None].contiguous(), d.to(dev)[None].contiguous()
+            self.set_len = torch.tensor(lengths, **i32)
+            self.data_index = torch.tensor([lengths.index(_data.padded_length(train_size, e.users_count))
+                                            for e in self.experiments], **i32)
+            self.test_index = torch.zeros(len(self.experiments), **i32)
         B, self.D = len(self.experiments), w0[seeds[0]].numel()
         self.B = B
         self.N = max(e.users_count for e in self.experiments)
-        i32 = dict(dtype=torch.int32, device=dev)
-        self.data_index = torch.tensor([seeds.index(e.seed) for e in self.experiments], **i32)
         self.rows = torch.tensor([e.users_count for e in self.experiments], **i32)
         self.W = torch.stack([w0[e.seed] for e in self.experiments]).contiguous()
         self.V = torch.zeros_like(self.W)
@@ -273,7 +319,7 @@ class Sweep:
         self.correct = torch.zeros((self.n_tests, B), **i32)
         L = nat.lib()
         cifar = self.dataset == 'CIFAR10'
-        self._grads_fn = L.afl_cifar10_client_grads if cifar else L.afl_mnist_client_grads
+        self._grads_fn = L.afl_cifar10_client_grads_sets if cifar else L.afl_mnist_client_grads_sets
         self._evaluate_fn = L.afl_cifar10_evaluate if cifar else L.afl_mnist_evaluate
         ws_bytes = (L.afl_cifar10_evaluate_workspace_bytes if cifar else L.afl_mnist_evaluate_workspace_bytes)
         self._eval_ws = torch.empty(max(ws_bytes(B, test_size, batch_size), 256),
@@ -308,7 +354,7 @@ class Sweep:
         dev, i32 = self.device, dict(dtype=torch.int32, device=self.device)
         keys = list(dict.fromkeys((e.backdoor, e.seed) for e in bds))
         self.bd_x, self.bd_y, self.bd_len = backdoor_sets(
-            [(bd, xtr[seeds.index(s)], ytr[seeds.index(s)], s) for bd, s in keys])
+            [(bd, xtr[seeds.index(s)], ytr[seeds.index(s)], s) for bd, s in keys], sampled=self.data_dir is not None)
         self.bd_index = torch.tensor([keys.index((e.backdoor, e.seed)) for e in bds], **i32)
         self._bd_f = torch.zeros(nb, **i32)
         self._bd_z = torch.zeros(nb, dtype=torch.float64, device=dev)
@@ -325,9 +371,9 @@ class Sweep:
         with torch.cuda.device(self.device):
             nat.check(self._grads_fn(
                 self.W.data_ptr(), self.B, self.D, self.x_train.data_ptr(), self.y_train.data_ptr(),
-                self.x_train.shape[0], self.train_size, self.data_index.data_ptr(), self.rows.data_ptr(), self.N,
-                self.batch_size, self.epoch_counter.data_ptr(), G.data_ptr(), G.stride(0), G.stride(1),
-                torch.cuda.current_stream(self.device).cuda_stream))
+                self.x_train.shape[0], self.x_train.shape[1], self.set_len.data_ptr(), self.data_index.data_ptr(),
+                self.rows.data_ptr(), self.N, self.batch_size, self.epoch_counter.data_ptr(), G.data_ptr(), G.stride(0),
+                G.stride(1), torch.cuda.current_stream(self.device).cuda_stream))
 
     def backdoor_train(self, k=None):
         """The malicious networks of the backdoor experiments bd0 + k (all of them by default) in one launch
@@ -376,7 +422,7 @@ class Sweep:
         with torch.cuda.device(self.device):
             nat.check(self._evaluate_fn(
                 self.W.data_ptr(), self.B, self.D, self.x_test.data_ptr(), self.y_test.data_ptr(),
-                self.x_test.shape[0], self.test_size, self.data_index.data_ptr(), self.batch_size,
+                self.x_test.shape[0], self.test_size, self.test_index.data_ptr(), self.batch_size,
                 self.test_slot.data_ptr(), self.n_tests, self.loss_sum.data_ptr(), self.correct.data_ptr(),
                 self._eval_ws.data_ptr(), self._eval_ws.numel(), stream))
             if self.n_backdoor:
@@ -443,15 +489,17 @@ class Sweep:
         return out
 
 
-def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=20000, test_size=4000,
-        test_step=5, out_dir='.', capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000, dataset='MNIST'):
+def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None, test_size=None,
+        test_step=5, out_dir='.', capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000, dataset='MNIST',
+        data_dir=None):
     """Train every experiment for `epochs` epochs as one batch; write each one's accuracy CSV and the summary CSV under
     out_dir/logs.  Returns `Sweep.results()` with `csv` (None for a failed experiment) added to each dict.  Raises
     before any GPU work for an experiment main.py would reject (see `check`).  alpha, mal_epochs and fading_rate are
     harness.main's (the backdoor experiments' malicious training and client learning rate), and so is dataset ('MNIST'
-    or 'CIFAR10', main.py -s)."""
+    or 'CIFAR10', main.py -s).  data_dir: the real dataset's files (see the module docstring); train_size and test_size
+    are then None or the files' row counts, and None means 20,000 and 4,000 synthetic rows otherwise."""
     sw = Sweep(experiments, epochs, learning_rate, momentum, batch_size, train_size, test_size, test_step, capture,
-               device, alpha, mal_epochs, fading_rate, dataset)
+               device, alpha, mal_epochs, fading_rate, dataset, data_dir)
     with torch.cuda.device(sw.device):
         for epoch in range(epochs):
             sw.step(epoch)
@@ -467,7 +515,7 @@ def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, tra
             r['csv'] = None
             head = list(e[:5]) + ([e.backdoor] if with_bd else [])
             if r['error'] is None:
-                r['csv'] = os.path.join(logs, csv_name(e, learning_rate, alpha, sw.dataset))
+                r['csv'] = os.path.join(logs, csv_name(e, learning_rate, alpha, sw.dataset, sw.data_dir))
                 np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
                 bd = r.get('backdoor_accuracies')
                 tail = ([max(bd), bd[-1]] if bd else ['', '']) if with_bd else []
@@ -492,8 +540,11 @@ def main(argv=None):
     p.add_argument('-l', '--learning_rate', type=float, default=0.1)
     p.add_argument('--out-dir', default='.')
     p.add_argument('--no-capture', action='store_true')
+    p.add_argument('--data-dir', default=None, help="the directory holding torchvision's MNIST or CIFAR10 files (the "
+                   "reference's ./mnist_data or ./cifar10_data); without it the synthetic stand-in is trained")
     a = p.parse_args(argv)
-    kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size,
+    train_size = 20000 if a.data_dir is None else len(harness.real_sizes(a.dataset, a.data_dir)[0][0])
+    kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size, train_size,
                          backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)], dataset=a.dataset)
     for cell, e in dropped:
         print(f"skipped {cell}: {type(e).__name__}: {e}")
@@ -501,7 +552,7 @@ def main(argv=None):
         print("no experiment left to run")
         return []
     res = run(kept, a.epochs, a.learning_rate, batch_size=a.batch_size, out_dir=a.out_dir, capture=not a.no_capture,
-              fading_rate=FADING_RATE[a.dataset], dataset=a.dataset)
+              fading_rate=FADING_RATE[a.dataset], dataset=a.dataset, data_dir=a.data_dir)
     for r in res:
         e = r['experiment']
         if r['error'] is None:

@@ -550,6 +550,13 @@ int afl_backdoor_finish_batched_dev(int batch, int n, int64_t d, const int* f, c
  * harness.Client.step's cycling position.  1 <= n <= 1024 clients and n <= n_train, else AFL_ERR_BAD_ARG /
  * AFL_ERR_UNSUPPORTED; ld >= d and (batch > 1) batch_stride >= (n - 1) * ld + d, else AFL_ERR_BAD_ARG.
  *
+ * afl_mnist_client_grads_sets — afl_mnist_client_grads over training sets of their own lengths: set s starts at row
+ * s * n_rows of x and y and its first set_len[s] rows are its training set (set_len: device int32 [n_sets], read when
+ * the kernel runs), so client u of problem b takes rows u, u + n_b, ... of set data_index[b] with n_train =
+ * set_len[data_index[b]].  A problem whose set length lies outside [n_b, n_rows] is skipped: none of its rows is
+ * written.  The host checks are afl_mnist_client_grads' with n_rows for n_train, and a NULL set_len -> AFL_ERR_BAD_ARG.
+ * With every set_len[s] = n_rows the results equal afl_mnist_client_grads(..., n_train = n_rows, ...) bit for bit.
+ *
  * afl_mnist_evaluate — server.py:92-112 / harness.main's test loop for every problem: test batches of m rows (the last
  * one shorter), each batch's mean NLL in fp32, summed over the batches in order in float64 into
  * loss_sum[slot][b] (divide by n_test for the reported loss), and correct[slot][b] = the number of rows whose argmax
@@ -560,6 +567,10 @@ int afl_backdoor_finish_batched_dev(int batch, int n, int64_t d, const int* f, c
 int afl_mnist_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                            int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
                            float* G, int64_t batch_stride, int64_t ld, void* stream);
+int afl_mnist_client_grads_sets(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                                int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
+                                int n, int m, const int* epoch, float* G, int64_t batch_stride, int64_t ld,
+                                void* stream);
 size_t afl_mnist_evaluate_workspace_bytes(int batch, int n_test, int m);
 int afl_mnist_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                        int n_test, const int* data_index, int m, const int* slot_index, int n_slots, double* loss_sum,
@@ -614,12 +625,19 @@ int afl_mnist_backdoor_test(const float* weights, int batch, int64_t d, const fl
  * clients, shards, minibatches (from *epoch) and limits on n, ld and batch_stride.  Only columns [0, d) of rows u <
  * min(rows[b], n) of each problem are written.  No workspace: the kernel accumulates the weight gradients in the row.
  *
+ * afl_cifar10_client_grads_sets — afl_cifar10_client_grads over sets of their own lengths: afl_mnist_client_grads_sets'
+ * pitch n_rows, device set_len, skip rule and checks.
+ *
  * afl_cifar10_evaluate — server.py:92-112 / harness.main's test loop with Cifar10Net: afl_mnist_evaluate's batches,
  * float64 loss sums, first-maximum correct counts, NaN loss for a label outside 0..9, slot rule and workspace
  * (afl_cifar10_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned). */
 int afl_cifar10_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                              int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
                              float* G, int64_t batch_stride, int64_t ld, void* stream);
+int afl_cifar10_client_grads_sets(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                                  int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
+                                  int n, int m, const int* epoch, float* G, int64_t batch_stride, int64_t ld,
+                                  void* stream);
 size_t afl_cifar10_evaluate_workspace_bytes(int batch, int n_test, int m);
 int afl_cifar10_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                          int n_test, const int* data_index, int m, const int* slot_index, int n_slots,

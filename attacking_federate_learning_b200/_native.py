@@ -105,6 +105,11 @@ SIGNATURES = {
                                            _i64, _vp]),
     "afl_cifar10_evaluate_workspace_bytes": (_sz, [_i, _i, _i]),
     "afl_cifar10_evaluate": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "afl_cifar10_backdoor_train_workspace_bytes": (_sz, [_i]),
+    "afl_cifar10_backdoor_train": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _d, _i, _i, _vp,
+                                        _sz, _vp]),
+    "afl_cifar10_backdoor_test_workspace_bytes": (_sz, [_i, _i, _i]),
+    "afl_cifar10_backdoor_test": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }
 
 _lib = None

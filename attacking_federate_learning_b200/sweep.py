@@ -38,11 +38,14 @@ key, so the experiments of a batch would overwrite one file.
     python -m attacking_federate_learning_b200.sweep -d Krum TrimmedMean -z 0.5 1.5 -m 0.1 0.24 -n 10 --seeds 0 1 -e 30
     python -m attacking_federate_learning_b200.sweep -d Krum NoDefense -z 1.0 -b No pattern 1 --seeds 0 1 -e 30
     python -m attacking_federate_learning_b200.sweep -s CIFAR10 -d Krum TrimmedMean -z 0.5 1.5 --seeds 0 1 -e 30
+    python -m attacking_federate_learning_b200.sweep -s CIFAR10 -d Krum NoDefense -z 1.0 -b pattern 1 --cifar10-backdoor
 
 dataset='CIFAR10' (main.py -s CIFAR10) runs the same loop on harness.Cifar10Net and `synthetic_cifar_problem`, with
 the CIFAR10 kernels (C ABI `afl_cifar10_client_grads` and `afl_cifar10_evaluate`) in steps 1 and 4 and SYNTH-CIFAR10
-log names.  A batch holds one dataset: the two models have different D.  CIFAR10 backdoor experiments are not batched
-(the trainer kernel is MnistNet's); `check` raises NotImplementedError for them and `harness.main` runs them.
+log names.  A batch holds one dataset: the two models have different D.  CIFAR10 backdoor experiments
+(main.py -s CIFAR10 -b ...) are batched with cifar10_backdoor=True (--cifar10-backdoor): the attacker's Cifar10Net
+trains in the CIFAR10 trainer kernel (C ABI `afl_cifar10_backdoor_train`) and its backdoor test is
+`afl_cifar10_backdoor_test`.  Without the switch `check` raises NotImplementedError for them, as before.
 
 data_dir (--data-dir) trains on the real dataset's files there, as `harness.main(..., data_dir=...)` does: data.load's
 rows, each client's DistributedSampler shard (user.py:49-54) and the backdoor loaders' rows (backdoor.py:30-42), with
@@ -125,15 +128,17 @@ def minibatch(n_train, users_count, user, batch_size, epoch):
     return k * batch_size, min(k * batch_size + batch_size, length)
 
 
-def check(exp, batch_size=83, train_size=20000, dataset='MNIST'):
+def check(exp, batch_size=83, train_size=20000, dataset='MNIST', cifar10_backdoor=False):
     """Raise what main.py would raise for this experiment at its first `defend` (AssertionError for the reference's
-    asserts), or for what the sweep's kernels do not take.  Returns the normalised Experiment."""
+    asserts), or for what the sweep's kernels do not take.  A CIFAR10 backdoor experiment is taken only with
+    cifar10_backdoor=True.  Returns the normalised Experiment."""
     if len(exp) not in (5, 6):
         raise ValueError(f"{exp}: an experiment has 5 or 6 elements")
     exp = Experiment(str(exp[0]), float(exp[1]), float(exp[2]), int(exp[3]), int(exp[4]),
                      normalise_backdoor(exp[5]) if len(exp) == 6 else False)
-    if harness.check_dataset(dataset) == 'CIFAR10' and exp.backdoor is not False:
-        raise NotImplementedError(f"{exp}: the sweep trains no CIFAR10 backdoor attacker (harness.main runs it)")
+    if harness.check_dataset(dataset) == 'CIFAR10' and exp.backdoor is not False and not cifar10_backdoor:
+        raise NotImplementedError(f"{exp}: CIFAR10 backdoor experiments need cifar10_backdoor=True "
+                                  "(--cifar10-backdoor)")
     if exp.backdoor not in (False, 'pattern') and exp.backdoor > train_size:
         raise ValueError(f"{exp}: backdoor sample {exp.backdoor} lies past the training set ({train_size} rows)")
     if exp.defense not in RULES:
@@ -155,7 +160,7 @@ def check(exp, batch_size=83, train_size=20000, dataset='MNIST'):
 
 
 def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000, backdoors=(False,),
-         dataset='MNIST'):
+         dataset='MNIST', cifar10_backdoor=False):
     """The Cartesian grid (defence-major, backdoor-minor) as (kept experiments, [(experiment, rejection), ...]): a cell
     main.py would reject is dropped with the exception `check` raises for it.  A drift cell (backdoor False) has 5
     elements, a backdoor cell 6."""
@@ -164,7 +169,7 @@ def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, trai
         if cell[5] is False:
             cell = cell[:5]
         try:
-            kept.append(check(cell, batch_size, train_size, dataset))
+            kept.append(check(cell, batch_size, train_size, dataset, cifar10_backdoor))
         except (AssertionError, KeyError, ValueError, NotImplementedError) as e:
             dropped.append((cell, e))
     return kept, dropped
@@ -192,11 +197,11 @@ def fading_lr(epoch, learning_rate, fading_rate):
 def backdoor_sets(specs, sampled=False):
     """The trainer kernel's backdoor sets from [(backdoor, x_train, y_train, seed), ...]: harness.backdoor_set (what
     BackdoorTrainer trains and tests on, from the reference's sampler rows when sampled) per spec, as x fp32
-    [n_sets, max_len, 784] and y int64 [n_sets, max_len], each set zero-padded to the longest, and set_len int32
-    [n_sets], on the training sets' device."""
+    [n_sets, max_len, *row shape] ([.., 784] for MNIST, [.., 3, 32, 32] for CIFAR10) and y int64 [n_sets, max_len],
+    each set zero-padded to the longest, and set_len int32 [n_sets], on the training sets' device."""
     sets = [harness.backdoor_set(bd, x, y, seed, BACKDOOR_BATCH, sampled) for bd, x, y, seed in specs]
     dev, max_len = sets[0][0].device, max(len(x) for x, _ in sets)
-    xs = torch.zeros((len(sets), max_len, sets[0][0].shape[-1]), dtype=torch.float32, device=dev)
+    xs = torch.zeros((len(sets), max_len) + tuple(sets[0][0].shape[1:]), dtype=torch.float32, device=dev)
     ys = torch.zeros((len(sets), max_len), dtype=torch.int64, device=dev)
     for k, (x, y) in enumerate(sets):
         xs[k, :len(x)] = x
@@ -239,11 +244,11 @@ class Sweep:
     Problem b trains on the first set_len[data_index[b]] rows of x_train[data_index[b]] and is tested on
     x_test[test_index[b]]: one set per seed for the synthetic data; with data_dir one training set per padded length
     (data.sampler_order) and one test set.  train_size and test_size: None (20,000 and 4,000 synthetic rows, or the
-    files' row counts), or those sizes."""
+    files' row counts), or those sizes.  cifar10_backdoor: take CIFAR10 backdoor experiments (see `check`)."""
 
     def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None,
                  test_size=None, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000,
-                 dataset='MNIST', data_dir=None):
+                 dataset='MNIST', data_dir=None, cifar10_backdoor=False):
         self.dataset = harness.check_dataset(dataset)
         self.data_dir = data_dir
         real = None
@@ -252,7 +257,7 @@ class Sweep:
             train_size, test_size = len(real[0][0]), len(real[1][0])
         train_size = 20000 if train_size is None else train_size
         test_size = 4000 if test_size is None else test_size
-        exps = [check(e, batch_size, train_size, dataset) for e in experiments]
+        exps = [check(e, batch_size, train_size, dataset, cifar10_backdoor) for e in experiments]
         if not exps:
             raise ValueError("sweep: no experiment")
         if epochs < 1 or test_step < 1 or test_size < 1:
@@ -346,7 +351,8 @@ class Sweep:
 
     def _setup_backdoor(self, xtr, ytr, seeds):
         """The backdoor experiments' sets (harness.backdoor_set, one per (backdoor, seed), padded to the longest),
-        their trainer state and their backdoor-test tables."""
+        their trainer state and their backdoor-test tables; for CIFAR10 also the trainer's gradient rows and the
+        backdoor test's batch tables, allocated once so that captured graphs keep their pointers."""
         bds = self.experiments[self.bd0:]
         self.n_backdoor = nb = len(bds)
         if not nb:
@@ -364,6 +370,13 @@ class Sweep:
         self.bd_mal = torch.empty((nb, self.D), dtype=torch.float32, device=dev)
         self.bd_loss_sum = torch.zeros((self.n_tests, nb), dtype=torch.float64, device=dev)
         self.bd_correct = torch.zeros((self.n_tests, nb), **i32)
+        if self.dataset == 'CIFAR10':
+            L = nat.lib()
+            self._bd_train_ws = torch.empty(L.afl_cifar10_backdoor_train_workspace_bytes(nb), dtype=torch.uint8,
+                                            device=dev)
+            self._bd_test_ws = torch.empty(
+                L.afl_cifar10_backdoor_test_workspace_bytes(nb, self.bd_x.shape[1], BACKDOOR_BATCH), dtype=torch.uint8,
+                device=dev)
 
     def client_grads(self):
         """Step 1: every client's gradient into G at the current device epoch."""
@@ -379,13 +392,19 @@ class Sweep:
         """The malicious networks of the backdoor experiments bd0 + k (all of them by default) in one launch
         (BackdoorTrainer.train), from bd_initial[k] into bd_mal[k]."""
         k = slice(0, self.n_backdoor) if k is None else k
-        with torch.cuda.device(self.device):
-            nat.check(nat.lib().afl_mnist_backdoor_train(
-                self.bd_initial[k].data_ptr(), self.bd_mal[k].data_ptr(), k.stop - k.start, self.D,
+        args = (self.bd_initial[k].data_ptr(), self.bd_mal[k].data_ptr(), k.stop - k.start, self.D,
                 self.bd_x.data_ptr(), self.bd_y.data_ptr(), self.bd_x.shape[0], self.bd_x.shape[1],
                 self.bd_len.data_ptr(), self.bd_index[k].data_ptr(), self._bd_f[k].data_ptr(), self._bd_z[k].data_ptr(),
-                self._bd_status[k].data_ptr(), float(self.alpha), self.mal_epochs, BACKDOOR_BATCH,
-                torch.cuda.current_stream(self.device).cuda_stream))
+                self._bd_status[k].data_ptr(), float(self.alpha), self.mal_epochs, BACKDOOR_BATCH)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        with torch.cuda.device(self.device):
+            if self.dataset == 'CIFAR10':                                 # problem b's gradient row: D floats at b D
+                L = nat.lib()
+                nat.check(L.afl_cifar10_backdoor_train(
+                    *args, self._bd_train_ws.data_ptr() + k.start * self.D * 4,
+                    L.afl_cifar10_backdoor_train_workspace_bytes(k.stop - k.start), stream))
+            else:
+                nat.check(nat.lib().afl_mnist_backdoor_train(*args, stream))
 
     def _defend(self, r, sl, rnd):
         agg = {DefenseTypes.Krum: rnd.krum, DefenseTypes.Bulyan: rnd.bulyan,
@@ -426,11 +445,15 @@ class Sweep:
                 self.test_slot.data_ptr(), self.n_tests, self.loss_sum.data_ptr(), self.correct.data_ptr(),
                 self._eval_ws.data_ptr(), self._eval_ws.numel(), stream))
             if self.n_backdoor:
-                nat.check(nat.lib().afl_mnist_backdoor_test(
-                    self.W[self.bd0:].data_ptr(), self.n_backdoor, self.D, self.bd_x.data_ptr(), self.bd_y.data_ptr(),
-                    self.bd_x.shape[0], self.bd_x.shape[1], self.bd_len.data_ptr(), self.bd_index.data_ptr(),
-                    BACKDOOR_BATCH, self.test_slot.data_ptr(), self.n_tests, self.bd_loss_sum.data_ptr(),
-                    self.bd_correct.data_ptr(), stream))
+                args = (self.W[self.bd0:].data_ptr(), self.n_backdoor, self.D, self.bd_x.data_ptr(),
+                        self.bd_y.data_ptr(), self.bd_x.shape[0], self.bd_x.shape[1], self.bd_len.data_ptr(),
+                        self.bd_index.data_ptr(), BACKDOOR_BATCH, self.test_slot.data_ptr(), self.n_tests,
+                        self.bd_loss_sum.data_ptr(), self.bd_correct.data_ptr())
+                if self.dataset == 'CIFAR10':
+                    nat.check(nat.lib().afl_cifar10_backdoor_test(*args, self._bd_test_ws.data_ptr(),
+                                                                  self._bd_test_ws.numel(), stream))
+                else:
+                    nat.check(nat.lib().afl_mnist_backdoor_test(*args, stream))
         self.test_slot.add_(1)
 
     def is_test_epoch(self, epoch):
@@ -491,15 +514,16 @@ class Sweep:
 
 def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None, test_size=None,
         test_step=5, out_dir='.', capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000, dataset='MNIST',
-        data_dir=None):
+        data_dir=None, cifar10_backdoor=False):
     """Train every experiment for `epochs` epochs as one batch; write each one's accuracy CSV and the summary CSV under
     out_dir/logs.  Returns `Sweep.results()` with `csv` (None for a failed experiment) added to each dict.  Raises
     before any GPU work for an experiment main.py would reject (see `check`).  alpha, mal_epochs and fading_rate are
     harness.main's (the backdoor experiments' malicious training and client learning rate), and so is dataset ('MNIST'
     or 'CIFAR10', main.py -s).  data_dir: the real dataset's files (see the module docstring); train_size and test_size
-    are then None or the files' row counts, and None means 20,000 and 4,000 synthetic rows otherwise."""
+    are then None or the files' row counts, and None means 20,000 and 4,000 synthetic rows otherwise.
+    cifar10_backdoor=True takes CIFAR10 backdoor experiments (main.py -s CIFAR10 -b ...)."""
     sw = Sweep(experiments, epochs, learning_rate, momentum, batch_size, train_size, test_size, test_step, capture,
-               device, alpha, mal_epochs, fading_rate, dataset, data_dir)
+               device, alpha, mal_epochs, fading_rate, dataset, data_dir, cifar10_backdoor)
     with torch.cuda.device(sw.device):
         for epoch in range(epochs):
             sw.step(epoch)
@@ -542,17 +566,21 @@ def main(argv=None):
     p.add_argument('--no-capture', action='store_true')
     p.add_argument('--data-dir', default=None, help="the directory holding torchvision's MNIST or CIFAR10 files (the "
                    "reference's ./mnist_data or ./cifar10_data); without it the synthetic stand-in is trained")
+    p.add_argument('--cifar10-backdoor', action='store_true', help="train CIFAR10 backdoor experiments (-s CIFAR10 "
+                   "-b pattern|1|2|3) in the CIFAR10 trainer kernel; without it they are skipped")
     a = p.parse_args(argv)
     train_size = 20000 if a.data_dir is None else len(harness.real_sizes(a.dataset, a.data_dir)[0][0])
     kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size, train_size,
-                         backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)], dataset=a.dataset)
+                         backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)], dataset=a.dataset,
+                         cifar10_backdoor=a.cifar10_backdoor)
     for cell, e in dropped:
         print(f"skipped {cell}: {type(e).__name__}: {e}")
     if not kept:
         print("no experiment left to run")
         return []
     res = run(kept, a.epochs, a.learning_rate, batch_size=a.batch_size, out_dir=a.out_dir, capture=not a.no_capture,
-              fading_rate=FADING_RATE[a.dataset], dataset=a.dataset, data_dir=a.data_dir)
+              fading_rate=FADING_RATE[a.dataset], dataset=a.dataset, data_dir=a.data_dir,
+              cifar10_backdoor=a.cifar10_backdoor)
     for r in res:
         e = r['experiment']
         if r['error'] is None:

@@ -643,6 +643,35 @@ int afl_cifar10_evaluate(const float* weights, int batch, int64_t d, const float
                          int n_test, const int* data_index, int m, const int* slot_index, int n_slots,
                          double* loss_sum, int* correct, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- the backdoor attacker's Cifar10Net (csrc/cifar_backdoor.cu): the model half of a CIFAR10 backdoor sweep epoch --
+ * The afl_mnist_backdoor_* entries above with Cifar10Net (D = 117,706): the same backdoor sets, activity condition,
+ * BEFORE test, SGD steps, status codes, slot rule and outputs, with x device fp32 [n_sets][max_len][3072] (the NCHW
+ * [3, 32, 32] images flattened) and the MSE term over Cifar10Net's ten tensors.  The forward and backward passes are
+ * afl_cifar10_client_grads' (the 23x23 corner, torch's max_pool2d rules), so one training step's NLL gradient is that
+ * call's on the same rows bit for bit.  One CTA per problem for the training, fp32 FFMA throughout, no atomics and
+ * every sum in a fixed order, so a problem's result depends only on its own inputs; no allocation, copy or
+ * synchronisation, so the calls can be captured in a CUDA graph.  Checked before any CUDA call: a NULL pointer, batch /
+ * n_sets / max_len / m < 1, mal_epochs < 0, a NaN alpha or a short workspace -> AFL_ERR_BAD_ARG; d != 117,706,
+ * m > 200 or batch > 65535 -> AFL_ERR_UNSUPPORTED.
+ *
+ * afl_cifar10_backdoor_train — afl_mnist_backdoor_train's contract.  workspace: device memory of at least
+ * afl_cifar10_backdoor_train_workspace_bytes(batch) bytes (4-byte aligned; problem b's step gradient lives in floats
+ * [b d, b d + d)), overlapping neither initial nor out.
+ *
+ * afl_cifar10_backdoor_test — afl_mnist_backdoor_test's contract, as one CTA per (test batch, problem) and a finish
+ * kernel that sums the batches in order.  workspace: afl_cifar10_backdoor_test_workspace_bytes(batch, max_len, m)
+ * bytes, 256-byte aligned; ceil(max_len / m) > 65535 -> AFL_ERR_UNSUPPORTED. */
+size_t afl_cifar10_backdoor_train_workspace_bytes(int batch);
+int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int64_t d, const float* x, const int64_t* y,
+                               int n_sets, int max_len, const int* set_len, const int* data_index, const int* f,
+                               const double* z, int* status, double alpha, int mal_epochs, int m, void* workspace,
+                               size_t workspace_bytes, void* stream);
+size_t afl_cifar10_backdoor_test_workspace_bytes(int batch, int max_len, int m);
+int afl_cifar10_backdoor_test(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                              int max_len, const int* set_len, const int* data_index, int m, const int* slot_index,
+                              int n_slots, double* loss_sum, int* correct, void* workspace, size_t workspace_bytes,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

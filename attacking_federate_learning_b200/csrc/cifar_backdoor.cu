@@ -15,7 +15,6 @@
 // parameters being trained, which are the output vector itself.  Every sum is one thread's loop in a fixed order and
 // nothing is atomic, so a problem's result depends only on its own initial vector, its set and the hyperparameters.
 // Full fp32 FFMA throughout (no TF32).
-#include "afl_common.cuh"
 #include "cifar_net.cuh"
 
 namespace afl {
@@ -23,40 +22,12 @@ namespace cifar {
 
 constexpr int kMaxRows = 200;                       // BackdoorTrainer's minibatch and test batch
 constexpr size_t kSmemRows = smem_bytes(kMaxRows);
-constexpr float kLr = 0.1f, kWeightDecay = 1e-4f;   // backdoor.py:134
 
 // mse_loss's backward factor 2 / numel of the tensor holding parameter o (ParamLayout order).
 __device__ __forceinline__ float mse_norm(int o) {
   return o < kOffB1c ? 2.f / 432   : o < kOffW2c ? 2.f / 16  : o < kOffB2c ? 2.f / 16'384 : o < kOffW1 ? 2.f / 64
        : o < kOffB1  ? 2.f / 24'576 : o < kOffW2  ? 2.f / 384 : o < kOffB2  ? 2.f / 73'728 : o < kOffW3 ? 2.f / 192
        : o < kOffB3  ? 2.f / 1'920  : 2.f / 10;
-}
-
-// backdoor_train.cu's sgd: one SGD step of one element from a fresh optimiser.  g is the NLL gradient; with alpha > 0
-// the MSE term's ((p - p0) * 2/numel) * alpha is added; then d_p = g + 1e-4 p and p - 0.1 d_p.  *bad is set when the
-// new p - p0 is NaN, which makes the next dist loss NaN.
-__device__ __forceinline__ float sgd(float p, float p0, float g, float norm, float alpha, bool dist, bool* bad) {
-  if (dist) g = __fadd_rn(g, __fmul_rn(__fmul_rn(__fsub_rn(p, p0), norm), alpha));
-  const float dp = __fmaf_rn(kWeightDecay, p, g);
-  const float np = __fmaf_rn(-kLr, dp, p);
-  const float r = __fsub_rn(np, p0);
-  if (r != r) *bad = true;
-  return np;
-}
-
-// Row i of the chunk (logits in s.Z): its NLL (-logp[label]; NaN for a label outside 0..9) and whether torch's
-// out.max(1)[1] is the label (the first NaN, else the first maximum).
-__device__ __forceinline__ float row_nll(const Smem& s, int i, int yi, bool* hit) {
-  float z[kOut], lp[kOut];
-#pragma unroll
-  for (int c = 0; c < kOut; ++c) z[c] = s.Z[i * kOut + c];
-  log_softmax_row(z, lp);
-  int best = 0;
-#pragma unroll
-  for (int c = 1; c < kOut; ++c)
-    if (lp[best] == lp[best] && (lp[c] != lp[c] || lp[c] > lp[best])) best = c;
-  *hit = best == yi;
-  return yi >= 0 && yi < kOut ? -lp[yi] : __int_as_float(0x7fc00000);
 }
 
 // Rows lo .. lo + mb of the set into s.row / s.label.  Ends at a barrier.
@@ -106,7 +77,7 @@ backdoor_train_kernel(const float* __restrict__ initial, float* out, const float
       const int mc = min(kS, mb - c0);
       forward_chunk<true>(xs, p0, c0, mc, s);
       bool hit = false;
-      if (t < mc) row_nll(s, t, s.label[c0 + t], &hit);
+      if (t < mc) train::row_head(s.Z + t * kOut, s.label[c0 + t], &hit);
       correct += __syncthreads_count(hit);
     }
   }
@@ -130,7 +101,7 @@ backdoor_train_kernel(const float* __restrict__ initial, float* out, const float
         forward_chunk<false>(xs, p, c0, mc, s);
         if (t < mc) {
           bool hit;
-          const float l = row_nll(s, t, s.label[c0 + t], &hit);
+          const float l = train::row_head(s.Z + t * kOut, s.label[c0 + t], &hit);
           nan_row |= l != l;
         }
         backward_chunk<false>(xs, p, c0, mc, mb, c0 == 0, s, g);
@@ -140,7 +111,7 @@ backdoor_train_kernel(const float* __restrict__ initial, float* out, const float
         return;
       }
       bad = false;
-      for (int o = t; o < kD; o += kThreads) p[o] = sgd(p[o], p0[o], g[o], mse_norm(o), alpha, dist, &bad);
+      for (int o = t; o < kD; o += kThreads) p[o] = train::sgd(p[o], p0[o], g[o], mse_norm(o), alpha, dist, &bad);
       dist_nan = __syncthreads_or(bad);                                 // also: every update lands before the next read
     }
   }
@@ -171,7 +142,7 @@ backdoor_test_kernel(const float* __restrict__ weights, const float* __restrict_
     forward_chunk<true>(xs, w, c0, mc, s);
     if (threadIdx.x < mc) {
       bool hit;
-      s.nll[c0 + threadIdx.x] = row_nll(s, threadIdx.x, s.label[c0 + threadIdx.x], &hit);
+      s.nll[c0 + threadIdx.x] = train::row_head(s.Z + threadIdx.x * kOut, s.label[c0 + threadIdx.x], &hit);
       s.hit[c0 + threadIdx.x] = hit ? 1.f : 0.f;
     }
     __syncthreads();
@@ -213,29 +184,6 @@ __global__ void backdoor_test_finish_kernel(int batch, int nb, int n_sets, int m
 static int smem_done_bd_train[kMaxDevices];
 static int smem_done_bd_test[kMaxDevices];
 
-// The checks both calls share: pointers are checked by the callers.
-static int check_backdoor(const char* who, int batch, int64_t d, int n_sets, int max_len, int m) {
-  if (batch < 1 || n_sets < 1 || max_len < 1 || m < 1) {
-    set_error("%s: batch, n_sets, max_len and m must be >= 1 (got %d, %d, %d, %d)", who, batch, n_sets, max_len, m);
-    return AFL_ERR_BAD_ARG;
-  }
-  if (d != kD) {
-    set_error("%s: the Cifar10Net layout has D = %lld parameters (got %lld)", who, static_cast<long long>(kD),
-              static_cast<long long>(d));
-    return AFL_ERR_UNSUPPORTED;
-  }
-  if (m > kMaxRows) { set_error("%s: batch size m <= %d (got %d)", who, kMaxRows, m); return AFL_ERR_UNSUPPORTED; }
-  if (batch > 65535) { set_error("%s: batch <= 65535 problems (got %d)", who, batch); return AFL_ERR_UNSUPPORTED; }
-  return AFL_OK;
-}
-
-static int64_t test_batches(int max_len, int m) { return (int64_t(max_len) + m - 1) / m; }
-
-static bool overlap(const void* a, size_t na, const void* b, size_t nb) {
-  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
-  return x < y + nb && y < x + na;
-}
-
 }  // namespace cifar
 }  // namespace afl
 
@@ -257,7 +205,9 @@ int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int6
     set_error("%s: a pointer argument is NULL", who);
     return AFL_ERR_BAD_ARG;
   }
-  if (int rc = cifar::check_backdoor(who, batch, d, n_sets, max_len, m)) return rc;
+  if (int rc = train::check_common(who, "Cifar10Net", cifar::kD, cifar::kMaxRows, "max_len", batch, d, n_sets,
+                                   max_len, m))
+    return rc;
   if (mal_epochs < 0 || alpha != alpha) {
     set_error("%s: mal_epochs must be >= 0 and alpha a number (got %d, %g)", who, mal_epochs, alpha);
     return AFL_ERR_BAD_ARG;
@@ -268,8 +218,8 @@ int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int6
     return AFL_ERR_BAD_ARG;
   }
   const size_t span = static_cast<size_t>(batch) * cifar::kD * sizeof(float);
-  if (cifar::overlap(initial, span, out, span) || cifar::overlap(workspace, need, out, span) ||
-      cifar::overlap(workspace, need, initial, span)) {
+  if (train::overlap(initial, span, out, span) || train::overlap(workspace, need, out, span) ||
+      train::overlap(workspace, need, initial, span)) {
     set_error("%s: out, initial and the workspace must not overlap", who);
     return AFL_ERR_BAD_ARG;
   }
@@ -285,9 +235,7 @@ int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int6
 }
 
 size_t afl_cifar10_backdoor_test_workspace_bytes(int batch, int max_len, int m) {
-  if (batch < 1 || max_len < 1 || m < 1) return 0;
-  const size_t per = static_cast<size_t>(batch) * cifar::test_batches(max_len, m);
-  return align_up(per * sizeof(float), 256) + align_up(per * sizeof(int), 256);
+  return train::eval_workspace_bytes(batch, max_len, m);
 }
 
 int afl_cifar10_backdoor_test(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
@@ -299,26 +247,21 @@ int afl_cifar10_backdoor_test(const float* weights, int batch, int64_t d, const 
     set_error("%s: a pointer argument is NULL", who);
     return AFL_ERR_BAD_ARG;
   }
-  if (int rc = cifar::check_backdoor(who, batch, d, n_sets, max_len, m)) return rc;
+  if (int rc = train::check_common(who, "Cifar10Net", cifar::kD, cifar::kMaxRows, "max_len", batch, d, n_sets,
+                                   max_len, m))
+    return rc;
   if (n_slots < 1) { set_error("%s: n_slots must be >= 1 (got %d)", who, n_slots); return AFL_ERR_BAD_ARG; }
-  const size_t need = afl_cifar10_backdoor_test_workspace_bytes(batch, max_len, m);
-  if (workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 256) {
-    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, workspace_bytes, need);
-    return AFL_ERR_BAD_ARG;
-  }
-  const int64_t nb = cifar::test_batches(max_len, m);
-  if (nb > 65535) { set_error("%s: at most 65535 test batches (got %lld)", who, static_cast<long long>(nb)); return AFL_ERR_UNSUPPORTED; }
-  float* batch_loss = static_cast<float*>(workspace);
-  int* batch_correct = reinterpret_cast<int*>(static_cast<char*>(workspace) +
-                                              align_up(static_cast<size_t>(batch) * nb * sizeof(float), 256));
+  train::EvalWorkspace ws;
+  if (int rc = train::carve_eval_workspace(who, workspace, workspace_bytes, batch, max_len, m, AFL_ERR_BAD_ARG, &ws))
+    return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   AFL_CUDA(ensure_dyn_smem(cifar::backdoor_test_kernel, static_cast<int>(cifar::kSmemRows), cifar::smem_done_bd_test));
-  cifar::backdoor_test_kernel<<<dim3(static_cast<unsigned>(nb), batch), cifar::kThreads, cifar::kSmemRows, st>>>(
-      weights, x, y, n_sets, max_len, set_len, data_index, m, slot_index, n_slots, batch_loss, batch_correct);
+  cifar::backdoor_test_kernel<<<dim3(ws.nb, batch), cifar::kThreads, cifar::kSmemRows, st>>>(
+      weights, x, y, n_sets, max_len, set_len, data_index, m, slot_index, n_slots, ws.batch_loss, ws.batch_correct);
   AFL_LAUNCH_CHECK("cifar10_backdoor_test_kernel");
   cifar::backdoor_test_finish_kernel<<<(batch + 127) / 128, 128, 0, st>>>(
-      batch, static_cast<int>(nb), n_sets, max_len, set_len, data_index, m, batch_loss, batch_correct, slot_index,
-      n_slots, loss_sum, correct);
+      batch, ws.nb, n_sets, max_len, set_len, data_index, m, ws.batch_loss, ws.batch_correct, slot_index, n_slots,
+      loss_sum, correct);
   AFL_LAUNCH_CHECK("cifar10_backdoor_test_finish_kernel");
   return AFL_OK;
 }

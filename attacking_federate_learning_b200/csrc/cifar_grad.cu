@@ -17,22 +17,10 @@
 // of a window is its first maximum in row-major order, a NaN takes the index, and the backward routes the window's
 // gradient to that index alone.  The chunk passes and the shared-memory carve live in cifar_net.cuh, which the backdoor
 // attacker's trainer (cifar_backdoor.cu) shares.
-#include "afl_common.cuh"
 #include "cifar_net.cuh"
 
 namespace afl {
 namespace cifar {
-
-// Client u's minibatch at epoch e: client_grad.cu's batch_start (harness.Client.step's cycling position).
-__device__ __forceinline__ int batch_start(int n_train, int n, int u, int m, int e, int* mb) {
-  const int L = (n_train - u + n - 1) / n;
-  const int q = (L + m - 1) / m;
-  int k = e % q;
-  if (k < 0) k += q;
-  const int lo = k * m;
-  *mb = min(lo + m, L) - lo;
-  return lo;
-}
 
 __global__ void __launch_bounds__(kThreads, 2)
 client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ x, const int64_t* __restrict__ y,
@@ -51,7 +39,7 @@ client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ 
   const float* xs = x + int64_t(set) * n_rows * kImg;
   const int64_t* ys = y + int64_t(set) * n_rows;
   int mb;
-  const int lo = batch_start(n_train, n, u, m, *epoch, &mb);
+  const int lo = train::batch_start(n_train, n, u, m, *epoch, &mb);
   for (int i = threadIdx.x; i < mb; i += kThreads) {
     const int r = u + n * (lo + i);
     s.row[i] = r;
@@ -91,18 +79,11 @@ evaluate_kernel(const float* __restrict__ weights, const float* __restrict__ x, 
   for (int c0 = 0; c0 < mb; c0 += kS) {
     const int mc = min(kS, mb - c0);
     forward_chunk<true>(xs, w, c0, mc, s);
-    // per row: its NLL, and 1 when the argmax (first maximum) is the label
+    // per row: its NLL, and 1 when the argmax is the label
     for (int i = threadIdx.x; i < mc; i += kThreads) {
-      float z[kOut], lp[kOut];
-#pragma unroll
-      for (int c = 0; c < kOut; ++c) z[c] = s.Z[i * kOut + c];
-      log_softmax_row(z, lp);
-      int best = 0;
-#pragma unroll
-      for (int c = 1; c < kOut; ++c) best = lp[c] > lp[best] ? c : best;
-      const int yi = s.label[c0 + i];
-      s.nll[c0 + i] = yi >= 0 && yi < kOut ? -lp[yi] : __int_as_float(0x7fc00000);   // a label outside 0..9: NaN
-      s.hit[c0 + i] = best == yi ? 1.f : 0.f;
+      bool hit;
+      s.nll[c0 + i] = train::row_head(s.Z + i * kOut, s.label[c0 + i], &hit);
+      s.hit[c0 + i] = hit ? 1.f : 0.f;
     }
     __syncthreads();
   }
@@ -118,60 +99,15 @@ evaluate_kernel(const float* __restrict__ weights, const float* __restrict__ x, 
   }
 }
 
-// loss_sum[slot][b] = sum_t batch_loss[b][t] in float64, t in order (harness.main's `test_loss += ....item()`);
-// correct[slot][b] = sum_t batch_correct[b][t].  A slot outside [0, n_slots) writes nothing.
-__global__ void evaluate_finish_kernel(int batch, int nb, const int* __restrict__ data_index, int n_sets,
-                                       const float* __restrict__ batch_loss, const int* __restrict__ batch_correct,
-                                       const int* __restrict__ slot, int n_slots, double* __restrict__ loss_sum,
-                                       int* __restrict__ correct) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  const int sl = *slot;
-  if (b >= batch || sl < 0 || sl >= n_slots) return;
-  const int set = data_index[b];
-  if (set < 0 || set >= n_sets) return;
-  double loss = 0.0;
-  int c = 0;
-  for (int t = 0; t < nb; ++t) {
-    loss += static_cast<double>(batch_loss[int64_t(b) * nb + t]);
-    c += batch_correct[int64_t(b) * nb + t];
-  }
-  loss_sum[int64_t(sl) * batch + b] = loss;
-  correct[int64_t(sl) * batch + b] = c;
-}
-
 static int smem_done_grad[kMaxDevices];
 static int smem_done_eval[kMaxDevices];
-
-static int check_common(const char* who, int batch, int64_t d, int n_sets, int n_rows, int m) {
-  if (batch < 1 || n_sets < 1 || n_rows < 1 || m < 1) {
-    set_error("%s: batch, n_sets, the set size and m must be >= 1 (got %d, %d, %d, %d)", who, batch, n_sets, n_rows, m);
-    return AFL_ERR_BAD_ARG;
-  }
-  if (d != kD) {
-    set_error("%s: the Cifar10Net layout has D = %lld parameters (got %lld)", who, static_cast<long long>(kD),
-              static_cast<long long>(d));
-    return AFL_ERR_UNSUPPORTED;
-  }
-  if (m > kMaxBatch) { set_error("%s: batch size m <= %d (got %d)", who, kMaxBatch, m); return AFL_ERR_UNSUPPORTED; }
-  if (batch > 65535) { set_error("%s: batch <= 65535 problems (got %d)", who, batch); return AFL_ERR_UNSUPPORTED; }
-  return AFL_OK;
-}
 
 static int client_grads(const char* who, const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
                         int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows, int n, int m,
                         const int* epoch, float* G, int64_t batch_stride, int64_t ld, void* stream) {
-  if (!weights || !x || !y || !data_index || !rows || !epoch || !G) {
-    set_error("%s: a pointer argument is NULL", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  if (int rc = check_common(who, batch, d, n_sets, n_rows, m)) return rc;
-  if (n < 1 || n > 1024) { set_error("%s: 1 <= n <= 1024 clients per problem (got %d)", who, n); return n < 1 ? AFL_ERR_BAD_ARG : AFL_ERR_UNSUPPORTED; }
-  if (n > n_rows) { set_error("%s: n (%d) exceeds the training set size (%d)", who, n, n_rows); return AFL_ERR_BAD_ARG; }
-  if (ld < d || (batch > 1 && batch_stride < (n - 1) * ld + d)) {
-    set_error("%s: ld (%lld) < d or batch_stride (%lld) makes problems overlap", who, static_cast<long long>(ld),
-              static_cast<long long>(batch_stride));
-    return AFL_ERR_BAD_ARG;
-  }
+  if (int rc = train::check_client_grads(who, "Cifar10Net", kD, kMaxBatch, weights, batch, d, x, y, n_sets, n_rows,
+                                         data_index, rows, n, m, epoch, G, batch_stride, ld))
+    return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   AFL_CUDA(ensure_dyn_smem(client_grad_kernel, static_cast<int>(kSmemBytes), smem_done_grad));
   client_grad_kernel<<<dim3(n, batch), kThreads, kSmemBytes, st>>>(
@@ -179,8 +115,6 @@ static int client_grads(const char* who, const float* weights, int batch, int64_
   AFL_LAUNCH_CHECK("cifar_client_grad_kernel");
   return AFL_OK;
 }
-
-static int64_t eval_batches(int n_test, int m) { return (int64_t(n_test) + m - 1) / m; }
 
 }  // namespace cifar
 }  // namespace afl
@@ -206,41 +140,23 @@ int afl_cifar10_client_grads_sets(const float* weights, int batch, int64_t d, co
 }
 
 size_t afl_cifar10_evaluate_workspace_bytes(int batch, int n_test, int m) {
-  if (batch < 1 || n_test < 1 || m < 1) return 0;
-  const size_t per = static_cast<size_t>(batch) * cifar::eval_batches(n_test, m);
-  return align_up(per * sizeof(float), 256) + align_up(per * sizeof(int), 256);
+  return train::eval_workspace_bytes(batch, n_test, m);
 }
 
 int afl_cifar10_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                          int n_test, const int* data_index, int m, const int* slot_index, int n_slots, double* loss_sum,
                          int* correct, void* workspace, size_t workspace_bytes, void* stream) {
-  const char* who = "afl_cifar10_evaluate";
-  if (!weights || !x || !y || !data_index || !slot_index || !loss_sum || !correct || !workspace) {
-    set_error("%s: a pointer argument is NULL", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  if (int rc = cifar::check_common(who, batch, d, n_sets, n_test, m)) return rc;
-  if (n_slots < 1) { set_error("%s: n_slots must be >= 1 (got %d)", who, n_slots); return AFL_ERR_BAD_ARG; }
-  const size_t need = afl_cifar10_evaluate_workspace_bytes(batch, n_test, m);
-  if (workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 256) {
-    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, workspace_bytes, need);
-    return AFL_ERR_WORKSPACE;
-  }
-  const int64_t nb = cifar::eval_batches(n_test, m);
-  if (nb > 65535) { set_error("%s: at most 65535 test batches (got %lld)", who, static_cast<long long>(nb)); return AFL_ERR_UNSUPPORTED; }
-  float* batch_loss = static_cast<float*>(workspace);
-  int* batch_correct = reinterpret_cast<int*>(static_cast<char*>(workspace) +
-                                              align_up(static_cast<size_t>(batch) * nb * sizeof(float), 256));
+  train::EvalWorkspace ws;
+  if (int rc = train::check_evaluate("afl_cifar10_evaluate", "Cifar10Net", cifar::kD, cifar::kMaxBatch, weights, batch,
+                                     d, x, y, n_sets, n_test, data_index, m, slot_index, n_slots, loss_sum, correct,
+                                     workspace, workspace_bytes, &ws))
+    return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   AFL_CUDA(ensure_dyn_smem(cifar::evaluate_kernel, static_cast<int>(cifar::kSmemBytes), cifar::smem_done_eval));
-  cifar::evaluate_kernel<<<dim3(static_cast<unsigned>(nb), batch), cifar::kThreads, cifar::kSmemBytes, st>>>(
-      weights, x, y, n_sets, n_test, data_index, m, batch_loss, batch_correct);
+  cifar::evaluate_kernel<<<dim3(ws.nb, batch), cifar::kThreads, cifar::kSmemBytes, st>>>(
+      weights, x, y, n_sets, n_test, data_index, m, ws.batch_loss, ws.batch_correct);
   AFL_LAUNCH_CHECK("cifar_evaluate_kernel");
-  cifar::evaluate_finish_kernel<<<(batch + 127) / 128, 128, 0, st>>>(batch, static_cast<int>(nb), data_index, n_sets,
-                                                                     batch_loss, batch_correct, slot_index, n_slots,
-                                                                     loss_sum, correct);
-  AFL_LAUNCH_CHECK("cifar_evaluate_finish_kernel");
-  return AFL_OK;
+  return train::evaluate_finish(st, batch, ws, data_index, n_sets, slot_index, n_slots, loss_sum, correct);
 }
 
 }  // extern "C"

@@ -2,13 +2,13 @@
 // attacker's trainer and backdoor test (cifar_backdoor.cu): the layout, the shared-memory carve and one chunk's
 // forward and backward pass (DESIGN 2.9).
 #pragma once
-#include "afl_common.cuh"
+#include "train_common.cuh"
 
 namespace afl {
 namespace cifar {
 
 constexpr int kImg = 3 * 32 * 32;                       // one NCHW image, flattened
-constexpr int kC1 = 16, kC2 = 64, kH1 = 384, kH2 = 192, kOut = 10;
+constexpr int kC1 = 16, kC2 = 64, kH1 = 384, kH2 = 192, kOut = train::kClasses;
 constexpr int kOffW1c = 0, kOffB1c = 432, kOffW2c = 448, kOffB2c = 16'832, kOffW1 = 16'896, kOffB1 = 41'472;
 constexpr int kOffW2 = 41'856, kOffB2 = 115'584, kOffW3 = 115'776, kOffB3 = 117'696;
 constexpr int64_t kD = 117'706;
@@ -47,35 +47,13 @@ __device__ __forceinline__ Smem carve(float* base, int rows = kMaxBatch) {
   return s;
 }
 
-// A weight load.  kNc: through the read-only data cache (__ldg), for weights no thread writes while the kernel runs;
-// otherwise an ordinary load, for the backdoor trainer's parameters, which the kernel updates in place between steps.
-template <bool kNc>
-__device__ __forceinline__ float ldw(const float* p) {
-  if constexpr (kNc) return __ldg(p);
-  else return *p;
-}
-
-// torch.relu: NaN stays NaN (fmaxf would turn it into 0).  (client_grad.cu and backdoor_train.cu hold the same.)
-__device__ __forceinline__ float relu(float v) { return v > 0.f || v != v ? v : 0.f; }
+using train::ldw;
+using train::relu;
 
 // torch's max_pool2d window step: a larger value or a NaN takes the index, so ties keep the first maximum.
 __device__ __forceinline__ void pool_step(float v, int k, float& mx, int& mi) {
   if (v > mx || v != v) { mx = v; mi = k; }
 }
-
-// torch's log_softmax: z - max - log(sum_c exp(z_c - max)), c in order.
-__device__ __forceinline__ void log_softmax_row(const float* z, float* logp) {
-  float mx = z[0];
-#pragma unroll
-  for (int c = 1; c < kOut; ++c) mx = fmaxf(mx, z[c]);
-  float sum = 0.f;
-#pragma unroll
-  for (int c = 0; c < kOut; ++c) sum += expf(z[c] - mx);
-  const float lse = logf(sum);
-#pragma unroll
-  for (int c = 0; c < kOut; ++c) logp[c] = z[c] - mx - lse;
-}
-
 
 // The forward pass of rows row[c0 .. c0 + mc) into the chunk buffers: P1/I1, H/I2, A1, A2 and the logits Z.
 // s.w1c must hold conv1's weights and bias.
@@ -209,13 +187,9 @@ __device__ void backward_chunk(const float* __restrict__ xs, const float* __rest
   // delta3 = (softmax - onehot) / mb: NLLLoss(mean) through log_softmax's backward
   const float fmb = static_cast<float>(mb);
   for (int i = t; i < mc; i += kThreads) {
-    float z[kOut], lp[kOut];
-#pragma unroll
-    for (int c = 0; c < kOut; ++c) z[c] = s.Z[i * kOut + c];
-    log_softmax_row(z, lp);
-    const int yi = s.label[c0 + i];
-#pragma unroll
-    for (int c = 0; c < kOut; ++c) s.Z[i * kOut + c] = (expf(lp[c]) - (c == yi ? 1.f : 0.f)) / fmb;
+    float lp[kOut];
+    train::log_softmax_row(s.Z + i * kOut, lp);
+    train::row_delta(lp, s.label[c0 + i], fmb, s.Z + i * kOut);
   }
   __syncthreads();
   // fc3: dW3[c][j] += sum_i delta3[i][c] A2[i][j], db3[c] += sum_i delta3[i][c]

@@ -560,9 +560,9 @@ int afl_backdoor_finish_batched_dev(int batch, int n, int64_t d, const int* f, c
  * afl_mnist_evaluate — server.py:92-112 / harness.main's test loop for every problem: test batches of m rows (the last
  * one shorter), each batch's mean NLL in fp32, summed over the batches in order in float64 into
  * loss_sum[slot][b] (divide by n_test for the reported loss), and correct[slot][b] = the number of rows whose argmax
- * (the first maximum of the log-probabilities) is the label.  slot = *slot_index (device int32, read when the kernel
- * runs); a slot outside [0, n_slots) writes nothing.  loss_sum: device float64 [n_slots][batch], correct: device int32
- * [n_slots][batch].  Workspace: afl_mnist_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned (else
+ * (torch's max(1) of the log-probabilities: the first NaN, else the first maximum) is the label.  slot = *slot_index
+ * (device int32, read when the kernel runs); a slot outside [0, n_slots) writes nothing.  loss_sum: device float64
+ * [n_slots][batch], correct: device int32 [n_slots][batch].  Workspace: afl_mnist_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned (else
  * AFL_ERR_WORKSPACE); 0 on bad arguments.  More than 65535 test batches -> AFL_ERR_UNSUPPORTED. */
 int afl_mnist_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                            int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
@@ -629,7 +629,7 @@ int afl_mnist_backdoor_test(const float* weights, int batch, int64_t d, const fl
  * pitch n_rows, device set_len, skip rule and checks.
  *
  * afl_cifar10_evaluate — server.py:92-112 / harness.main's test loop with Cifar10Net: afl_mnist_evaluate's batches,
- * float64 loss sums, first-maximum correct counts, NaN loss for a label outside 0..9, slot rule and workspace
+ * float64 loss sums, correct counts by torch's argmax, NaN loss for a label outside 0..9, slot rule and workspace
  * (afl_cifar10_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned). */
 int afl_cifar10_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                              int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,

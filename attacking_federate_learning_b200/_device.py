@@ -167,6 +167,22 @@ def momentum_step(weights: torch.Tensor, velocity: torch.Tensor, grads: torch.Te
                                               float(momentum), float(lr), _stream_ptr(weights)))
 
 
+def momentum_step_batched(weights: torch.Tensor, velocity: torch.Tensor, grads: torch.Tensor, momentum: float,
+                          lr: torch.Tensor):
+    """momentum_step on each row b of contiguous fp32 [B, D] weights, velocity and grads at lr[b] (a device fp32 [B]
+    tensor, read when the kernel runs), in one launch."""
+    B = lr.numel()
+    for t in (weights, velocity, grads):
+        if not (t.is_contiguous() and t.dtype == torch.float32 and t.dim() == 2 and t.shape[0] == B):
+            raise ValueError("momentum_step_batched: contiguous float32 [B, D] rows, one learning rate per row")
+    if not (lr.is_contiguous() and lr.dtype == torch.float32):
+        raise ValueError("momentum_step_batched: lr must be a contiguous float32 tensor")
+    with torch.cuda.device(weights.device):
+        nat.check(nat.lib().afl_momentum_step_batched(weights.data_ptr(), velocity.data_ptr(), grads.data_ptr(), B,
+                                                      weights.shape[1], float(momentum), lr.data_ptr(),
+                                                      _stream_ptr(weights)))
+
+
 # ---------------------------------------------------------------------------------------------------------
 # multi-GPU exchange over NVLink peer memory (csrc/xgpu.cu)
 # ---------------------------------------------------------------------------------------------------------

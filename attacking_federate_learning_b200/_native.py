@@ -41,6 +41,7 @@ SIGNATURES = {
     "afl_alie": (_i, [_vp, _i, _i64, _i64, _i, _d, _vp, _vp, _vp, _vp, _i64, _vp]),
     "afl_alie_band": (_i, [_vp, _vp, _d, _vp, _vp, _i64, _vp]),
     "afl_momentum_step": (_i, [_vp, _vp, _vp, _i64, _f, _f, _vp]),
+    "afl_momentum_step_batched": (_i, [_vp, _vp, _vp, _i, _i64, _f, _vp, _vp]),
     "afl_xgpu_create": (_i, [_i, _i, _i, C.POINTER(_vp)]),
     "afl_xgpu_handle": (_i, [_vp, C.c_char_p]),
     "afl_xgpu_connect": (_i, [_vp, C.c_char_p]),
@@ -94,6 +95,10 @@ SIGNATURES = {
                                          _vp]),
     "afl_mnist_evaluate_workspace_bytes": (_sz, [_i, _i, _i]),
     "afl_mnist_evaluate": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "afl_mnist_client_grads_each": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i64,
+                                         _i64, _vp]),
+    "afl_mnist_evaluate_each": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _sz,
+                                     _vp]),
     "afl_backdoor_start_batched_dev": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp,
                                             _vp, _sz, _vp, _vp]),
     "afl_backdoor_finish_batched_dev": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
@@ -105,6 +110,10 @@ SIGNATURES = {
                                            _i64, _vp]),
     "afl_cifar10_evaluate_workspace_bytes": (_sz, [_i, _i, _i]),
     "afl_cifar10_evaluate": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "afl_cifar10_client_grads_each": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i64,
+                                           _i64, _vp]),
+    "afl_cifar10_evaluate_each": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _sz,
+                                       _vp]),
     "afl_cifar10_backdoor_train_workspace_bytes": (_sz, [_i]),
     "afl_cifar10_backdoor_train": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _d, _i, _i, _vp,
                                         _sz, _vp]),

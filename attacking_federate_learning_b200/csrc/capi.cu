@@ -142,6 +142,8 @@ int alie_batched_dev(const void* G, int f_bound, int64_t d, int64_t ld, int dtyp
 int gather_row(const void* G, int n, int64_t d, int64_t ld, int dtype, const int* idx_dev, float* out,
                cudaStream_t stream);
 int momentum_step(float* w, float* v, const float* g, int64_t d, float momentum, float lr, cudaStream_t stream);
+int momentum_step_batched(float* w, float* v, const float* g, int batch, int64_t d, float momentum, const float* lr,
+                          cudaStream_t stream);
 int alie_band(const float* mu, const float* sigma, double z, const float* x, float* out, int64_t d, cudaStream_t stream);
 int64_t deviation_tiles(int64_t d, int dtype);
 int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, int64_t ld, int dtype, int f,
@@ -1513,6 +1515,12 @@ int afl_momentum_step(float* weights, float* velocity, const float* grads, int64
                       float learning_rate, void* stream) {
   return colstats::momentum_step(weights, velocity, grads, d, momentum, learning_rate,
                                  static_cast<cudaStream_t>(stream));
+}
+
+int afl_momentum_step_batched(float* weights, float* velocity, const float* grads, int batch, int64_t d,
+                              float momentum, const float* learning_rate, void* stream) {
+  return colstats::momentum_step_batched(weights, velocity, grads, batch, d, momentum, learning_rate,
+                                         static_cast<cudaStream_t>(stream));
 }
 
 int afl_defend_host(const char* rule, const float* G_host, int n, int64_t d, int64_t ld, int users_count,

@@ -25,14 +25,16 @@ namespace cifar {
 __global__ void __launch_bounds__(kThreads, 2)
 client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ x, const int64_t* __restrict__ y,
                    int n_sets, int n_rows, const int* __restrict__ set_len, const int* __restrict__ data_index,
-                   const int* __restrict__ rows, int n_max, int m, const int* __restrict__ epoch, float* __restrict__ G,
-                   int64_t batch_stride, int64_t ld) {
+                   const int* __restrict__ rows, int n_max, int max_m, const int* __restrict__ m_each,
+                   const int* __restrict__ epoch, float* __restrict__ G, int64_t batch_stride, int64_t ld) {
   const int u = blockIdx.x, b = blockIdx.y;
   const int n = min(rows[b], n_max);
   const int set = data_index[b];
   if (u >= n || set < 0 || set >= n_sets) return;                 // block-uniform, before any barrier
   const int n_train = set_len ? set_len[set] : n_rows;            // no set_len: every set is n_rows long
   if (n_train < n || n_train > n_rows) return;
+  const int m = train::problem_m(m_each, b, 1, max_m);            // m_each: problem b's own minibatch size
+  if (!m) return;
   extern __shared__ float smem[];
   const Smem s = carve(smem);
   const float* w = weights + int64_t(b) * kD;
@@ -55,15 +57,17 @@ client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ 
   }
 }
 
-// Evaluation: CTA (t, b) runs test batch t of problem b's test set (rows [t m, min(t m + m, n_test))) and writes the
-// batch's mean NLL (a fp32 sum over rows in order, divided by the row count) and its correct count to the workspace.
+// Evaluation: CTA (t, b) runs test batch t of problem b's test set (rows [t m, min(t m + m, n_test)), m = max_m or
+// problem b's own size, train::problem_m) and writes the batch's mean NLL (a fp32 sum over rows in order, divided by
+// the row count) and its correct count to the workspace.  The grid covers the batch count at min_m.
 __global__ void __launch_bounds__(kThreads, 2)
 evaluate_kernel(const float* __restrict__ weights, const float* __restrict__ x, const int64_t* __restrict__ y,
-                int n_sets, int n_test, const int* __restrict__ data_index, int m, float* __restrict__ batch_loss,
-                int* __restrict__ batch_correct) {
+                int n_sets, int n_test, const int* __restrict__ data_index, int min_m, int max_m,
+                const int* __restrict__ m_each, float* __restrict__ batch_loss, int* __restrict__ batch_correct) {
   const int t = blockIdx.x, b = blockIdx.y, nb = gridDim.x;
   const int set = data_index[b];
-  if (set < 0 || set >= n_sets) return;
+  const int m = train::problem_m(m_each, b, min_m, max_m);
+  if (set < 0 || set >= n_sets || !m || t * m >= n_test) return;  // past problem b's own batch count
   extern __shared__ float smem[];
   const Smem s = carve(smem);
   const float* w = weights + int64_t(b) * kD;
@@ -104,14 +108,15 @@ static int smem_done_eval[kMaxDevices];
 
 static int client_grads(const char* who, const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
                         int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows, int n, int m,
-                        const int* epoch, float* G, int64_t batch_stride, int64_t ld, void* stream) {
+                        const int* m_each, const int* epoch, float* G, int64_t batch_stride, int64_t ld,
+                        void* stream) {
   if (int rc = train::check_client_grads(who, "Cifar10Net", kD, kMaxBatch, weights, batch, d, x, y, n_sets, n_rows,
                                          data_index, rows, n, m, epoch, G, batch_stride, ld))
     return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   AFL_CUDA(ensure_dyn_smem(client_grad_kernel, static_cast<int>(kSmemBytes), smem_done_grad));
   client_grad_kernel<<<dim3(n, batch), kThreads, kSmemBytes, st>>>(
-      weights, x, y, n_sets, n_rows, set_len, data_index, rows, n, m, epoch, G, batch_stride, ld);
+      weights, x, y, n_sets, n_rows, set_len, data_index, rows, n, m, m_each, epoch, G, batch_stride, ld);
   AFL_LAUNCH_CHECK("cifar_client_grad_kernel");
   return AFL_OK;
 }
@@ -127,7 +132,7 @@ int afl_cifar10_client_grads(const float* weights, int batch, int64_t d, const f
                              int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
                              float* G, int64_t batch_stride, int64_t ld, void* stream) {
   return cifar::client_grads("afl_cifar10_client_grads", weights, batch, d, x, y, n_sets, n_train, nullptr, data_index,
-                             rows, n, m, epoch, G, batch_stride, ld, stream);
+                             rows, n, m, nullptr, epoch, G, batch_stride, ld, stream);
 }
 
 int afl_cifar10_client_grads_sets(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
@@ -136,7 +141,16 @@ int afl_cifar10_client_grads_sets(const float* weights, int batch, int64_t d, co
                                   void* stream) {
   if (!set_len) { set_error("afl_cifar10_client_grads_sets: a pointer argument is NULL"); return AFL_ERR_BAD_ARG; }
   return cifar::client_grads("afl_cifar10_client_grads_sets", weights, batch, d, x, y, n_sets, n_rows, set_len,
-                             data_index, rows, n, m, epoch, G, batch_stride, ld, stream);
+                             data_index, rows, n, m, nullptr, epoch, G, batch_stride, ld, stream);
+}
+
+int afl_cifar10_client_grads_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                                  int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
+                                  int n, const int* m, int max_m, const int* epoch, float* G, int64_t batch_stride,
+                                  int64_t ld, void* stream) {
+  if (!set_len || !m) { set_error("afl_cifar10_client_grads_each: a pointer argument is NULL"); return AFL_ERR_BAD_ARG; }
+  return cifar::client_grads("afl_cifar10_client_grads_each", weights, batch, d, x, y, n_sets, n_rows, set_len,
+                             data_index, rows, n, max_m, m, epoch, G, batch_stride, ld, stream);
 }
 
 size_t afl_cifar10_evaluate_workspace_bytes(int batch, int n_test, int m) {
@@ -154,9 +168,27 @@ int afl_cifar10_evaluate(const float* weights, int batch, int64_t d, const float
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   AFL_CUDA(ensure_dyn_smem(cifar::evaluate_kernel, static_cast<int>(cifar::kSmemBytes), cifar::smem_done_eval));
   cifar::evaluate_kernel<<<dim3(ws.nb, batch), cifar::kThreads, cifar::kSmemBytes, st>>>(
-      weights, x, y, n_sets, n_test, data_index, m, ws.batch_loss, ws.batch_correct);
+      weights, x, y, n_sets, n_test, data_index, m, m, nullptr, ws.batch_loss, ws.batch_correct);
   AFL_LAUNCH_CHECK("cifar_evaluate_kernel");
   return train::evaluate_finish(st, batch, ws, data_index, n_sets, slot_index, n_slots, loss_sum, correct);
+}
+
+int afl_cifar10_evaluate_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                              int n_sets, int n_test, const int* data_index, const int* m, int min_m, int max_m,
+                              const int* slot_index, int n_slots, double* loss_sum, int* correct, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  train::EvalWorkspace ws;
+  if (int rc = train::check_evaluate_each("afl_cifar10_evaluate_each", "Cifar10Net", cifar::kD, cifar::kMaxBatch,
+                                          weights, batch, d, x, y, n_sets, n_test, data_index, m, min_m, max_m,
+                                          slot_index, n_slots, loss_sum, correct, workspace, workspace_bytes, &ws))
+    return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  AFL_CUDA(ensure_dyn_smem(cifar::evaluate_kernel, static_cast<int>(cifar::kSmemBytes), cifar::smem_done_eval));
+  cifar::evaluate_kernel<<<dim3(ws.nb, batch), cifar::kThreads, cifar::kSmemBytes, st>>>(
+      weights, x, y, n_sets, n_test, data_index, min_m, max_m, m, ws.batch_loss, ws.batch_correct);
+  AFL_LAUNCH_CHECK("cifar_evaluate_kernel");
+  return train::evaluate_finish(st, batch, ws, data_index, n_sets, slot_index, n_slots, loss_sum, correct, m, min_m,
+                                max_m, n_test);
 }
 
 }  // extern "C"

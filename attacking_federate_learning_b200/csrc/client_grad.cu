@@ -20,14 +20,16 @@ template <int RT>
 __global__ void __launch_bounds__(kThreads, 2)
 client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ x, const int64_t* __restrict__ y,
                    int n_sets, int n_rows, const int* __restrict__ set_len, const int* __restrict__ data_index,
-                   const int* __restrict__ rows, int n_max, int m, const int* __restrict__ epoch, float* __restrict__ G,
-                   int64_t batch_stride, int64_t ld) {
+                   const int* __restrict__ rows, int n_max, int max_m, const int* __restrict__ m_each,
+                   const int* __restrict__ epoch, float* __restrict__ G, int64_t batch_stride, int64_t ld) {
   const int u = blockIdx.x, b = blockIdx.y;
   const int n = min(rows[b], n_max);
   const int set = data_index[b];
   if (u >= n || set < 0 || set >= n_sets) return;                 // block-uniform, before any barrier
   const int n_train = set_len ? set_len[set] : n_rows;            // no set_len: every set is n_rows long
   if (n_train < n || n_train > n_rows) return;
+  const int m = train::problem_m(m_each, b, 1, max_m);
+  if (!m) return;
   extern __shared__ float smem[];
   const Smem s = carve<Geo>(smem);
   const float* w = weights + int64_t(b) * kD;
@@ -79,16 +81,18 @@ client_grad_kernel(const float* __restrict__ weights, const float* __restrict__ 
   }
 }
 
-// Evaluation: CTA (t, b) runs test batch t of problem b's test set (rows [t m, min(t m + m, n_test))) and writes the
-// batch's mean NLL (a fp32 sum over rows in order, divided by the row count) and its correct count to the workspace.
+// Evaluation: CTA (t, b) runs test batch t of problem b's test set (rows [t m, min(t m + m, n_test)), m = max_m or
+// problem b's own size, train::problem_m) and writes the batch's mean NLL (a fp32 sum over rows in order, divided by
+// the row count) and its correct count to the workspace.  The grid covers the batch count at min_m.
 template <int RT>
 __global__ void __launch_bounds__(kThreads, 2)
 evaluate_kernel(const float* __restrict__ weights, const float* __restrict__ x, const int64_t* __restrict__ y,
-                int n_sets, int n_test, const int* __restrict__ data_index, int m, float* __restrict__ batch_loss,
-                int* __restrict__ batch_correct) {
+                int n_sets, int n_test, const int* __restrict__ data_index, int min_m, int max_m,
+                const int* __restrict__ m_each, float* __restrict__ batch_loss, int* __restrict__ batch_correct) {
   const int t = blockIdx.x, b = blockIdx.y, nb = gridDim.x;
   const int set = data_index[b];
-  if (set < 0 || set >= n_sets) return;
+  const int m = train::problem_m(m_each, b, min_m, max_m);
+  if (set < 0 || set >= n_sets || !m || t * m >= n_test) return;  // past problem b's own batch count
   extern __shared__ float smem[];
   const Smem s = carve<Geo>(smem);
   const float* w = weights + int64_t(b) * kD;
@@ -127,20 +131,22 @@ static int smem_done_eval[8][kMaxDevices];
 template <int RT>
 static int launch_grad(dim3 grid, cudaStream_t stream, const float* weights, const float* x, const int64_t* y,
                        int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
-                       int n_max, int m, const int* epoch, float* G, int64_t batch_stride, int64_t ld) {
+                       int n_max, int m, const int* m_each, const int* epoch, float* G, int64_t batch_stride,
+                       int64_t ld) {
   AFL_CUDA(ensure_dyn_smem(client_grad_kernel<RT>, static_cast<int>(kSmemBytes), smem_done_grad[RT - 1]));
   client_grad_kernel<RT><<<grid, kThreads, kSmemBytes, stream>>>(weights, x, y, n_sets, n_rows, set_len, data_index,
-                                                                  rows, n_max, m, epoch, G, batch_stride, ld);
+                                                                  rows, n_max, m, m_each, epoch, G, batch_stride, ld);
   AFL_LAUNCH_CHECK("client_grad_kernel");
   return AFL_OK;
 }
 
 template <int RT>
 static int launch_eval(dim3 grid, cudaStream_t stream, const float* weights, const float* x, const int64_t* y,
-                       int n_sets, int n_test, const int* data_index, int m, float* batch_loss, int* batch_correct) {
+                       int n_sets, int n_test, const int* data_index, int min_m, int m, const int* m_each,
+                       float* batch_loss, int* batch_correct) {
   AFL_CUDA(ensure_dyn_smem(evaluate_kernel<RT>, static_cast<int>(kSmemBytes), smem_done_eval[RT - 1]));
-  evaluate_kernel<RT><<<grid, kThreads, kSmemBytes, stream>>>(weights, x, y, n_sets, n_test, data_index, m,
-                                                               batch_loss, batch_correct);
+  evaluate_kernel<RT><<<grid, kThreads, kSmemBytes, stream>>>(weights, x, y, n_sets, n_test, data_index, min_m, m,
+                                                               m_each, batch_loss, batch_correct);
   AFL_LAUNCH_CHECK("evaluate_kernel");
   return AFL_OK;
 }
@@ -157,21 +163,25 @@ static int launch_eval(dim3 grid, cudaStream_t stream, const float* weights, con
     default: return FN<8>(__VA_ARGS__);                                                       \
   }
 
+// m: the test batch size, or with m_each the largest one (the RT instance follows it)
 static int run_eval(dim3 grid, cudaStream_t stream, const float* weights, const float* x, const int64_t* y, int n_sets,
-                    int n_test, const int* data_index, int m, float* batch_loss, int* batch_correct) {
-  AFL_MNIST_BY_ROWS((m + 15) / 16, launch_eval, grid, stream, weights, x, y, n_sets, n_test, data_index, m, batch_loss,
-                    batch_correct)
+                    int n_test, const int* data_index, int min_m, int m, const int* m_each, float* batch_loss,
+                    int* batch_correct) {
+  AFL_MNIST_BY_ROWS((m + 15) / 16, launch_eval, grid, stream, weights, x, y, n_sets, n_test, data_index, min_m, m,
+                    m_each, batch_loss, batch_correct)
 }
 
+// m: the minibatch size, or with m_each (the _each calls) the largest one, which picks the RT instance
 static int client_grads(const char* who, const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
                         int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows, int n, int m,
-                        const int* epoch, float* G, int64_t batch_stride, int64_t ld, void* stream) {
+                        const int* m_each, const int* epoch, float* G, int64_t batch_stride, int64_t ld,
+                        void* stream) {
   if (int rc = train::check_client_grads(who, "MnistNet", kD, kMaxBatch, weights, batch, d, x, y, n_sets, n_rows,
                                          data_index, rows, n, m, epoch, G, batch_stride, ld))
     return rc;
   const dim3 grid(n, batch);
   AFL_MNIST_BY_ROWS((m + 15) / 16, launch_grad, grid, static_cast<cudaStream_t>(stream), weights, x, y, n_sets, n_rows,
-                    set_len, data_index, rows, n, m, epoch, G, batch_stride, ld)
+                    set_len, data_index, rows, n, m, m_each, epoch, G, batch_stride, ld)
 }
 
 }  // namespace mnist
@@ -183,15 +193,22 @@ namespace train {
 __global__ void evaluate_finish_kernel(int batch, int nb, const int* __restrict__ data_index, int n_sets,
                                        const float* __restrict__ batch_loss, const int* __restrict__ batch_correct,
                                        const int* __restrict__ slot, int n_slots, double* __restrict__ loss_sum,
-                                       int* __restrict__ correct) {
+                                       int* __restrict__ correct, const int* __restrict__ m_each, int min_m,
+                                       int max_m, int n_test) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   const int sl = *slot;
   if (b >= batch || sl < 0 || sl >= n_slots) return;
   const int set = data_index[b];
   if (set < 0 || set >= n_sets) return;
+  int nb_b = nb;                                                  // problem b's own batch count
+  if (m_each) {
+    const int m = problem_m(m_each, b, min_m, max_m);
+    if (!m) return;
+    nb_b = (n_test + m - 1) / m;
+  }
   double loss = 0.0;
   int c = 0;
-  for (int t = 0; t < nb; ++t) {
+  for (int t = 0; t < nb_b; ++t) {
     loss += static_cast<double>(batch_loss[int64_t(b) * nb + t]);
     c += batch_correct[int64_t(b) * nb + t];
   }
@@ -200,10 +217,11 @@ __global__ void evaluate_finish_kernel(int batch, int nb, const int* __restrict_
 }
 
 int evaluate_finish(cudaStream_t stream, int batch, const EvalWorkspace& ws, const int* data_index, int n_sets,
-                    const int* slot_index, int n_slots, double* loss_sum, int* correct) {
+                    const int* slot_index, int n_slots, double* loss_sum, int* correct, const int* m_each, int min_m,
+                    int max_m, int n_test) {
   evaluate_finish_kernel<<<(batch + 127) / 128, 128, 0, stream>>>(batch, ws.nb, data_index, n_sets, ws.batch_loss,
                                                                   ws.batch_correct, slot_index, n_slots, loss_sum,
-                                                                  correct);
+                                                                  correct, m_each, min_m, max_m, n_test);
   AFL_LAUNCH_CHECK("evaluate_finish_kernel");
   return AFL_OK;
 }
@@ -219,7 +237,7 @@ int afl_mnist_client_grads(const float* weights, int batch, int64_t d, const flo
                            int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
                            float* G, int64_t batch_stride, int64_t ld, void* stream) {
   return mnist::client_grads("afl_mnist_client_grads", weights, batch, d, x, y, n_sets, n_train, nullptr, data_index,
-                             rows, n, m, epoch, G, batch_stride, ld, stream);
+                             rows, n, m, nullptr, epoch, G, batch_stride, ld, stream);
 }
 
 int afl_mnist_client_grads_sets(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
@@ -228,7 +246,16 @@ int afl_mnist_client_grads_sets(const float* weights, int batch, int64_t d, cons
                                 void* stream) {
   if (!set_len) { set_error("afl_mnist_client_grads_sets: a pointer argument is NULL"); return AFL_ERR_BAD_ARG; }
   return mnist::client_grads("afl_mnist_client_grads_sets", weights, batch, d, x, y, n_sets, n_rows, set_len,
-                             data_index, rows, n, m, epoch, G, batch_stride, ld, stream);
+                             data_index, rows, n, m, nullptr, epoch, G, batch_stride, ld, stream);
+}
+
+int afl_mnist_client_grads_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                                int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
+                                int n, const int* m, int max_m, const int* epoch, float* G, int64_t batch_stride,
+                                int64_t ld, void* stream) {
+  if (!set_len || !m) { set_error("afl_mnist_client_grads_each: a pointer argument is NULL"); return AFL_ERR_BAD_ARG; }
+  return mnist::client_grads("afl_mnist_client_grads_each", weights, batch, d, x, y, n_sets, n_rows, set_len,
+                             data_index, rows, n, max_m, m, epoch, G, batch_stride, ld, stream);
 }
 
 size_t afl_mnist_evaluate_workspace_bytes(int batch, int n_test, int m) {
@@ -244,10 +271,27 @@ int afl_mnist_evaluate(const float* weights, int batch, int64_t d, const float* 
                                      workspace, workspace_bytes, &ws))
     return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = mnist::run_eval(dim3(ws.nb, batch), st, weights, x, y, n_sets, n_test, data_index, m, ws.batch_loss,
-                               ws.batch_correct))
+  if (int rc = mnist::run_eval(dim3(ws.nb, batch), st, weights, x, y, n_sets, n_test, data_index, m, m, nullptr,
+                               ws.batch_loss, ws.batch_correct))
     return rc;
   return train::evaluate_finish(st, batch, ws, data_index, n_sets, slot_index, n_slots, loss_sum, correct);
+}
+
+int afl_mnist_evaluate_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                            int n_test, const int* data_index, const int* m, int min_m, int max_m,
+                            const int* slot_index, int n_slots, double* loss_sum, int* correct, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  train::EvalWorkspace ws;
+  if (int rc = train::check_evaluate_each("afl_mnist_evaluate_each", "MnistNet", mnist::kD, mnist::kMaxBatch, weights,
+                                          batch, d, x, y, n_sets, n_test, data_index, m, min_m, max_m, slot_index,
+                                          n_slots, loss_sum, correct, workspace, workspace_bytes, &ws))
+    return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int rc = mnist::run_eval(dim3(ws.nb, batch), st, weights, x, y, n_sets, n_test, data_index, min_m, max_m, m,
+                               ws.batch_loss, ws.batch_correct))
+    return rc;
+  return train::evaluate_finish(st, batch, ws, data_index, n_sets, slot_index, n_slots, loss_sum, correct, m, min_m,
+                                max_m, n_test);
 }
 
 }  // extern "C"

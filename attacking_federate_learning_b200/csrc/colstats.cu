@@ -277,7 +277,13 @@ gather_row_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, const i
 
 __global__ void __launch_bounds__(kBlock)
 momentum_kernel(float* __restrict__ w, float* __restrict__ v, const float* __restrict__ g, int64_t d, float momentum,
-                float lr) {
+                float lr, const float* __restrict__ lr_each) {
+  // lr_each: row blockIdx.y of [batch, d] rows at its own learning rate (the scalar call's grid has one row)
+  if (lr_each) {
+    const int64_t off = static_cast<int64_t>(blockIdx.y) * d;
+    w += off; v += off; g += off;
+    lr = lr_each[blockIdx.y];
+  }
   for (int64_t c = static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x; c < d;
        c += static_cast<int64_t>(gridDim.x) * kBlock) {
     // server.py:89  velocity = momentum*velocity - lr*grads  (two products, one subtraction, fp32)
@@ -678,7 +684,24 @@ int momentum_step(float* w, float* v, const float* g, int64_t d, float momentum,
   if (!w || !v || !g || d < 1) { set_error("afl_momentum_step: bad argument"); return AFL_ERR_BAD_ARG; }
   int64_t blocks = ceil_div64(d, kBlock);
   if (blocks > 132 * 16) blocks = 132 * 16;
-  momentum_kernel<<<static_cast<unsigned>(blocks), kBlock, 0, stream>>>(w, v, g, d, momentum, lr);
+  momentum_kernel<<<static_cast<unsigned>(blocks), kBlock, 0, stream>>>(w, v, g, d, momentum, lr, nullptr);
+  AFL_LAUNCH_CHECK("momentum_kernel");
+  return AFL_OK;
+}
+
+int momentum_step_batched(float* w, float* v, const float* g, int batch, int64_t d, float momentum, const float* lr,
+                          cudaStream_t stream) {
+  if (!w || !v || !g || !lr || batch < 1 || d < 1) {
+    set_error("afl_momentum_step_batched: bad argument");
+    return AFL_ERR_BAD_ARG;
+  }
+  if (batch > 65535) {
+    set_error("afl_momentum_step_batched: batch <= 65535 rows (got %d)", batch);
+    return AFL_ERR_UNSUPPORTED;
+  }
+  int64_t blocks = ceil_div64(d, kBlock);
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  momentum_kernel<<<dim3(static_cast<unsigned>(blocks), batch), kBlock, 0, stream>>>(w, v, g, d, momentum, 0.f, lr);
   AFL_LAUNCH_CHECK("momentum_kernel");
   return AFL_OK;
 }

@@ -71,6 +71,14 @@ __device__ __forceinline__ int batch_start(int n_train, int n, int u, int m, int
   return lo;
 }
 
+// Problem b's minibatch (or test batch) size: m, or m_each[b] for the per-problem (_each) calls, where a size outside
+// [lo, m] returns 0 and the caller skips the problem.  The scalar calls pass m_each = nullptr.
+__device__ __forceinline__ int problem_m(const int* m_each, int b, int lo, int m) {
+  if (!m_each) return m;
+  const int mb = m_each[b];
+  return mb >= lo && mb <= m ? mb : 0;
+}
+
 // One SGD step of one element (backdoor.py:134-153 with torch.optim.SGD's first step of a fresh optimiser): g is the
 // NLL gradient; with alpha > 0 the MSE term's ((p - p0) * 2/numel) * alpha is added (mse_loss's backward); then
 // d_p = g + 1e-4 p and p - 0.1 d_p.  *bad is set when the new p - p0 is NaN, which makes the next dist loss NaN.
@@ -173,11 +181,29 @@ inline int check_evaluate(const char* who, const char* net, int64_t net_d, int m
   return carve_eval_workspace(who, workspace, workspace_bytes, batch, n_test, m, AFL_ERR_WORKSPACE, ws);
 }
 
+// The arguments of afl_*_evaluate_each: afl_*_evaluate's with the per-problem sizes m (device int32 [batch]) in
+// [min_m, max_m], and the workspace carved for the batch count at min_m.
+inline int check_evaluate_each(const char* who, const char* net, int64_t net_d, int max_batch, const float* weights,
+                               int batch, int64_t d, const float* x, const int64_t* y, int n_sets, int n_test,
+                               const int* data_index, const int* m, int min_m, int max_m, const int* slot_index,
+                               int n_slots, const double* loss_sum, const int* correct, void* workspace,
+                               size_t workspace_bytes, EvalWorkspace* ws) {
+  if (!m) { set_error("%s: a pointer argument is NULL", who); return AFL_ERR_BAD_ARG; }
+  if (min_m > max_m) { set_error("%s: min_m (%d) > max_m (%d)", who, min_m, max_m); return AFL_ERR_BAD_ARG; }
+  if (int rc = check_evaluate(who, net, net_d, max_batch, weights, batch, d, x, y, n_sets, n_test, data_index, max_m,
+                              slot_index, n_slots, loss_sum, correct, workspace, workspace_bytes, ws))
+    return rc;
+  if (min_m < 1) { set_error("%s: min_m must be >= 1 (got %d)", who, min_m); return AFL_ERR_BAD_ARG; }
+  return carve_eval_workspace(who, workspace, workspace_bytes, batch, n_test, min_m, AFL_ERR_WORKSPACE, ws);
+}
+
 // loss_sum[slot][b] = sum_t batch_loss[b][t] in float64, t in order (harness.main's `test_loss += ....item()`);
-// correct[slot][b] = sum_t batch_correct[b][t], for every problem whose set index is in range.  Defined in
+// correct[slot][b] = sum_t batch_correct[b][t], for every problem whose set index is in range: t < ws.nb, or with
+// m_each t < ceil(n_test / m_each[b]) for a size in [min_m, max_m] (any other size writes nothing).  Defined in
 // client_grad.cu.
 int evaluate_finish(cudaStream_t stream, int batch, const EvalWorkspace& ws, const int* data_index, int n_sets,
-                    const int* slot_index, int n_slots, double* loss_sum, int* correct);
+                    const int* slot_index, int n_slots, double* loss_sum, int* correct, const int* m_each = nullptr,
+                    int min_m = 0, int max_m = 0, int n_test = 0);
 
 inline bool overlap(const void* a, size_t na, const void* b, size_t nb) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);

@@ -32,13 +32,14 @@ backdoor experiment whose malicious training meets a NaN loss: Exception('...: G
 Outputs per experiment: the accuracy list and the CSV `harness.main` writes (np.savetxt(..., delimiter=',') in
 out_dir/logs, with `_seed_<s>` before `.csv` so that seeds do not overwrite one another), and one summary CSV with the
 parameters, max and final accuracy and status (and, when the run has a backdoor experiment, the backdoor and its max
-and final backdoor accuracy).  No checkpoint is written: main.py's checkpoint path has no experiment
-key, so the experiments of a batch would overwrite one file.
+and final backdoor accuracy; when it has an 8-tuple, every experiment's learning rate and batch size).  No checkpoint
+is written: main.py's checkpoint path has no experiment key, so the experiments of a batch would overwrite one file.
 
     python -m attacking_federate_learning_b200.sweep -d Krum TrimmedMean -z 0.5 1.5 -m 0.1 0.24 -n 10 --seeds 0 1 -e 30
     python -m attacking_federate_learning_b200.sweep -d Krum NoDefense -z 1.0 -b No pattern 1 --seeds 0 1 -e 30
     python -m attacking_federate_learning_b200.sweep -s CIFAR10 -d Krum TrimmedMean -z 0.5 1.5 --seeds 0 1 -e 30
     python -m attacking_federate_learning_b200.sweep -s CIFAR10 -d Krum NoDefense -z 1.0 -b pattern 1 --cifar10-backdoor
+    python -m attacking_federate_learning_b200.sweep -d Krum NoDefense -z 1.0 -l 0.05 0.1 0.2 -c 32 83 128 -e 30
 
 dataset='CIFAR10' (main.py -s CIFAR10) runs the same loop on harness.Cifar10Net and `synthetic_cifar_problem`, with
 the CIFAR10 kernels (C ABI `afl_cifar10_client_grads` and `afl_cifar10_evaluate`) in steps 1 and 4 and SYNTH-CIFAR10
@@ -54,6 +55,14 @@ length ceil(N / n) * n (users counts 10, 100, 250, 500 and 1000 share the 60,000
 each problem's set length from the device (C ABI `afl_*_client_grads_sets`); the test set is one copy for all seeds.
 
     python -m attacking_federate_learning_b200.sweep --data-dir ./mnist_data -d Krum NoDefense -z 1.0 -n 10 51 -e 30
+
+Learning rate and batch size per experiment (main.py -l and -c; several values on the CLI, `grid(learning_rates=...,
+batch_sizes=...)`): the 8-tuple experiments carry their own, and experiments of any (lr, c) train in one batch.  The
+kernels take problem b's minibatch and test batch size from a device array (C ABI `afl_*_client_grads_each` and
+`afl_*_evaluate_each`) and the momentum step its learning rate (`afl_momentum_step_batched`), and the backdoor's lr_t
+starts from its own learning_rate * fading_rate; each problem's bits equal a sweep of its own (lr, c).  The backdoor
+trainer keeps its own batch (200) and lr (0.1); epochs, momentum and fading rate stay per run.  An 8-tuple's CSV
+takes its own learning rate and adds `_batch_<c>` before the seed, since main.py's name has no batch size.
 """
 from __future__ import annotations
 
@@ -70,7 +79,7 @@ from . import _native as nat
 from . import batched
 from . import data as _data
 from . import harness
-from ._device import momentum_step
+from ._device import momentum_step_batched
 from .defences import DefenseTypes
 
 RULES = (DefenseTypes.Krum, DefenseTypes.Bulyan, DefenseTypes.TrimmedMean, DefenseTypes.NoDefense)
@@ -83,25 +92,42 @@ FADING_RATE = {'MNIST': 10000, 'CIFAR10': 2000}         # main.py:144-147
 
 class Experiment(tuple):
     """(defense, mal_prop, num_std, users_count, seed[, backdoor]): a drift experiment (backdoor False) is the 5-tuple,
-    so it equals, prints and writes as before; a backdoor experiment carries 'pattern', 1, 2 or 3 as a sixth element."""
+    so it equals, prints and writes as before; a backdoor experiment carries 'pattern', 1, 2 or 3 as a sixth element.
+    An experiment with its own learning rate and batch size (main.py's -l and -c) is the 8-tuple (defense, mal_prop,
+    num_std, users_count, seed, backdoor, learning_rate, batch_size), backdoor False for a drift experiment; the short
+    forms take the run's and return None for both."""
     __slots__ = ()
     _fields = ('defense', 'mal_prop', 'num_std', 'users_count', 'seed')     # a drift experiment's
+    _hyper = ('backdoor', 'learning_rate', 'batch_size')
 
-    def __new__(cls, defense, mal_prop, num_std, users_count, seed, backdoor=False):
+    def __new__(cls, defense, mal_prop, num_std, users_count, seed, backdoor=False, learning_rate=None,
+                batch_size=None):
         t = (defense, mal_prop, num_std, users_count, seed)
-        return tuple.__new__(cls, t if backdoor is False else t + (backdoor,))
+        if learning_rate is None and batch_size is None:
+            return tuple.__new__(cls, t if backdoor is False else t + (backdoor,))
+        if learning_rate is None or batch_size is None:
+            raise ValueError("an experiment gives both learning_rate and batch_size, or neither")
+        return tuple.__new__(cls, t + (backdoor, learning_rate, batch_size))
 
     def __getnewargs__(self):
         return tuple(self)
 
     def __repr__(self):
-        return 'Experiment(' + ', '.join(f'{n}={v!r}' for n, v in zip(self._fields + ('backdoor',), self)) + ')'
+        return 'Experiment(' + ', '.join(f'{n}={v!r}' for n, v in zip(self._fields + self._hyper, self)) + ')'
 
     defense, mal_prop, num_std, users_count, seed = (property(itemgetter(i)) for i in range(5))
 
     @property
     def backdoor(self):
         return self[5] if len(self) > 5 else False
+
+    @property
+    def learning_rate(self):
+        return self[6] if len(self) == 8 else None
+
+    @property
+    def batch_size(self):
+        return self[7] if len(self) == 8 else None
 
     @property
     def corrupted_count(self):
@@ -131,11 +157,15 @@ def minibatch(n_train, users_count, user, batch_size, epoch):
 def check(exp, batch_size=83, train_size=20000, dataset='MNIST', cifar10_backdoor=False):
     """Raise what main.py would raise for this experiment at its first `defend` (AssertionError for the reference's
     asserts), or for what the sweep's kernels do not take.  A CIFAR10 backdoor experiment is taken only with
-    cifar10_backdoor=True.  Returns the normalised Experiment."""
-    if len(exp) not in (5, 6):
-        raise ValueError(f"{exp}: an experiment has 5 or 6 elements")
+    cifar10_backdoor=True.  batch_size is the run's, which an 8-tuple's own replaces.  Returns the normalised
+    Experiment."""
+    if len(exp) not in (5, 6, 8):
+        raise ValueError(f"{exp}: an experiment has 5, 6 or 8 elements")
     exp = Experiment(str(exp[0]), float(exp[1]), float(exp[2]), int(exp[3]), int(exp[4]),
-                     normalise_backdoor(exp[5]) if len(exp) == 6 else False)
+                     normalise_backdoor(exp[5]) if len(exp) > 5 else False,
+                     *((float(exp[6]), int(exp[7])) if len(exp) == 8 else ()))
+    if exp.batch_size is not None:
+        batch_size = exp.batch_size
     if harness.check_dataset(dataset) == 'CIFAR10' and exp.backdoor is not False and not cifar10_backdoor:
         raise NotImplementedError(f"{exp}: CIFAR10 backdoor experiments need cifar10_backdoor=True "
                                   "(--cifar10-backdoor)")
@@ -160,13 +190,20 @@ def check(exp, batch_size=83, train_size=20000, dataset='MNIST', cifar10_backdoo
 
 
 def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000, backdoors=(False,),
-         dataset='MNIST', cifar10_backdoor=False):
+         dataset='MNIST', cifar10_backdoor=False, learning_rates=None, batch_sizes=None, learning_rate=0.1):
     """The Cartesian grid (defence-major, backdoor-minor) as (kept experiments, [(experiment, rejection), ...]): a cell
     main.py would reject is dropped with the exception `check` raises for it.  A drift cell (backdoor False) has 5
-    elements, a backdoor cell 6."""
+    elements, a backdoor cell 6.  When learning_rates or batch_sizes is given, every cell is an 8-tuple over the product
+    with the learning rate and then the batch size as the innermost axes; the one not given is [learning_rate] or
+    [batch_size]."""
+    hyper = learning_rates is not None or batch_sizes is not None
+    axes = (defenses, mal_props, num_stds, users_counts, seeds, backdoors)
+    if hyper:
+        axes += ([learning_rate] if learning_rates is None else learning_rates,
+                 [batch_size] if batch_sizes is None else batch_sizes)
     kept, dropped = [], []
-    for cell in itertools.product(defenses, mal_props, num_stds, users_counts, seeds, backdoors):
-        if cell[5] is False:
+    for cell in itertools.product(*axes):
+        if cell[5] is False and not hyper:
             cell = cell[:5]
         try:
             kept.append(check(cell, batch_size, train_size, dataset, cifar10_backdoor))
@@ -176,22 +213,36 @@ def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, trai
 
 
 def csv_name(exp, learning_rate, alpha=4, dataset='MNIST', data_dir=None):
-    """harness.main's log name for this experiment, with `_seed_<s>` before `.csv`."""
+    """harness.main's log name for this experiment, with `_seed_<s>` before `.csv`.  An 8-tuple's name takes its own
+    learning rate and adds `_batch_<c>` before the seed: main.py's name has no batch size."""
+    if exp.learning_rate is not None:
+        learning_rate = exp.learning_rate
     name = harness.csv_name(exp.num_std, exp.defense, exp.backdoor, exp.mal_prop, exp.users_count, alpha, learning_rate,
                             dataset, data_dir)
-    return name[:-len('.csv')] + f'_seed_{exp.seed}.csv'
+    batch = '' if exp.batch_size is None else f'_batch_{exp.batch_size}'
+    return name[:-len('.csv')] + f'{batch}_seed_{exp.seed}.csv'
 
 
 def test_epochs(epochs, test_step):
     return [e for e in range(epochs) if e % test_step == 0 or e == epochs - 1]
 
 
-def fading_lr(epoch, learning_rate, fading_rate):
+def fading_lr(epoch, learning_rate, fading_rate, out=None):
     """harness.main's client learning rate lr_t = learning_rate * fading_rate / (epoch + fading_rate) (server.py:50-52)
     as float64 tensor arithmetic on `epoch` (an integer tensor), in the Python expression's order: one product, one
-    sum and one IEEE division, so each value is the harness's Python double."""
-    num = torch.full(epoch.shape, learning_rate * fading_rate, dtype=torch.float64, device=epoch.device)
-    return torch.div(num, epoch.to(torch.float64) + fading_rate)
+    sum and one IEEE division, so each value is the harness's Python double.  learning_rate: a float, or a float64
+    tensor of per-problem products learning_rate * fading_rate already taken in Python (`lr_products`), which the
+    epoch broadcasts against."""
+    if isinstance(learning_rate, torch.Tensor):
+        num = learning_rate
+    else:
+        num = torch.full(epoch.shape, learning_rate * fading_rate, dtype=torch.float64, device=epoch.device)
+    return torch.div(num, epoch.to(torch.float64) + fading_rate, out=out)
+
+
+def lr_products(learning_rates, fading_rate, device):
+    """float64 [len(learning_rates)]: each learning_rate * fading_rate as the Python double `fading_lr` starts from."""
+    return torch.tensor([lr * fading_rate for lr in learning_rates], dtype=torch.float64, device=device)
 
 
 def backdoor_sets(specs, sampled=False):
@@ -209,10 +260,12 @@ def backdoor_sets(specs, sampled=False):
     return xs, ys, torch.tensor([len(x) for x, _ in sets], dtype=torch.int32, device=dev)
 
 
-def summary_header(with_backdoor):
-    """The summary CSV's columns; the backdoor ones only when the run has a backdoor experiment."""
+def summary_header(with_backdoor, with_hyper=False):
+    """The summary CSV's columns; the backdoor ones only when the run has a backdoor experiment, the learning rate and
+    batch size only when it has an 8-tuple."""
     bd = with_backdoor
-    return list(Experiment._fields) + (['backdoor'] if bd else []) + ['max_accuracy', 'final_accuracy'] + \
+    return list(Experiment._fields) + (['backdoor'] if bd else []) + \
+        (['learning_rate', 'batch_size'] if with_hyper else []) + ['max_accuracy', 'final_accuracy'] + \
         (['max_backdoor_accuracy', 'final_backdoor_accuracy'] if bd else []) + ['status']
 
 
@@ -244,7 +297,12 @@ class Sweep:
     Problem b trains on the first set_len[data_index[b]] rows of x_train[data_index[b]] and is tested on
     x_test[test_index[b]]: one set per seed for the synthetic data; with data_dir one training set per padded length
     (data.sampler_order) and one test set.  train_size and test_size: None (20,000 and 4,000 synthetic rows, or the
-    files' row counts), or those sizes.  cifar10_backdoor: take CIFAR10 backdoor experiments (see `check`)."""
+    files' row counts), or those sizes.  cifar10_backdoor: take CIFAR10 backdoor experiments (see `check`).
+
+    Per problem: `batch_sizes` and `learning_rates` (an 8-tuple's own, else the run's batch_size and learning_rate),
+    on the device as m (int32: the client minibatches and the test batches), lr (fp32: the momentum step) and
+    lr_fading (float64: learning_rate * fading_rate, the backdoor's lr_t numerator), allocated once so that captured
+    graphs keep their pointers."""
 
     def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None,
                  test_size=None, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000,
@@ -311,6 +369,11 @@ class Sweep:
         B, self.D = len(self.experiments), w0[seeds[0]].numel()
         self.B = B
         self.N = max(e.users_count for e in self.experiments)
+        self.batch_sizes = [batch_size if e.batch_size is None else e.batch_size for e in self.experiments]
+        self.learning_rates = [learning_rate if e.learning_rate is None else e.learning_rate for e in self.experiments]
+        self.m = torch.tensor(self.batch_sizes, **i32)
+        self.lr = torch.tensor(self.learning_rates, dtype=torch.float32, device=dev)
+        self.lr_fading = lr_products(self.learning_rates, fading_rate, dev)
         self.rows = torch.tensor([e.users_count for e in self.experiments], **i32)
         self.W = torch.stack([w0[e.seed] for e in self.experiments]).contiguous()
         self.V = torch.zeros_like(self.W)
@@ -324,10 +387,10 @@ class Sweep:
         self.correct = torch.zeros((self.n_tests, B), **i32)
         L = nat.lib()
         cifar = self.dataset == 'CIFAR10'
-        self._grads_fn = L.afl_cifar10_client_grads_sets if cifar else L.afl_mnist_client_grads_sets
-        self._evaluate_fn = L.afl_cifar10_evaluate if cifar else L.afl_mnist_evaluate
+        self._grads_fn = L.afl_cifar10_client_grads_each if cifar else L.afl_mnist_client_grads_each
+        self._evaluate_fn = L.afl_cifar10_evaluate_each if cifar else L.afl_mnist_evaluate_each
         ws_bytes = (L.afl_cifar10_evaluate_workspace_bytes if cifar else L.afl_mnist_evaluate_workspace_bytes)
-        self._eval_ws = torch.empty(max(ws_bytes(B, test_size, batch_size), 256),
+        self._eval_ws = torch.empty(max(ws_bytes(B, test_size, min(self.batch_sizes)), 256),
                                     dtype=torch.uint8, device=dev)
         self.bd0 = sum(e.backdoor is False for e in self.experiments)
         self._setup_backdoor(xtr, ytr, seeds)
@@ -385,8 +448,8 @@ class Sweep:
             nat.check(self._grads_fn(
                 self.W.data_ptr(), self.B, self.D, self.x_train.data_ptr(), self.y_train.data_ptr(),
                 self.x_train.shape[0], self.x_train.shape[1], self.set_len.data_ptr(), self.data_index.data_ptr(),
-                self.rows.data_ptr(), self.N, self.batch_size, self.epoch_counter.data_ptr(), G.data_ptr(), G.stride(0),
-                G.stride(1), torch.cuda.current_stream(self.device).cuda_stream))
+                self.rows.data_ptr(), self.N, self.m.data_ptr(), max(self.batch_sizes), self.epoch_counter.data_ptr(),
+                G.data_ptr(), G.stride(0), G.stride(1), torch.cuda.current_stream(self.device).cuda_stream))
 
     def backdoor_train(self, k=None):
         """The malicious networks of the backdoor experiments bd0 + k (all of them by default) in one launch
@@ -409,7 +472,7 @@ class Sweep:
     def _defend(self, r, sl, rnd):
         agg = {DefenseTypes.Krum: rnd.krum, DefenseTypes.Bulyan: rnd.bulyan,
                DefenseTypes.TrimmedMean: rnd.trimmed_mean, DefenseTypes.NoDefense: rnd.no_defense}[r]()
-        momentum_step(self.W[sl], self.V[sl], agg, self.momentum, self.learning_rate)
+        momentum_step_batched(self.W[sl], self.V[sl], agg, self.momentum, self.lr[sl])
 
     def aggregate(self, rule=None):
         """Step 2 for one defence (every defence when rule is None): the attack, the rule and the momentum step."""
@@ -421,7 +484,7 @@ class Sweep:
         bd = [(r, sl, rnd) for r, (sl, rnd) in self.backdoor_rounds.items() if rule is None or r == rule]
         if not bd:
             return
-        self._bd_lr.copy_(fading_lr(self.epoch_counter, self.learning_rate, self.fading_rate).expand(self.n_backdoor))
+        fading_lr(self.epoch_counter, self.lr_fading[self.bd0:], self.fading_rate, out=self._bd_lr)
         for r, sl, rnd in bd:
             rnd.backdoor_start(self.W[sl], initial=self.bd_initial[sl.start - self.bd0:sl.stop - self.bd0])
         self.backdoor_train(None if rule is None else slice(bd[0][1].start - self.bd0, bd[0][1].stop - self.bd0))
@@ -441,8 +504,8 @@ class Sweep:
         with torch.cuda.device(self.device):
             nat.check(self._evaluate_fn(
                 self.W.data_ptr(), self.B, self.D, self.x_test.data_ptr(), self.y_test.data_ptr(),
-                self.x_test.shape[0], self.test_size, self.test_index.data_ptr(), self.batch_size,
-                self.test_slot.data_ptr(), self.n_tests, self.loss_sum.data_ptr(), self.correct.data_ptr(),
+                self.x_test.shape[0], self.test_size, self.test_index.data_ptr(), self.m.data_ptr(),
+                min(self.batch_sizes), max(self.batch_sizes), self.test_slot.data_ptr(), self.n_tests, self.loss_sum.data_ptr(), self.correct.data_ptr(),
                 self._eval_ws.data_ptr(), self._eval_ws.numel(), stream))
             if self.n_backdoor:
                 args = (self.W[self.bd0:].data_ptr(), self.n_backdoor, self.D, self.bd_x.data_ptr(),
@@ -531,13 +594,15 @@ def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, tra
     logs = os.path.join(out_dir, 'logs')
     os.makedirs(logs, exist_ok=True)
     with_bd = sw.n_backdoor > 0
+    with_hyper = any(e.batch_size is not None for e in sw.experiments)
+    hyper = {pos: [sw.learning_rates[i], sw.batch_sizes[i]] for i, pos in enumerate(sw.order)}
     with open(os.path.join(logs, SUMMARY), 'w', newline='') as fh:
         w = _csv.writer(fh)
-        w.writerow(summary_header(with_bd))
-        for r in res:
+        w.writerow(summary_header(with_bd, with_hyper))
+        for k, r in enumerate(res):
             e = r['experiment']
             r['csv'] = None
-            head = list(e[:5]) + ([e.backdoor] if with_bd else [])
+            head = list(e[:5]) + ([e.backdoor] if with_bd else []) + (hyper[k] if with_hyper else [])
             if r['error'] is None:
                 r['csv'] = os.path.join(logs, csv_name(e, learning_rate, alpha, sw.dataset, sw.data_dir))
                 np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
@@ -560,8 +625,8 @@ def main(argv=None):
     p.add_argument('-b', '--backdoor', nargs='+', default=['No'], choices=['No', 'pattern', '1', '2', '3'])
     p.add_argument('-s', '--dataset', default='MNIST', choices=list(harness.DATASETS))
     p.add_argument('-e', '--epochs', type=int, default=300)
-    p.add_argument('-c', '--batch_size', type=int, default=83)
-    p.add_argument('-l', '--learning_rate', type=float, default=0.1)
+    p.add_argument('-c', '--batch_size', nargs='+', type=int, default=[83])
+    p.add_argument('-l', '--learning_rate', nargs='+', type=float, default=[0.1])
     p.add_argument('--out-dir', default='.')
     p.add_argument('--no-capture', action='store_true')
     p.add_argument('--data-dir', default=None, help="the directory holding torchvision's MNIST or CIFAR10 files (the "
@@ -570,15 +635,17 @@ def main(argv=None):
                    "-b pattern|1|2|3) in the CIFAR10 trainer kernel; without it they are skipped")
     a = p.parse_args(argv)
     train_size = 20000 if a.data_dir is None else len(harness.real_sizes(a.dataset, a.data_dir)[0][0])
-    kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, a.batch_size, train_size,
+    lrs, cs = list(dict.fromkeys(a.learning_rate)), list(dict.fromkeys(a.batch_size))
+    hyper = dict(learning_rates=lrs, batch_sizes=cs) if len(lrs) > 1 or len(cs) > 1 else {}   # 8-tuple cells
+    kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, cs[0], train_size,
                          backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)], dataset=a.dataset,
-                         cifar10_backdoor=a.cifar10_backdoor)
+                         cifar10_backdoor=a.cifar10_backdoor, **hyper)
     for cell, e in dropped:
         print(f"skipped {cell}: {type(e).__name__}: {e}")
     if not kept:
         print("no experiment left to run")
         return []
-    res = run(kept, a.epochs, a.learning_rate, batch_size=a.batch_size, out_dir=a.out_dir, capture=not a.no_capture,
+    res = run(kept, a.epochs, lrs[0], batch_size=cs[0], out_dir=a.out_dir, capture=not a.no_capture,
               fading_rate=FADING_RATE[a.dataset], dataset=a.dataset, data_dir=a.data_dir,
               cifar10_backdoor=a.cifar10_backdoor)
     for r in res:

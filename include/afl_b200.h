@@ -161,6 +161,12 @@ int afl_alie_band(const float* mu, const float* sigma, double z, const float* x,
  * v = momentum*v - lr*g ;  w += v   (fp32, in place). */
 int afl_momentum_step(float* weights, float* velocity, const float* grads, int64_t d, float momentum,
                       float learning_rate, void* stream);
+/* afl_momentum_step on `batch` contiguous rows of d floats (weights, velocity and grads: device fp32 [batch][d]), row b
+ * at its own learning rate learning_rate[b] (device fp32 [batch], read when the kernel runs) in one launch: row b's
+ * bits equal afl_momentum_step's at learning_rate[b].  A NULL pointer, batch < 1 or d < 1 -> AFL_ERR_BAD_ARG;
+ * batch > 65535 -> AFL_ERR_UNSUPPORTED. */
+int afl_momentum_step_batched(float* weights, float* velocity, const float* grads, int batch, int64_t d,
+                              float momentum, const float* learning_rate, void* stream);
 
 /* ---- multi-GPU exchange over NVLink peer memory (SURVEY 8e: "exactly one sum of the n x n partial table") ------
  * One process per GPU.  Every rank creates a context, exports its 64-byte CUDA IPC handle, the host layer gathers
@@ -563,7 +569,19 @@ int afl_backdoor_finish_batched_dev(int batch, int n, int64_t d, const int* f, c
  * (torch's max(1) of the log-probabilities: the first NaN, else the first maximum) is the label.  slot = *slot_index
  * (device int32, read when the kernel runs); a slot outside [0, n_slots) writes nothing.  loss_sum: device float64
  * [n_slots][batch], correct: device int32 [n_slots][batch].  Workspace: afl_mnist_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned (else
- * AFL_ERR_WORKSPACE); 0 on bad arguments.  More than 65535 test batches -> AFL_ERR_UNSUPPORTED. */
+ * AFL_ERR_WORKSPACE); 0 on bad arguments.  More than 65535 test batches -> AFL_ERR_UNSUPPORTED.
+ *
+ * afl_mnist_client_grads_each — afl_mnist_client_grads_sets with a minibatch size per problem: m is device int32
+ * [batch] (read when the kernel runs) and problem b uses m[b] where the _sets call uses its scalar m, so its rows equal
+ * afl_mnist_client_grads_sets(..., m = m[b], ...) bit for bit, whatever the other problems' sizes.  A problem whose
+ * m[b] lies outside [1, max_m] is skipped: none of its rows is written.  The host checks are the _sets call's with
+ * max_m for m (1 <= max_m <= 128), and a NULL m -> AFL_ERR_BAD_ARG.
+ *
+ * afl_mnist_evaluate_each — afl_mnist_evaluate with a test batch size per problem: problem b's test set runs in batches
+ * of m[b] rows (m: device int32 [batch], read when the kernel runs), so loss_sum[slot][b] and correct[slot][b] equal
+ * afl_mnist_evaluate's at m = m[b] bit for bit.  1 <= min_m <= max_m <= 128 (else AFL_ERR_BAD_ARG / _UNSUPPORTED); a
+ * problem whose m[b] lies outside [min_m, max_m] writes nothing.  Workspace: afl_mnist_evaluate_workspace_bytes(batch,
+ * n_test, min_m) bytes, 256-byte aligned (else AFL_ERR_WORKSPACE). */
 int afl_mnist_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                            int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
                            float* G, int64_t batch_stride, int64_t ld, void* stream);
@@ -575,6 +593,14 @@ size_t afl_mnist_evaluate_workspace_bytes(int batch, int n_test, int m);
 int afl_mnist_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                        int n_test, const int* data_index, int m, const int* slot_index, int n_slots, double* loss_sum,
                        int* correct, void* workspace, size_t workspace_bytes, void* stream);
+int afl_mnist_client_grads_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                                int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
+                                int n, const int* m, int max_m, const int* epoch, float* G, int64_t batch_stride,
+                                int64_t ld, void* stream);
+int afl_mnist_evaluate_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
+                            int n_test, const int* data_index, const int* m, int min_m, int max_m,
+                            const int* slot_index, int n_slots, double* loss_sum, int* correct, void* workspace,
+                            size_t workspace_bytes, void* stream);
 
 /* ---- the backdoor attacker's MnistNet (csrc/backdoor_train.cu): the model half of a backdoor sweep epoch ----------
  * Backdoor sets: x device fp32 [n_sets][max_len][784], y device int64 [n_sets][max_len], set_len device int32 [n_sets]
@@ -630,7 +656,11 @@ int afl_mnist_backdoor_test(const float* weights, int batch, int64_t d, const fl
  *
  * afl_cifar10_evaluate — server.py:92-112 / harness.main's test loop with Cifar10Net: afl_mnist_evaluate's batches,
  * float64 loss sums, correct counts by torch's argmax, NaN loss for a label outside 0..9, slot rule and workspace
- * (afl_cifar10_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned). */
+ * (afl_cifar10_evaluate_workspace_bytes(batch, n_test, m) bytes, 256-byte aligned).
+ *
+ * afl_cifar10_client_grads_each, afl_cifar10_evaluate_each — the MnistNet _each calls with Cifar10Net: per-problem m
+ * (device int32 [batch]), max_m (and min_m for the test), the skip rules and the workspace at min_m; each problem's
+ * results equal the scalar call's at m = m[b] bit for bit. */
 int afl_cifar10_client_grads(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                              int n_train, const int* data_index, const int* rows, int n, int m, const int* epoch,
                              float* G, int64_t batch_stride, int64_t ld, void* stream);
@@ -642,6 +672,14 @@ size_t afl_cifar10_evaluate_workspace_bytes(int batch, int n_test, int m);
 int afl_cifar10_evaluate(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                          int n_test, const int* data_index, int m, const int* slot_index, int n_slots,
                          double* loss_sum, int* correct, void* workspace, size_t workspace_bytes, void* stream);
+int afl_cifar10_client_grads_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                                  int n_sets, int n_rows, const int* set_len, const int* data_index, const int* rows,
+                                  int n, const int* m, int max_m, const int* epoch, float* G, int64_t batch_stride,
+                                  int64_t ld, void* stream);
+int afl_cifar10_evaluate_each(const float* weights, int batch, int64_t d, const float* x, const int64_t* y,
+                              int n_sets, int n_test, const int* data_index, const int* m, int min_m, int max_m,
+                              const int* slot_index, int n_slots, double* loss_sum, int* correct, void* workspace,
+                              size_t workspace_bytes, void* stream);
 
 /* ---- the backdoor attacker's Cifar10Net (csrc/cifar_backdoor.cu): the model half of a CIFAR10 backdoor sweep epoch --
  * The afl_mnist_backdoor_* entries above with Cifar10Net (D = 117,706): the same backdoor sets, activity condition,

@@ -87,6 +87,9 @@ SIGNATURES = {
                                   _vp, _vp]),
     "afl_attack_metrics_batched_dev": (_i, [_vp, _i, _i64, _i, _i64, _i64, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
                                             _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "afl_attack_trace_workspace_bytes": (_sz, [_i, _i64]),
+    "afl_attack_trace_dev": (_i, [_vp, _i, _i64, _i, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i64, _vp, _vp,
+                                  _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "afl_batched_large_dev_workspace_bytes": (_sz, [C.c_char_p, _i, _i, _i64, _i]),
     "afl_defend_batched_large_dev": (_i, [C.c_char_p, _vp, _i, _i64, _i, _i64, _i64, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp,
                                           _i, _vp, _sz, _vp, _vp]),

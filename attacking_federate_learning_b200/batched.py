@@ -505,6 +505,7 @@ class DeviceRound:
         self._problems = torch.arange(B, dtype=torch.int64, device=dev)
         self.initial = None                              # backdoor_start's [B, D], allocated by its first call
         self._initial_used = None                        # the initial the last backdoor_start wrote
+        self._trace_ws = None                            # attack_trace's workspace, allocated by its first call
 
     @staticmethod
     def _ptr(t):
@@ -642,6 +643,53 @@ class DeviceRound:
         if honest is not None:
             res["honest_mean"] = honest
         return res
+
+    TRACE_TABLES = {"agg_deviation": torch.float32, "malicious_deviation": torch.float32, "krum_index": torch.int32,
+                    "bulyan_malicious": torch.int32, "bulyan_selected": torch.int32}
+
+    def attack_trace(self, aggregated, slot, tables, *, krum_index=None, selection=None):
+        """This round's attack figures into row `slot` (a device int32 [1], e.g. a sweep's epoch counter) of the
+        caller's tables (C ABI `afl_attack_trace_dev`, fp32 client matrices): per problem b, `agg_deviation`
+        ||a_b - h_b|| / ||h_b|| of `aggregated` (fp32 [B, D]; for Krum the gathered rows `krum` returns),
+        `malicious_deviation` the same for row 0 (NaN when f_b = 0), `krum_index` (needs krum_index) and Bulyan's
+        `bulyan_malicious` / `bulyan_selected` counts (need selection) -- attack_metrics' figures bit for bit.
+        tables: {name: tensor} of any of those names (TRACE_TABLES gives the dtypes), each an [n_slots, B] view with
+        unit column stride and one row pitch >= B, e.g. a column slice of an [n_slots, B_total] tensor allocated once,
+        so that a captured round keeps its pointers.  A slot outside [0, n_slots) writes nothing.  Allocates nothing
+        per call: the workspace comes with the first call and is kept."""
+        if self.G.dtype != torch.float32:
+            raise TypeError("DeviceRound.attack_trace takes fp32 client matrices only")
+        for t, name, dtype, shape in ((aggregated, "aggregated", torch.float32, (self.B, self.D)),
+                                      (slot, "slot", torch.int32, (1,)),
+                                      (krum_index, "krum_index", torch.int32, (self.B,)),
+                                      (selection, "selection", torch.int32, None)):
+            if t is not None and not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == dtype
+                                      and t.is_contiguous() and (t.shape == shape if shape else
+                                                                 (t.dim() == 2 and t.shape[0] == self.B))):
+                raise ValueError(f"{name}: expected a contiguous {dtype} tensor for {self.B} problems on {self.device}")
+        if aggregated is None or slot is None:
+            raise ValueError("attack_trace: aggregated and slot are required")
+        unknown = set(tables) - set(self.TRACE_TABLES)
+        if unknown or not tables:
+            raise ValueError(f"attack_trace: tables names one or more of {', '.join(self.TRACE_TABLES)} "
+                             f"(got {sorted(tables)})")
+        first = next(iter(tables.values()))
+        n_slots, table_ld = first.shape[0], first.stride(0)
+        for name, t in tables.items():
+            if not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == self.TRACE_TABLES[name]
+                    and t.dim() == 2 and tuple(t.shape) == (n_slots, self.B) and t.stride(1) == 1
+                    and t.stride(0) == table_ld and table_ld >= self.B):
+                raise ValueError(f"tables[{name!r}]: expected a {self.TRACE_TABLES[name]} [{n_slots}, {self.B}] view "
+                                 f"with unit column stride and row pitch {table_ld} >= {self.B} on {self.device}")
+        L = nat.lib()
+        if self._trace_ws is None:
+            self._trace_ws = torch.empty(L.afl_attack_trace_workspace_bytes(self.B, self.D), dtype=torch.uint8,
+                                         device=self.device)
+        self._call(L.afl_attack_trace_dev, self.G.data_ptr(), self.B, self._bs, self.N, self.D, self._ld,
+                   self._ptr(self.rows), self.f.data_ptr(), aggregated.data_ptr(), self._ptr(krum_index),
+                   self._ptr(selection), 0 if selection is None else selection.shape[1], slot.data_ptr(), n_slots,
+                   table_ld, *(self._ptr(tables.get(k)) for k in self.TRACE_TABLES), self._trace_ws.data_ptr(),
+                   self._trace_ws.numel(), self.status.data_ptr(), _stream_ptr(self.G))
 
     def clear_status(self):
         """Zero `status` (enqueued)."""

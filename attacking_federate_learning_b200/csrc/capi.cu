@@ -150,6 +150,10 @@ int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, 
                    const ProblemParams* each, const float* agg, const int* idx, const int* sel, int sel_ld,
                    float* dev_out, double* sums_out, float* honest_out, int* krum_hit, int* mal_count, int* sel_count,
                    void* partial, cudaStream_t stream, bool rows = false);
+int attack_trace(const float* G, int batch, int64_t g_batch, int n, int64_t d, int64_t ld, const ProblemParams* each,
+                 const float* agg, const int* idx, const int* sel, int sel_ld, const int* slot, int n_slots,
+                 int64_t table_ld, float* agg_dev, float* mal_dev, int* idx_out, int* mal_count, int* sel_count,
+                 void* partial, cudaStream_t stream, bool rows);
 int backdoor_start(const void* G, int fmax, int64_t d, int64_t ld, int dtype, int batch, int64_t g_batch,
                    const ProblemParams* each, const float* w, int64_t w_batch, float* mu_out, float* sigma_out,
                    float* initial_out, cudaStream_t stream);
@@ -1424,6 +1428,41 @@ static int attack_metrics_dev(const void* G, int batch, int64_t batch_stride, in
                                   static_cast<uint8_t*>(ws) + table_bytes(batch), stream, rows != nullptr);
 }
 
+// afl_attack_trace_dev's workspace: the T_METRICS table, then double[batch][tiles][3] partial sums.
+static size_t trace_workspace_bytes(int batch, int64_t d) {
+  return table_bytes(batch) +
+         align_up(static_cast<size_t>(batch) * colstats::deviation_tiles(d, AFL_F32) * 3 * sizeof(double), 256);
+}
+
+// One epoch's attack figures of an fp32 batch into row *slot of caller-held tables: afl_attack_metrics_batched_dev's
+// table and checks, then colstats::attack_trace.
+static int attack_trace_dev(const float* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
+                            const int* rows, const int* fs, const float* agg, const int* idx, const int* sel,
+                            int sel_ld, const int* slot, int n_slots, int64_t table_ld, float* agg_dev,
+                            float* mal_dev, int* idx_out, int* mal_count, int* sel_count, void* ws, size_t ws_bytes,
+                            int* status, cudaStream_t stream) {
+  const char* who = "afl_attack_trace_dev";
+  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, AFL_F32, INT32_MAX);
+  if (rc) return rc;
+  if (!agg || !slot) { set_error("%s: the aggregate agg and the device slot are required (NULL given)", who); return AFL_ERR_BAD_ARG; }
+  if (n_slots < 1) { set_error("%s: n_slots must be >= 1 (got %d)", who, n_slots); return AFL_ERR_BAD_ARG; }
+  if (table_ld < batch) {
+    set_error("%s: table_ld %lld is less than batch %d", who, static_cast<long long>(table_ld), batch);
+    return AFL_ERR_BAD_ARG;
+  }
+  if (sel && sel_ld < 1) { set_error("%s: sel_ld must be >= 1 (got %d)", who, sel_ld); return AFL_ERR_BAD_ARG; }
+  if ((mal_count || sel_count) && !sel) { set_error("%s: mal_count and sel_count need sel", who); return AFL_ERR_BAD_ARG; }
+  if (idx_out && !idx) { set_error("%s: idx_out needs idx", who); return AFL_ERR_BAD_ARG; }
+  if ((rc = check_dev(who, fs, status, ws, ws_bytes, trace_workspace_bytes(batch, d)))) return rc;
+  TableArgs a{};
+  a.rule = T_METRICS; a.batch = batch; a.n = n; a.rows = rows; a.fs = fs; a.table = static_cast<ProblemParams*>(ws);
+  a.status = status;
+  if ((rc = launch_table(a, stream))) return rc;
+  return colstats::attack_trace(G, batch, batch_stride, n, d, ld, a.table, agg, idx, sel, sel_ld, slot, n_slots,
+                                table_ld, agg_dev, mal_dev, idx_out, mal_count, sel_count,
+                                static_cast<uint8_t*>(ws) + table_bytes(batch), stream, rows != nullptr);
+}
+
 }  // namespace afl
 
 using namespace afl;
@@ -1748,6 +1787,21 @@ int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_strid
   return attack_metrics_dev(G, batch, batch_stride, n, d, ld, dtype, rows, corrupted_counts, agg, idx, sel, sel_ld,
                             dev_out, sums_out, honest_out, krum_hit, mal_count, sel_count, workspace, workspace_bytes,
                             status, static_cast<cudaStream_t>(stream));
+}
+
+size_t afl_attack_trace_workspace_bytes(int batch, int64_t d) {
+  if (batch < 1 || batch > kBatchMax || d < 1) return 0;
+  return trace_workspace_bytes(batch, d);
+}
+
+int afl_attack_trace_dev(const float* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, const int* rows,
+                         const int* corrupted_counts, const float* agg, const int* idx, const int* sel, int sel_ld,
+                         const int* slot, int n_slots, int64_t table_ld, float* agg_dev, float* mal_dev, int* idx_out,
+                         int* mal_count, int* sel_count, void* workspace, size_t workspace_bytes, int* status,
+                         void* stream) {
+  return attack_trace_dev(G, batch, batch_stride, n, d, ld, rows, corrupted_counts, agg, idx, sel, sel_ld, slot,
+                          n_slots, table_ld, agg_dev, mal_dev, idx_out, mal_count, sel_count, workspace,
+                          workspace_bytes, status, static_cast<cudaStream_t>(stream));
 }
 
 int afl_backdoor_start_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,

@@ -398,13 +398,30 @@ __device__ __forceinline__ void cta_sum2(double& a, double& b) {
   }
 }
 
+// cta_sum2 with a third sum: each of the three takes cta_sum2's order, so a and b come out as cta_sum2 gives them.
+__device__ __forceinline__ void cta_sum3(double& a, double& b, double& c) {
+  __shared__ double s[3][kBlock / 32];
+  a = warp_sum(a);
+  b = warp_sum(b);
+  c = warp_sum(c);
+  if (lane_id() == 0) { s[0][threadIdx.x / 32] = a; s[1][threadIdx.x / 32] = b; s[2][threadIdx.x / 32] = c; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    a = s[0][0]; b = s[1][0]; c = s[2][0];
+#pragma unroll
+    for (int w = 1; w < kBlock / 32; ++w) { a += s[0][w]; b += s[1][w]; c += s[2][w]; }
+  }
+}
+
 // h = mean of rows f..n-1: mean_kernel's sequential fp32 row sum and one IEEE division on that row range, so h is
 // afl_mean of G[f:] bit for bit.  a = the aggregate: agg[b] (fp32, pitch d), or row idx[b] of G[b] upcast to fp32
 // (Krum's result, read in place).  partial[b][tile] = (sum (a - h)^2, sum h^2) over the tile's columns in float64; the
 // differences and squares are formed from the fp32 values as float64, so nothing cancels.  f >= n (no honest row)
 // reads no row and gives h = 0 / 0 = NaN; an idx outside [0, n) reads no row and gives a = NaN.  partial == NULL:
 // only honest_out is wanted.  kRows (a ragged batch): problem b has each[b].tm.n_rows rows instead of n.
-template <typename T, int V, bool VL, bool kRows>
+// kTrace (afl_attack_trace_dev, agg given): also sum (r0 - h)^2 with r0 = row 0 when f > 0 (0 otherwise), formed as
+// (a - h)^2 is, so that sum equals the first with a = row 0; partial is then read as double[3] per (problem, tile).
+template <typename T, int V, bool VL, bool kRows, bool kTrace = false>
 __global__ void __launch_bounds__(kBlock)
 honest_deviation_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, int64_t g_batch, int f,
                         const ProblemParams* __restrict__ each, const float* __restrict__ agg,
@@ -416,6 +433,7 @@ honest_deviation_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, i
   f = f < n ? f : n;
   const int64_t c0 = (static_cast<int64_t>(blockIdx.x) * kBlock + threadIdx.x) * V;
   double sd = 0.0, sh = 0.0;
+  [[maybe_unused]] double sm = 0.0;
   if (c0 < d) {
     const T* p = G + b * g_batch + c0;
     float acc[V];
@@ -447,6 +465,10 @@ honest_deviation_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, i
       for (int k = 0; k < V; ++k)
         if (c0 + k < d) a.v[k] = __ldg(agg + b * d + c0 + k);
     }
+    [[maybe_unused]] Pack<V> m;
+    if constexpr (kTrace) {
+      if (f > 0) m = load_cols<T, V, VL>(p, c0, d);
+    }
     const float fn = static_cast<float>(n - f);
     const int64_t o = b * d + c0;
 #pragma unroll
@@ -457,12 +479,23 @@ honest_deviation_kernel(const T* __restrict__ G, int n, int64_t d, int64_t ld, i
         const double hd = static_cast<double>(h), df = static_cast<double>(a.v[k]) - hd;
         sd = fma(df, df, sd);
         sh = fma(hd, hd, sh);
+        if constexpr (kTrace) {
+          if (f > 0) { const double dm = static_cast<double>(m.v[k]) - hd; sm = fma(dm, dm, sm); }
+        }
       }
     }
   }
-  if (!partial) return;
-  cta_sum2(sd, sh);
-  if (threadIdx.x == 0) partial[static_cast<int64_t>(b) * gridDim.x + blockIdx.x] = make_double2(sd, sh);
+  if constexpr (kTrace) {
+    cta_sum3(sd, sh, sm);
+    if (threadIdx.x == 0) {
+      double* q = reinterpret_cast<double*>(partial) + 3 * (static_cast<int64_t>(b) * gridDim.x + blockIdx.x);
+      q[0] = sd; q[1] = sh; q[2] = sm;
+    }
+  } else {
+    if (!partial) return;
+    cta_sum2(sd, sh);
+    if (threadIdx.x == 0) partial[static_cast<int64_t>(b) * gridDim.x + blockIdx.x] = make_double2(sd, sh);
+  }
 }
 
 // One CTA per problem: thread t adds tiles t, t + kBlock, ... in that order, then cta_sum2.  The order depends on
@@ -502,6 +535,40 @@ selection_stats_kernel(int batch, int f, const ProblemParams* __restrict__ each,
     }
     if (mal_count) mal_count[b] = mal;
     if (sel_count) sel_count[b] = cnt;
+  }
+}
+
+// afl_attack_trace_dev's finish, one CTA per problem: deviation_finish_kernel's order on three sums, then entry
+// [*slot][b] of each given table (pitch table_ld): agg_dev = sqrt(sum (a - h)^2 / sum h^2), mal_dev the same with row 0
+// (NaN when f_b = 0), idx_out = idx[b], and selection_stats_kernel's two counts.  A slot outside [0, n_slots) writes
+// nothing.
+__global__ void __launch_bounds__(kBlock)
+trace_finish_kernel(const double* __restrict__ partial, int tiles, const ProblemParams* __restrict__ each,
+                    const int* __restrict__ slot, int n_slots, int64_t table_ld, const int* __restrict__ idx,
+                    const int* __restrict__ sel, int sel_ld, float* __restrict__ agg_dev, float* __restrict__ mal_dev,
+                    int* __restrict__ idx_out, int* __restrict__ mal_count, int* __restrict__ sel_count) {
+  const int b = blockIdx.x;
+  const int s = *slot;
+  if (s < 0 || s >= n_slots) return;                   // the whole CTA, before any barrier
+  const double* p = partial + 3 * static_cast<int64_t>(b) * tiles;
+  double sd = 0.0, sh = 0.0, sm = 0.0;
+  for (int t = threadIdx.x; t < tiles; t += kBlock) { sd += p[3 * t]; sh += p[3 * t + 1]; sm += p[3 * t + 2]; }
+  cta_sum3(sd, sh, sm);
+  if (threadIdx.x != 0) return;
+  const int f = each[b].f;
+  const int64_t o = static_cast<int64_t>(s) * table_ld + b;
+  if (agg_dev) agg_dev[o] = static_cast<float>(sqrt(sd / sh));
+  if (mal_dev) mal_dev[o] = f > 0 ? static_cast<float>(sqrt(sm / sh)) : __int_as_float(0x7fc00000);
+  if (idx_out) idx_out[o] = idx[b];
+  if (sel) {
+    int mal = 0, cnt = 0;
+    for (int j = 0; j < sel_ld; ++j) {
+      const int i = sel[static_cast<int64_t>(b) * sel_ld + j];
+      cnt += i >= 0;
+      mal += i >= 0 && i < f;
+    }
+    if (mal_count) mal_count[o] = mal;
+    if (sel_count) sel_count[o] = cnt;
   }
 }
 
@@ -677,6 +744,33 @@ int attack_metrics(const void* G, int batch, int64_t g_batch, int n, int64_t d, 
         batch, f, each, idx, sel, sel_ld, krum_hit, mal_count, sel_count);
     AFL_LAUNCH_CHECK("selection_stats_kernel");
   }
+  return AFL_OK;
+}
+
+// afl_attack_trace_dev's two kernels on `batch` fp32 problems (arguments checked by the caller, capi.cu): the trace
+// instance of honest_deviation_kernel against agg, then trace_finish_kernel.  partial: double[batch][tiles][3].
+int attack_trace(const float* G, int batch, int64_t g_batch, int n, int64_t d, int64_t ld, const ProblemParams* each,
+                 const float* agg, const int* idx, const int* sel, int sel_ld, const int* slot, int n_slots,
+                 int64_t table_ld, float* agg_dev, float* mal_dev, int* idx_out, int* mal_count, int* sel_count,
+                 void* partial, cudaStream_t stream, bool rows) {
+  const int tiles = static_cast<int>(deviation_tiles(d, AFL_F32));
+  const dim3 grid(tiles, batch);
+  const bool v = vec_ok(G, ld, AFL_F32, batch, g_batch);
+  double2* part = static_cast<double2*>(partial);
+  ProfScope ps("attack_trace", stream);
+#define AFL_TRACE_LAUNCH(VL)                                                                                             \
+  do {                                                                                                                   \
+    if (rows) honest_deviation_kernel<float, 4, VL, true, true><<<grid, kBlock, 0, stream>>>(G, n, d, ld, g_batch, 0, each, agg, nullptr, nullptr, part); \
+    else honest_deviation_kernel<float, 4, VL, false, true><<<grid, kBlock, 0, stream>>>(G, n, d, ld, g_batch, 0, each, agg, nullptr, nullptr, part); \
+  } while (0)
+  if (v) AFL_TRACE_LAUNCH(true);
+  else AFL_TRACE_LAUNCH(false);
+#undef AFL_TRACE_LAUNCH
+  AFL_LAUNCH_CHECK("honest_deviation_kernel");
+  trace_finish_kernel<<<batch, kBlock, 0, stream>>>(static_cast<const double*>(partial), tiles, each, slot, n_slots,
+                                                     table_ld, idx, sel, sel_ld, agg_dev, mal_dev, idx_out, mal_count,
+                                                     sel_count);
+  AFL_LAUNCH_CHECK("trace_finish_kernel");
   return AFL_OK;
 }
 

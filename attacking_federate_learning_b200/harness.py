@@ -44,8 +44,11 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import batched
 from . import data as _data
+from . import defences
 from . import malicious
+from . import metrics
 from .ingest import ParamLayout
 from .server import AggregationServer
 
@@ -273,10 +276,17 @@ class BackdoorTrainer:
 
 def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0.1, fading_rate=10000, momentum=0.9,
          batch_size=83, output=None, device="cuda", out_dir=".", seed=0, train_size=None, test_size=None, test_step=5,
-         backdoor=False, alpha=4, mal_epochs=5, dataset='MNIST', data_dir=None):
+         backdoor=False, alpha=4, mal_epochs=5, dataset='MNIST', data_dir=None, trace=False):
     """main.py's experiment.  train_size and test_size (None: 20,000 and 4,000) size the synthetic problem; with
     data_dir the data are the real dataset's files there (see the module docstring) and the sizes, when given, must
-    be the files' row counts."""
+    be the files' row counts.  Returns (accuracies, accuracies_epochs, csv).
+
+    trace=True also records every epoch's attack figures after `defend` (sweep.run(trace=True)'s, from the existing
+    calls): batched.attack_metrics on the [1, N, D] matrix against the applied aggregate and against row 0, Krum's
+    index from a second `krum(..., return_index=True)` and Bulyan's selection from a second `bulyan(...,
+    return_selection=True)`.  So a traced Krum or Bulyan epoch runs its rule twice and each traced epoch synchronises
+    the host.  It writes the trace CSV beside the accuracy CSV (`..._trace.csv`, metrics.TRACE_HEADER) and returns the
+    trace (metrics.trace_record's dict) as a fourth element."""
     synth = dataset_name(dataset, data_dir)
     if output:
         def my_print(s, end='\n'):
@@ -306,6 +316,8 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     my_print("\nStarting Training...")
     criterion = nn.NLLLoss()
     accuracies, accuracies_epochs = [], []
+    figures = {k: [] for k in ('agg_deviation', 'malicious_deviation', 'krum_index', 'bulyan_malicious',
+                               'bulyan_selected')}
     for epoch in range(epochs):
         lr_t = learning_rate * fading_rate / (epoch + fading_rate)       # server.py:50-52
         for u in users:                                                   # server.py:54-56 dispatch_weights
@@ -314,7 +326,9 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
             attacker.attack_rows(srv.users_grads, corrupted_count, users[0].original_params, users[0].learning_rate)
         else:
             attacker.attack_rows(srv.users_grads, corrupted_count)
-        srv.defend(defense, epoch)                                        # main.py:71
+        aggregate = srv.defend(defense, epoch)                            # main.py:71
+        if trace:
+            attack_figures(srv.users_grads, users_count, corrupted_count, defense, aggregate, figures)
         if epoch % test_step == 0 or epoch == epochs - 1:
             layout.row_into_parameters(srv.current_weights, list(test_net.parameters()))
             test_net.eval()
@@ -344,10 +358,36 @@ def main(mal_prop, num_std, defense, users_count=10, epochs=150, learning_rate=0
     csv = os.path.join(out_dir, 'logs', csv_name(num_std, defense, backdoor, mal_prop, users_count, alpha, learning_rate,
                                                  dataset, data_dir))
     np.savetxt(csv, accuracies, delimiter=',')                            # main.py:100
-    return accuracies, accuracies_epochs, csv
+    if not trace:
+        return accuracies, accuracies_epochs, csv
+    tr = metrics.trace_record(defense, corrupted_count, *figures.values())
+    metrics.write_trace_csv(csv[:-len('.csv')] + '_trace.csv', tr)
+    return accuracies, accuracies_epochs, csv, tr
 
 
-if __name__ == '__main__':
+def attack_figures(G, users_count, corrupted_count, defense, aggregate, figures):
+    """One epoch's trace figures of main's server matrix G ([N, D]) and the aggregate `defend` applied, appended to
+    figures' lists (metrics.trace_record's arguments)."""
+    f, G3 = corrupted_count, G[None]
+    sel = None
+    if defense == 'Krum':
+        figures['krum_index'].append(defences.krum(G, users_count, f, return_index=True))
+    elif defense == 'Bulyan':
+        sel = defences.bulyan(G, users_count, f, return_selection=True)[1].to(torch.int32)
+        s = sel.cpu().numpy()
+        figures['bulyan_malicious'].append(int(((s >= 0) & (s < f)).sum()))
+        figures['bulyan_selected'].append(int((s >= 0).sum()))
+    met = batched.attack_metrics(G3, f, aggregated=aggregate.float()[None], selection=None if sel is None else sel[None])
+    figures['agg_deviation'].append(float(met['rel_deviation'][0]))
+    mal = float('nan')
+    if f > 0:
+        row0 = torch.zeros(1, dtype=torch.int32, device=G.device)
+        mal = float(batched.attack_metrics(G3, f, krum_index=row0)['rel_deviation'][0])
+    figures['malicious_deviation'].append(mal)
+
+
+def parser():
+    """main.py's command line (the flags that apply here), plus --trace."""
     p = argparse.ArgumentParser()                                         # main.py:104-131 (the flags that apply here)
     p.add_argument('-m', '--mal-prop', default=0.24, type=float)
     p.add_argument('-z', '--num_std', default=1.5, type=float)
@@ -361,8 +401,14 @@ if __name__ == '__main__':
     p.add_argument('-s', '--dataset', default='MNIST', choices=list(DATASETS))
     p.add_argument('--data-dir', default=None, help="the directory holding torchvision's MNIST or CIFAR10 files "
                    "(the reference's ./mnist_data or ./cifar10_data); without it a synthetic stand-in is trained")
-    a = p.parse_args()
+    p.add_argument('--trace', action='store_true', help="record every epoch's attack figures into a _trace.csv beside "
+                   "the accuracy log (runs Krum and Bulyan twice per epoch)")
+    return p
+
+
+if __name__ == '__main__':
+    a = parser().parse_args()
     bd = False if a.backdoor == 'No' else a.backdoor if a.backdoor == 'pattern' else int(a.backdoor)
     main(a.mal_prop, a.num_std, a.defense, users_count=a.users_count, epochs=a.epochs, learning_rate=a.learning_rate,
          batch_size=a.batch_size, output=a.output, backdoor=bd, dataset=a.dataset, data_dir=a.data_dir,
-         fading_rate=2000 if a.dataset == 'CIFAR10' else 10000)                 # main.py:144-147
+         fading_rate=2000 if a.dataset == 'CIFAR10' else 10000, trace=a.trace)   # main.py:144-147

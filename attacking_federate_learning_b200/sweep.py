@@ -63,6 +63,16 @@ kernels take problem b's minibatch and test batch size from a device array (C AB
 starts from its own learning_rate * fading_rate; each problem's bits equal a sweep of its own (lr, c).  The backdoor
 trainer keeps its own batch (200) and lr (0.1); epochs, momentum and fading rate stay per run.  An 8-tuple's CSV
 takes its own learning rate and adds `_batch_<c>` before the seed, since main.py's name has no batch size.
+
+trace=True (--trace) records why accuracy moves: in every epoch, after each rule, one `DeviceRound.attack_trace`
+call (C ABI `afl_attack_trace_dev`) per (defence, attack) slice writes each experiment's ||aggregate - honest mean|| /
+||honest mean||, the same for its first malicious row (the crafted vector when the attack wrote one), Krum's index and
+Bulyan's malicious and selected counts into row `epoch` of [epochs, B] device tables, inside the captured epoch and
+with no host synchronisation.  It reads G and the aggregates and writes only its tables, so every other output keeps
+its bits.  `results()` gains `trace` per experiment (metrics.trace_record), and `run` writes one
+`..._seed_<s>_trace.csv` per experiment (metrics.TRACE_HEADER) and four more summary columns (metrics.TRACE_SUMMARY).
+
+    python -m attacking_federate_learning_b200.sweep -d Krum Bulyan TrimmedMean NoDefense -z 0.5 1.5 -m 0.1 0.24 -e 10 --trace
 """
 from __future__ import annotations
 
@@ -79,6 +89,7 @@ from . import _native as nat
 from . import batched
 from . import data as _data
 from . import harness
+from . import metrics
 from ._device import momentum_step_batched
 from .defences import DefenseTypes
 
@@ -88,6 +99,7 @@ MAX_BATCH_SIZE = 128                     # minibatch rows of the client-gradient
 BACKDOOR_BATCH = 200                     # BackdoorTrainer's minibatch and test batch (the trainer kernel's limit)
 SUMMARY = 'sweep_summary.csv'
 FADING_RATE = {'MNIST': 10000, 'CIFAR10': 2000}         # main.py:144-147
+TRACE_UNSET = -9                         # a trace table entry no epoch has written
 
 
 class Experiment(tuple):
@@ -260,13 +272,49 @@ def backdoor_sets(specs, sampled=False):
     return xs, ys, torch.tensor([len(x) for x, _ in sets], dtype=torch.int32, device=dev)
 
 
-def summary_header(with_backdoor, with_hyper=False):
+def summary_header(with_backdoor, with_hyper=False, with_trace=False):
     """The summary CSV's columns; the backdoor ones only when the run has a backdoor experiment, the learning rate and
-    batch size only when it has an 8-tuple."""
+    batch size only when it has an 8-tuple, the trace's (metrics.TRACE_SUMMARY) only when the run traces."""
     bd = with_backdoor
     return list(Experiment._fields) + (['backdoor'] if bd else []) + \
         (['learning_rate', 'batch_size'] if with_hyper else []) + ['max_accuracy', 'final_accuracy'] + \
-        (['max_backdoor_accuracy', 'final_backdoor_accuracy'] if bd else []) + ['status']
+        (['max_backdoor_accuracy', 'final_backdoor_accuracy'] if bd else []) + \
+        (metrics.TRACE_SUMMARY if with_trace else []) + ['status']
+
+
+def trace_csv_name(name):
+    """The trace CSV beside the accuracy CSV `name`: `..._seed_<s>_trace.csv`."""
+    return name[:-len('.csv')] + '_trace.csv'
+
+
+def write_logs(res, logs, names, with_backdoor=False, hyper=None, trace=False):
+    """`run`'s files under `logs` from `results()`-style dicts: each successful experiment's accuracy CSV names[k]
+    (np.savetxt, main.py:100) and, with trace, its trace CSV; then the summary CSV.  hyper: None, or [learning_rate,
+    batch_size] per result for the summary.  Sets each dict's `csv` (and with trace `trace_csv`), None when it failed."""
+    with_bd, with_hyper = with_backdoor, hyper is not None
+    with open(os.path.join(logs, SUMMARY), 'w', newline='') as fh:
+        w = _csv.writer(fh)
+        w.writerow(summary_header(with_bd, with_hyper, trace))
+        for k, r in enumerate(res):
+            e = r['experiment']
+            r['csv'] = None
+            if trace:
+                r['trace_csv'] = None
+            head = list(e[:5]) + ([e.backdoor] if with_bd else []) + (hyper[k] if with_hyper else [])
+            if r['error'] is None:
+                r['csv'] = os.path.join(logs, names[k])
+                np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
+                bd = r.get('backdoor_accuracies')
+                tail = ([max(bd), bd[-1]] if bd else ['', '']) if with_bd else []
+                if trace:
+                    r['trace_csv'] = os.path.join(logs, trace_csv_name(names[k]))
+                    metrics.write_trace_csv(r['trace_csv'], r['trace'])
+                    tail += metrics.trace_summary(r['trace'])
+                w.writerow(head + [max(r['accuracies']), r['accuracies'][-1]] + tail + ['ok'])
+            else:
+                w.writerow(head + ['', ''] + (['', ''] if with_bd else []) +
+                           ([''] * len(metrics.TRACE_SUMMARY) if trace else []) +
+                           [f"failed: {type(r['error']).__name__}: {r['error']}"])
 
 
 def status_error(code, name):
@@ -302,11 +350,12 @@ class Sweep:
     Per problem: `batch_sizes` and `learning_rates` (an 8-tuple's own, else the run's batch_size and learning_rate),
     on the device as m (int32: the client minibatches and the test batches), lr (fp32: the momentum step) and
     lr_fading (float64: learning_rate * fading_rate, the backdoor's lr_t numerator), allocated once so that captured
-    graphs keep their pointers."""
+    graphs keep their pointers.  trace=True: `trace` holds the [epochs, B] tables of DeviceRound.TRACE_TABLES (TRACE_UNSET
+    until an epoch writes them), filled after each rule at row epoch_counter; None otherwise."""
 
     def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None,
                  test_size=None, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000,
-                 dataset='MNIST', data_dir=None, cifar10_backdoor=False):
+                 dataset='MNIST', data_dir=None, cifar10_backdoor=False, trace=False):
         self.dataset = harness.check_dataset(dataset)
         self.data_dir = data_dir
         real = None
@@ -410,6 +459,10 @@ class Sweep:
                 rnd.z.copy_(torch.tensor([e.num_std for e in sub], dtype=torch.float64))
                 rnd.rows.copy_(torch.tensor([e.users_count for e in sub], dtype=torch.int32))
                 rounds[r] = (sl, rnd)
+        self.trace = None
+        if trace:                                                         # [epochs, B] per DeviceRound.TRACE_TABLES
+            self.trace = {k: torch.full((epochs, B), TRACE_UNSET, dtype=t, device=dev)
+                          for k, t in batched.DeviceRound.TRACE_TABLES.items()}
         self._graphs = None
 
     def _setup_backdoor(self, xtr, ytr, seeds):
@@ -472,6 +525,13 @@ class Sweep:
     def _defend(self, r, sl, rnd):
         agg = {DefenseTypes.Krum: rnd.krum, DefenseTypes.Bulyan: rnd.bulyan,
                DefenseTypes.TrimmedMean: rnd.trimmed_mean, DefenseTypes.NoDefense: rnd.no_defense}[r]()
+        if self.trace is not None:       # reads G, agg and the rule's indices; the counter is still this epoch's
+            names = ['agg_deviation', 'malicious_deviation'] + (
+                ['krum_index'] if r == DefenseTypes.Krum else
+                ['bulyan_malicious', 'bulyan_selected'] if r == DefenseTypes.Bulyan else [])
+            rnd.attack_trace(agg, self.epoch_counter, {k: self.trace[k][:, sl] for k in names},
+                             krum_index=rnd.krum_index if r == DefenseTypes.Krum else None,
+                             selection=rnd.selection if r == DefenseTypes.Bulyan else None)
         momentum_step_batched(self.W[sl], self.V[sl], agg, self.momentum, self.lr[sl])
 
     def aggregate(self, rule=None):
@@ -552,8 +612,10 @@ class Sweep:
     def results(self):
         """Synchronise and return, in the order of `experiments` as given, one dict per experiment: experiment,
         accuracies, accuracies_epochs, losses (harness.main's test loss), error (None, or the exception), and for a
-        backdoor experiment backdoor_accuracies and backdoor_losses (BackdoorTrainer.test('POST') at each test epoch)."""
+        backdoor experiment backdoor_accuracies and backdoor_losses (BackdoorTrainer.test('POST') at each test epoch).
+        With trace, also `trace`: metrics.trace_record's dict over epochs, None for a failed experiment."""
         st = self.status()
+        tables = None if self.trace is None else {k: v.cpu().numpy() for k, v in self.trace.items()}
         correct = self.correct.cpu().numpy()
         loss = self.loss_sum.cpu().numpy()
         if self.n_backdoor:
@@ -567,6 +629,9 @@ class Sweep:
             err = status_error(int(st[i]), f"experiment {tuple(e)}") if st[i] else None
             out[pos] = dict(experiment=e, accuracies=acc, accuracies_epochs=epochs,
                             losses=[float(loss[t, i]) / self.test_size for t in range(self.n_tests)], error=err)
+            if tables is not None:
+                out[pos]['trace'] = None if err is not None else metrics.trace_record(
+                    e.defense, e.corrupted_count, *(tables[k][:, i] for k in batched.DeviceRound.TRACE_TABLES))
             if i >= self.bd0:
                 k = i - self.bd0
                 n = int(bd_len[bd_index[k]])
@@ -577,45 +642,33 @@ class Sweep:
 
 def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None, test_size=None,
         test_step=5, out_dir='.', capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000, dataset='MNIST',
-        data_dir=None, cifar10_backdoor=False):
+        data_dir=None, cifar10_backdoor=False, trace=False):
     """Train every experiment for `epochs` epochs as one batch; write each one's accuracy CSV and the summary CSV under
     out_dir/logs.  Returns `Sweep.results()` with `csv` (None for a failed experiment) added to each dict.  Raises
     before any GPU work for an experiment main.py would reject (see `check`).  alpha, mal_epochs and fading_rate are
     harness.main's (the backdoor experiments' malicious training and client learning rate), and so is dataset ('MNIST'
     or 'CIFAR10', main.py -s).  data_dir: the real dataset's files (see the module docstring); train_size and test_size
     are then None or the files' row counts, and None means 20,000 and 4,000 synthetic rows otherwise.
-    cifar10_backdoor=True takes CIFAR10 backdoor experiments (main.py -s CIFAR10 -b ...)."""
+    cifar10_backdoor=True takes CIFAR10 backdoor experiments (main.py -s CIFAR10 -b ...).  trace=True records every
+    epoch's attack figures (see the module docstring) and adds `trace_csv` to each dict."""
     sw = Sweep(experiments, epochs, learning_rate, momentum, batch_size, train_size, test_size, test_step, capture,
-               device, alpha, mal_epochs, fading_rate, dataset, data_dir, cifar10_backdoor)
+               device, alpha, mal_epochs, fading_rate, dataset, data_dir, cifar10_backdoor, trace)
     with torch.cuda.device(sw.device):
         for epoch in range(epochs):
             sw.step(epoch)
     res = sw.results()
     logs = os.path.join(out_dir, 'logs')
     os.makedirs(logs, exist_ok=True)
-    with_bd = sw.n_backdoor > 0
     with_hyper = any(e.batch_size is not None for e in sw.experiments)
     hyper = {pos: [sw.learning_rates[i], sw.batch_sizes[i]] for i, pos in enumerate(sw.order)}
-    with open(os.path.join(logs, SUMMARY), 'w', newline='') as fh:
-        w = _csv.writer(fh)
-        w.writerow(summary_header(with_bd, with_hyper))
-        for k, r in enumerate(res):
-            e = r['experiment']
-            r['csv'] = None
-            head = list(e[:5]) + ([e.backdoor] if with_bd else []) + (hyper[k] if with_hyper else [])
-            if r['error'] is None:
-                r['csv'] = os.path.join(logs, csv_name(e, learning_rate, alpha, sw.dataset, sw.data_dir))
-                np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
-                bd = r.get('backdoor_accuracies')
-                tail = ([max(bd), bd[-1]] if bd else ['', '']) if with_bd else []
-                w.writerow(head + [max(r['accuracies']), r['accuracies'][-1]] + tail + ['ok'])
-            else:
-                w.writerow(head + ['', ''] + (['', ''] if with_bd else []) +
-                           [f"failed: {type(r['error']).__name__}: {r['error']}"])
+    names = [csv_name(r['experiment'], learning_rate, alpha, sw.dataset, sw.data_dir) for r in res]
+    write_logs(res, logs, names, sw.n_backdoor > 0, [hyper[k] for k in range(len(res))] if with_hyper else None,
+               trace)
     return res
 
 
-def main(argv=None):
+def parser():
+    """The command line of `python -m attacking_federate_learning_b200.sweep`."""
     p = argparse.ArgumentParser(description="A grid of main.py experiments as one batched training run.")
     p.add_argument('-d', '--defense', nargs='+', default=['NoDefense'], choices=list(RULES))
     p.add_argument('-z', '--num_std', nargs='+', type=float, default=[1.5])
@@ -633,7 +686,14 @@ def main(argv=None):
                    "reference's ./mnist_data or ./cifar10_data); without it the synthetic stand-in is trained")
     p.add_argument('--cifar10-backdoor', action='store_true', help="train CIFAR10 backdoor experiments (-s CIFAR10 "
                    "-b pattern|1|2|3) in the CIFAR10 trainer kernel; without it they are skipped")
-    a = p.parse_args(argv)
+    p.add_argument('--trace', action='store_true', help="record every epoch's attack figures (aggregate and malicious "
+                   "row deviation from the honest mean, Krum's pick, Bulyan's malicious share) into a _trace.csv per "
+                   "experiment and four more summary columns")
+    return p
+
+
+def main(argv=None):
+    a = parser().parse_args(argv)
     train_size = 20000 if a.data_dir is None else len(harness.real_sizes(a.dataset, a.data_dir)[0][0])
     lrs, cs = list(dict.fromkeys(a.learning_rate)), list(dict.fromkeys(a.batch_size))
     hyper = dict(learning_rates=lrs, batch_sizes=cs) if len(lrs) > 1 or len(cs) > 1 else {}   # 8-tuple cells
@@ -647,7 +707,7 @@ def main(argv=None):
         return []
     res = run(kept, a.epochs, lrs[0], batch_size=cs[0], out_dir=a.out_dir, capture=not a.no_capture,
               fading_rate=FADING_RATE[a.dataset], dataset=a.dataset, data_dir=a.data_dir,
-              cifar10_backdoor=a.cifar10_backdoor)
+              cifar10_backdoor=a.cifar10_backdoor, trace=a.trace)
     for r in res:
         e = r['experiment']
         if r['error'] is None:

@@ -519,6 +519,33 @@ int afl_attack_metrics_batched_dev(const void* G, int batch, int64_t batch_strid
                                    float* honest_out, int* krum_hit, int* mal_count, int* sel_count, void* workspace,
                                    size_t workspace_bytes, int* status, void* stream);
 
+/* afl_attack_trace_dev — one round's attack figures of an fp32 batch, written into row *slot of caller-held tables, so
+ * that a captured round replayed with an advancing slot (a training sweep's epoch counter) records every round.  The
+ * device-parameter arguments (G .. ld, rows, corrupted_counts, workspace, status) are afl_attack_metrics_batched_dev's,
+ * and the per-problem table and its status flags are that call's.  agg (fp32 [batch][d], required): the aggregate the
+ * round applied; Krum's is the gathered winning row, so index -1 is measured as the row applied.  idx (int32 [batch],
+ * may be NULL): Krum's index.  sel (int32 [batch][sel_ld], may be NULL): Bulyan's selection.  slot: a DEVICE int32.
+ * Each output (may be NULL) is a table of n_slots rows at pitch table_ld >= batch; problem b writes entry
+ * [*slot][b]:
+ *   agg_dev   (fp32)  ||agg_b - h_b|| / ||h_b||, h_b the mean of the honest rows f_b .. rows_b - 1: the dev_out
+ *                     afl_attack_metrics_batched_dev(agg = agg) gives, bit for bit;
+ *   mal_dev   (fp32)  ||G[b, 0] - h_b|| / ||h_b|| when f_b > 0 (that call's dev_out with idx = 0, bit for bit), NaN
+ *                     when f_b = 0;
+ *   idx_out   (int32) idx[b] as given, -1 included (needs idx);
+ *   mal_count, sel_count (int32)  that call's counts over row b of sel (need sel).
+ * A slot outside [0, n_slots) writes nothing.  One column pass over the honest rows, agg and row 0, then one CTA per
+ * problem; no host copy, synchronisation or allocation after the host checks, so the call can be captured.  Host
+ * checks: NULL G, agg, slot, corrupted_counts or status, n_slots < 1, table_ld < batch, sel_ld < 1 with sel, a count
+ * without sel, idx_out without idx and a short batch_stride -> AFL_ERR_BAD_ARG; a short or misaligned workspace ->
+ * AFL_ERR_WORKSPACE.  Workspace: afl_attack_trace_workspace_bytes(batch, d) bytes, 256-byte aligned (0 on bad
+ * arguments). */
+size_t afl_attack_trace_workspace_bytes(int batch, int64_t d);
+int afl_attack_trace_dev(const float* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, const int* rows,
+                         const int* corrupted_counts, const float* agg, const int* idx, const int* sel, int sel_ld,
+                         const int* slot, int n_slots, int64_t table_ld, float* agg_dev, float* mal_dev, int* idx_out,
+                         int* mal_count, int* sel_count, void* workspace, size_t workspace_bytes, int* status,
+                         void* stream);
+
 /* ---- device-parameter backdoor crafting: afl_backdoor_start_batched / _finish_batched with f (int32), z and lr
  * (float64) as DEVICE arrays of `batch` values and a status array, as the other _dev calls take them.  The table is
  * built on the device, the host calls' row field for field, so on the same values each result equals the host call's

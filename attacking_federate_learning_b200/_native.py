@@ -107,6 +107,8 @@ SIGNATURES = {
     "afl_backdoor_finish_batched_dev": (_i, [_i, _i, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
                                              _i64, _vp, _sz, _vp, _vp]),
     "afl_mnist_backdoor_train": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _d, _i, _i, _vp]),
+    "afl_mnist_backdoor_train_each": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i,
+                                           _vp]),
     "afl_mnist_backdoor_test": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "afl_cifar10_client_grads": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i64, _i64, _vp]),
     "afl_cifar10_client_grads_sets": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _i64,
@@ -120,6 +122,8 @@ SIGNATURES = {
     "afl_cifar10_backdoor_train_workspace_bytes": (_sz, [_i]),
     "afl_cifar10_backdoor_train": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _d, _i, _i, _vp,
                                         _sz, _vp]),
+    "afl_cifar10_backdoor_train_each": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                             _i, _vp, _sz, _vp]),
     "afl_cifar10_backdoor_test_workspace_bytes": (_sz, [_i, _i, _i]),
     "afl_cifar10_backdoor_test": (_i, [_vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }

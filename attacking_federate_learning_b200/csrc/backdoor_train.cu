@@ -60,17 +60,26 @@ __device__ int test_set(const float* __restrict__ xs, const int64_t* __restrict_
   return correct;
 }
 
+// kEach: the _each call, which reads problem b's alpha and epochs from alpha_each and epochs_each and checks them here.
+// The scalar call's instance takes the host's checked values from the parameter bank and reads no array: on a batch
+// that shares one (alpha, epochs) it runs faster than the kEach instance (DESIGN 2.14).
+template <bool kEach>
 __global__ void __launch_bounds__(kBdThreads, 1)
 backdoor_train_kernel(const float* __restrict__ initial, float* out, const float* __restrict__ x,
                       const int64_t* __restrict__ y, int n_sets, int max_len, const int* __restrict__ set_len,
                       const int* __restrict__ data_index, const int* __restrict__ fs, const double* __restrict__ zs,
-                      int* status, float alpha, int epochs, int m) {
+                      int* status, float alpha, int epochs, int m, const float* __restrict__ alpha_each,
+                      const int* __restrict__ epochs_each) {
   const int b = blockIdx.x, t = threadIdx.x;
   if (fs[b] <= 0 || zs[b] == 0.0 || status[b] != AFL_OK) return;       // batched.backdoor_rows' attacking problems
   const int set = data_index[b];
   const int len = set >= 0 && set < n_sets ? set_len[set] : 0;
+  if constexpr (kEach) {
+    alpha = alpha_each[b];
+    epochs = epochs_each[b];
+  }
   __syncthreads();                                                      // every thread has read status[b]
-  if (len < 1 || len > max_len) {
+  if (len < 1 || len > max_len || (kEach && (alpha != alpha || epochs < 0))) {
     if (t == 0) status[b] = AFL_ERR_BAD_ARG;
     return;
   }
@@ -185,7 +194,7 @@ backdoor_test_kernel(const float* __restrict__ weights, int batch, const float* 
   }
 }
 
-static int smem_done_train[kMaxDevices];
+static int smem_done_train[2][kMaxDevices];                             // [kEach]
 static int smem_done_test[kMaxDevices];
 
 }  // namespace mnist
@@ -193,12 +202,12 @@ static int smem_done_test[kMaxDevices];
 
 using namespace afl;
 
-extern "C" {
-
-int afl_mnist_backdoor_train(const float* initial, float* out, int batch, int64_t d, const float* x, const int64_t* y,
-                             int n_sets, int max_len, const int* set_len, const int* data_index, const int* f,
-                             const double* z, int* status, double alpha, int mal_epochs, int m, void* stream) {
-  const char* who = "afl_mnist_backdoor_train";
+// afl_mnist_backdoor_train and its _each form.  The scalar call passes alpha_each = epochs_each = nullptr and has
+// alpha and mal_epochs checked here; the _each call's values are checked by the kernel, problem by problem.
+static int mnist_backdoor_train(const char* who, const float* initial, float* out, int batch, int64_t d, const float* x,
+                                const int64_t* y, int n_sets, int max_len, const int* set_len, const int* data_index,
+                                const int* f, const double* z, int* status, double alpha, int mal_epochs,
+                                const float* alpha_each, const int* epochs_each, int m, void* stream) {
   if (!initial || !out || !x || !y || !set_len || !data_index || !f || !z || !status) {
     set_error("%s: a pointer argument is NULL", who);
     return AFL_ERR_BAD_ARG;
@@ -206,19 +215,40 @@ int afl_mnist_backdoor_train(const float* initial, float* out, int batch, int64_
   if (int rc = train::check_common(who, "MnistNet", mnist::kD, mnist::kBdRows, "max_len", batch, d, n_sets,
                                    max_len, m))
     return rc;
-  if (mal_epochs < 0 || alpha != alpha) {
+  if (!alpha_each && (mal_epochs < 0 || alpha != alpha)) {
     set_error("%s: mal_epochs must be >= 0 and alpha a number (got %d, %g)", who, mal_epochs, alpha);
     return AFL_ERR_BAD_ARG;
   }
   const size_t span = static_cast<size_t>(batch) * mnist::kD * sizeof(float);
   if (train::overlap(initial, span, out, span)) { set_error("%s: out overlaps initial", who); return AFL_ERR_BAD_ARG; }
-  AFL_CUDA(ensure_dyn_smem(mnist::backdoor_train_kernel, static_cast<int>(mnist::BdGeo::kSmemBytes),
-                           mnist::smem_done_train));
+  const bool each = alpha_each != nullptr;
+  auto kernel = each ? mnist::backdoor_train_kernel<true> : mnist::backdoor_train_kernel<false>;
+  AFL_CUDA(ensure_dyn_smem(kernel, static_cast<int>(mnist::BdGeo::kSmemBytes), mnist::smem_done_train[each]));
   ProfScope ps("backdoor_train", static_cast<cudaStream_t>(stream));
-  mnist::backdoor_train_kernel<<<batch, mnist::kBdThreads, mnist::BdGeo::kSmemBytes, static_cast<cudaStream_t>(stream)>>>(
-      initial, out, x, y, n_sets, max_len, set_len, data_index, f, z, status, static_cast<float>(alpha), mal_epochs, m);
+  kernel<<<batch, mnist::kBdThreads, mnist::BdGeo::kSmemBytes, static_cast<cudaStream_t>(stream)>>>(
+      initial, out, x, y, n_sets, max_len, set_len, data_index, f, z, status, static_cast<float>(alpha), mal_epochs, m,
+      alpha_each, epochs_each);
   AFL_LAUNCH_CHECK("backdoor_train_kernel");
   return AFL_OK;
+}
+
+extern "C" {
+
+int afl_mnist_backdoor_train(const float* initial, float* out, int batch, int64_t d, const float* x, const int64_t* y,
+                             int n_sets, int max_len, const int* set_len, const int* data_index, const int* f,
+                             const double* z, int* status, double alpha, int mal_epochs, int m, void* stream) {
+  return mnist_backdoor_train("afl_mnist_backdoor_train", initial, out, batch, d, x, y, n_sets, max_len, set_len,
+                              data_index, f, z, status, alpha, mal_epochs, nullptr, nullptr, m, stream);
+}
+
+int afl_mnist_backdoor_train_each(const float* initial, float* out, int batch, int64_t d, const float* x,
+                                  const int64_t* y, int n_sets, int max_len, const int* set_len, const int* data_index,
+                                  const int* f, const double* z, int* status, const float* alpha,
+                                  const int* mal_epochs, int m, void* stream) {
+  const char* who = "afl_mnist_backdoor_train_each";
+  if (!alpha || !mal_epochs) { set_error("%s: a pointer argument is NULL", who); return AFL_ERR_BAD_ARG; }
+  return mnist_backdoor_train(who, initial, out, batch, d, x, y, n_sets, max_len, set_len, data_index, f, z, status,
+                              0.0, 0, alpha, mal_epochs, m, stream);
 }
 
 int afl_mnist_backdoor_test(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,

@@ -39,17 +39,24 @@ __device__ __forceinline__ void stage_rows(const int64_t* __restrict__ ys, int l
   __syncthreads();
 }
 
+// kEach: the _each call, as backdoor_train.cu's kernel.
+template <bool kEach>
 __global__ void __launch_bounds__(kThreads, 1)
 backdoor_train_kernel(const float* __restrict__ initial, float* out, const float* __restrict__ x,
                       const int64_t* __restrict__ y, int n_sets, int max_len, const int* __restrict__ set_len,
                       const int* __restrict__ data_index, const int* __restrict__ fs, const double* __restrict__ zs,
-                      int* status, float alpha, int epochs, int m, float* __restrict__ grad) {
+                      int* status, float alpha, int epochs, int m, float* __restrict__ grad,
+                      const float* __restrict__ alpha_each, const int* __restrict__ epochs_each) {
   const int b = blockIdx.x, t = threadIdx.x;
   if (fs[b] <= 0 || zs[b] == 0.0 || status[b] != AFL_OK) return;       // batched.backdoor_rows' attacking problems
   const int set = data_index[b];
   const int len = set >= 0 && set < n_sets ? set_len[set] : 0;
+  if constexpr (kEach) {
+    alpha = alpha_each[b];
+    epochs = epochs_each[b];
+  }
   __syncthreads();                                                      // every thread has read status[b]
-  if (len < 1 || len > max_len) {
+  if (len < 1 || len > max_len || (kEach && (alpha != alpha || epochs < 0))) {
     if (t == 0) status[b] = AFL_ERR_BAD_ARG;
     return;
   }
@@ -181,7 +188,7 @@ __global__ void backdoor_test_finish_kernel(int batch, int nb, int n_sets, int m
   correct[int64_t(sl) * batch + b] = c;
 }
 
-static int smem_done_bd_train[kMaxDevices];
+static int smem_done_bd_train[2][kMaxDevices];                          // [kEach]
 static int smem_done_bd_test[kMaxDevices];
 
 }  // namespace cifar
@@ -189,18 +196,12 @@ static int smem_done_bd_test[kMaxDevices];
 
 using namespace afl;
 
-extern "C" {
-
-size_t afl_cifar10_backdoor_train_workspace_bytes(int batch) {
-  if (batch < 1) return 0;
-  return static_cast<size_t>(batch) * cifar::kD * sizeof(float);
-}
-
-int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int64_t d, const float* x,
-                               const int64_t* y, int n_sets, int max_len, const int* set_len, const int* data_index,
-                               const int* f, const double* z, int* status, double alpha, int mal_epochs, int m,
-                               void* workspace, size_t workspace_bytes, void* stream) {
-  const char* who = "afl_cifar10_backdoor_train";
+// afl_cifar10_backdoor_train and its _each form, as mnist_backdoor_train (backdoor_train.cu).
+static int cifar10_backdoor_train(const char* who, const float* initial, float* out, int batch, int64_t d,
+                                  const float* x, const int64_t* y, int n_sets, int max_len, const int* set_len,
+                                  const int* data_index, const int* f, const double* z, int* status, double alpha,
+                                  int mal_epochs, const float* alpha_each, const int* epochs_each, int m,
+                                  void* workspace, size_t workspace_bytes, void* stream) {
   if (!initial || !out || !x || !y || !set_len || !data_index || !f || !z || !status || !workspace) {
     set_error("%s: a pointer argument is NULL", who);
     return AFL_ERR_BAD_ARG;
@@ -208,7 +209,7 @@ int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int6
   if (int rc = train::check_common(who, "Cifar10Net", cifar::kD, cifar::kMaxRows, "max_len", batch, d, n_sets,
                                    max_len, m))
     return rc;
-  if (mal_epochs < 0 || alpha != alpha) {
+  if (!alpha_each && (mal_epochs < 0 || alpha != alpha)) {
     set_error("%s: mal_epochs must be >= 0 and alpha a number (got %d, %g)", who, mal_epochs, alpha);
     return AFL_ERR_BAD_ARG;
   }
@@ -224,14 +225,42 @@ int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int6
     return AFL_ERR_BAD_ARG;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  AFL_CUDA(ensure_dyn_smem(cifar::backdoor_train_kernel, static_cast<int>(cifar::kSmemRows),
-                           cifar::smem_done_bd_train));
+  const bool each = alpha_each != nullptr;
+  auto kernel = each ? cifar::backdoor_train_kernel<true> : cifar::backdoor_train_kernel<false>;
+  AFL_CUDA(ensure_dyn_smem(kernel, static_cast<int>(cifar::kSmemRows), cifar::smem_done_bd_train[each]));
   ProfScope ps("cifar10_backdoor_train", st);
-  cifar::backdoor_train_kernel<<<batch, cifar::kThreads, cifar::kSmemRows, st>>>(
+  kernel<<<batch, cifar::kThreads, cifar::kSmemRows, st>>>(
       initial, out, x, y, n_sets, max_len, set_len, data_index, f, z, status, static_cast<float>(alpha), mal_epochs, m,
-      static_cast<float*>(workspace));
+      static_cast<float*>(workspace), alpha_each, epochs_each);
   AFL_LAUNCH_CHECK("cifar10_backdoor_train_kernel");
   return AFL_OK;
+}
+
+extern "C" {
+
+size_t afl_cifar10_backdoor_train_workspace_bytes(int batch) {
+  if (batch < 1) return 0;
+  return static_cast<size_t>(batch) * cifar::kD * sizeof(float);
+}
+
+int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int64_t d, const float* x,
+                               const int64_t* y, int n_sets, int max_len, const int* set_len, const int* data_index,
+                               const int* f, const double* z, int* status, double alpha, int mal_epochs, int m,
+                               void* workspace, size_t workspace_bytes, void* stream) {
+  return cifar10_backdoor_train("afl_cifar10_backdoor_train", initial, out, batch, d, x, y, n_sets, max_len, set_len,
+                                data_index, f, z, status, alpha, mal_epochs, nullptr, nullptr, m, workspace,
+                                workspace_bytes, stream);
+}
+
+int afl_cifar10_backdoor_train_each(const float* initial, float* out, int batch, int64_t d, const float* x,
+                                    const int64_t* y, int n_sets, int max_len, const int* set_len,
+                                    const int* data_index, const int* f, const double* z, int* status,
+                                    const float* alpha, const int* mal_epochs, int m, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  const char* who = "afl_cifar10_backdoor_train_each";
+  if (!alpha || !mal_epochs) { set_error("%s: a pointer argument is NULL", who); return AFL_ERR_BAD_ARG; }
+  return cifar10_backdoor_train(who, initial, out, batch, d, x, y, n_sets, max_len, set_len, data_index, f, z, status,
+                                0.0, 0, alpha, mal_epochs, m, workspace, workspace_bytes, stream);
 }
 
 size_t afl_cifar10_backdoor_test_workspace_bytes(int batch, int max_len, int m) {

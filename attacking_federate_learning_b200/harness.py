@@ -387,7 +387,8 @@ def attack_figures(G, users_count, corrupted_count, defense, aggregate, figures)
 
 
 def parser():
-    """main.py's command line (the flags that apply here), plus --trace."""
+    """main.py's command line (the flags that apply here), plus --trace, and --alpha and --mal-epochs for the backdoor
+    attack's values, which main.py hard-codes."""
     p = argparse.ArgumentParser()                                         # main.py:104-131 (the flags that apply here)
     p.add_argument('-m', '--mal-prop', default=0.24, type=float)
     p.add_argument('-z', '--num_std', default=1.5, type=float)
@@ -403,12 +404,23 @@ def parser():
                    "(the reference's ./mnist_data or ./cifar10_data); without it a synthetic stand-in is trained")
     p.add_argument('--trace', action='store_true', help="record every epoch's attack figures into a _trace.csv beside "
                    "the accuracy log (runs Krum and Bulyan twice per epoch)")
+    p.add_argument('--alpha', default=4, type=float, help="the backdoor attack's distance-loss weight (main.py's 4; "
+                   "the log name's _alpha_ field)")
+    p.add_argument('--mal-epochs', default=5, type=int, help="the backdoor attacker's training passes per round "
+                   "(main.py's 5)")
     return p
 
 
-if __name__ == '__main__':
-    a = parser().parse_args()
+def cli(argv=None):
+    """`python -m attacking_federate_learning_b200.harness`: main.py's command line into `main`."""
+    a = parser().parse_args(argv)
     bd = False if a.backdoor == 'No' else a.backdoor if a.backdoor == 'pattern' else int(a.backdoor)
-    main(a.mal_prop, a.num_std, a.defense, users_count=a.users_count, epochs=a.epochs, learning_rate=a.learning_rate,
-         batch_size=a.batch_size, output=a.output, backdoor=bd, dataset=a.dataset, data_dir=a.data_dir,
-         fading_rate=2000 if a.dataset == 'CIFAR10' else 10000, trace=a.trace)   # main.py:144-147
+    return main(a.mal_prop, a.num_std, a.defense, users_count=a.users_count, epochs=a.epochs,
+                learning_rate=a.learning_rate, batch_size=a.batch_size, output=a.output, backdoor=bd,
+                dataset=a.dataset, data_dir=a.data_dir,
+                fading_rate=2000 if a.dataset == 'CIFAR10' else 10000,                    # main.py:144-147
+                trace=a.trace, alpha=a.alpha, mal_epochs=a.mal_epochs)
+
+
+if __name__ == '__main__':
+    cli()

@@ -32,7 +32,8 @@ backdoor experiment whose malicious training meets a NaN loss: Exception('...: G
 Outputs per experiment: the accuracy list and the CSV `harness.main` writes (np.savetxt(..., delimiter=',') in
 out_dir/logs, with `_seed_<s>` before `.csv` so that seeds do not overwrite one another), and one summary CSV with the
 parameters, max and final accuracy and status (and, when the run has a backdoor experiment, the backdoor and its max
-and final backdoor accuracy; when it has an 8-tuple, every experiment's learning rate and batch size).  No checkpoint
+and final backdoor accuracy; when it has an 8-tuple, every experiment's learning rate and batch size; when it has a
+10-tuple, every backdoor experiment's α and mal_epochs).  No checkpoint
 is written: main.py's checkpoint path has no experiment key, so the experiments of a batch would overwrite one file.
 
     python -m attacking_federate_learning_b200.sweep -d Krum TrimmedMean -z 0.5 1.5 -m 0.1 0.24 -n 10 --seeds 0 1 -e 30
@@ -61,8 +62,17 @@ batch_sizes=...)`): the 8-tuple experiments carry their own, and experiments of 
 kernels take problem b's minibatch and test batch size from a device array (C ABI `afl_*_client_grads_each` and
 `afl_*_evaluate_each`) and the momentum step its learning rate (`afl_momentum_step_batched`), and the backdoor's lr_t
 starts from its own learning_rate * fading_rate; each problem's bits equal a sweep of its own (lr, c).  The backdoor
-trainer keeps its own batch (200) and lr (0.1); epochs, momentum and fading rate stay per run.  An 8-tuple's CSV
+trainer keeps its own batch (200) and lr (0.1).  An 8-tuple's CSV
 takes its own learning rate and adds `_batch_<c>` before the seed, since main.py's name has no batch size.
+
+The backdoor attack's α and malicious epochs per experiment (--alpha and --mal-epochs with several values,
+`grid(alphas=..., mal_epochs=...)`): a backdoor experiment may be the 10-tuple (..., learning_rate, batch_size, alpha,
+mal_epochs), and experiments of any (α, mal_epochs) train in one launch of the trainer kernel, which takes problem b's
+α and epoch count from device arrays (C ABI `afl_*_backdoor_train_each`); each problem's bits equal a sweep of its own
+(α, mal_epochs).  The trainer's batch (200), lr (0.1) and momentum, and the run's momentum and fading rate, stay per
+run.  A 10-tuple's CSV takes its own α in main.py's `_alpha_` field and adds `_malepochs_<k>` after `_batch_<c>`.
+
+    python -m attacking_federate_learning_b200.sweep -d Krum NoDefense -z 1.0 -b pattern --alpha 0.2 1 4 --mal-epochs 1 5
 
 trace=True (--trace) records why accuracy moves: in every epoch, after each rule, one `DeviceRound.attack_trace`
 call (C ABI `afl_attack_trace_dev`) per (defence, attack) slice writes each experiment's ||aggregate - honest mean|| /
@@ -107,19 +117,24 @@ class Experiment(tuple):
     so it equals, prints and writes as before; a backdoor experiment carries 'pattern', 1, 2 or 3 as a sixth element.
     An experiment with its own learning rate and batch size (main.py's -l and -c) is the 8-tuple (defense, mal_prop,
     num_std, users_count, seed, backdoor, learning_rate, batch_size), backdoor False for a drift experiment; the short
-    forms take the run's and return None for both."""
+    forms take the run's and return None for both.  A backdoor experiment with its own attack α and malicious epochs is
+    the 10-tuple (..., learning_rate, batch_size, alpha, mal_epochs); the shorter forms take the run's and return None
+    for both."""
     __slots__ = ()
     _fields = ('defense', 'mal_prop', 'num_std', 'users_count', 'seed')     # a drift experiment's
-    _hyper = ('backdoor', 'learning_rate', 'batch_size')
+    _hyper = ('backdoor', 'learning_rate', 'batch_size', 'alpha', 'mal_epochs')
 
     def __new__(cls, defense, mal_prop, num_std, users_count, seed, backdoor=False, learning_rate=None,
-                batch_size=None):
+                batch_size=None, alpha=None, mal_epochs=None):
         t = (defense, mal_prop, num_std, users_count, seed)
-        if learning_rate is None and batch_size is None:
+        if (alpha is None) != (mal_epochs is None):
+            raise ValueError("an experiment gives both alpha and mal_epochs, or neither")
+        if learning_rate is None and batch_size is None and alpha is None:
             return tuple.__new__(cls, t if backdoor is False else t + (backdoor,))
         if learning_rate is None or batch_size is None:
             raise ValueError("an experiment gives both learning_rate and batch_size, or neither")
-        return tuple.__new__(cls, t + (backdoor, learning_rate, batch_size))
+        return tuple.__new__(cls, t + (backdoor, learning_rate, batch_size) +
+                             (() if alpha is None else (alpha, mal_epochs)))
 
     def __getnewargs__(self):
         return tuple(self)
@@ -135,11 +150,19 @@ class Experiment(tuple):
 
     @property
     def learning_rate(self):
-        return self[6] if len(self) == 8 else None
+        return self[6] if len(self) >= 8 else None
 
     @property
     def batch_size(self):
-        return self[7] if len(self) == 8 else None
+        return self[7] if len(self) >= 8 else None
+
+    @property
+    def alpha(self):
+        return self[8] if len(self) == 10 else None
+
+    @property
+    def mal_epochs(self):
+        return self[9] if len(self) == 10 else None
 
     @property
     def corrupted_count(self):
@@ -169,13 +192,20 @@ def minibatch(n_train, users_count, user, batch_size, epoch):
 def check(exp, batch_size=83, train_size=20000, dataset='MNIST', cifar10_backdoor=False):
     """Raise what main.py would raise for this experiment at its first `defend` (AssertionError for the reference's
     asserts), or for what the sweep's kernels do not take.  A CIFAR10 backdoor experiment is taken only with
-    cifar10_backdoor=True.  batch_size is the run's, which an 8-tuple's own replaces.  Returns the normalised
+    cifar10_backdoor=True.  batch_size is the run's, which an 8- or 10-tuple's own replaces.  A 10-tuple must be a
+    backdoor experiment with a number for α and mal_epochs >= 0 (else ValueError).  Returns the normalised
     Experiment."""
-    if len(exp) not in (5, 6, 8):
-        raise ValueError(f"{exp}: an experiment has 5, 6 or 8 elements")
+    if len(exp) not in (5, 6, 8, 10):
+        raise ValueError(f"{exp}: an experiment has 5, 6, 8 or 10 elements")
     exp = Experiment(str(exp[0]), float(exp[1]), float(exp[2]), int(exp[3]), int(exp[4]),
                      normalise_backdoor(exp[5]) if len(exp) > 5 else False,
-                     *((float(exp[6]), int(exp[7])) if len(exp) == 8 else ()))
+                     *((float(exp[6]), int(exp[7])) if len(exp) >= 8 else ()),
+                     *((float(exp[8]), int(exp[9])) if len(exp) == 10 else ()))
+    if exp.alpha is not None:
+        if exp.backdoor is False:
+            raise ValueError(f"{exp}: only a backdoor experiment takes its own alpha and mal_epochs")
+        if exp.alpha != exp.alpha or exp.mal_epochs < 0:
+            raise ValueError(f"{exp}: alpha must be a number and mal_epochs >= 0")
     if exp.batch_size is not None:
         batch_size = exp.batch_size
     if harness.check_dataset(dataset) == 'CIFAR10' and exp.backdoor is not False and not cifar10_backdoor:
@@ -202,37 +232,50 @@ def check(exp, batch_size=83, train_size=20000, dataset='MNIST', cifar10_backdoo
 
 
 def grid(defenses, num_stds, mal_props, users_counts, seeds, batch_size=83, train_size=20000, backdoors=(False,),
-         dataset='MNIST', cifar10_backdoor=False, learning_rates=None, batch_sizes=None, learning_rate=0.1):
+         dataset='MNIST', cifar10_backdoor=False, learning_rates=None, batch_sizes=None, learning_rate=0.1, alphas=None,
+         mal_epochs=None, alpha=4, run_mal_epochs=5):
     """The Cartesian grid (defence-major, backdoor-minor) as (kept experiments, [(experiment, rejection), ...]): a cell
     main.py would reject is dropped with the exception `check` raises for it.  A drift cell (backdoor False) has 5
     elements, a backdoor cell 6.  When learning_rates or batch_sizes is given, every cell is an 8-tuple over the product
     with the learning rate and then the batch size as the innermost axes; the one not given is [learning_rate] or
-    [batch_size]."""
+    [batch_size].  When alphas or mal_epochs is given, every backdoor cell is a 10-tuple over the product with α and
+    then mal_epochs innermost (the one not given is [alpha] or [run_mal_epochs], the run's values), its learning rate
+    and batch size as above; drift cells are left as they are."""
     hyper = learning_rates is not None or batch_sizes is not None
-    axes = (defenses, mal_props, num_stds, users_counts, seeds, backdoors)
-    if hyper:
-        axes += ([learning_rate] if learning_rates is None else learning_rates,
-                 [batch_size] if batch_sizes is None else batch_sizes)
+    attack = alphas is not None or mal_epochs is not None
+    lrs = [learning_rate] if learning_rates is None else learning_rates
+    cs = [batch_size] if batch_sizes is None else batch_sizes
+    pairs = list(itertools.product([alpha] if alphas is None else alphas,
+                                   [run_mal_epochs] if mal_epochs is None else mal_epochs))
     kept, dropped = [], []
-    for cell in itertools.product(*axes):
-        if cell[5] is False and not hyper:
-            cell = cell[:5]
-        try:
-            kept.append(check(cell, batch_size, train_size, dataset, cifar10_backdoor))
-        except (AssertionError, KeyError, ValueError, NotImplementedError) as e:
-            dropped.append((cell, e))
+    for base in itertools.product(defenses, mal_props, num_stds, users_counts, seeds, backdoors):
+        if attack and base[5] is not False:
+            cells = [base + (lr, c) + p for lr in lrs for c in cs for p in pairs]
+        elif hyper:
+            cells = [base + (lr, c) for lr in lrs for c in cs]
+        else:
+            cells = [base if base[5] is not False else base[:5]]
+        for cell in cells:
+            try:
+                kept.append(check(cell, batch_size, train_size, dataset, cifar10_backdoor))
+            except (AssertionError, KeyError, ValueError, NotImplementedError) as e:
+                dropped.append((cell, e))
     return kept, dropped
 
 
 def csv_name(exp, learning_rate, alpha=4, dataset='MNIST', data_dir=None):
     """harness.main's log name for this experiment, with `_seed_<s>` before `.csv`.  An 8-tuple's name takes its own
-    learning rate and adds `_batch_<c>` before the seed: main.py's name has no batch size."""
+    learning rate and adds `_batch_<c>` before the seed: main.py's name has no batch size.  A 10-tuple's also takes its
+    own α and adds `_malepochs_<k>` after the batch size, since main.py's name has no epoch count either."""
     if exp.learning_rate is not None:
         learning_rate = exp.learning_rate
+    if exp.alpha is not None:
+        alpha = exp.alpha
     name = harness.csv_name(exp.num_std, exp.defense, exp.backdoor, exp.mal_prop, exp.users_count, alpha, learning_rate,
                             dataset, data_dir)
     batch = '' if exp.batch_size is None else f'_batch_{exp.batch_size}'
-    return name[:-len('.csv')] + f'{batch}_seed_{exp.seed}.csv'
+    mal = '' if exp.mal_epochs is None else f'_malepochs_{exp.mal_epochs}'
+    return name[:-len('.csv')] + f'{batch}{mal}_seed_{exp.seed}.csv'
 
 
 def test_epochs(epochs, test_step):
@@ -272,12 +315,14 @@ def backdoor_sets(specs, sampled=False):
     return xs, ys, torch.tensor([len(x) for x, _ in sets], dtype=torch.int32, device=dev)
 
 
-def summary_header(with_backdoor, with_hyper=False, with_trace=False):
+def summary_header(with_backdoor, with_hyper=False, with_trace=False, with_attack=False):
     """The summary CSV's columns; the backdoor ones only when the run has a backdoor experiment, the learning rate and
-    batch size only when it has an 8-tuple, the trace's (metrics.TRACE_SUMMARY) only when the run traces."""
+    batch size only when it has an 8-tuple, α and mal_epochs only when it has a 10-tuple, the trace's
+    (metrics.TRACE_SUMMARY) only when the run traces."""
     bd = with_backdoor
     return list(Experiment._fields) + (['backdoor'] if bd else []) + \
-        (['learning_rate', 'batch_size'] if with_hyper else []) + ['max_accuracy', 'final_accuracy'] + \
+        (['learning_rate', 'batch_size'] if with_hyper else []) + (['alpha', 'mal_epochs'] if with_attack else []) + \
+        ['max_accuracy', 'final_accuracy'] + \
         (['max_backdoor_accuracy', 'final_backdoor_accuracy'] if bd else []) + \
         (metrics.TRACE_SUMMARY if with_trace else []) + ['status']
 
@@ -287,20 +332,22 @@ def trace_csv_name(name):
     return name[:-len('.csv')] + '_trace.csv'
 
 
-def write_logs(res, logs, names, with_backdoor=False, hyper=None, trace=False):
+def write_logs(res, logs, names, with_backdoor=False, hyper=None, trace=False, attack=None):
     """`run`'s files under `logs` from `results()`-style dicts: each successful experiment's accuracy CSV names[k]
     (np.savetxt, main.py:100) and, with trace, its trace CSV; then the summary CSV.  hyper: None, or [learning_rate,
-    batch_size] per result for the summary.  Sets each dict's `csv` (and with trace `trace_csv`), None when it failed."""
-    with_bd, with_hyper = with_backdoor, hyper is not None
+    batch_size] per result for the summary; attack: None, or [alpha, mal_epochs] per result (empty strings for a drift
+    experiment).  Sets each dict's `csv` (and with trace `trace_csv`), None when it failed."""
+    with_bd, with_hyper, with_attack = with_backdoor, hyper is not None, attack is not None
     with open(os.path.join(logs, SUMMARY), 'w', newline='') as fh:
         w = _csv.writer(fh)
-        w.writerow(summary_header(with_bd, with_hyper, trace))
+        w.writerow(summary_header(with_bd, with_hyper, trace, with_attack))
         for k, r in enumerate(res):
             e = r['experiment']
             r['csv'] = None
             if trace:
                 r['trace_csv'] = None
-            head = list(e[:5]) + ([e.backdoor] if with_bd else []) + (hyper[k] if with_hyper else [])
+            head = list(e[:5]) + ([e.backdoor] if with_bd else []) + (hyper[k] if with_hyper else []) + \
+                (attack[k] if with_attack else [])
             if r['error'] is None:
                 r['csv'] = os.path.join(logs, names[k])
                 np.savetxt(r['csv'], r['accuracies'], delimiter=',')     # main.py:100
@@ -350,8 +397,10 @@ class Sweep:
     Per problem: `batch_sizes` and `learning_rates` (an 8-tuple's own, else the run's batch_size and learning_rate),
     on the device as m (int32: the client minibatches and the test batches), lr (fp32: the momentum step) and
     lr_fading (float64: learning_rate * fading_rate, the backdoor's lr_t numerator), allocated once so that captured
-    graphs keep their pointers.  trace=True: `trace` holds the [epochs, B] tables of DeviceRound.TRACE_TABLES (TRACE_UNSET
-    until an epoch writes them), filled after each rule at row epoch_counter; None otherwise."""
+    graphs keep their pointers.  Per backdoor problem, the same way: `bd_alpha` (fp32) and `bd_mal_epochs` (int32), a
+    10-tuple's own or the run's alpha and mal_epochs, which the trainer kernel reads when they differ.  trace=True:
+    `trace` holds the [epochs, B] tables of DeviceRound.TRACE_TABLES (TRACE_UNSET until an epoch writes them), filled
+    after each rule at row epoch_counter; None otherwise."""
 
     def __init__(self, experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, train_size=None,
                  test_size=None, test_step=5, capture=True, device='cuda', alpha=4, mal_epochs=5, fading_rate=10000,
@@ -478,6 +527,12 @@ class Sweep:
         self.bd_x, self.bd_y, self.bd_len = backdoor_sets(
             [(bd, xtr[seeds.index(s)], ytr[seeds.index(s)], s) for bd, s in keys], sampled=self.data_dir is not None)
         self.bd_index = torch.tensor([keys.index((e.backdoor, e.seed)) for e in bds], **i32)
+        self._bd_alphas = [self.alpha if e.alpha is None else e.alpha for e in bds]
+        self._bd_epochs = [self.mal_epochs if e.mal_epochs is None else e.mal_epochs for e in bds]
+        if any(a != a for a in self._bd_alphas):
+            raise ValueError("sweep: alpha must be a number")
+        self.bd_alpha = torch.tensor(self._bd_alphas, dtype=torch.float32, device=dev)
+        self.bd_mal_epochs = torch.tensor(self._bd_epochs, **i32)
         self._bd_f = torch.zeros(nb, **i32)
         self._bd_z = torch.zeros(nb, dtype=torch.float64, device=dev)
         self._bd_lr = torch.zeros(nb, dtype=torch.float64, device=dev)
@@ -506,21 +561,27 @@ class Sweep:
 
     def backdoor_train(self, k=None):
         """The malicious networks of the backdoor experiments bd0 + k (all of them by default) in one launch
-        (BackdoorTrainer.train), from bd_initial[k] into bd_mal[k]."""
+        (BackdoorTrainer.train), from bd_initial[k] into bd_mal[k], each at its own bd_alpha and bd_mal_epochs.  When
+        the launch's problems share one (alpha, mal_epochs) it is the scalar call: its kernel instance reads no
+        per-problem array and runs faster on such a grid (DESIGN 2.14); both give the same bits."""
         k = slice(0, self.n_backdoor) if k is None else k
+        alphas, epochs = set(self._bd_alphas[k]), set(self._bd_epochs[k])
+        each = len(alphas) > 1 or len(epochs) > 1
+        attack = (self.bd_alpha[k].data_ptr(), self.bd_mal_epochs[k].data_ptr()) if each else \
+            (float(alphas.pop()), epochs.pop())
         args = (self.bd_initial[k].data_ptr(), self.bd_mal[k].data_ptr(), k.stop - k.start, self.D,
                 self.bd_x.data_ptr(), self.bd_y.data_ptr(), self.bd_x.shape[0], self.bd_x.shape[1],
                 self.bd_len.data_ptr(), self.bd_index[k].data_ptr(), self._bd_f[k].data_ptr(), self._bd_z[k].data_ptr(),
-                self._bd_status[k].data_ptr(), float(self.alpha), self.mal_epochs, BACKDOOR_BATCH)
+                self._bd_status[k].data_ptr(), *attack, BACKDOOR_BATCH)
         stream = torch.cuda.current_stream(self.device).cuda_stream
+        L, suffix = nat.lib(), '_each' if each else ''
         with torch.cuda.device(self.device):
             if self.dataset == 'CIFAR10':                                 # problem b's gradient row: D floats at b D
-                L = nat.lib()
-                nat.check(L.afl_cifar10_backdoor_train(
+                nat.check(getattr(L, 'afl_cifar10_backdoor_train' + suffix)(
                     *args, self._bd_train_ws.data_ptr() + k.start * self.D * 4,
                     L.afl_cifar10_backdoor_train_workspace_bytes(k.stop - k.start), stream))
             else:
-                nat.check(nat.lib().afl_mnist_backdoor_train(*args, stream))
+                nat.check(getattr(L, 'afl_mnist_backdoor_train' + suffix)(*args, stream))
 
     def _defend(self, r, sl, rnd):
         agg = {DefenseTypes.Krum: rnd.krum, DefenseTypes.Bulyan: rnd.bulyan,
@@ -646,9 +707,10 @@ def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, tra
     """Train every experiment for `epochs` epochs as one batch; write each one's accuracy CSV and the summary CSV under
     out_dir/logs.  Returns `Sweep.results()` with `csv` (None for a failed experiment) added to each dict.  Raises
     before any GPU work for an experiment main.py would reject (see `check`).  alpha, mal_epochs and fading_rate are
-    harness.main's (the backdoor experiments' malicious training and client learning rate), and so is dataset ('MNIST'
-    or 'CIFAR10', main.py -s).  data_dir: the real dataset's files (see the module docstring); train_size and test_size
-    are then None or the files' row counts, and None means 20,000 and 4,000 synthetic rows otherwise.
+    harness.main's (the backdoor experiments' malicious training and client learning rate; a 10-tuple's own alpha and
+    mal_epochs replace the first two), and so is dataset ('MNIST' or 'CIFAR10', main.py -s).  data_dir: the real
+    dataset's files (see the module docstring); train_size and test_size are then None or the files' row counts, and
+    None means 20,000 and 4,000 synthetic rows otherwise.
     cifar10_backdoor=True takes CIFAR10 backdoor experiments (main.py -s CIFAR10 -b ...).  trace=True records every
     epoch's attack figures (see the module docstring) and adds `trace_csv` to each dict."""
     sw = Sweep(experiments, epochs, learning_rate, momentum, batch_size, train_size, test_size, test_step, capture,
@@ -661,9 +723,13 @@ def run(experiments, epochs, learning_rate=0.1, momentum=0.9, batch_size=83, tra
     os.makedirs(logs, exist_ok=True)
     with_hyper = any(e.batch_size is not None for e in sw.experiments)
     hyper = {pos: [sw.learning_rates[i], sw.batch_sizes[i]] for i, pos in enumerate(sw.order)}
+    attack = None
+    if any(e.alpha is not None for e in sw.experiments):                 # a 10-tuple: α and mal_epochs columns
+        attack = [['', ''] if e.backdoor is False else [alpha, mal_epochs] if e.alpha is None else
+                  [e.alpha, e.mal_epochs] for e in (r['experiment'] for r in res)]
     names = [csv_name(r['experiment'], learning_rate, alpha, sw.dataset, sw.data_dir) for r in res]
     write_logs(res, logs, names, sw.n_backdoor > 0, [hyper[k] for k in range(len(res))] if with_hyper else None,
-               trace)
+               trace, attack)
     return res
 
 
@@ -680,6 +746,10 @@ def parser():
     p.add_argument('-e', '--epochs', type=int, default=300)
     p.add_argument('-c', '--batch_size', nargs='+', type=int, default=[83])
     p.add_argument('-l', '--learning_rate', nargs='+', type=float, default=[0.1])
+    p.add_argument('--alpha', nargs='+', type=float, default=[4], help="the backdoor attack's distance-loss weight "
+                   "(main.py's alpha = 4); several values make one backdoor experiment per value")
+    p.add_argument('--mal-epochs', nargs='+', type=int, default=[5], help="the backdoor attacker's training passes per "
+                   "round (main.py's 5); several values make one backdoor experiment per value")
     p.add_argument('--out-dir', default='.')
     p.add_argument('--no-capture', action='store_true')
     p.add_argument('--data-dir', default=None, help="the directory holding torchvision's MNIST or CIFAR10 files (the "
@@ -697,6 +767,9 @@ def main(argv=None):
     train_size = 20000 if a.data_dir is None else len(harness.real_sizes(a.dataset, a.data_dir)[0][0])
     lrs, cs = list(dict.fromkeys(a.learning_rate)), list(dict.fromkeys(a.batch_size))
     hyper = dict(learning_rates=lrs, batch_sizes=cs) if len(lrs) > 1 or len(cs) > 1 else {}   # 8-tuple cells
+    alphas, mal_epochs = list(dict.fromkeys(a.alpha)), list(dict.fromkeys(a.mal_epochs))
+    if len(alphas) > 1 or len(mal_epochs) > 1:                                                 # 10-tuple backdoor cells
+        hyper.update(alphas=alphas, mal_epochs=mal_epochs, learning_rate=lrs[0])
     kept, dropped = grid(a.defense, a.num_std, a.mal_prop, a.users_count, a.seeds, cs[0], train_size,
                          backdoors=[normalise_backdoor(b) for b in dict.fromkeys(a.backdoor)], dataset=a.dataset,
                          cifar10_backdoor=a.cifar10_backdoor, **hyper)
@@ -706,7 +779,8 @@ def main(argv=None):
         print("no experiment left to run")
         return []
     res = run(kept, a.epochs, lrs[0], batch_size=cs[0], out_dir=a.out_dir, capture=not a.no_capture,
-              fading_rate=FADING_RATE[a.dataset], dataset=a.dataset, data_dir=a.data_dir,
+              alpha=alphas[0], mal_epochs=mal_epochs[0], fading_rate=FADING_RATE[a.dataset], dataset=a.dataset,
+              data_dir=a.data_dir,
               cifar10_backdoor=a.cifar10_backdoor, trace=a.trace)
     for r in res:
         e = r['experiment']

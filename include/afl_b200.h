@@ -649,6 +649,15 @@ int afl_mnist_evaluate_each(const float* weights, int batch, int64_t d, const fl
  * index outside [0, n_sets) or a set length outside [1, max_len] sets AFL_ERR_BAD_ARG.  Any other problem's out[b] is
  * neither read nor written.  mal_epochs < 0 or a NaN alpha -> AFL_ERR_BAD_ARG.
  *
+ * afl_mnist_backdoor_train_each — afl_mnist_backdoor_train with alpha and mal_epochs per problem: alpha is device fp32
+ * [batch] and mal_epochs device int32 [batch] (read when the kernel runs), and problem b trains at alpha[b] and
+ * mal_epochs[b], so its out[b] and status[b] equal afl_mnist_backdoor_train(..., alpha = alpha[b], mal_epochs =
+ * mal_epochs[b], ...) bit for bit, whatever the other problems' values.  The MSE term, and AFL_ERR_NAN_DIST_LOSS, apply
+ * only to problems with alpha[b] > 0; mal_epochs[b] = 0 returns initial[b] after the BEFORE test.  An attacking problem
+ * whose alpha[b] is NaN or whose mal_epochs[b] < 0 gets status[b] = AFL_ERR_BAD_ARG, and its out[b] is neither read
+ * nor written.  The host checks are the scalar call's without the value checks, and a NULL alpha or mal_epochs ->
+ * AFL_ERR_BAD_ARG.
+ *
  * afl_mnist_backdoor_test — BackdoorTrainer.test (backdoor.py:67-102; main.py:91-95's 'POST') at weights[b] (device
  * fp32 [batch][d]) for every problem: loss_sum[slot][b] = the float64 sum of the batches' fp32 mean NLL (divide by the
  * set length for the reported loss) and correct[slot][b] = the rows whose argmax (torch's: the first NaN, else the
@@ -658,6 +667,10 @@ int afl_mnist_evaluate_each(const float* weights, int batch, int64_t d, const fl
 int afl_mnist_backdoor_train(const float* initial, float* out, int batch, int64_t d, const float* x, const int64_t* y,
                              int n_sets, int max_len, const int* set_len, const int* data_index, const int* f,
                              const double* z, int* status, double alpha, int mal_epochs, int m, void* stream);
+int afl_mnist_backdoor_train_each(const float* initial, float* out, int batch, int64_t d, const float* x,
+                                  const int64_t* y, int n_sets, int max_len, const int* set_len, const int* data_index,
+                                  const int* f, const double* z, int* status, const float* alpha,
+                                  const int* mal_epochs, int m, void* stream);
 int afl_mnist_backdoor_test(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                             int max_len, const int* set_len, const int* data_index, int m, const int* slot_index,
                             int n_slots, double* loss_sum, int* correct, void* stream);
@@ -723,6 +736,11 @@ int afl_cifar10_evaluate_each(const float* weights, int batch, int64_t d, const 
  * afl_cifar10_backdoor_train_workspace_bytes(batch) bytes (4-byte aligned; problem b's step gradient lives in floats
  * [b d, b d + d)), overlapping neither initial nor out.
  *
+ * afl_cifar10_backdoor_train_each — afl_mnist_backdoor_train_each's per-problem alpha (device fp32 [batch]) and
+ * mal_epochs (device int32 [batch]) with afl_cifar10_backdoor_train's workspace: each problem equals the scalar call at
+ * its own values bit for bit, and a NaN alpha[b] or a negative mal_epochs[b] sets status[b] = AFL_ERR_BAD_ARG before
+ * out[b] is touched.  A NULL alpha or mal_epochs -> AFL_ERR_BAD_ARG.
+ *
  * afl_cifar10_backdoor_test — afl_mnist_backdoor_test's contract, as one CTA per (test batch, problem) and a finish
  * kernel that sums the batches in order.  workspace: afl_cifar10_backdoor_test_workspace_bytes(batch, max_len, m)
  * bytes, 256-byte aligned; ceil(max_len / m) > 65535 -> AFL_ERR_UNSUPPORTED. */
@@ -731,6 +749,11 @@ int afl_cifar10_backdoor_train(const float* initial, float* out, int batch, int6
                                int n_sets, int max_len, const int* set_len, const int* data_index, const int* f,
                                const double* z, int* status, double alpha, int mal_epochs, int m, void* workspace,
                                size_t workspace_bytes, void* stream);
+int afl_cifar10_backdoor_train_each(const float* initial, float* out, int batch, int64_t d, const float* x,
+                                    const int64_t* y, int n_sets, int max_len, const int* set_len,
+                                    const int* data_index, const int* f, const double* z, int* status,
+                                    const float* alpha, const int* mal_epochs, int m, void* workspace,
+                                    size_t workspace_bytes, void* stream);
 size_t afl_cifar10_backdoor_test_workspace_bytes(int batch, int max_len, int m);
 int afl_cifar10_backdoor_test(const float* weights, int batch, int64_t d, const float* x, const int64_t* y, int n_sets,
                               int max_len, const int* set_len, const int* data_index, int m, const int* slot_index,

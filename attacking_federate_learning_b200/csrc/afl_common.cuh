@@ -139,7 +139,7 @@ __host__ __device__ inline TmShape shape(int n_rows, int corrupted_count) {
 
 // The slot class of n_rows <= 1024 participating rows: c = 0 .. kSlotClasses - 1 for the kernel with S = 4 (c + 1)
 // slots per lane, the instance that trimmed_mean_batched launches for them.  The host grouping (capi.cu,
-// upload_class_table) and the device grouping (class_perm_kernel) share this definition.
+// upload_table) and the device grouping (class_perm_kernel) share this definition.
 __host__ __device__ inline int slot_class(int n_rows) { return n_rows <= 128 ? 0 : (n_rows - 1) / 128; }
 }  // namespace tmean
 

@@ -595,9 +595,8 @@ static int alie_host(const float* const* rows, int f, int64_t d, double z, float
 //   Krum   [d2: batch x n x n float64][gram workspace][selection workspace]
 //   Bulyan [d2: batch x n x n float64][dist: batch x n x n fp32][gram workspace][selection workspace]
 // The per-problem calls (*_each) take corrupted_count (and ALIE's z) per problem.  Their host arrays become one
-// ProblemParams row per problem, built here with the single call's own host code (krum_take, tmean::shape) and copied
-// to the start of the workspace; the scalar call's layout follows it.  The scalar calls pass no table and run as they
-// always have.
+// ProblemParams row per problem (problem_row, the builder problem_table_kernel runs on the device) copied to the start
+// of the workspace; the scalar call's layout follows it.  The scalar calls pass no table and run as they always have.
 // The large calls (afl_defend_batched_large) take up to 1024 clients per problem: every Gram form is batched for any
 // tile count, and the register-resident trimmed-mean kernels end at 1024 rows.
 // ------------------------------------------------------------------------------------------------
@@ -605,7 +604,8 @@ constexpr int kBatchMaxClients = 128;            // one Gram tile
 constexpr int kBatchLargeMaxClients = 1024;      // the largest register-resident trimmed-mean kernel (S = 32)
 constexpr int kBatchMax = 65535;                 // grid y / z limit
 
-enum BatchedRule { B_BAD, B_MEAN, B_KRUM, B_TM, B_BULYAN };
+// The rule of a batched call: the defences, then the attacks and the metrics, whose tables the same builders make.
+enum BatchedRule { B_BAD, B_MEAN, B_KRUM, B_TM, B_BULYAN, T_ALIE, T_METRICS, T_BACKDOOR };
 static BatchedRule batched_rule(const char* rule) {
   if (!rule) return B_BAD;
   if (!strcmp(rule, "NoDefense")) return B_MEAN;
@@ -613,6 +613,47 @@ static BatchedRule batched_rule(const char* rule) {
   if (!strcmp(rule, "TrimmedMean")) return B_TM;
   if (!strcmp(rule, "Bulyan")) return B_BULYAN;
   return B_BAD;
+}
+
+// The defence `rule` names; with `attacks` (afl_batched_table_dev) also "ALIE" and "AttackMetrics".
+static int parse_rule(const char* who, const char* rule, bool attacks, BatchedRule* r) {
+  *r = batched_rule(rule);
+  if (attacks && rule && !strcmp(rule, "ALIE")) *r = T_ALIE;
+  if (attacks && rule && !strcmp(rule, "AttackMetrics")) *r = T_METRICS;
+  if (*r != B_BAD) return AFL_OK;
+  set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)");
+  return AFL_ERR_BAD_ARG;
+}
+
+// Problem b's table row, built by the host calls (upload_table) and by problem_table_kernel alike:
+//   defences: m rows (rows_b, or n), users count uc and f; Bulyan's table for its second stage (`second`) holds the
+//     trimmed mean of the theta_b selected rows with 2 f_b;
+//   ALIE and the backdoor: f, (float)z and write, and the backdoor's (float)lr (ALIE's is 0, so the union's bits are);
+//   the metrics: f and tm.n_rows = m, which a call without rows passes as 0 (its kernels read no row count).
+__host__ __device__ inline ProblemParams problem_row(int rule, int m, int uc, int f, double z, double lr, bool second) {
+  ProblemParams q{};
+  q.f = f;
+  if (rule == T_METRICS) {
+    q.tm.n_rows = m;
+  } else if (rule == T_ALIE || rule == T_BACKDOOR) {
+    q.z = static_cast<float>(z);
+    q.lr = static_cast<float>(lr);
+    q.write = f > 0 && z != 0.0;                         // malicious.py:20-21: z == 0 computes the statistics only
+  } else {
+    q.take = select::krum_take(m, uc, f);
+    q.theta = uc - 2 * f;
+    q.tm = rule == B_BULYAN && second ? tmean::shape(q.theta, 2 * f) : tmean::shape(m, f);
+  }
+  return q;
+}
+
+// The reference's asserts (defences.py:24-25, 56) and Bulyan's users_count == rows for one problem of m rows, users
+// count uc and corrupted count f: the host calls' check_problems and the device's problem_code.
+__host__ __device__ inline int problem_assert(int rule, int m, int uc, int f) {
+  if (rule == B_KRUM && uc < 2 * static_cast<int64_t>(f) + 1) return AFL_ERR_PRECONDITION;
+  if (rule == B_BULYAN && uc < 4 * static_cast<int64_t>(f) + 3) return AFL_ERR_PRECONDITION;
+  if (rule == B_BULYAN && uc != m) return AFL_ERR_UNSUPPORTED;
+  return AFL_OK;
 }
 
 // Shape checks shared by the batched calls, before any CUDA call.  max_rows: one Gram tile for the defences and ALIE.
@@ -634,6 +675,12 @@ static int check_batch(const char* who, const void* G, int batch, int64_t batch_
   return AFL_OK;
 }
 
+static int check_workspace(const char* who, const void* ws, size_t ws_bytes, size_t need) {
+  if (ws && ws_bytes >= need && reinterpret_cast<uintptr_t>(ws) % 256 == 0) return AFL_OK;
+  set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
+  return AFL_ERR_WORKSPACE;
+}
+
 // Per-problem counts: non-NULL, each in [0, f_cap]; their range in *fmin, *fmax.
 static int check_counts(const char* who, const int* fs, int batch, int f_cap, int* fmin, int* fmax) {
   if (!fs) { set_error("%s: the per-problem corrupted counts are NULL", who); return AFL_ERR_BAD_ARG; }
@@ -649,6 +696,74 @@ static int check_counts(const char* who, const int* fs, int batch, int f_cap, in
   return AFL_OK;
 }
 
+// The per-problem checks of the host-array defences and metrics, each phase up to its first failing problem: the
+// arrays are non-NULL (with `ragged`, rows and ucs too), every f_b is in [0, f_cap], every rows_b in [1, n], then the
+// caller's outputs(), then problem_assert.  fs == NULL: the scalar call's f in every problem; rows == NULL: n rows;
+// ucs == NULL: users_count.  Without rows, Bulyan's users_count == n is one condition of the call, checked after every
+// problem's asserts.  The smallest f_b goes to *fmin, Bulyan's largest theta_b to *theta_max.
+template <typename Outputs>
+static int check_problems(const char* who, BatchedRule rule, int batch, int n, int f_cap, bool ragged, const int* rows,
+                          const int* ucs, int users_count, const int* fs, int f, Outputs outputs, int* fmin,
+                          int* theta_max) {
+  if (ragged && (!rows || !ucs)) {
+    set_error("%s: the per-problem row counts or users counts are NULL", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  int fmax = f, rc = AFL_OK;
+  *fmin = f;
+  if ((fs || ragged) && (rc = check_counts(who, fs, batch, f_cap, fmin, &fmax))) return rc;
+  for (int b = 0; rows && b < batch; ++b)
+    if (rows[b] < 1 || rows[b] > n) {
+      set_error("%s: row count %d of problem %d is outside [1, %d]", who, rows[b], b, n);
+      return AFL_ERR_BAD_ARG;
+    }
+  if ((rc = outputs())) return rc;
+  *theta_max = 0;
+  for (int b = 0; b < batch; ++b) {
+    const int m = rows ? rows[b] : n, uc = ucs ? ucs[b] : users_count, fb = fs ? fs[b] : f;
+    const int code = problem_assert(rule, m, uc, fb);
+    if (code == AFL_ERR_PRECONDITION) {
+      const char* what = rule == B_KRUM ? "krum: users_count >= 2*corrupted_count + 1"
+                                        : "bulyan: users_count >= 4*corrupted_count + 3";
+      if (fs) set_error("%s violated (%d, %d) in problem %d", what, uc, fb, b);
+      else set_error("%s violated (%d, %d)", what, uc, fb);
+      return code;
+    }
+    if (code == AFL_ERR_UNSUPPORTED && rows) {
+      set_error("%s: Bulyan's users_count (%d) must equal the number of rows (%d) in problem %d", who, uc, m, b);
+      return code;
+    }
+    if (rule == B_BULYAN && uc - 2 * fb > *theta_max) *theta_max = uc - 2 * fb;
+  }
+  if (rule == B_BULYAN && !rows && users_count != n) {
+    set_error("%s: Bulyan's users_count (%d) must equal the number of rows (%d)", who, users_count, n);
+    return AFL_ERR_UNSUPPORTED;
+  }
+  return AFL_OK;
+}
+
+// The outputs a defence writes: out (all but Krum), idx_out (Krum), sel_out (Bulyan).  The scalar call's negative
+// corrupted_count f is refused with the same message.
+static int check_outputs(const char* who, const char* rule, BatchedRule r, const float* out, const int* idx_out,
+                         const int* sel_out, int f = 0) {
+  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out) || f < 0) {
+    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
+    return AFL_ERR_BAD_ARG;
+  }
+  return AFL_OK;
+}
+
+// Rows 0 .. rows_max - 1 of every problem written at bcast_ld / bcast_batch_stride must not overlap.
+static int check_bcast(const char* who, const void* bcast_rows, int rows_max, int64_t d, int batch,
+                       int64_t bcast_batch_stride, int64_t bcast_ld) {
+  if (bcast_rows && rows_max > 0 &&
+      (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(rows_max - 1) * bcast_ld + d))) {
+    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  return AFL_OK;
+}
+
 static size_t table_bytes(int batch) { return align_up(static_cast<size_t>(batch) * sizeof(ProblemParams), 256); }
 // The table of a batch with more than kBatchMaxClients rows per slot: ProblemParams[batch], then int perm[batch], the
 // problems grouped by trimmed-mean slot class (tmean::trimmed_mean_classes).
@@ -657,47 +772,48 @@ static size_t class_table_bytes(int batch, int n) {
   return align_up(static_cast<size_t>(batch) * (sizeof(ProblemParams) + sizeof(int)), 256);
 }
 
-// The rule's scratch after the table (0: the rule needs none).
-static size_t batched_ws_parts(BatchedRule r, int batch, int n, int64_t d, int dtype, size_t* gram_ws, size_t* tabs) {
-  *gram_ws = 0; *tabs = 0;
-  if (r != B_KRUM && r != B_BULYAN) return 0;
+// The rule's scratch after the table, in this order: d², Bulyan's dist, the Gram workspace, the selection workspace
+// (bytes == 0: the rule needs none).  With `at`, the parts' addresses in a workspace whose scratch starts there.
+struct RuleScratch {
+  size_t bytes = 0, gram_bytes = 0, sel_bytes = 0;
+  double* d2 = nullptr;
+  float* dist = nullptr;
+  void* gram = nullptr;
+  void* sel = nullptr;
+};
+static RuleScratch rule_scratch(BatchedRule r, int batch, int n, int64_t d, int dtype, void* at = nullptr) {
+  RuleScratch s;
+  if (r != B_KRUM && r != B_BULYAN) return s;
   const size_t nn = static_cast<size_t>(batch) * n * n;
-  *gram_ws = align_up(gram::workspace_bytes(n, d, dtype, 0, batch), 256);
-  *tabs = align_up(nn * 8, 256) + (r == B_BULYAN ? align_up(nn * 4, 256) : 0);
-  return *gram_ws + *tabs + select::workspace_bytes(n, batch);
+  const size_t tabs = align_up(nn * 8, 256) + (r == B_BULYAN ? align_up(nn * 4, 256) : 0);
+  s.gram_bytes = align_up(gram::workspace_bytes(n, d, dtype, 0, batch), 256);
+  s.sel_bytes = select::workspace_bytes(n, batch);
+  s.bytes = tabs + s.gram_bytes + s.sel_bytes;
+  if (uint8_t* p = static_cast<uint8_t*>(at)) {
+    s.d2 = reinterpret_cast<double*>(p);
+    s.dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
+    s.gram = p + tabs;
+    s.sel = p + tabs + s.gram_bytes;
+  }
+  return s;
 }
 
-// Workspace check, then the table built by `row(b, ProblemParams&)` copied to the workspace start (pageable source:
-// the copy has taken the values when cudaMemcpyAsync returns).  Returns the device table in *table.
+// The table of rows row(b), b < batch, copied to the workspace start (pageable source: the copy has taken the values
+// when cudaMemcpyAsync returns).  With counts, the same copy appends int perm[batch]: the problems grouped by the
+// trimmed-mean slot class of their tm.n_rows, in problem order within a class, whose sizes go to counts[kSlotClasses]
+// (host).
 template <typename Row>
-static int upload_table(const char* who, int batch, void* ws, size_t ws_bytes, size_t need, cudaStream_t stream,
-                        Row row, const ProblemParams** table) {
-  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
-    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
-    return AFL_ERR_WORKSPACE;
-  }
-  std::vector<ProblemParams> host(static_cast<size_t>(batch));
-  for (int b = 0; b < batch; ++b) row(b, host[b]);
-  AFL_CUDA(cudaMemcpyAsync(ws, host.data(), host.size() * sizeof(ProblemParams), cudaMemcpyHostToDevice, stream));
-  *table = static_cast<const ProblemParams*>(ws);
-  return AFL_OK;
-}
-
-// upload_table followed by the problems grouped by the trimmed-mean slot class of their tm.n_rows, in one copy: the
-// device permutation in *perm, the class sizes in counts[kSlotClasses] (host).
-template <typename Row>
-static int upload_class_table(const char* who, int batch, void* ws, size_t ws_bytes, size_t need, cudaStream_t stream,
-                              Row row, const ProblemParams** table, const int** perm, int* counts) {
-  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
-    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
-    return AFL_ERR_WORKSPACE;
-  }
+static int upload_table(int batch, void* ws, cudaStream_t stream, Row row, int* counts = nullptr) {
   const size_t nb = static_cast<size_t>(batch);
   std::vector<ProblemParams> host(nb);
+  for (int b = 0; b < batch; ++b) host[b] = row(b);
+  if (!counts) {
+    AFL_CUDA(cudaMemcpyAsync(ws, host.data(), nb * sizeof(ProblemParams), cudaMemcpyHostToDevice, stream));
+    return AFL_OK;
+  }
   std::vector<int> cls(nb), order(nb);
   for (int c = 0; c < kSlotClasses; ++c) counts[c] = 0;
   for (int b = 0; b < batch; ++b) {
-    row(b, host[b]);
     cls[b] = tmean::slot_class(host[b].tm.n_rows);
     ++counts[cls[b]];
   }
@@ -708,173 +824,61 @@ static int upload_class_table(const char* who, int batch, void* ws, size_t ws_by
   memcpy(bytes.data(), host.data(), nb * sizeof(ProblemParams));
   memcpy(bytes.data() + nb * sizeof(ProblemParams), order.data(), nb * sizeof(int));
   AFL_CUDA(cudaMemcpyAsync(ws, bytes.data(), bytes.size(), cudaMemcpyHostToDevice, stream));
-  *table = static_cast<const ProblemParams*>(ws);
-  *perm = reinterpret_cast<const int*>(static_cast<const uint8_t*>(ws) + nb * sizeof(ProblemParams));
   return AFL_OK;
 }
 
-// fs == NULL: every problem has corrupted_count f (afl_defend_batched).  Otherwise problem b has fs[b]
-// (afl_defend_batched_each): f is unused, the preconditions hold per problem, and the workspace starts with the table.
-static int defend_batched(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
-                          int dtype, int users_count, int f, const int* fs, float* out, int* idx_out, int* sel_out,
-                          void* ws, size_t ws_bytes, cudaStream_t stream) {
-  const char* who = fs ? "afl_defend_batched_each" : "afl_defend_batched";
-  const BatchedRule r = batched_rule(rule);
-  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
-  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
+// The host-array defences: afl_defend_batched (fs == NULL: the scalar f), _each (rows == NULL: n rows and users_count in
+// every problem), _rows and _large (`ragged`: rows_b and users_count_b per problem; the large call passes rows = n when
+// it gets none).  Every check runs before any CUDA call.  Problem b's row is problem_row on (rows_b, users_count_b,
+// f_b); NoDefense without rows takes no table, as it ignores f.  Each kernel of a ragged batch reads the problem's row
+// count from the table: tm.n_rows (the Gram centre, Krum, TrimmedMean, NoDefense), theta + 2f (Bulyan's selection,
+// whose users_count is its row count).  Bulyan's second stage needs tm = shape(theta_b, 2 f_b): without rows the one
+// table holds it; with rows a second upload replaces the first after the selection kernels, in stream order.  Slots of
+// more than kBatchMaxClients rows append the class permutation to the table (class_table_bytes), and the trimmed mean
+// runs one launch per class (tmean::trimmed_mean_classes).
+static int defend_batched(const char* who, int max_clients, bool ragged, const char* rule, const void* G, int batch,
+                          int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, const int* rows,
+                          const int* ucs, int users_count, const int* fs, int f, float* out, int* idx_out,
+                          int* sel_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  BatchedRule r;
+  int rc = parse_rule(who, rule, false, &r);
+  if (rc || (rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, max_clients))) return rc;
+  int fmin = 0, theta_max = 0;
+  rc = check_problems(who, r, batch, n, INT32_MAX / 4, ragged, rows, ucs, users_count, fs, f,
+                      [&] { return check_outputs(who, rule, r, out, idx_out, sel_out, f); }, &fmin, &theta_max);
   if (rc) return rc;
-  int fmin = f, fmax = f;
-  if (fs && (rc = check_counts(who, fs, batch, INT32_MAX / 4, &fmin, &fmax))) return rc;
-  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out) || fmin < 0) {
-    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
-    return AFL_ERR_BAD_ARG;
-  }
-  // the reference's asserts (defences.py:24-25, 56), per problem
-  const int need_f = r == B_KRUM ? 2 * fmax + 1 : r == B_BULYAN ? 4 * fmax + 3 : 0;
-  if (users_count < need_f) {
-    const char* what = r == B_KRUM ? "krum: users_count >= 2*corrupted_count + 1" : "bulyan: users_count >= 4*corrupted_count + 3";
-    int b = 0;
-    while (fs && fs[b] != fmax) ++b;
-    if (fs) set_error("%s violated (%d, %d) in problem %d", what, users_count, fmax, b);
-    else set_error("%s violated (%d, %d)", what, users_count, f);
-    return AFL_ERR_PRECONDITION;
-  }
-  if (r == B_BULYAN && users_count != n) {
-    set_error("%s: Bulyan's users_count (%d) must equal the number of rows (%d)", who, users_count, n);
-    return AFL_ERR_UNSUPPORTED;
-  }
-  size_t gram_ws = 0, tabs = 0;
-  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
-  const ProblemParams* each = nullptr;
-  uint8_t* p = static_cast<uint8_t*>(ws);
-  if (fs && r != B_MEAN) {                              // NoDefense ignores f, as the reference does
-    rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch) + rule_ws, stream, [&](int b, ProblemParams& q) {
-      q.f = fs[b];
-      q.take = select::krum_take(n, users_count, fs[b]);
-      q.theta = users_count - 2 * fs[b];
-      q.tm = r == B_BULYAN ? tmean::shape(q.theta, 2 * fs[b]) : tmean::shape(n, fs[b]);
-    }, &each);
-    if (rc) return rc;
-    p += table_bytes(batch);
-    ws_bytes -= table_bytes(batch);
-  }
-  if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream);
-  if (r == B_TM)
-    return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, fmin, out, batch, batch_stride, 0, d, stream, each);
-  if (ws_bytes < rule_ws || !p || reinterpret_cast<uintptr_t>(p) % 256 != 0) {
-    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, rule_ws);
-    return AFL_ERR_WORKSPACE;
-  }
-  const size_t nn = static_cast<size_t>(batch) * n * n;
-  double* d2 = reinterpret_cast<double*>(p);
-  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
-  void* sel_ws = p + tabs + gram_ws;
-  const size_t sel_ws_bytes = ws_bytes - tabs - gram_ws;
-  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream);
-  if (rc) return rc;
-  if (r == B_KRUM)
-    return select::krum_from_sqdist(d2, n, users_count, fmin, idx_out, sel_ws, sel_ws_bytes, stream, batch, each);
-  const int theta = users_count - 2 * fmin;             // the row length of sel_out
-  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
-  rc = select::bulyan_select(dist, n, users_count, fmin, sel_out, sel_ws, sel_ws_bytes, stream, batch, each);
-  if (rc) return rc;
-  return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, theta, 2 * fmin, out, batch, batch_stride, theta, d,
-                                     stream, each);
-}
-
-// A ragged batch (afl_defend_batched_rows): problem b is rows 0..rows[b]-1 of its n-row slot, with its own users_count
-// ucs[b] and corrupted count fs[b].  Every check is the single call's, per problem and before any CUDA call; the table
-// rows come from the single call's host helpers on (rows[b], ucs[b], fs[b]), and each kernel reads the problem's row
-// count from them: tm.n_rows (the Gram centre, Krum, TrimmedMean, NoDefense), theta + 2f (Bulyan's selection, whose
-// users_count is its row count).  Bulyan's second stage needs tm = shape(theta, 2f): that table is copied over the
-// first one after the selection kernels, in stream order.  The workspace layout is afl_defend_batched_each's.
-// max_clients: kBatchMaxClients (afl_defend_batched_rows) or kBatchLargeMaxClients (afl_defend_batched_large).  Slots of
-// more than kBatchMaxClients rows append the problems' trimmed-mean class permutation to the table
-// (class_table_bytes), and the trimmed mean runs one launch per class (tmean::trimmed_mean_classes).
-static int defend_batched_rows(const char* who, int max_clients, const char* rule, const void* G, int batch,
-                               int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, const int* rows,
-                               const int* ucs, const int* fs, float* out, int* idx_out, int* sel_out, void* ws,
-                               size_t ws_bytes, cudaStream_t stream) {
-  const BatchedRule r = batched_rule(rule);
-  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
-  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, max_clients);
-  if (rc) return rc;
-  if (!rows || !ucs) { set_error("%s: the per-problem row counts or users counts are NULL", who); return AFL_ERR_BAD_ARG; }
-  int fmin = 0, fmax = 0;
-  if ((rc = check_counts(who, fs, batch, INT32_MAX / 4, &fmin, &fmax))) return rc;
-  for (int b = 0; b < batch; ++b)
-    if (rows[b] < 1 || rows[b] > n) {
-      set_error("%s: row count %d of problem %d is outside [1, %d]", who, rows[b], b, n);
-      return AFL_ERR_BAD_ARG;
-    }
-  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out)) {
-    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
-    return AFL_ERR_BAD_ARG;
-  }
-  int theta_max = 0;
-  for (int b = 0; b < batch; ++b) {
-    // the reference's asserts (defences.py:24-25, 56), per problem
-    const int64_t need = r == B_KRUM ? 2 * static_cast<int64_t>(fs[b]) + 1 : r == B_BULYAN ? 4 * static_cast<int64_t>(fs[b]) + 3 : 0;
-    if (ucs[b] < need) {
-      set_error("%s violated (%d, %d) in problem %d",
-                r == B_KRUM ? "krum: users_count >= 2*corrupted_count + 1" : "bulyan: users_count >= 4*corrupted_count + 3",
-                ucs[b], fs[b], b);
-      return AFL_ERR_PRECONDITION;
-    }
-    if (r == B_BULYAN && ucs[b] != rows[b]) {
-      set_error("%s: Bulyan's users_count (%d) must equal the number of rows (%d) in problem %d", who, ucs[b], rows[b], b);
-      return AFL_ERR_UNSUPPORTED;
-    }
-    const int theta = ucs[b] - 2 * fs[b];
-    theta_max = theta > theta_max ? theta : theta_max;
-  }
-  size_t gram_ws = 0, tabs = 0;
-  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
-  const bool classes = n > kBatchMaxClients;
-  const size_t tab_bytes = class_table_bytes(batch, n);
-  const ProblemParams* each = nullptr;
-  const int* perm = nullptr;
+  const bool table = fs && (rows || r != B_MEAN), classes = n > kBatchMaxClients;
+  const size_t tab_bytes = table ? class_table_bytes(batch, n) : 0;
+  const RuleScratch s = rule_scratch(r, batch, n, d, dtype, static_cast<uint8_t*>(ws) + tab_bytes);
+  if (tab_bytes + s.bytes > 0 && (rc = check_workspace(who, ws, ws_bytes, tab_bytes + s.bytes))) return rc;
+  const ProblemParams* each = table ? static_cast<const ProblemParams*>(ws) : nullptr;
+  const int* perm = classes ? reinterpret_cast<const int*>(each + batch) : nullptr;
   int counts[kSlotClasses];
-  auto row = [&](int b, ProblemParams& q) {
-    q.f = fs[b];
-    q.take = select::krum_take(rows[b], ucs[b], fs[b]);
-    q.theta = ucs[b] - 2 * fs[b];
-    q.tm = tmean::shape(rows[b], fs[b]);
+  auto upload = [&](bool second) {
+    return upload_table(batch, ws, stream, [&](int b) {
+      return problem_row(r, rows ? rows[b] : n, ucs ? ucs[b] : users_count, fs[b], 0.0, 0.0, second);
+    }, classes ? counts : nullptr);
   };
-  rc = classes ? upload_class_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row, &each, &perm, counts)
-               : upload_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row, &each);
-  if (rc) return rc;
-  uint8_t* p = static_cast<uint8_t*>(ws) + tab_bytes;
+  if (table && (rc = upload(!rows))) return rc;
   if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, each);
   if (r == B_TM && classes)
     return tmean::trimmed_mean_classes(G, n, d, ld, dtype, nullptr, out, batch, batch_stride, 0, d, stream, each, perm,
                                        counts);
   if (r == B_TM)
     return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, fmin, out, batch, batch_stride, 0, d, stream, each);
-  const size_t nn = static_cast<size_t>(batch) * n * n;
-  double* d2 = reinterpret_cast<double*>(p);
-  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
-  void* sel_ws = p + tabs + gram_ws;
-  const size_t sel_ws_bytes = ws_bytes - tab_bytes - tabs - gram_ws;
-  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream, each);
+  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, s.d2, s.gram, s.gram_bytes, 0, stream,
+                            rows ? each : nullptr);
   if (rc) return rc;
-  if (r == B_KRUM)
-    return select::krum_from_sqdist(d2, n, 0, 0, idx_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
-  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
-  rc = select::bulyan_rounds(dist, n, fmin, theta_max, sel_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
-  if (rc) return rc;
-  auto row2 = [&](int b, ProblemParams& q) {
-    row(b, q);
-    q.tm = tmean::shape(q.theta, 2 * fs[b]);              // the trimmed mean of the theta_b selected rows with 2 f_b
-  };
-  if (classes) {
-    rc = upload_class_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row2, &each, &perm, counts);
-    if (rc) return rc;
+  if (r == B_KRUM)                                       // a ragged table's take stands for users_count and f
+    return select::krum_from_sqdist(s.d2, n, rows ? 0 : users_count, rows ? 0 : fmin, idx_out, s.sel, s.sel_bytes,
+                                    stream, batch, each, rows != nullptr);
+  if ((rc = gram::sqdist_to_dist(s.d2, n, s.dist, stream, batch))) return rc;
+  rc = select::bulyan_rounds(s.dist, n, fmin, theta_max, sel_out, s.sel, s.sel_bytes, stream, batch, each,
+                             rows != nullptr);
+  if (rc || (rows && (rc = upload(true)))) return rc;
+  if (classes)
     return tmean::trimmed_mean_classes(G, n, d, ld, dtype, sel_out, out, batch, batch_stride, theta_max, d, stream, each,
                                        perm, counts);
-  }
-  rc = upload_table(who, batch, ws, ws_bytes, tab_bytes + rule_ws, stream, row2, &each);
-  if (rc) return rc;
   return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, theta_max, 2 * fmin, out, batch, batch_stride, theta_max,
                                      d, stream, each);
 }
@@ -893,28 +897,41 @@ static int alie_batched(const char* who, const void* G, int batch, int64_t batch
     if (!zs) { set_error("%s: the per-problem attack strengths are NULL", who); return AFL_ERR_BAD_ARG; }
     if ((rc = check_counts(who, fs, batch, n, &fmin, &fmax))) return rc;
   }
-  if (bcast_rows && fmax > 0 &&
-      (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(fmax - 1) * bcast_ld + d))) {
-    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  const ProblemParams* each = nullptr;
+  if ((rc = check_bcast(who, bcast_rows, fmax, d, batch, bcast_batch_stride, bcast_ld))) return rc;
   if (fs) {
-    rc = upload_table(who, batch, ws, ws_bytes, table_bytes(batch), stream, [&](int b, ProblemParams& q) {
-      q.f = fs[b];
-      q.z = static_cast<float>(zs[b]);
-      q.write = fs[b] > 0 && zs[b] != 0.0;             // malicious.py:20-21: z == 0 computes the statistics only
-    }, &each);
+    if ((rc = check_workspace(who, ws, ws_bytes, table_bytes(batch)))) return rc;
+    rc = upload_table(batch, ws, stream, [&](int b) { return problem_row(T_ALIE, 0, 0, fs[b], zs[b], 0.0, false); });
     if (rc) return rc;
   }
   return colstats::alie_batched(G, fmax, d, ld, dtype, z, mu_out, sigma_out, crafted_out, bcast_rows, bcast_ld, batch,
-                                batch_stride, d, bcast_batch_stride, stream, each);
+                                batch_stride, d, bcast_batch_stride, stream,
+                                fs ? static_cast<const ProblemParams*>(ws) : nullptr);
 }
 
 // Attack-success metrics of a batch (afl_attack_metrics_batched; fs != NULL: afl_attack_metrics_batched_each).
 // Workspace: [ProblemParams table][partial sums: double2[batch][tiles]]; the scalar call leaves the table unused.
 static size_t metrics_partial_bytes(int batch, int64_t d, int dtype) {
   return align_up(static_cast<size_t>(batch) * colstats::deviation_tiles(d, dtype) * sizeof(double2), 256);
+}
+
+// The selection inputs of the metrics: the counts need sel, whose rows are sel_ld >= 1 apart.
+static int check_sel(const char* who, const int* sel, int sel_ld, const int* mal_count, const int* sel_count) {
+  if ((mal_count || sel_count) && !sel) { set_error("%s: mal_count and sel_count need sel", who); return AFL_ERR_BAD_ARG; }
+  if (sel && sel_ld < 1) { set_error("%s: sel_ld must be >= 1 (got %d)", who, sel_ld); return AFL_ERR_BAD_ARG; }
+  return AFL_OK;
+}
+
+// The metrics' pointer rules: the aggregate as agg or as idx, not both, and each output with the input it needs.
+static int check_metrics_inputs(const char* who, const float* agg, const int* idx, const int* sel, int sel_ld,
+                                const float* dev_out, const double* sums_out, const int* krum_hit, const int* mal_count,
+                                const int* sel_count) {
+  if (agg && idx) { set_error("%s: give the aggregate as agg or as idx, not both", who); return AFL_ERR_BAD_ARG; }
+  if ((dev_out || sums_out) && !agg && !idx) {
+    set_error("%s: dev_out and sums_out need an aggregate (agg or idx)", who);
+    return AFL_ERR_BAD_ARG;
+  }
+  if (krum_hit && !idx) { set_error("%s: krum_hit needs idx", who); return AFL_ERR_BAD_ARG; }
+  return check_sel(who, sel, sel_ld, mal_count, sel_count);
 }
 
 // rows != NULL (afl_attack_metrics_batched_rows, fs required): problem b has rows[b] rows, in [1, n].
@@ -925,39 +942,47 @@ static int attack_metrics(const void* G, int batch, int64_t batch_stride, int n,
   const char* who = rows ? "afl_attack_metrics_batched_rows" : fs ? "afl_attack_metrics_batched_each" : "afl_attack_metrics_batched";
   int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
   if (rc) return rc;
-  int fmin = f, fmax = f;
-  if (fs && (rc = check_counts(who, fs, batch, INT32_MAX, &fmin, &fmax))) return rc;
-  for (int b = 0; rows && b < batch; ++b)
-    if (rows[b] < 1 || rows[b] > n) {
-      set_error("%s: row count %d of problem %d is outside [1, %d]", who, rows[b], b, n);
-      return AFL_ERR_BAD_ARG;
-    }
-  if (fmin < 0) { set_error("%s: corrupted_count %d is negative", who, f); return AFL_ERR_BAD_ARG; }
-  if (agg && idx) { set_error("%s: give the aggregate as agg or as idx, not both", who); return AFL_ERR_BAD_ARG; }
-  if ((dev_out || sums_out) && !agg && !idx) {
-    set_error("%s: dev_out and sums_out need an aggregate (agg or idx)", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  if (krum_hit && !idx) { set_error("%s: krum_hit needs idx", who); return AFL_ERR_BAD_ARG; }
-  if ((mal_count || sel_count) && !sel) { set_error("%s: mal_count and sel_count need sel", who); return AFL_ERR_BAD_ARG; }
-  if (sel && sel_ld < 1) { set_error("%s: sel_ld must be >= 1 (got %d)", who, sel_ld); return AFL_ERR_BAD_ARG; }
+  int fmin = 0, theta_max = 0;
+  rc = check_problems(who, T_METRICS, batch, n, INT32_MAX, false, rows, nullptr, 0, fs, f, [&]() -> int {
+    if (f < 0) { set_error("%s: corrupted_count %d is negative", who, f); return AFL_ERR_BAD_ARG; }
+    return check_metrics_inputs(who, agg, idx, sel, sel_ld, dev_out, sums_out, krum_hit, mal_count, sel_count);
+  }, &fmin, &theta_max);
+  if (rc) return rc;
   const bool pass = dev_out || sums_out || honest_out;          // the column pass and its partial sums
   const size_t need = table_bytes(batch) + metrics_partial_bytes(batch, d, dtype);
-  if ((fs || pass) && (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0)) {
-    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
-    return AFL_ERR_WORKSPACE;
-  }
-  const ProblemParams* each = nullptr;
+  if ((fs || pass) && (rc = check_workspace(who, ws, ws_bytes, need))) return rc;
   if (fs) {
-    rc = upload_table(who, batch, ws, ws_bytes, need, stream, [&](int b, ProblemParams& q) {
-      q.f = fs[b];
-      if (rows) q.tm.n_rows = rows[b];
-    }, &each);
+    rc = upload_table(batch, ws, stream, [&](int b) {
+      return problem_row(T_METRICS, rows ? rows[b] : 0, 0, fs[b], 0.0, 0.0, false);
+    });
     if (rc) return rc;
   }
-  return colstats::attack_metrics(G, batch, batch_stride, n, d, ld, dtype, f, each, agg, idx, sel, sel_ld, dev_out,
+  return colstats::attack_metrics(G, batch, batch_stride, n, d, ld, dtype, f,
+                                  fs ? static_cast<const ProblemParams*>(ws) : nullptr, agg, idx, sel, sel_ld, dev_out,
                                   sums_out, honest_out, krum_hit, mal_count, sel_count,
                                   static_cast<uint8_t*>(ws) + table_bytes(batch), stream, rows != nullptr);
+}
+
+// The backdoor crafting's own arguments.  Start: w and every output, and w_batch_stride 0 (one shared w) or >= d.
+static int check_backdoor_start(const char* who, int64_t d, const float* w, int64_t w_batch_stride, const float* mu_out,
+                                const float* sigma_out, const float* initial_out) {
+  if (!w || !mu_out || !sigma_out || !initial_out) { set_error("%s: w and every output are required", who); return AFL_ERR_BAD_ARG; }
+  if (w_batch_stride < 0 || (w_batch_stride > 0 && w_batch_stride < d)) {
+    set_error("%s: w_batch_stride %lld must be 0 (one shared w) or >= d", who, static_cast<long long>(w_batch_stride));
+    return AFL_ERR_BAD_ARG;
+  }
+  return AFL_OK;
+}
+
+// Finish: 1 <= batch <= kBatchMax, and the problems' trained vectors mal do not overlap.
+static int check_backdoor_finish(const char* who, int batch, int64_t d, int64_t mal_batch_stride) {
+  if (batch < 1) { set_error("%s: batch must be >= 1 (got %d)", who, batch); return AFL_ERR_BAD_ARG; }
+  if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
+  if (batch > 1 && mal_batch_stride < d) {
+    set_error("%s: mal_batch_stride %lld makes problems overlap", who, static_cast<long long>(mal_batch_stride));
+    return AFL_ERR_BAD_ARG;
+  }
+  return AFL_OK;
 }
 
 // The backdoor's per-problem values (afl_backdoor_start_batched / _finish_batched): non-NULL, counts in [0, f_cap].
@@ -970,13 +995,10 @@ static int backdoor_values(const char* who, int batch, const int* fs, int f_cap,
 
 // Their table (f, (float)z, (float)lr, write) at the start of the workspace: the calls' first CUDA call.
 static int backdoor_table(const char* who, int batch, const int* fs, const double* zs, const double* lrs, void* ws,
-                          size_t ws_bytes, cudaStream_t stream, const ProblemParams** each) {
-  return upload_table(who, batch, ws, ws_bytes, table_bytes(batch), stream, [&](int b, ProblemParams& q) {
-    q.f = fs[b];
-    q.z = static_cast<float>(zs[b]);
-    q.lr = static_cast<float>(lrs[b]);
-    q.write = fs[b] > 0 && zs[b] != 0.0;               // malicious.py:20-21: z == 0 computes the statistics only
-  }, each);
+                          size_t ws_bytes, cudaStream_t stream) {
+  const int rc = check_workspace(who, ws, ws_bytes, table_bytes(batch));
+  if (rc) return rc;
+  return upload_table(batch, ws, stream, [&](int b) { return problem_row(T_BACKDOOR, 0, 0, fs[b], zs[b], lrs[b], false); });
 }
 
 static int backdoor_start(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
@@ -985,18 +1007,12 @@ static int backdoor_start(const void* G, int batch, int64_t batch_stride, int n,
                           cudaStream_t stream) {
   const char* who = "afl_backdoor_start_batched";
   int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
-  if (rc) return rc;
-  if (!w || !mu_out || !sigma_out || !initial_out) { set_error("%s: w and every output are required", who); return AFL_ERR_BAD_ARG; }
-  if (w_batch_stride < 0 || (w_batch_stride > 0 && w_batch_stride < d)) {
-    set_error("%s: w_batch_stride %lld must be 0 (one shared w) or >= d", who, static_cast<long long>(w_batch_stride));
-    return AFL_ERR_BAD_ARG;
-  }
+  if (rc || (rc = check_backdoor_start(who, d, w, w_batch_stride, mu_out, sigma_out, initial_out))) return rc;
   int fmax = 0;
   if ((rc = backdoor_values(who, batch, fs, n, zs, lrs, &fmax))) return rc;
-  const ProblemParams* each = nullptr;
-  if ((rc = backdoor_table(who, batch, fs, zs, lrs, ws, ws_bytes, stream, &each))) return rc;
-  return colstats::backdoor_start(G, fmax, d, ld, dtype, batch, batch_stride, each, w, w_batch_stride, mu_out,
-                                  sigma_out, initial_out, stream);
+  if ((rc = backdoor_table(who, batch, fs, zs, lrs, ws, ws_bytes, stream))) return rc;
+  return colstats::backdoor_start(G, fmax, d, ld, dtype, batch, batch_stride, static_cast<const ProblemParams*>(ws), w,
+                                  w_batch_stride, mu_out, sigma_out, initial_out, stream);
 }
 
 static int backdoor_finish(int batch, int64_t d, const int* fs, const double* zs, const double* lrs, const float* mu,
@@ -1005,60 +1021,53 @@ static int backdoor_finish(int batch, int64_t d, const int* fs, const double* zs
                            size_t ws_bytes, cudaStream_t stream) {
   const char* who = "afl_backdoor_finish_batched";
   if (!mu || !sigma || !initial || !mal || !crafted_out || d < 1) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
-  if (batch < 1) { set_error("%s: batch must be >= 1 (got %d)", who, batch); return AFL_ERR_BAD_ARG; }
-  if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
-  if (batch > 1 && mal_batch_stride < d) {
-    set_error("%s: mal_batch_stride %lld makes problems overlap", who, static_cast<long long>(mal_batch_stride));
-    return AFL_ERR_BAD_ARG;
-  }
-  int fmax = 0;
-  int rc = backdoor_values(who, batch, fs, INT32_MAX, zs, lrs, &fmax);
+  int rc = check_backdoor_finish(who, batch, d, mal_batch_stride);
   if (rc) return rc;
-  if (bcast_rows && fmax > 0 &&
-      (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(fmax - 1) * bcast_ld + d))) {
-    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  const ProblemParams* each = nullptr;
-  if ((rc = backdoor_table(who, batch, fs, zs, lrs, ws, ws_bytes, stream, &each))) return rc;
-  return colstats::backdoor_finish(batch, d, each, mu, sigma, initial, mal, mal_batch_stride, crafted_out, bcast_rows,
-                                   bcast_batch_stride, bcast_ld, stream);
+  int fmax = 0;
+  if ((rc = backdoor_values(who, batch, fs, INT32_MAX, zs, lrs, &fmax))) return rc;
+  if ((rc = check_bcast(who, bcast_rows, fmax, d, batch, bcast_batch_stride, bcast_ld))) return rc;
+  if ((rc = backdoor_table(who, batch, fs, zs, lrs, ws, ws_bytes, stream))) return rc;
+  return colstats::backdoor_finish(batch, d, static_cast<const ProblemParams*>(ws), mu, sigma, initial, mal,
+                                   mal_batch_stride, crafted_out, bcast_rows, bcast_batch_stride, bcast_ld, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Device-parameter calls (afl_*_dev): the per-problem arrays are device memory, so a call never reads them on the host.
-// problem_table_kernel builds the table the host calls above build, one thread per problem, and runs their per-problem
-// checks in the same order.  A problem that fails a check gets its first code in the caller's sticky status[b] and
-// the safe row of rows_b = n, users_count_b = n, f_b = 0, which keeps every kernel inside its slot; its outputs are
-// then not the reference's, and only status says so.  After the host checks of shapes, pointers and the workspace,
-// a call makes no host copy, synchronisation or allocation, so it can be captured into a CUDA graph.
+// problem_table_kernel runs the host calls' per-problem checks in the same order (problem_code, whose asserts are
+// problem_assert) and builds their rows with problem_row, one thread per problem.  A problem that fails a check gets
+// its first code in the caller's sticky status[b] and the safe row of rows_b = n, users_count_b = n, f_b = 0, which
+// keeps every kernel inside its slot; its outputs are then not the reference's, and only status says so.  After the
+// host checks of shapes, pointers and the workspace, a call makes no host copy, synchronisation or allocation, so it
+// can be captured into a CUDA graph.
 // ------------------------------------------------------------------------------------------------
-enum TableRule { T_ALIE = B_BULYAN + 1, T_METRICS };
-
 struct TableArgs {
-  int rule;                   // BatchedRule, T_ALIE or T_METRICS
+  int rule;                   // a BatchedRule
   int batch, n;
   const int* rows;            // NULL: n rows in every problem
   const int* ucs;             // NULL: users_count without rows, rows with them
   int users_count;
   const int* fs;
-  const double* zs;           // ALIE only
+  const double* zs;           // ALIE and the backdoor only
+  const double* lrs;          // the backdoor only
   ProblemParams* table;
   int* status;
   const int* sel;             // Bulyan's second stage: rows of sel_ld entries, sel[b][theta_b - 1] < 0 = failed round
   int sel_ld;
 };
 
+static TableArgs table_args(BatchedRule rule, int batch, int n, const int* fs, void* ws, int* status) {
+  TableArgs a{};
+  a.rule = rule; a.batch = batch; a.n = n; a.fs = fs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
+  return a;
+}
+
 // The first code of the host calls' checks for one problem: afl_defend_batched_rows / _each (rows = n),
-// afl_alie_batched_each, afl_attack_metrics_batched_rows / _each.
+// afl_alie_batched_each, afl_attack_metrics_batched_rows / _each, and the backdoor's (ALIE's count range).
 __device__ int problem_code(int rule, int n, bool ragged, int m, int uc, int f) {
-  if (rule == T_ALIE) return f < 0 || f > n ? AFL_ERR_BAD_ARG : AFL_OK;
+  if (rule == T_ALIE || rule == T_BACKDOOR) return f < 0 || f > n ? AFL_ERR_BAD_ARG : AFL_OK;
   if (f < 0 || (rule != T_METRICS && f > INT32_MAX / 4)) return AFL_ERR_BAD_ARG;
   if (ragged && (m < 1 || m > n)) return AFL_ERR_BAD_ARG;
-  if (rule == B_KRUM && uc < 2 * static_cast<int64_t>(f) + 1) return AFL_ERR_PRECONDITION;
-  if (rule == B_BULYAN && uc < 4 * static_cast<int64_t>(f) + 3) return AFL_ERR_PRECONDITION;
-  if (rule == B_BULYAN && uc != m) return AFL_ERR_UNSUPPORTED;
-  return AFL_OK;
+  return problem_assert(rule, m, uc, f);
 }
 
 __global__ void __launch_bounds__(128) problem_table_kernel(const TableArgs a) {
@@ -1069,19 +1078,9 @@ __global__ void __launch_bounds__(128) problem_table_kernel(const TableArgs a) {
   int uc = a.ucs ? a.ucs[b] : a.rows ? m : a.users_count;
   const int code = problem_code(a.rule, a.n, a.rows != nullptr, m, uc, f);
   if (code != AFL_OK) { m = a.n; uc = a.n; f = 0; }
-  ProblemParams q{};
-  q.f = f;
-  if (a.rule == T_ALIE) {
-    q.z = static_cast<float>(a.zs[b]);
-    q.write = f > 0 && a.zs[b] != 0.0;                  // malicious.py:20-21: z == 0 computes the statistics only
-  } else if (a.rule == T_METRICS) {
-    if (a.rows) q.tm.n_rows = m;
-  } else {
-    q.take = select::krum_take(m, uc, f);
-    q.theta = uc - 2 * f;
-    // Bulyan's second stage: the trimmed mean of the theta_b selected rows with 2 f_b (the whole-slot call's only table)
-    q.tm = a.rule == B_BULYAN && (a.sel || !a.rows) ? tmean::shape(q.theta, 2 * f) : tmean::shape(m, f);
-  }
+  // Bulyan's second stage: the table after the selection, or the whole-slot call's only table
+  const ProblemParams q = problem_row(a.rule, (a.rows || a.rule != T_METRICS) ? m : 0, uc, f, a.zs ? a.zs[b] : 0.0,
+                                      a.lrs ? a.lrs[b] : 0.0, a.sel || !a.rows);
   a.table[b] = q;
   int st = code;
   if (st == AFL_OK && a.sel && a.sel[static_cast<int64_t>(b) * a.sel_ld + q.theta - 1] < 0) st = AFL_ERR_NO_WINNER;
@@ -1095,7 +1094,7 @@ static int launch_table(const TableArgs& a, cudaStream_t stream) {
 }
 
 // The problems of a table grouped by the trimmed-mean slot class of their tm.n_rows, on the device: perm[batch] lists
-// them class by class and in problem order within a class (upload_class_table's order), and start[kSlotClasses + 1]
+// them class by class and in problem order within a class (upload_table's order), and start[kSlotClasses + 1]
 // holds the offset of each class in perm.  One CTA walks the problems in chunks of its size: a first pass counts the
 // classes (__syncthreads_count), a second places each problem at its class's running offset plus its rank in the
 // chunk (warp ballots, then the counts of the warps before it).  No atomics and no waits between CTAs, so the order is
@@ -1170,140 +1169,80 @@ static int launch_class_perm(const ProblemParams* table, int batch, int* perm, i
 // `need` bytes at a 256-byte boundary.
 static int check_dev(const char* who, const int* fs, const int* status, void* ws, size_t ws_bytes, size_t need) {
   if (!fs || !status) { set_error("%s: the per-problem corrupted counts or the status array are NULL", who); return AFL_ERR_BAD_ARG; }
-  if (!ws || ws_bytes < need || reinterpret_cast<uintptr_t>(ws) % 256 != 0) {
-    set_error("%s: workspace too small or misaligned (%zu < %zu)", who, ws_bytes, need);
-    return AFL_ERR_WORKSPACE;
-  }
-  return AFL_OK;
+  return check_workspace(who, ws, ws_bytes, need);
 }
 
 static int table_dev(const char* rule, int batch, int n, const int* rows, int users_count, const int* ucs,
                      const int* fs, const double* zs, void* ws, size_t ws_bytes, int* status, cudaStream_t stream) {
   const char* who = "afl_batched_table_dev";
-  const bool alie = rule && !strcmp(rule, "ALIE"), metrics = rule && !strcmp(rule, "AttackMetrics");
-  const BatchedRule r = batched_rule(rule);
-  if (r == B_BAD && !alie && !metrics) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
+  BatchedRule r;
+  int rc = parse_rule(who, rule, true, &r);
+  if (rc) return rc;
   if (batch < 1 || n < 1) { set_error("%s: batch and n must be >= 1 (got %d, %d)", who, batch, n); return AFL_ERR_BAD_ARG; }
   if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
-  if (alie && !zs) { set_error("%s: the per-problem attack strengths are NULL", who); return AFL_ERR_BAD_ARG; }
-  int rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch));
-  if (rc) return rc;
-  TableArgs a{};
-  a.rule = alie ? static_cast<int>(T_ALIE) : metrics ? static_cast<int>(T_METRICS) : static_cast<int>(r);
-  a.batch = batch; a.n = n; a.rows = alie ? nullptr : rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
-  a.fs = fs; a.zs = zs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
+  if (r == T_ALIE && !zs) { set_error("%s: the per-problem attack strengths are NULL", who); return AFL_ERR_BAD_ARG; }
+  if ((rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch)))) return rc;
+  TableArgs a = table_args(r, batch, n, fs, ws, status);
+  a.rows = r == T_ALIE ? nullptr : rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
+  a.zs = r == T_ALIE ? zs : nullptr;
   return launch_table(a, stream);
 }
 
-// afl_defend_batched_rows (rows != NULL) or afl_defend_batched_each (rows == NULL, n rows and users_count in every
-// problem) with device arrays: the same kernels on a device-built table.  Host scalars of those calls become bounds
-// that hold for every accepted value: Bulyan's selection width is the caller's sel_ld >= n >= theta_b (the host calls
-// use theta_max), and the corrupted counts and users counts that only fill fields a table overrides are passed as 0.
-static int defend_batched_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
-                              int64_t ld, int dtype, const int* rows, int users_count, const int* ucs, const int* fs,
-                              float* out, int* idx_out, int* sel_out, int sel_ld, void* ws, size_t ws_bytes,
-                              int* status, cudaStream_t stream) {
-  const char* who = "afl_defend_batched_dev";
-  const BatchedRule r = batched_rule(rule);
-  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
-  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype);
-  if (rc) return rc;
-  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out)) {
-    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
-    return AFL_ERR_BAD_ARG;
-  }
+// afl_defend_batched_dev (max_clients = kBatchMaxClients) and afl_defend_batched_large_dev (kBatchLargeMaxClients):
+// afl_defend_batched_rows / _large (rows != NULL) or _each (rows == NULL: n rows and users_count in every problem) with
+// device arrays, the same kernels on a device-built table.  Host scalars of those calls become bounds that hold for
+// every accepted value: Bulyan's selection width is the caller's sel_ld >= n >= theta_b (the host calls use
+// theta_max), and the corrupted counts and users counts that only fill fields a table overrides are passed as 0.
+// Above kBatchMaxClients the workspace is the large call's (ProblemParams[batch], perm[batch], then the rule's scratch)
+// followed by one kClassStartBytes block for start[]: after each table launch class_perm_kernel groups the problems on
+// the device, and the trimmed mean runs one device-count launch per class (tmean::trimmed_mean_classes_dev).  Every
+// kernel then reads the table as afl_defend_batched_large does, except the Gram without rows: with n rows in every
+// problem its multi-tile centre is the same without the table, and the table of a whole-slot Bulyan holds the second
+// stage's tm already.
+static int defend_batched_dev(const char* who, int max_clients, const char* rule, const void* G, int batch,
+                              int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype, const int* rows,
+                              int users_count, const int* ucs, const int* fs, float* out, int* idx_out, int* sel_out,
+                              int sel_ld, void* ws, size_t ws_bytes, int* status, cudaStream_t stream) {
+  BatchedRule r;
+  int rc = parse_rule(who, rule, false, &r);
+  if (rc || (rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, max_clients))) return rc;
+  if (n <= kBatchMaxClients) who = "afl_defend_batched_dev";      // the large call's small form is that call
+  if ((rc = check_outputs(who, rule, r, out, idx_out, sel_out))) return rc;
   if (r == B_BULYAN && sel_ld < n) {
     set_error("%s: Bulyan's selection width sel_ld (%d) must be at least n (%d)", who, sel_ld, n);
     return AFL_ERR_BAD_ARG;
   }
-  size_t gram_ws = 0, tabs = 0;
-  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
-  if ((rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch) + rule_ws))) return rc;
-
-  TableArgs a{};
-  a.rule = r; a.batch = batch; a.n = n; a.rows = rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
-  a.fs = fs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
-  if ((rc = launch_table(a, stream))) return rc;
-  const ProblemParams* each = a.table;
-  const ProblemParams* ragged = rows ? each : nullptr;
-  if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, ragged);
-  if (r == B_TM) return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, 0, out, batch, batch_stride, 0, d, stream, each);
-  uint8_t* p = static_cast<uint8_t*>(ws) + table_bytes(batch);
-  const size_t nn = static_cast<size_t>(batch) * n * n;
-  double* d2 = reinterpret_cast<double*>(p);
-  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
-  void* sel_ws = p + tabs + gram_ws;
-  const size_t sel_ws_bytes = ws_bytes - table_bytes(batch) - tabs - gram_ws;
-  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream, ragged);
-  if (rc) return rc;
-  if (r == B_KRUM) return select::krum_from_sqdist(d2, n, 0, 0, idx_out, sel_ws, sel_ws_bytes, stream, batch, each, rows != nullptr);
-  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
-  rc = select::bulyan_rounds(dist, n, 0, sel_ld, sel_out, sel_ws, sel_ws_bytes, stream, batch, each, rows != nullptr);
-  if (rc) return rc;
-  a.sel = sel_out; a.sel_ld = sel_ld;                    // second stage's table, and a failed round's status
-  if ((rc = launch_table(a, stream))) return rc;
-  return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, n, 0, out, batch, batch_stride, sel_ld, d, stream, each);
-}
-
-// afl_defend_batched_large with device arrays (afl_defend_batched_large_dev): n <= 128 is afl_defend_batched_dev.  Above,
-// the workspace is the large call's (ProblemParams[batch], perm[batch], then the rule's scratch) followed by one
-// kClassStartBytes block for start[].  After each table launch class_perm_kernel groups the problems on the device, and
-// the trimmed mean runs one device-count launch per class (tmean::trimmed_mean_classes_dev).  Every kernel reads the
-// table as afl_defend_batched_large does, except the Gram without rows: with n rows in every problem its multi-tile
-// centre is the same without the table, and the table of a whole-slot Bulyan holds the second stage's tm already.
-static int defend_batched_large_dev(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
-                                    int64_t ld, int dtype, const int* rows, int users_count, const int* ucs,
-                                    const int* fs, float* out, int* idx_out, int* sel_out, int sel_ld, void* ws,
-                                    size_t ws_bytes, int* status, cudaStream_t stream) {
-  const char* who = "afl_defend_batched_large_dev";
-  const BatchedRule r = batched_rule(rule);
-  if (r == B_BAD) { set_error("%s: unknown rule '%s'", who, rule ? rule : "(null)"); return AFL_ERR_BAD_ARG; }
-  int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, kBatchLargeMaxClients);
-  if (rc) return rc;
-  if (n <= kBatchMaxClients)
-    return defend_batched_dev(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_count, ucs, fs, out, idx_out,
-                              sel_out, sel_ld, ws, ws_bytes, status, stream);
-  if ((r != B_KRUM && !out) || (r == B_KRUM && !idx_out) || (r == B_BULYAN && !sel_out)) {
-    set_error("%s: %s needs %s", who, rule, r == B_KRUM ? "idx_out" : r == B_BULYAN ? "out and sel_out" : "out");
-    return AFL_ERR_BAD_ARG;
-  }
-  if (r == B_BULYAN && sel_ld < n) {
-    set_error("%s: Bulyan's selection width sel_ld (%d) must be at least n (%d)", who, sel_ld, n);
-    return AFL_ERR_BAD_ARG;
-  }
-  size_t gram_ws = 0, tabs = 0;
-  const size_t rule_ws = batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  const bool classes = n > kBatchMaxClients, ragged = rows || classes;   // ragged: kernels read rows_b from the table
   const size_t tab_bytes = class_table_bytes(batch, n);
-  if ((rc = check_dev(who, fs, status, ws, ws_bytes, tab_bytes + rule_ws + kClassStartBytes))) return rc;
-
-  TableArgs a{};
-  a.rule = r; a.batch = batch; a.n = n; a.rows = rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
-  a.fs = fs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
-  const ProblemParams* each = a.table;
   uint8_t* p = static_cast<uint8_t*>(ws) + tab_bytes;
-  int* perm = reinterpret_cast<int*>(static_cast<uint8_t*>(ws) + static_cast<size_t>(batch) * sizeof(ProblemParams));
-  int* start = reinterpret_cast<int*>(p + rule_ws);
+  const RuleScratch s = rule_scratch(r, batch, n, d, dtype, p);
+  if ((rc = check_dev(who, fs, status, ws, ws_bytes, tab_bytes + s.bytes + (classes ? kClassStartBytes : 0)))) return rc;
+
+  TableArgs a = table_args(r, batch, n, fs, ws, status);
+  a.rows = rows; a.ucs = rows ? ucs : nullptr; a.users_count = users_count;
   if ((rc = launch_table(a, stream))) return rc;
-  if (r == B_MEAN) return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, each);
-  if (r == B_TM) {
+  const ProblemParams* each = a.table;
+  int* perm = reinterpret_cast<int*>(a.table + batch);
+  int* start = reinterpret_cast<int*>(p + s.bytes);
+  if (r == B_MEAN)
+    return colstats::mean_batched(G, n, d, ld, dtype, out, batch, batch_stride, d, stream, ragged ? each : nullptr);
+  if (r == B_TM && classes) {
     if ((rc = launch_class_perm(each, batch, perm, start, stream))) return rc;
     return tmean::trimmed_mean_classes_dev(G, n, d, ld, dtype, nullptr, out, batch, batch_stride, 0, d, stream, each,
                                            perm, start);
   }
-  const size_t nn = static_cast<size_t>(batch) * n * n;
-  double* d2 = reinterpret_cast<double*>(p);
-  float* dist = reinterpret_cast<float*>(p + align_up(nn * 8, 256));
-  void* sel_ws = p + tabs + gram_ws;
-  const size_t sel_ws_bytes = rule_ws - tabs - gram_ws;
-  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, d2, p + tabs, gram_ws, 0, stream,
+  if (r == B_TM) return tmean::trimmed_mean_batched(G, n, d, ld, dtype, nullptr, n, 0, out, batch, batch_stride, 0, d, stream, each);
+  rc = gram::sqdist_batched(G, batch, batch_stride, n, d, ld, dtype, s.d2, s.gram, s.gram_bytes, 0, stream,
                             rows ? each : nullptr);
   if (rc) return rc;
-  if (r == B_KRUM) return select::krum_from_sqdist(d2, n, 0, 0, idx_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
-  rc = gram::sqdist_to_dist(d2, n, dist, stream, batch); if (rc) return rc;
-  rc = select::bulyan_rounds(dist, n, 0, sel_ld, sel_out, sel_ws, sel_ws_bytes, stream, batch, each, true);
+  if (r == B_KRUM) return select::krum_from_sqdist(s.d2, n, 0, 0, idx_out, s.sel, s.sel_bytes, stream, batch, each, ragged);
+  if ((rc = gram::sqdist_to_dist(s.d2, n, s.dist, stream, batch))) return rc;
+  rc = select::bulyan_rounds(s.dist, n, 0, sel_ld, sel_out, s.sel, s.sel_bytes, stream, batch, each, ragged);
   if (rc) return rc;
-  a.sel = sel_out; a.sel_ld = sel_ld;                    // second stage's table (theta_b classes), and a failed round's status
+  a.sel = sel_out; a.sel_ld = sel_ld;                    // second stage's table, and a failed round's status
   if ((rc = launch_table(a, stream))) return rc;
+  if (!classes)
+    return tmean::trimmed_mean_batched(G, n, d, ld, dtype, sel_out, n, 0, out, batch, batch_stride, sel_ld, d, stream, each);
   if ((rc = launch_class_perm(each, batch, perm, start, stream))) return rc;
   return tmean::trimmed_mean_classes_dev(G, n, d, ld, dtype, sel_out, out, batch, batch_stride, sel_ld, d, stream, each,
                                          perm, start);
@@ -1318,45 +1257,26 @@ static int alie_batched_dev(const void* G, int batch, int64_t batch_stride, int 
   int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
   if (rc) return rc;
   if (!zs) { set_error("%s: the per-problem attack strengths are NULL", who); return AFL_ERR_BAD_ARG; }
-  if (bcast_rows && (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(n - 1) * bcast_ld + d))) {
-    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
-    return AFL_ERR_BAD_ARG;
-  }
+  if ((rc = check_bcast(who, bcast_rows, n, d, batch, bcast_batch_stride, bcast_ld))) return rc;
   if ((rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch)))) return rc;
-  TableArgs a{};
-  a.rule = T_ALIE; a.batch = batch; a.n = n; a.fs = fs; a.zs = zs; a.table = static_cast<ProblemParams*>(ws); a.status = status;
+  TableArgs a = table_args(T_ALIE, batch, n, fs, ws, status);
+  a.zs = zs;
   if ((rc = launch_table(a, stream))) return rc;
   return colstats::alie_batched_dev(G, n, d, ld, dtype, mu_out, sigma_out, crafted_out, bcast_rows, bcast_ld, batch,
                                     batch_stride, d, bcast_batch_stride, stream, a.table);
 }
 
-// The backdoor crafting's table from device arrays (afl_backdoor_start_batched_dev / _finish_batched_dev): backdoor_table's
-// row, with the host calls' count check per problem (f_b < 0 or f_b > n -> AFL_ERR_BAD_ARG, and the safe f_b = 0).
-__global__ void __launch_bounds__(128) backdoor_table_kernel(int batch, int n, const int* fs, const double* zs,
-                                                             const double* lrs, ProblemParams* table, int* status) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= batch) return;
-  int f = fs[b];
-  const int code = f < 0 || f > n ? AFL_ERR_BAD_ARG : AFL_OK;
-  if (code != AFL_OK) f = 0;
-  ProblemParams q{};
-  q.f = f;
-  q.z = static_cast<float>(zs[b]);
-  q.lr = static_cast<float>(lrs[b]);
-  q.write = f > 0 && zs[b] != 0.0;                      // malicious.py:20-21: z == 0 computes the statistics only
-  table[b] = q;
-  if (code != AFL_OK && status[b] == AFL_OK) status[b] = code;
-}
-
+// The backdoor crafting's table from device arrays (afl_backdoor_start_batched_dev / _finish_batched_dev):
+// backdoor_table's row, with the host calls' count check per problem (f_b < 0 or f_b > n -> AFL_ERR_BAD_ARG, and the
+// safe f_b = 0).
 static int backdoor_table_dev(const char* who, int batch, int n, const int* fs, const double* zs, const double* lrs,
                               void* ws, size_t ws_bytes, int* status, cudaStream_t stream) {
   if (!zs || !lrs) { set_error("%s: the per-problem attack strengths or learning rates are NULL", who); return AFL_ERR_BAD_ARG; }
   int rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch));
   if (rc) return rc;
-  backdoor_table_kernel<<<static_cast<unsigned>((batch + 127) / 128), 128, 0, stream>>>(
-      batch, n, fs, zs, lrs, static_cast<ProblemParams*>(ws), status);
-  AFL_LAUNCH_CHECK("backdoor_table_kernel");
-  return AFL_OK;
+  TableArgs a = table_args(T_BACKDOOR, batch, n, fs, ws, status);
+  a.zs = zs; a.lrs = lrs;
+  return launch_table(a, stream);
 }
 
 // afl_backdoor_start_batched with device arrays: n bounds every f_b (the host call's fmax).
@@ -1366,12 +1286,7 @@ static int backdoor_start_dev(const void* G, int batch, int64_t batch_stride, in
                               int* status, cudaStream_t stream) {
   const char* who = "afl_backdoor_start_batched_dev";
   int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
-  if (rc) return rc;
-  if (!w || !mu_out || !sigma_out || !initial_out) { set_error("%s: w and every output are required", who); return AFL_ERR_BAD_ARG; }
-  if (w_batch_stride < 0 || (w_batch_stride > 0 && w_batch_stride < d)) {
-    set_error("%s: w_batch_stride %lld must be 0 (one shared w) or >= d", who, static_cast<long long>(w_batch_stride));
-    return AFL_ERR_BAD_ARG;
-  }
+  if (rc || (rc = check_backdoor_start(who, d, w, w_batch_stride, mu_out, sigma_out, initial_out))) return rc;
   if ((rc = backdoor_table_dev(who, batch, n, fs, zs, lrs, ws, ws_bytes, status, stream))) return rc;
   return colstats::backdoor_start(G, n, d, ld, dtype, batch, batch_stride, static_cast<const ProblemParams*>(ws), w,
                                   w_batch_stride, mu_out, sigma_out, initial_out, stream);
@@ -1385,18 +1300,9 @@ static int backdoor_finish_dev(int batch, int n, int64_t d, const int* fs, const
                                cudaStream_t stream) {
   const char* who = "afl_backdoor_finish_batched_dev";
   if (!mu || !sigma || !initial || !mal || !crafted_out || d < 1 || n < 1) { set_error("%s: bad argument", who); return AFL_ERR_BAD_ARG; }
-  if (batch < 1) { set_error("%s: batch must be >= 1 (got %d)", who, batch); return AFL_ERR_BAD_ARG; }
-  if (batch > kBatchMax) { set_error("%s: batch <= %d problems (got %d)", who, kBatchMax, batch); return AFL_ERR_UNSUPPORTED; }
-  if (batch > 1 && mal_batch_stride < d) {
-    set_error("%s: mal_batch_stride %lld makes problems overlap", who, static_cast<long long>(mal_batch_stride));
-    return AFL_ERR_BAD_ARG;
-  }
-  if (bcast_rows && (bcast_ld < d || (batch > 1 && bcast_batch_stride < static_cast<int64_t>(n - 1) * bcast_ld + d))) {
-    set_error("%s: bcast_ld / bcast_batch_stride make the written rows overlap", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  int rc = backdoor_table_dev(who, batch, n, fs, zs, lrs, ws, ws_bytes, status, stream);
-  if (rc) return rc;
+  int rc = check_backdoor_finish(who, batch, d, mal_batch_stride);
+  if (rc || (rc = check_bcast(who, bcast_rows, n, d, batch, bcast_batch_stride, bcast_ld))) return rc;
+  if ((rc = backdoor_table_dev(who, batch, n, fs, zs, lrs, ws, ws_bytes, status, stream))) return rc;
   return colstats::backdoor_finish(batch, d, static_cast<const ProblemParams*>(ws), mu, sigma, initial, mal,
                                    mal_batch_stride, crafted_out, bcast_rows, bcast_batch_stride, bcast_ld, stream);
 }
@@ -1409,19 +1315,11 @@ static int attack_metrics_dev(const void* G, int batch, int64_t batch_stride, in
                               cudaStream_t stream) {
   const char* who = "afl_attack_metrics_batched_dev";
   int rc = check_batch(who, G, batch, batch_stride, n, d, ld, dtype, INT32_MAX);
-  if (rc) return rc;
-  if (agg && idx) { set_error("%s: give the aggregate as agg or as idx, not both", who); return AFL_ERR_BAD_ARG; }
-  if ((dev_out || sums_out) && !agg && !idx) {
-    set_error("%s: dev_out and sums_out need an aggregate (agg or idx)", who);
-    return AFL_ERR_BAD_ARG;
-  }
-  if (krum_hit && !idx) { set_error("%s: krum_hit needs idx", who); return AFL_ERR_BAD_ARG; }
-  if ((mal_count || sel_count) && !sel) { set_error("%s: mal_count and sel_count need sel", who); return AFL_ERR_BAD_ARG; }
-  if (sel && sel_ld < 1) { set_error("%s: sel_ld must be >= 1 (got %d)", who, sel_ld); return AFL_ERR_BAD_ARG; }
+  if (rc || (rc = check_metrics_inputs(who, agg, idx, sel, sel_ld, dev_out, sums_out, krum_hit, mal_count, sel_count)))
+    return rc;
   if ((rc = check_dev(who, fs, status, ws, ws_bytes, table_bytes(batch) + metrics_partial_bytes(batch, d, dtype)))) return rc;
-  TableArgs a{};
-  a.rule = T_METRICS; a.batch = batch; a.n = n; a.rows = rows; a.fs = fs; a.table = static_cast<ProblemParams*>(ws);
-  a.status = status;
+  TableArgs a = table_args(T_METRICS, batch, n, fs, ws, status);
+  a.rows = rows;
   if ((rc = launch_table(a, stream))) return rc;
   return colstats::attack_metrics(G, batch, batch_stride, n, d, ld, dtype, 0, a.table, agg, idx, sel, sel_ld, dev_out,
                                   sums_out, honest_out, krum_hit, mal_count, sel_count,
@@ -1435,7 +1333,7 @@ static size_t trace_workspace_bytes(int batch, int64_t d) {
 }
 
 // One epoch's attack figures of an fp32 batch into row *slot of caller-held tables: afl_attack_metrics_batched_dev's
-// table and checks, then colstats::attack_trace.
+// table and selection checks, then colstats::attack_trace.
 static int attack_trace_dev(const float* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
                             const int* rows, const int* fs, const float* agg, const int* idx, const int* sel,
                             int sel_ld, const int* slot, int n_slots, int64_t table_ld, float* agg_dev,
@@ -1450,13 +1348,11 @@ static int attack_trace_dev(const float* G, int batch, int64_t batch_stride, int
     set_error("%s: table_ld %lld is less than batch %d", who, static_cast<long long>(table_ld), batch);
     return AFL_ERR_BAD_ARG;
   }
-  if (sel && sel_ld < 1) { set_error("%s: sel_ld must be >= 1 (got %d)", who, sel_ld); return AFL_ERR_BAD_ARG; }
-  if ((mal_count || sel_count) && !sel) { set_error("%s: mal_count and sel_count need sel", who); return AFL_ERR_BAD_ARG; }
+  if ((rc = check_sel(who, sel, sel_ld, mal_count, sel_count))) return rc;
   if (idx_out && !idx) { set_error("%s: idx_out needs idx", who); return AFL_ERR_BAD_ARG; }
   if ((rc = check_dev(who, fs, status, ws, ws_bytes, trace_workspace_bytes(batch, d)))) return rc;
-  TableArgs a{};
-  a.rule = T_METRICS; a.batch = batch; a.n = n; a.rows = rows; a.fs = fs; a.table = static_cast<ProblemParams*>(ws);
-  a.status = status;
+  TableArgs a = table_args(T_METRICS, batch, n, fs, ws, status);
+  a.rows = rows;
   if ((rc = launch_table(a, stream))) return rc;
   return colstats::attack_trace(G, batch, batch_stride, n, d, ld, a.table, agg, idx, sel, sel_ld, slot, n_slots,
                                 table_ld, agg_dev, mal_dev, idx_out, mal_count, sel_count,
@@ -1586,23 +1482,22 @@ size_t afl_batched_workspace_bytes(const char* rule, int batch, int n, int64_t d
   const BatchedRule r = batched_rule(rule);
   if (r == B_BAD || batch < 1 || batch > kBatchMax || n < 1 || n > kBatchMaxClients || d < 1) return 0;
   if (r == B_MEAN || r == B_TM) return 256;
-  size_t gram_ws = 0, tabs = 0;
-  return batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  return rule_scratch(r, batch, n, d, dtype).bytes;
 }
 
 size_t afl_batched_each_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
   const bool alie = rule && !strcmp(rule, "ALIE");
   const BatchedRule r = batched_rule(rule);
   if ((r == B_BAD && !alie) || batch < 1 || batch > kBatchMax || n < 1 || n > kBatchMaxClients || d < 1) return 0;
-  size_t gram_ws = 0, tabs = 0;
-  return table_bytes(batch) + batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  return table_bytes(batch) + rule_scratch(r, batch, n, d, dtype).bytes;
 }
 
 int afl_defend_batched(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld,
                        int dtype, int users_count, int corrupted_count, float* out, int* idx_out, int* sel_out,
                        void* workspace, size_t workspace_bytes, void* stream) {
-  return defend_batched(rule, G, batch, batch_stride, n, d, ld, dtype, users_count, corrupted_count, nullptr, out, idx_out,
-                        sel_out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  return defend_batched("afl_defend_batched", kBatchMaxClients, false, rule, G, batch, batch_stride, n, d, ld, dtype,
+                        nullptr, nullptr, users_count, nullptr, corrupted_count, out, idx_out, sel_out, workspace,
+                        workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 int afl_defend_batched_each(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
@@ -1612,8 +1507,9 @@ int afl_defend_batched_each(const char* rule, const void* G, int batch, int64_t 
     set_error("afl_defend_batched_each: the per-problem corrupted counts are NULL");
     return AFL_ERR_BAD_ARG;
   }
-  return defend_batched(rule, G, batch, batch_stride, n, d, ld, dtype, users_count, 0, corrupted_counts, out, idx_out,
-                        sel_out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  return defend_batched("afl_defend_batched_each", kBatchMaxClients, false, rule, G, batch, batch_stride, n, d, ld, dtype,
+                        nullptr, nullptr, users_count, corrupted_counts, 0, out, idx_out, sel_out, workspace,
+                        workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 int afl_alie_batched(const void* G_mal, int batch, int64_t batch_stride, int f, int64_t d, int64_t ld, int dtype, double z,
@@ -1643,9 +1539,9 @@ int afl_defend_batched_rows(const char* rule, const void* G, int batch, int64_t 
                             int64_t ld, int dtype, const int* rows, const int* users_counts, const int* corrupted_counts,
                             float* out, int* idx_out, int* sel_out, void* workspace, size_t workspace_bytes,
                             void* stream) {
-  return defend_batched_rows("afl_defend_batched_rows", kBatchMaxClients, rule, G, batch, batch_stride, n, d, ld, dtype,
-                             rows, users_counts, corrupted_counts, out, idx_out, sel_out, workspace, workspace_bytes,
-                             static_cast<cudaStream_t>(stream));
+  return defend_batched("afl_defend_batched_rows", kBatchMaxClients, true, rule, G, batch, batch_stride, n, d, ld, dtype,
+                        rows, users_counts, 0, corrupted_counts, 0, out, idx_out, sel_out, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream));
 }
 
 size_t afl_batched_large_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
@@ -1653,8 +1549,7 @@ size_t afl_batched_large_workspace_bytes(const char* rule, int batch, int n, int
   if (r == B_BAD || n < 1 || n > kBatchLargeMaxClients) return 0;
   if (n <= kBatchMaxClients) return afl_batched_rows_workspace_bytes(rule, batch, n, d, dtype);
   if (batch < 1 || batch > kBatchMax || d < 1 || (dtype != AFL_F32 && dtype != AFL_BF16 && dtype != AFL_F16)) return 0;
-  size_t gram_ws = 0, tabs = 0;
-  return class_table_bytes(batch, n) + batched_ws_parts(r, batch, n, d, dtype, &gram_ws, &tabs);
+  return class_table_bytes(batch, n) + rule_scratch(r, batch, n, d, dtype).bytes;
 }
 
 int afl_defend_batched_large(const char* rule, const void* G, int batch, int64_t batch_stride, int n, int64_t d,
@@ -1666,9 +1561,9 @@ int afl_defend_batched_large(const char* rule, const void* G, int batch, int64_t
     all.assign(static_cast<size_t>(batch), n);
     rows = all.data();
   }
-  return defend_batched_rows("afl_defend_batched_large", kBatchLargeMaxClients, rule, G, batch, batch_stride, n, d, ld,
-                             dtype, rows, users_counts, corrupted_counts, out, idx_out, sel_out, workspace,
-                             workspace_bytes, static_cast<cudaStream_t>(stream));
+  return defend_batched("afl_defend_batched_large", kBatchLargeMaxClients, true, rule, G, batch, batch_stride, n, d, ld,
+                        dtype, rows, users_counts, 0, corrupted_counts, 0, out, idx_out, sel_out, workspace,
+                        workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 int afl_alie_batched_large(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,
@@ -1750,9 +1645,9 @@ int afl_defend_batched_dev(const char* rule, const void* G, int batch, int64_t b
                            int dtype, const int* rows, int users_count, const int* users_counts,
                            const int* corrupted_counts, float* out, int* idx_out, int* sel_out, int sel_ld,
                            void* workspace, size_t workspace_bytes, int* status, void* stream) {
-  return defend_batched_dev(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_count, users_counts,
-                            corrupted_counts, out, idx_out, sel_out, sel_ld, workspace, workspace_bytes, status,
-                            static_cast<cudaStream_t>(stream));
+  return defend_batched_dev("afl_defend_batched_dev", kBatchMaxClients, rule, G, batch, batch_stride, n, d, ld, dtype,
+                            rows, users_count, users_counts, corrupted_counts, out, idx_out, sel_out, sel_ld, workspace,
+                            workspace_bytes, status, static_cast<cudaStream_t>(stream));
 }
 
 size_t afl_batched_large_dev_workspace_bytes(const char* rule, int batch, int n, int64_t d, int dtype) {
@@ -1765,9 +1660,9 @@ int afl_defend_batched_large_dev(const char* rule, const void* G, int batch, int
                                  int64_t ld, int dtype, const int* rows, int users_count, const int* users_counts,
                                  const int* corrupted_counts, float* out, int* idx_out, int* sel_out, int sel_ld,
                                  void* workspace, size_t workspace_bytes, int* status, void* stream) {
-  return defend_batched_large_dev(rule, G, batch, batch_stride, n, d, ld, dtype, rows, users_count, users_counts,
-                                  corrupted_counts, out, idx_out, sel_out, sel_ld, workspace, workspace_bytes, status,
-                                  static_cast<cudaStream_t>(stream));
+  return defend_batched_dev("afl_defend_batched_large_dev", kBatchLargeMaxClients, rule, G, batch, batch_stride, n, d,
+                            ld, dtype, rows, users_count, users_counts, corrupted_counts, out, idx_out, sel_out, sel_ld,
+                            workspace, workspace_bytes, status, static_cast<cudaStream_t>(stream));
 }
 
 int afl_alie_batched_dev(const void* G, int batch, int64_t batch_stride, int n, int64_t d, int64_t ld, int dtype,

@@ -73,6 +73,10 @@ def test_defend_each_preconditions_name_the_problem(nat):
     assert b"2*corrupted_count + 1" in msg and b"problem 2" in msg
     with pytest.raises(AssertionError, match="problem 2"):
         nat.check(defend(nat, counts(1, 2, 5, 1), rule=b"Krum"))
+    # every problem fails: the first failing one is named, not the first with the largest count
+    assert defend(nat, counts(5, 9), rule=b"Krum") == nat.AFL_ERR_PRECONDITION
+    msg = L.afl_last_error()
+    assert b"(10, 5) in problem 0" in msg
     # Bulyan: users_count >= 4 f_b + 3 for every b (defences.py:56); f = 2 holds at 11 users, f = 3 does not
     assert defend(nat, counts(2, 3, 0), rule=b"Bulyan", n=11, users=11, stride=11 * 64) == nat.AFL_ERR_PRECONDITION
     msg = L.afl_last_error()
